@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""bench.py -- items/s for the BGE-base embed .map() hot path on N B200s (BASELINE.json's metric).
+"""bench.py -- items/s for the BGE-base embed .map() hot path on N H100s (BASELINE.json's metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
     python bench.py --impl reference [...]                          # the CPU reference arm
+    python bench.py --dump-outputs DIR [...]                        # also write the timed path's last outputs as DIR/*.npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W   # N > 1: one rank per GPU
 
-A "step" is one pass of the hot path over one batch of synthetic input: 32 waves (32 x 148 = 4736 on a B200;
+A "step" is one pass of the hot path over one batch of synthetic input: 32 waves (32 x 132 = 4224 on an H100 SXM;
 BENCH_ITEMS_PER_STEP overrides) of 512-token items per GPU, presented as .map() inputs of 32 items (the reference's BATCH_SIZE,
 06_gpu_and_ml/embeddings/text_embeddings_inference.py:19).  Weak scaling: every rank owns one GPU and an
 equal shard of the items; the path has no data-path collective (items are independent), so ranks only
@@ -36,7 +37,7 @@ sys.path.insert(0, os.path.join(ROOT, "modal-examples_b200"))
 METRIC = "items/sec for BGE-base embed .map()"
 SEQ = 512
 MAP_INPUT_ITEMS = 32           # reference BATCH_SIZE
-ITEMS_PER_STEP = int(os.environ.get("BENCH_ITEMS_PER_STEP", "0"))  # per GPU; 0 = 32 waves of the runtime's wave size (32 x 148 = 4736 on a B200)
+ITEMS_PER_STEP = int(os.environ.get("BENCH_ITEMS_PER_STEP", "0"))  # per GPU; 0 = 32 waves of the runtime's wave size (32 x 132 = 4224 on an H100 SXM)
 REF_ITEMS_PER_STEP = 8         # bounded sample for the CPU arm
 FLOPS_PER_ITEM = 96.64e9       # BASELINE.md §4 (2*m*n*k, all rows, 12 layers)
 
@@ -56,7 +57,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"], tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="MEASURED_PEAKS.json (measured)")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="B200_PROFILING.md fallback")
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 -- a bound, not a measured rate
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -107,6 +109,29 @@ class ClockSampler:
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["no sample inside the timed region"]}
         return {"sm_mhz": statistics.median(sm), "sm_max_mhz": max(mx), "power_w_max": max(pw), "samples": len(sm), "reasons": sorted(reasons)}
+
+
+DUMP_BUDGET_BYTES = 64 << 20  # --dump-outputs writes at most this much in all
+
+
+def dump_outputs(dump_dir, emb):
+    """Write what the timed path returned in its last step, `emb` [n, hidden], as DUMP_DIR/embeddings.npy (float32).  Over the
+    budget, a fixed sample of rows is written instead (sorted numpy default_rng(0).choice(n, k, replace=False), the same for a
+    given n on every run), with their row indices as DUMP_DIR/embeddings_rows.npy (float64: exact for any row index)."""
+    import numpy as np
+
+    emb = np.ascontiguousarray(emb, dtype=np.float32)
+    n, hidden = emb.shape
+    names = {"embeddings.npy": emb}
+    if emb.nbytes > DUMP_BUDGET_BYTES:
+        k = (DUMP_BUDGET_BYTES - 4096) // (hidden * 4 + 8)  # 4 KB left for the two .npy headers
+        rows = np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+        names = {"embeddings.npy": emb[rows], "embeddings_rows.npy": rows.astype(np.float64)}
+    os.makedirs(dump_dir, exist_ok=True)
+    paths = [os.path.join(dump_dir, name) for name in names]
+    for path, a in zip(paths, names.values()):
+        np.save(path, a)
+    assert sum(os.path.getsize(path) for path in paths) <= DUMP_BUDGET_BYTES
 
 
 def dist_env():
@@ -180,6 +205,8 @@ def main_reference(args):
         out = R.forward_hf(model, ids)
     dt = time.perf_counter() - t0
     assert np.isfinite(out).all()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out)
     value = args.steps * REF_ITEMS_PER_STEP / dt
     sample = f"{REF_ITEMS_PER_STEP} items x {SEQ} tokens per step (bounded sample of the 1M-item workload), HF BertModel fp32, torch {threads} threads (fastest of a sweep up to the visible cores)"
     line = {
@@ -257,7 +284,7 @@ def main_ours(args):
     if world != args.gpus and world > 1:
         raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={world}")
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU fallback for the CUDA path (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: there is no CPU fallback for the CUDA path (use --impl reference for the CPU arm)")
     N = args.gpus
     if torch.cuda.device_count() < N:
         raise SystemExit(f"--gpus {N} but only {torch.cuda.device_count()} visible")
@@ -376,6 +403,10 @@ def main_ours(args):
     tw1 = time.perf_counter()
     t_wall1 = time.time()
     assert abs(dev_ms - (tw1 - tw0) * 1e3) < 0.05 * dev_ms + 10.0, f"CUDA-event time {dev_ms} and synchronised wall time {(tw1 - tw0) * 1e3} disagree"
+    if args.dump_outputs:
+        # the L2-normalised embeddings of every replica's items, in item order (inputs are seeded: replica r's shard is
+        # synth_ids(n_step, 512, seed=r), weights default_rng(0))
+        dump_outputs(args.dump_outputs, np.concatenate([dev[r]["out"].cpu().numpy() for r in range(N)]))
     st1 = b200rt.stats()
     clocks = sampler.stop(t_wall0, t_wall1)
     launches = st1["kernel_launches"] - st0["kernel_launches"]
@@ -552,14 +583,10 @@ def main_ours(args):
     top = max((k for k in prof if k in KERNEL_FLOPS), key=lambda k: prof[k])
     n_launch = g.layers
     achieved = KERNEL_FLOPS[top] * cap * n_launch / (prof[top] / 1e3) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get(top)
     total_ms = sum(prof.values())
     roofline = {
         "bound": "tensor", "kernel": top, "achieved": achieved, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
-        "frac": achieved / peaks["tflops_sustained"], "traffic": traffic, "peak_source": peaks["source"] + ", sustained bf16/fp16 dense",
+        "frac": achieved / peaks["tflops_sustained"], "peak_source": peaks["source"] + ", sustained bf16/fp16 dense",
         "launch_ms": prof[top] / n_launch, "share_of_forward": prof[top] / total_ms,
         "forward": {"items_per_s_per_gpu": value / N, "tflops": value / N * FLOPS_PER_ITEM / 1e12,
                     "frac_of_tensor_peak": value / N * FLOPS_PER_ITEM / 1e12 / peaks["tflops_sustained"],
@@ -592,7 +619,7 @@ def main_ours(args):
                    "seq_len": SEQ, "items_per_step_per_gpu": n_step, "items_per_step": n_total, "map_input_items": MAP_INPUT_ITEMS, "device_batch_items": cap,
                    "weights": "HF default init, numpy default_rng(0), shared with the oracle",
                    "parallelism": f"ONE process, one pool of {N} replica(s): scatter kernel -> peer HBM, forward per replica, pool+normalise stores into the root's gather buffer (no NCCL on the data path)",
-                   "l2": "per-step working set (218 MB fp16 weights + ~1.3 GB activations per replica) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (218 MB fp16 weights + ~1.0 GB activations per replica) exceeds the 50 MB L2; no explicit flush",
                    "precision": "fp16 tensor-core operands, fp32 accumulate, fp32 residual/LayerNorm/softmax"},
         "pool": {"replicas": N, "driving_processes": 1, "peer_bytes_per_step": per_step(s0, s1, "peer_bytes", args.steps),
                  "waves_per_step": per_step(s0, s1, "waves", args.steps)},
@@ -649,6 +676,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-vit", action="store_true", help="skip the secondary CLIP ViT-B/16 measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the timed path's outputs of its last step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3  # timing rule: W >= 3

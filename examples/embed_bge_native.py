@@ -1,7 +1,7 @@
 # ---
 # cmd: ["modal", "run", "examples/embed_bge_native.py"]
 # ---
-# # BGE-base embeddings on the in-box B200 runtime
+# # BGE-base embeddings on the in-box H100 runtime
 #
 # The reference's `06_gpu_and_ml/embeddings/text_embeddings_inference.py` with the TEI subprocess replaced by the
 # b200rt engine: same `@app.cls` / `@modal.enter` / `@modal.method` shape, same `generate_batches()` (batches of 32,
@@ -29,9 +29,9 @@ def random_blob(seed: int = 0):
     return rb(GEOMETRY, seed)
 
 
-@app.cls(gpu="B200:8", max_containers=1)
+@app.cls(gpu="H100:8", max_containers=1)
 # Batches in flight; the C++ scheduler coalesces them into waves.  The reference allows 20 containers x 10 inputs = 200
-# (text_embeddings_inference.py:79-86); one wave of the 8-replica pool is 8 x 148 items = 37 batches of 32 and the scheduler
+# (text_embeddings_inference.py:79-86); one wave of the 8-replica pool is 8 x 132 items = 33 batches of 32 and the scheduler
 # wants two to three waves' worth of tickets pending, hence 96 (each a thread blocked in b200rt_wait with the GIL released).
 @modal.concurrent(max_inputs=96)
 class TextEmbeddings:

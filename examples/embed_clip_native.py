@@ -1,7 +1,7 @@
 # ---
 # cmd: ["modal", "run", "examples/embed_clip_native.py"]
 # ---
-# # CLIP ViT-B/16 image embeddings on the in-box B200 runtime
+# # CLIP ViT-B/16 image embeddings on the in-box H100 runtime
 #
 # The reference's `06_gpu_and_ml/embeddings/image_embeddings_infinity.py` with the `infinity_emb` engine replaced by the
 # b200rt engine: the same `@app.cls` + `@modal.concurrent` class with an `@modal.enter` that brings the model up, an `embed`
@@ -22,7 +22,7 @@ with modal.Image.debian_slim().imports():
     import numpy as np
 
 
-@app.cls(gpu="B200:8", max_containers=1)
+@app.cls(gpu="H100:8", max_containers=1)
 @modal.concurrent(max_inputs=32)
 class ClipEngine:
     weights: str = modal.parameter(default="")

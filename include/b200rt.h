@@ -1,4 +1,4 @@
-/* b200rt -- C ABI of the in-box B200 runtime behind the `modal` shim's .map() fan-out.
+/* b200rt -- C ABI of the in-box H100 runtime behind the `modal` shim's .map() fan-out.
  *
  * The reference (modal-labs/modal-examples) has no native interface for this path: its fan-out is
  *   Function.map  -> cloudpickle -> gRPC -> one container per input -> gather
@@ -24,9 +24,9 @@ extern "C" {
 #define B200RT_E_STATE (-2)     /* not initialised / already initialised / shut down */
 #define B200RT_E_CUDA (-3)      /* CUDA error; the context is poisoned and every later call fails fast */
 #define B200RT_E_NOMEM (-4)
-#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_100, or geometry is not BERT-base */
+#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is not BERT-base */
 
-/* Geometry of a BERT encoder (HF BertConfig fields).  The sm_100a kernels are specialised for the
+/* Geometry of a BERT encoder (HF BertConfig fields).  The sm_90a kernels are specialised for the
  * BGE-base geometry (hidden 768, 12 heads of 64, inter 3072, max_pos <= 512); `layers` is free.   */
 typedef struct b200rt_bert_config {
     int32_t vocab, hidden, layers, heads, inter, max_pos, type_vocab;
@@ -53,9 +53,9 @@ typedef struct b200rt_stats_t {
 } b200rt_stats_t;
 
 /* Replica pool.  Stands in for `@app.cls(gpu=..., max_containers=N)` + `@modal.concurrent`
- * (text_embeddings_inference.py:79-86): n_gpus local B200s instead of N cloud containers.  Enables peer
+ * (text_embeddings_inference.py:79-86): n_gpus local H100s instead of N cloud containers.  Enables peer
  * access between all of them and starts the scheduler threads.  devices = NULL means 0..n_gpus-1.    */
-/* flags: bits 0-15 = items of 512 tokens one replica takes per wave (0 = default: the SM count of the first device, 148 on a B200), see B200RT_INIT_WAVE_ITEMS */
+/* flags: bits 0-15 = items of 512 tokens one replica takes per wave (0 = default: the SM count of the first device, 132 on an H100 SXM), see B200RT_INIT_WAVE_ITEMS */
 #define B200RT_INIT_WAVE_ITEMS(n) ((uint32_t)(n) & 0xFFFFu)
 /*        bits 16-23 = k > 0: TWO replicas per GPU; each replica's GEMM launches ask for (SMs - k) SMs and its attention launches
  *        for k, so that one replica's attention (MUFU-bound, light on L2) runs beside the other's GEMMs (L2-fill-bound).       */

@@ -4,8 +4,8 @@ This is the host-side mirror of the reference's interface for the embed hot path
 reference's ``TextEmbeddingsInference.embed`` (``06_gpu_and_ml/embeddings/text_embeddings_inference.py:97-104``)
 POSTs strings to a TEI server and ``.map`` (``:167``) fans batches out to cloud containers, an
 :class:`EmbedModel` takes token-id batches and the library's C++ scheduler fans them out to the local
-B200s.  There is no CPU path: importing works anywhere, but :func:`init` raises unless the shared
-library is built and a B200 is visible.
+H100s.  There is no CPU path: importing works anywhere, but :func:`init` raises unless the shared
+library is built and an H100 is visible.
 """
 from __future__ import annotations
 
@@ -121,7 +121,7 @@ _initialised = False
 
 def init(n_gpus: int = 1, devices=None, flags: int = 0, wave_items: int = 0) -> int:
     """Start the replica pool on ``devices`` (default ``0..n_gpus-1``).  Idempotent per process.
-    ``wave_items``: 512-token items one replica takes per wave (0 = the library default: one per SM, 148 on a B200)."""
+    ``wave_items``: 512-token items one replica takes per wave (0 = the library default: one per SM, 132 on an H100 SXM)."""
     global _initialised
     lib = load_library()
     if _initialised:

@@ -1,0 +1,229 @@
+// Multi-head self-attention for S <= 512, d = 64, on wgmma (sm_90a): persistent CTAs.
+//
+// A work unit is one (item, head) -- or, for batches with fewer units than SMs, one (item, head, query tile).  Each CTA walks
+// the units u = blockIdx.x, blockIdx.x + gridDim.x, ...  For the unit in hand one thread TMA-loads the head's K and V
+// (<= 512 x 64 fp16 each, up to four 128-key tiles, one mbarrier per tile) and the unit's 128-row query tiles (double
+// buffered) into 128B-swizzled shared memory; everything is issued up front, so the first sub-block's MMAs start as soon as
+// its own tile has landed.
+//
+// Two warpgroups; warpgroup c takes query rows 64c .. 64c+63 of every tile and walks the keys in 64-key sub-blocks:
+//   S   = Q . K_c^T      four wgmma.m64n64k16 (Q and K from shared memory, both K-major), fp32 in registers;
+//   online softmax       row max over the quad of threads that share a row, P = exp2((S - m) k) with k = log2(e) / 8, the
+//                        output accumulator and the partial row sum rescaled by exp2((m_old - m) k);
+//   O  += P . V_c        four wgmma.m64n64k16 with A = P (fp16) straight from the registers -- the S accumulator fragment
+//                        is already the A-operand fragment of the same rows -- and B = V_c (MN-major) from shared memory.
+// The tile's output ctx = O / l is staged in the tile's own (now idle) query buffer and leaves with one TMA store.
+//
+// Keys >= len are masked to -inf before the max (exactly P = 0, matching HF's additive -inf mask); sub-blocks wholly past
+// len are skipped.  Every query tile is computed the same way whether the item travels as one unit or split by query tile,
+// alone or in any batch, on any CTA, so an item's embedding is bit-identical in any batch (tests: scheduler / size-independent
+// properties).
+//
+// Restates BertSelfAttention.forward (HF modeling_bert.py:143-207) for the TEI /embed path the
+// reference calls at 06_gpu_and_ml/embeddings/text_embeddings_inference.py:100.
+#include "kernels.h"
+#include "ptx.cuh"
+
+namespace b200 {
+namespace attn {
+
+constexpr int QT = 128;      // query rows per tile
+constexpr int KB = 128;      // keys per K/V smem tile (TMA box)
+constexpr int SB = 64;       // keys per sub-block
+constexpr int D = HEAD_DIM;  // 64
+constexpr int MAX_KB = 4;    // S <= 512
+constexpr int TILE_BYTES = 128 * D * 2;              // 16 KB: 128 rows x 128 B
+constexpr int OFF_Q = 0;                             // 2 x 16 KB (double buffered across tiles), also the output staging tile
+constexpr int OFF_K = OFF_Q + 2 * TILE_BYTES;        // 4 x 16 KB
+constexpr int OFF_V = OFF_K + MAX_KB * TILE_BYTES;   // 4 x 16 KB
+constexpr int OFF_BAR = OFF_V + MAX_KB * TILE_BYTES;
+constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+constexpr int NUM_THREADS = 256;
+static_assert(SMEM_BYTES <= 232448, "shared memory");
+
+// softmax_scale * log2(e) with softmax_scale = 1/sqrt(64)
+constexpr float kScaleLog2e = 0.125f * 1.4426950408889634f;
+
+struct Unit {
+    int b, h, t0, nq;  // item, head, first query tile, query tiles
+    int len, nsb, nkb; // valid keys, 64-key sub-blocks, 128-key K/V tiles
+};
+
+__device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const int32_t* __restrict__ lens, int S) {
+    Unit U;
+    int unit = u;
+    U.t0 = 0;
+    if (split) {
+        U.t0 = unit % nq_all;
+        unit /= nq_all;
+    }
+    U.b = unit / HEADS;
+    U.h = unit % HEADS;
+    int len = __ldg(lens + U.b);
+    len = len < 1 ? 1 : (len > S ? S : len);
+    U.len = len;
+    U.nq = split ? 1 : nq_all;
+    U.nsb = (len + SB - 1) / SB;
+    U.nkb = (U.nsb + 1) / 2;
+    return U;
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tctx,
+                 const int32_t* __restrict__ lens, int S, int split, int n_units) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
+    uint64_t* kv_full = bars;          // [MAX_KB]  K tile j and V tile j of the unit have landed
+    uint64_t* q_full = bars + MAX_KB;  // [2]
+
+    griddep_launch_dependents();
+    const int lane = lane_id();
+    const int wg = threadIdx.x >> 7;          // which 64 query rows of a tile
+    const int w4 = (threadIdx.x >> 5) & 3;    // warp within the warpgroup: rows 16 w4 .. 16 w4 + 15
+    const int nq_all = (S + QT - 1) / QT;
+    const bool loader = threadIdx.x == 0;
+
+    if (loader) {
+        prefetch_tmap(&tq);
+        prefetch_tmap(&tctx);
+        for (int i = 0; i < MAX_KB; ++i) mbar_init(&kv_full[i], 1);
+        for (int i = 0; i < 2; ++i) mbar_init(&q_full[i], 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    griddep_wait();  // the prologue above overlapped the previous kernel's tail; nothing it wrote (qkv, lens) has been read yet
+
+    // this thread's rows of a tile (first and +8) and their 16-byte chunk in a 128B-swizzled row: dims 8j .. 8j+7 of row r
+    // sit in chunk j ^ (r & 7)
+    const int rr = wg * 64 + w4 * 16 + (lane >> 2);
+    const uint32_t cq = 4 * (lane & 3);  // byte offset of this thread's two dims inside a chunk
+    uint32_t kv_par = 0;                 // bit j: parity of the number of loads of K/V tile j so far
+    uint32_t gt = 0;                     // the CTA's running query-tile index
+    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const Unit U = decode_unit(u, nq_all, split, lens, S);
+        auto load_q = [&](uint32_t g, int t) {
+            mbar_arrive_expect_tx(&q_full[g & 1], TILE_BYTES);
+            tma_load_3d(smem + OFF_Q + (g & 1) * TILE_BYTES, &tq, &q_full[g & 1], U.h * D, (U.t0 + t) * QT, U.b);
+        };
+        if (loader) {
+            load_q(gt, 0);
+            for (int j = 0; j < U.nkb; ++j) {
+                mbar_arrive_expect_tx(&kv_full[j], 2 * TILE_BYTES);
+                tma_load_3d(smem + OFF_K + j * TILE_BYTES, &tq, &kv_full[j], HIDDEN + U.h * D, j * KB, U.b);
+                tma_load_3d(smem + OFF_V + j * TILE_BYTES, &tq, &kv_full[j], 2 * HIDDEN + U.h * D, j * KB, U.b);
+            }
+            if (U.nq > 1) load_q(gt + 1, 1);
+        }
+        for (int t = 0; t < U.nq; ++t) {
+            const uint32_t g = gt + t;
+            const uint32_t q_buf = smem_u32(smem + OFF_Q + (g & 1) * TILE_BYTES);
+            mbar_wait(&q_full[g & 1], (g >> 1) & 1);
+            float o[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) o[i] = 0.f;
+            float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+            const uint32_t q_addr = q_buf + wg * (64 * 128);
+#pragma unroll 1
+            for (int sb = 0; sb < U.nsb; ++sb) {
+                if ((sb & 1) == 0) mbar_wait(&kv_full[sb >> 1], (kv_par >> (sb >> 1)) & 1);
+                const uint32_t k_addr = smem_u32(smem + OFF_K) + sb * (SB * 128);
+                float s[32];
+                wgmma_fence();
+                fence_operands(s);
+#pragma unroll
+                for (int k = 0; k < D / 16; ++k)
+                    wgmma_m64n64k16_ss(s, make_sw128_desc(q_addr + k * 32), make_sw128_desc(k_addr + k * 32), k != 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_operands(s);
+                const int valid = U.len - sb * SB;  // keys [0, valid) of this sub-block are real (>= 1)
+                if (valid < SB) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i)
+                        if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) s[i] = -INFINITY;
+                }
+                uint32_t pa[4][4];  // P as the A fragments of the four 16-key steps
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float mx = -INFINITY;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffff, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffff, mx, 2));
+                    const float m_new = fmaxf(m_run[h], mx);
+                    const float alpha = ex2_approx((m_run[h] - m_new) * kScaleLog2e);  // 0 on the first sub-block
+                    m_run[h] = m_new;
+                    const float neg_ms = -m_new * kScaleLog2e;
+                    float ls = 0.f;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const float p0 = ex2_approx(fmaf(s[4 * j + 2 * h], kScaleLog2e, neg_ms));
+                        const float p1 = ex2_approx(fmaf(s[4 * j + 2 * h + 1], kScaleLog2e, neg_ms));
+                        ls += p0 + p1;
+                        // keys 8j .. 8j+7: k-step j/2, register 2 (j odd) + h
+                        pa[j >> 1][2 * (j & 1) + h] = pack_half2(p0, p1);
+                        o[4 * j + 2 * h] *= alpha;
+                        o[4 * j + 2 * h + 1] *= alpha;
+                    }
+                    l_run[h] = fmaf(l_run[h], alpha, ls);
+                }
+                const uint32_t v_addr = smem_u32(smem + OFF_V) + sb * (SB * 128);
+                wgmma_fence();
+                fence_operands(o);
+#pragma unroll
+                for (int kk = 0; kk < SB / 16; ++kk) wgmma_m64n64k16_rs_mn(o, pa[kk], make_sw128_desc(v_addr + kk * (16 * 128)), 1);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_operands(o);
+            }
+            // ctx = O / l, staged over this warpgroup's own rows of the tile's query buffer (its MMAs on them are complete)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float l = l_run[h];
+                l += __shfl_xor_sync(0xffffffff, l, 1);
+                l += __shfl_xor_sync(0xffffffff, l, 2);
+                const float inv_l = 1.0f / l;
+                const int r = rr + 8 * h;
+                const uint32_t row = q_buf + r * 128 + cq;
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(row + ((static_cast<uint32_t>(j) ^ (r & 7)) << 4)),
+                                 "r"(pack_half2(o[4 * j + 2 * h] * inv_l, o[4 * j + 2 * h + 1] * inv_l))
+                                 : "memory");
+            }
+            fence_proxy_async_smem();
+            __syncthreads();
+            if (loader) {  // rows past S are clipped by the tensor map
+                tma_store_3d(&tctx, smem + OFF_Q + (g & 1) * TILE_BYTES, U.h * D, (U.t0 + t) * QT, U.b);
+                tma_store_commit();
+                tma_store_wait_read<0>();  // the buffer is free again
+                if (t + 2 < U.nq) load_q(g + 2, t + 2);
+            }
+        }
+        kv_par ^= (1u << U.nkb) - 1;
+        gt += U.nq;
+        __syncthreads();  // K / V are reloaded for the next unit only once every warpgroup is done with them
+    }
+    if (loader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
+}
+
+}  // namespace attn
+
+cudaError_t attention_init_device() {
+    return cudaFuncSetAttribute(attn::attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SMEM_BYTES);
+}
+
+cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
+                             cudaStream_t stream) {
+    if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1) return cudaErrorInvalidValue;
+    // fewer (item, head) units than SMs: split them by query tile (K and V are then loaded once per tile, but a single item
+    // spreads over 48 SMs instead of 12)
+    const int nq = (S + attn::QT - 1) / attn::QT;
+    const int split = (B * HEADS < sm_count && nq > 1) ? 1 : 0;
+    const int n_units = B * HEADS * (split ? nq : 1);
+    const int grid = n_units < sm_count ? n_units : sm_count;
+    return launch_pdl(attn::attention_kernel, dim3(grid), dim3(attn::NUM_THREADS), attn::SMEM_BYTES, stream, tq, tctx, lens, S, split, n_units);
+}
+
+}  // namespace b200

@@ -98,20 +98,6 @@ int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, 
     return 0;
 }
 
-// fp16 2D row-major [rows, cols] -> box {32, 128} (64-byte rows), 64B swizzle: the residual epilogue's hi / lo staging chunks
-int make_map_2d_chunk(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols) {
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * 2};
-    cuuint32_t box[2] = {32, 128};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(B200RT_E_CUDA, "cuTensorMapEncodeTiled(chunk %llu x %llu) -> %d",
-                                       (unsigned long long)rows, (unsigned long long)cols, (int)r);
-    return 0;
-}
-
 // fp16 [B, S, width] (qkv: width 2304, ctx: width 768) -> box {64, 128, 1}, 128B swizzle (rows past S are zero-filled
 // on load and clipped on store)
 int make_map_qkv(CUtensorMap* m, const void* base, uint64_t B, uint64_t S, uint64_t width = QKV_DIM) {
@@ -140,7 +126,7 @@ struct LayerW {
     // LayerNorm folded into the consuming projections at load time (kernels.h):
     // qkv_w / ff1_w hold fp16(gamma o W, rows centred); *_c = W beta + b
     float *qkv_c, *ff1_c;
-    CUtensorMap m_qkv, m_ao, m_ff1, m_ff2;  // box {64,128}: each CTA of a pair stages half of the tile's columns
+    CUtensorMap m_qkv, m_ao, m_ff1, m_ff2;  // box {64,128}: GEMM B operands (two boxes per 256-column tile)
 };
 
 struct DevWeights {
@@ -171,9 +157,8 @@ struct Model {
 
 struct Dev {
     int id = -1;
-    int sm_count = 148;
-    int sm_gemm = 148, sm_attn = 148;  // SMs a GEMM / an attention launch of this replica asks for (see B200RT_INIT_SPLIT_SMS)
-    bool attn_pairs = false;           // launch the attention CTAs as clusters of 2 so that they take whole TPCs
+    int sm_count = 0;
+    int sm_gemm = 0, sm_attn = 0;  // SMs a GEMM / an attention launch of this replica asks for (see B200RT_INIT_SPLIT_SMS)
     cudaStream_t compute = nullptr;
     // workspace (capacity cap_rows rows)
     __half *yhi = nullptr, *ylo = nullptr;  // residual stream y = hi + lo, PRE-LayerNorm; hi doubles as the GEMM A operand
@@ -181,8 +166,6 @@ struct Dev {
     float* x32_dbg = nullptr;    // tests only (b200rt_debug_hidden): normalised fp32 rows, allocated on first use
     __half *qkv = nullptr, *ctx = nullptr, *ffn = nullptr;
     CUtensorMap m_yhi, m_ctx, m_ffn;      // fp16 [rows,*] box {64,128}: GEMM A operands (m_ffn is also FFN1's output map)
-    CUtensorMap m_qkv2d;                  // fp16 [rows,2304] box {64,128}: QKV GEMM output
-    CUtensorMap m_yhi_c, m_ylo_c;         // fp16 [rows,768] box {32,128} SW64: the residual epilogues update hi / lo in place
     std::unordered_map<int, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per padded length
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
     int32_t* ids_in[NSLOT] = {};
@@ -346,20 +329,20 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, c
         const LayerW& lw = w.layers[l];
         // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
         GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_yhi, lw.m_qkv, d.m_qkv2d, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
         ++nl; mark("gemm_qkv");
-        CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, nullptr, d.attn_pairs));
+        CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream));
         ++nl; mark("attention");
         // y <- ctx Wao^T + b + LN_prev(y); new row statistics (LN1's) into pstats[1]
         GemmEpi e_ao{lw.ao_b, d.pstats[0], STAT_PARTS, prev_g, prev_b, d.pstats[1], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ctx, lw.m_ao, d.m_yhi_c, &d.m_ylo_c, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
         ++nl; mark("gemm_attn_out");
         GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, d.m_yhi, lw.m_ff1, d.m_ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, d.m_yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
         ++nl; mark("gemm_ffn1_gelu");
         // y <- ffn W2^T + b + LN1(y); LN2's statistics into pstats[0]
         GemmEpi e_ff2{lw.ff2_b, d.pstats[1], STAT_PARTS, lw.ln1_g, lw.ln1_b, d.pstats[0], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ffn, lw.m_ff2, d.m_yhi_c, &d.m_ylo_c, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
         ++nl; mark("gemm_ffn2");
         prev_g = lw.ln2_g;
         prev_b = lw.ln2_b;
@@ -393,20 +376,20 @@ int forward_enqueue_vit(Dev& d, const Model& m, int dev_index, const float* pixe
     // embeddings, pre_layrnorm -> residual stream + statistics
     CUDA_TRY(launch_im2col(pixels, d.ffn, B, c.image, c.patch, stream));
     GemmEpi e_patch{w.zero_bias, nullptr, STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-    CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.m_ctx, nullptr, e_patch, M, HIDDEN, 3 * c.patch * c.patch, d.sm_gemm, stream));
+    CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, e_patch, M, HIDDEN, 3 * c.patch * c.patch, d.sm_gemm, stream));
     CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, T, c.eps, stream));
     nl += 3;
     for (int l = 0; l < L; ++l) {
         const LayerW& lw = w.layers[l];
         GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_yhi, lw.m_qkv, d.m_qkv2d, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
-        CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream, nullptr, d.attn_pairs));
+        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream));
         GemmEpi e_ao{lw.ao_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[1], c.eps};  // h += ctx Wo^T + b (raw residual)
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ctx, lw.m_ao, d.m_yhi_c, &d.m_ylo_c, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
         GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, d.m_yhi, lw.m_ff1, d.m_ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, d.m_yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
         GemmEpi e_ff2{lw.ff2_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[0], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ffn, lw.m_ff2, d.m_yhi_c, &d.m_ylo_c, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
         nl += 5;
     }
     if (n_layers < 0) {
@@ -470,11 +453,7 @@ int forward(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int
             cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr) {
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(stream, d.ev_ws, 0));
     int rc = 0;
-    bool use_graph = !(n_layers >= 0 || prof || B * S > GRAPH_MAX_ROWS);
-#ifdef B200RT_DIAG
-    static const bool no_graphs = getenv("B200RT_NO_GRAPHS") != nullptr;
-    if (no_graphs) use_graph = false;
-#endif
+    const bool use_graph = !(n_layers >= 0 || prof || B * S > GRAPH_MAX_ROWS);
     if (!use_graph) {
         rc = forward_enqueue(d, m, dev_index, ids, lens, B, S, out, stream, n_layers, prof, launches);
     } else {
@@ -930,16 +909,13 @@ int alloc_dev(Runtime& rt, Dev& d) {
     CUDA_TRY(cudaSetDevice(d.id));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, d.id));
-    if (prop.major != 10)
-        return fail(B200RT_E_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", d.id, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(B200RT_E_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", d.id, prop.major, prop.minor);
     d.sm_count = prop.multiProcessorCount;
     if (d.sm_attn >= d.sm_count || d.sm_attn < 2) {  // whole-GPU replica
         d.sm_gemm = d.sm_attn = d.sm_count;
-        d.attn_pairs = false;
     } else {  // two replicas share this GPU: GEMM launches leave sm_attn SMs to the other replica's attention launches
-        d.sm_attn &= ~1;
-        d.sm_gemm = (d.sm_count - d.sm_attn) & ~1;
-        d.attn_pairs = true;
+        d.sm_gemm = d.sm_count - d.sm_attn;
     }
     CUDA_TRY(kernels_init_device());
     CUDA_TRY(cudaStreamCreateWithFlags(&d.compute, cudaStreamNonBlocking));
@@ -963,9 +939,6 @@ int alloc_dev(Runtime& rt, Dev& d) {
     if (int rc = make_map_2d(&d.m_yhi, d.yhi, R, HIDDEN, 128)) return rc;
     if (int rc = make_map_2d(&d.m_ctx, d.ctx, R, HIDDEN, 128)) return rc;
     if (int rc = make_map_2d(&d.m_ffn, d.ffn, R, 3072, 128)) return rc;
-    if (int rc = make_map_2d(&d.m_qkv2d, d.qkv, R, QKV_DIM, 128)) return rc;
-    if (int rc = make_map_2d_chunk(&d.m_yhi_c, d.yhi, R, HIDDEN)) return rc;
-    if (int rc = make_map_2d_chunk(&d.m_ylo_c, d.ylo, R, HIDDEN)) return rc;
     for (int s = 0; s < NSLOT; ++s) {
         CUDA_TRY(cudaMalloc(&d.ids_in[s], R * 4));
         CUDA_TRY(cudaMalloc(&d.lens_in[s], R * 4));
@@ -989,10 +962,9 @@ int rt_init(const int* devices, int n, uint32_t flags) {
     auto rt = std::make_unique<Runtime>();
     if (flags & 0xFFFFu) rt->cap_items = static_cast<int>(flags & 0xFFFFu);  // B200RT_INIT_WAVE_ITEMS(n)
     if (rt->cap_items == 0) {
-        // Default: as many 512-token items as the GPU has SMs.  A wave of B items is 6B / 18B / 24B pair-GEMM tiles and 12B
-        // attention units, so with B = #SMs (= 2 x CTA pairs) every kernel of the forward runs a whole number of rounds
-        // (148 SMs: 12 / 36 / 48 tiles per pair, 12 units per SM); 128 items left attn-out, FFN2 and attention at 10.4 -> 11
-        // rounds (tools/wave_size_probe.py: 108.3 vs 110.2 us per item).
+        // Default: as many 512-token items as the GPU has SMs.  A wave of B items is 12B / 36B / 48B GEMM tiles (128 x 256)
+        // and 12B attention units, so with B = #SMs every kernel of the forward runs a whole number of rounds
+        // (H100 SXM, 132 SMs: 12 / 36 / 48 tiles and 12 attention units per SM).
         int sms = 0;
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, devices ? devices[0] : 0) != cudaSuccess || sms < 2) sms = 128;
         rt->cap_items = sms & ~1;
@@ -1695,9 +1667,7 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
                       const float* ln_gamma, const float* ln_beta, float eps, float* stats_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!a || !w || !bias || !out || M < 1 || N % 256 || K % 64 || epi < 0 || (epi & 0xFF) > 2) return fail(B200RT_E_INVALID, "bad gemm arguments");
-    const int epi_full = epi;  // bits 8+ = diagnostic mode of the pair kernel (B200RT_DIAG builds)
-    epi &= 0xFF;
+    if (!a || !w || !bias || !out || M < 1 || N % 256 || K % 64 || epi < 0 || epi > 2) return fail(B200RT_E_INVALID, "bad gemm arguments");
     if (ln_stats && epi != 2 && K % 128) return fail(B200RT_E_INVALID, "LayerNorm fold needs K % 128 == 0");
     if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
     Dev& d = *rt->devs[0];
@@ -1729,7 +1699,7 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     };
     CUDA_TRY(up(&dg, ln_gamma));
     CUDA_TRY(up(&dbt, ln_beta));
-    CUtensorMap ta, tb, tout, tlo;
+    CUtensorMap ta, tb;
     if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
     if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
     std::vector<__half> hhi, hlo;
@@ -1748,13 +1718,11 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
         CUDA_TRY(cudaMemcpy(dhi, dhi0, Mp * N * 2, cudaMemcpyDeviceToDevice));
         CUDA_TRY(cudaMemcpy(dlo, dlo0, Mp * N * 2, cudaMemcpyDeviceToDevice));
         CUDA_TRY(cudaMalloc(&dso, Mp * parts_out * sizeof(float2)));
-        if (int rc = make_map_2d_chunk(&tout, dhi, Mp, N)) return rc;
-        if (int rc = make_map_2d_chunk(&tlo, dlo, Mp, N)) return rc;
     } else {
         CUDA_TRY(cudaMalloc(&dout, Mp * N * 2));
         CUDA_TRY(cudaMemset(dout, 0xFF, Mp * N * 2));
-        if (int rc = make_map_2d(&tout, dout, Mp, N, 128)) return rc;
     }
+    __half* const o_hi = epi == 2 ? dhi : static_cast<__half*>(dout);
     GemmEpi e{db, dsi, parts_in, dg, dbt, dso, eps};
     // epi 2 updates hi / lo in place (y = acc + bias + LN(y)): reload the residual before the launch whose result is returned
     auto reload = [&]() -> cudaError_t {
@@ -1767,10 +1735,10 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     cudaEventCreate(&e1);
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi_full, ta, tb, tout, epi == 2 ? &tlo : nullptr, e, M, N, K, d.sm_count, d.compute));  // timing (values drift in place)
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, d.sm_count, d.compute));  // timing (values drift in place)
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(reload());
-    CUDA_TRY(launch_gemm(epi_full, ta, tb, tout, epi == 2 ? &tlo : nullptr, e, M, N, K, d.sm_count, d.compute));  // the result that is returned
+    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, d.sm_count, d.compute));  // the result that is returned
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
@@ -1822,36 +1790,6 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     cudaEventElapsedTime(&ms, e0, e1);
     if (ms_out) *ms_out = ms / iters;
     CUDA_TRY(cudaMemcpy(ctx, dc, M * HIDDEN * 2, cudaMemcpyDeviceToHost));
-#ifdef B200RT_DIAG
-    if (const char* path = getenv("B200RT_ATTN_STAMPS")) {  // diagnostics: per-phase clock stamps of CTA 0 -> text file
-        unsigned long long* dstamp = nullptr;
-        std::vector<unsigned long long> hs(10 * 32 * 8, 0);
-        CUDA_TRY(cudaMalloc(&dstamp, hs.size() * 8));
-        CUDA_TRY(cudaMemset(dstamp, 0, hs.size() * 8));
-        CUDA_TRY(launch_attention(tq, tc, dl_, B, S, d.sm_count, d.compute, dstamp));
-        CUDA_TRY(cudaStreamSynchronize(d.compute));
-        CUDA_TRY(cudaMemcpy(hs.data(), dstamp, hs.size() * 8, cudaMemcpyDeviceToHost));
-        unsigned long long t0 = ~0ull;
-        for (auto v : hs) if (v && v < t0) t0 = v;
-        if (FILE* f = fopen(path, "w")) {
-            const char* names[10] = {"exp_wg0", "exp_wg1", "exp_wg2", "epilogue", "pv", "s_issue", "tracker", "wg0_warp1", "wg0_warp2", "wg0_warp3"};
-            for (int o = 0; o < 10; ++o)
-                for (int c = 0; c < 32; ++c) {
-                    bool any = false;
-                    for (int sl = 0; sl < 8; ++sl) any |= hs[(o * 32 + c) * 8 + sl] != 0;
-                    if (!any) continue;
-                    fprintf(f, "%s c%02d:", names[o], c);
-                    for (int sl = 0; sl < 8; ++sl) {
-                        unsigned long long v = hs[(o * 32 + c) * 8 + sl];
-                        if (v) fprintf(f, " %llu", v - t0); else fprintf(f, " -");
-                    }
-                    fprintf(f, "\n");
-                }
-            fclose(f);
-        }
-        cudaFree(dstamp);
-    }
-#endif
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     cudaFree(dq); cudaFree(dc); cudaFree(dl_);
     return 0;

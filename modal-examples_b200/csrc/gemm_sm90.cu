@@ -1,0 +1,288 @@
+// Warp-specialised wgmma GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] . W[N,K]^T + bias)
+//
+// Persistent CTAs walk 128 x 256 output tiles (tile = blockIdx.x, blockIdx.x + gridDim.x, ...).  Three warpgroups:
+//   warpgroup 0  : one thread TMA-loads A [128 x 64] and W [256 x 64] per 64-wide k-block into a STAGES-deep ring
+//                  (48 KB per stage, 128B-swizzled), running ahead across tiles while the consumers are in their epilogue;
+//   warpgroups 1-2: consumer c owns rows 64c .. 64c+63 of the tile and all 256 columns: four wgmma.m64n256k16 per k-block
+//                  into 128 fp32 accumulator registers per thread, one k-block's MMAs kept in flight while the previous
+//                  stage is handed back to the producer; then the epilogue runs straight from the registers.
+//
+//   full[s]  : producer arrive.expect_tx(48 KB); the TMA loads complete_tx on it
+//   empty[s] : one arrival per consumer warp once the wgmma that read stage s have completed
+//
+// Epilogues (see kernels.h for the residual-stream format):
+//   EPI_BIAS(_GELU / _QGELU)_F16 : folded LayerNorm  rstd * acc + c  (c = W beta + b), optional GELU, fp16 out;
+//   EPI_BIAS_RES_SPLIT           : y' = acc + bias + LN(y) with the LayerNorm re-applied from the row's statistics, y' split
+//                                  into fp16 hi + lo in place, and the (sum, M2) partial of each new 128-column row slice.
+//
+// The accumulator fragment of thread (warp w of the consumer warpgroup, lane l) holds rows 16w + l/4 and 16w + l/4 + 8,
+// columns 8j + 2(l%4) + {0, 1} for j = 0..31: acc[4j + {0, 1}] on the first row, acc[4j + {2, 3}] on the second.
+//
+// Replaces (inside TEI, un-vendored; restated from HF modeling_bert.py): the Linear layers of
+// BertSelfAttention :143-207 (fused QKV), BertSelfOutput.dense :287-298, BertIntermediate :330-342
+// (dense + GELU) and BertOutput.dense :345-356.
+#include "kernels.h"
+#include "ptx.cuh"
+
+namespace b200 {
+namespace gemm {
+
+constexpr int BM = 128;  // rows per tile (two consumer warpgroups of 64)
+constexpr int BN = 256;  // columns per tile
+constexpr int BK = 64, STAGES = 4;
+constexpr int A_BYTES = BM * BK * 2;            // 16 KB
+constexpr int B_BYTES = BN * BK * 2;            // 32 KB (two TMA boxes of 128 rows)
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // 48 KB
+constexpr int OFF_BAR = STAGES * STAGE_BYTES;
+constexpr int NUM_THREADS = 384;
+constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+static_assert(SMEM_BYTES <= 232448, "shared memory");
+
+// erf-GELU x * Phi(x), erf by Abramowitz-Stegun 7.1.26 (abs err <= 1.5e-7): 2 MUFU (rcp, ex2) per value
+__device__ __forceinline__ float gelu_erf(float x) {
+    const float a = fabsf(x);
+    const float u = fmaf(a, 0.3275911f * 0.70710678118654752f, 1.0f);
+    float t;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(u));
+    float p = fmaf(0.5f * 1.061405429f, t, 0.5f * -1.453152027f);
+    p = fmaf(p, t, 0.5f * 1.421413741f);
+    p = fmaf(p, t, 0.5f * -0.284496736f);
+    p = fmaf(p, t, 0.5f * 0.254829592f);
+    const float q = p * t * ex2_approx(a * (-0.5f * 1.4426950408889634f) * a);
+    return x * (x >= 0.f ? 1.0f - q : q);
+}
+
+// CLIP's quick_gelu: x * sigmoid(1.702 x) = x / (1 + 2^(-1.702 log2(e) x))
+__device__ __forceinline__ float gelu_quick(float x) {
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(ex2_approx(x * (-1.702f * 1.4426950408889634f)) + 1.0f));
+    return x * r;
+}
+
+// LayerNorm statistics of a row from its STAT_PARTS (sum, M2) partials (Chan et al.)
+__device__ __forceinline__ void row_stats(const float2* __restrict__ st, float eps, float& mean, float& rstd) {
+    const float4* __restrict__ pp = reinterpret_cast<const float4*>(st);
+    const float4 a = __ldg(pp), b = __ldg(pp + 1), c = __ldg(pp + 2);
+    const float2 p[STAT_PARTS] = {make_float2(a.x, a.y), make_float2(a.z, a.w), make_float2(b.x, b.y),
+                                  make_float2(b.z, b.w), make_float2(c.x, c.y), make_float2(c.z, c.w)};
+    constexpr float inv_n = 1.0f / (128.0f * STAT_PARTS);
+    mean = (((p[0].x + p[1].x) + (p[2].x + p[3].x)) + (p[4].x + p[5].x)) * inv_n;
+    float m2[STAT_PARTS];
+#pragma unroll
+    for (int i = 0; i < STAT_PARTS; ++i) {
+        const float d = p[i].x * (1.0f / 128.0f) - mean;
+        m2[i] = fmaf(128.0f * d, d, p[i].y);
+    }
+    rstd = rsqrtf((((m2[0] + m2[1]) + (m2[2] + m2[3])) + (m2[4] + m2[5])) * inv_n + eps);
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
+            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
+    uint64_t* full = bars;            // [STAGES]
+    uint64_t* empty = bars + STAGES;  // [STAGES]
+
+    griddep_launch_dependents();
+    const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
+    const int lane = lane_id();
+    const int num_n = N / BN;
+    const int num_tiles = ((M + BM - 1) / BM) * num_n;
+    const int kblocks = K / BK;
+
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tma_a);
+        prefetch_tmap(&tma_b);
+        for (int s = 0; s < STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 8);  // the 8 consumer warps
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    griddep_wait();  // everything above overlapped the previous kernel's tail; nothing it wrote has been read yet
+
+    if (warp < 4) {
+        // -------------------------------------------------------------------- TMA producer
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
+                for (int kb = 0; kb < kblocks; ++kb) {
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    uint8_t* sa = smem + stage * STAGE_BYTES;
+                    mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
+                    tma_load_2d(sa, &tma_a, &full[stage], kb * BK, m0);
+                    tma_load_2d(sa + A_BYTES, &tma_b, &full[stage], kb * BK, n0);
+                    tma_load_2d(sa + A_BYTES + B_BYTES / 2, &tma_b, &full[stage], kb * BK, n0 + BN / 2);
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+        return;
+    }
+
+    // ------------------------------------------------------------------------ consumers
+    setmaxnreg_inc<232>();
+    const int cw = (warp >> 2) - 1;  // which 64 rows of the tile
+    const int w4 = warp & 3;
+    const float* __restrict__ bias = ep.bias;
+    const bool has_ln = ep.stats_in != nullptr;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM, n_blk = tile % num_n, n0 = n_blk * BN;
+        float acc[128];
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < kblocks; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t a_addr = smem_u32(smem + stage * STAGE_BYTES) + cw * (64 * 128);
+            const uint32_t b_addr = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
+            wgmma_fence();
+            fence_operands(acc);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+                wgmma_m64n256k16_ss(acc, make_sw128_desc(a_addr + k * 32), make_sw128_desc(b_addr + k * 32), (kb | k) != 0);
+            wgmma_commit();
+            fence_operands(acc);
+            if (prev >= 0) {
+                wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
+                if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_operands(acc);
+        if (lane == 0) mbar_arrive(&empty[prev]);
+
+        // -------------------------------------------------------------------- epilogue, straight from the registers
+        const int r0 = m0 + cw * 64 + w4 * 16 + (lane >> 2);  // this thread's rows r0 and r0 + 8
+        const int c0 = n0 + 2 * (lane & 3);                   // its columns c0 + 8j + {0, 1}
+        float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+        if (has_ln) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (r0 + 8 * h < M) row_stats(ep.stats_in + static_cast<size_t>(r0 + 8 * h) * STAT_PARTS, ep.eps, mean[h], rstd[h]);
+        }
+        if constexpr (EPI != EPI_BIAS_RES_SPLIT) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    // folded LayerNorm: rstd * acc + c -- the weight rows are centred at load time (sum_k W''[n,k] = 0), so the
+                    // row mean cancels inside the tensor core: sum_k (y_k - mean) W''_nk = sum_k y_k W''_nk
+                    float v0 = fmaf(rstd[h], acc[4 * j + 2 * h], bv.x);
+                    float v1 = fmaf(rstd[h], acc[4 * j + 2 * h + 1], bv.y);
+                    if constexpr (EPI == EPI_BIAS_GELU_F16) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                    if constexpr (EPI == EPI_BIAS_QGELU_F16) { v0 = gelu_quick(v0); v1 = gelu_quick(v1); }
+                    const int row = r0 + 8 * h;
+                    if (row < M) *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * N + c0 + 8 * j) = pack_half2(v0, v1);
+                }
+            }
+        } else {
+            // y' = acc + bias + LN(y); LN(y) = fmaf((y - mean) * rstd, gamma, beta) (stats_in NULL: the residual is added as is)
+            float csum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // [row][128-column half of the tile]
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                const int col = c0 + 8 * j;
+                const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + col));
+                float2 gm = make_float2(1.f, 1.f), bt = make_float2(0.f, 0.f);
+                if (has_ln) {
+                    gm = __ldg(reinterpret_cast<const float2*>(ep.ln_gamma + col));
+                    bt = __ldg(reinterpret_cast<const float2*>(ep.ln_beta + col));
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = r0 + 8 * h;
+                    float& v0 = acc[4 * j + 2 * h];
+                    float& v1 = acc[4 * j + 2 * h + 1];
+                    if (row < M) {
+                        const size_t off = static_cast<size_t>(row) * N + col;
+                        const float2 hv = __half22float2(*reinterpret_cast<const __half2*>(out + off));
+                        const float2 lv = __half22float2(*reinterpret_cast<const __half2*>(out_lo + off));
+                        v0 = v0 + bv.x + fmaf((hv.x + lv.x - mean[h]) * rstd[h], gm.x, bt.x);
+                        v1 = v1 + bv.y + fmaf((hv.y + lv.y - mean[h]) * rstd[h], gm.y, bt.y);
+                        // split y' = hi' + lo' and write both back in place
+                        const __half2 hp = __floats2half2_rn(v0, v1);
+                        const float2 hb = __half22float2(hp);
+                        *reinterpret_cast<__half2*>(out + off) = hp;
+                        *reinterpret_cast<uint32_t*>(out_lo + off) = pack_half2(v0 - hb.x, v1 - hb.y);
+                    }
+                    csum[h][j >> 4] += v0 + v1;
+                }
+            }
+            if (ep.stats_out != nullptr) {
+                // (sum, M2 about the slice mean) of each 128-column slice of the new rows: the four threads of a quad share a row
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int half = 0; half < 2; ++half) {
+                        float s = csum[h][half];
+                        s += __shfl_xor_sync(0xffffffff, s, 1);
+                        s += __shfl_xor_sync(0xffffffff, s, 2);
+                        const float mu = s * (1.0f / 128.0f);
+                        float m2 = 0.f;
+#pragma unroll
+                        for (int j = 16 * half; j < 16 * half + 16; ++j) {
+                            const float d0 = acc[4 * j + 2 * h] - mu, d1 = acc[4 * j + 2 * h + 1] - mu;
+                            m2 = fmaf(d0, d0, fmaf(d1, d1, m2));
+                        }
+                        m2 += __shfl_xor_sync(0xffffffff, m2, 1);
+                        m2 += __shfl_xor_sync(0xffffffff, m2, 2);
+                        const int row = r0 + 8 * h;
+                        if ((lane & 3) == 0 && row < M)
+                            ep.stats_out[static_cast<size_t>(row) * (N / 128) + n_blk * 2 + half] = make_float2(s, m2);
+                    }
+                }
+            }
+        }
+    }
+}
+
+}  // namespace gemm
+
+template <int EPI>
+static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
+                              int K, int sm_count, cudaStream_t stream) {
+    const int tiles = ((M + gemm::BM - 1) / gemm::BM) * (N / gemm::BN);
+    const int grid = tiles < sm_count ? tiles : sm_count;
+    return launch_pdl(gemm::gemm_kernel<EPI>, dim3(grid), dim3(gemm::NUM_THREADS), gemm::SMEM_BYTES, stream, ta, tb, e, out, out_lo, M, N, K);
+}
+
+cudaError_t gemm_init_device() {
+    cudaError_t e;
+    e = cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_GELU_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_QGELU_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_RES_SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
+}
+
+cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
+                        int K, int sm_count, cudaStream_t stream) {
+    if (N % gemm::BN != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
+    if (e.stats_in != nullptr && e.parts_in != STAT_PARTS) return cudaErrorInvalidValue;  // the LayerNorm'd width is HIDDEN
+    switch (epi) {
+        case EPI_BIAS_F16: return launch_one<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_GELU_F16: return launch_one<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_QGELU_F16: return launch_one<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_RES_SPLIT:
+            if (out_lo == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr))) return cudaErrorInvalidValue;
+            if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
+            return launch_one<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
+    }
+    return cudaErrorInvalidValue;
+}
+
+}  // namespace b200

@@ -1,4 +1,4 @@
-// Internal launch interface between the engine (host C++) and the sm_100a kernels.
+// Internal launch interface between the engine (host C++) and the sm_90a kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -32,13 +32,13 @@ cudaError_t kernels_init_device();
 //     row mean never has to be subtracted; its epilogue applies  rstd * acc + (W beta + b)   -- "LNfold";
 //   * a GEMM that adds the residual LN(y) re-applies (y - mean) * rstd * gamma + beta in its epilogue.
 //
-// C[M,N] = epi(A[M,K] . W[N,K]^T) on CTA pairs.  All operands move by TMA:
+// C[M,N] = epi(A[M,K] . W[N,K]^T).  A and W move by TMA:
 //   ta  : fp16 A   {K, rows>=M}  box {64,128} SW128     tb  : fp16 W {K, N} box {64,128} SW128
-//   EPI 0/1: tout = fp16 out {N, rows} box {64,128} SW128; e.stats_in (or NULL: plain acc + bias), e.bias
-//   EPI 2  : tout = hi, tlo = lo, both fp16 {N, rows} box {32,128} SW64 (read and written in place); e.stats_in + e.ln_gamma/
-//            e.ln_beta describe the LayerNorm of the residual (stats_in NULL: the residual is added as is); e.stats_out
-//            receives the partials of the new rows (N / 128 per row; must not alias stats_in: other tiles still read those).
-//   N % 256 == 0, K % 64 == 0; rows past M are clipped by the maps' own bounds.
+//   EPI 0/1/3: out = fp16 [M, N] row-major; e.stats_in (or NULL: plain acc + bias), e.bias
+//   EPI 2    : out = hi, out_lo = lo, both fp16 [M, N] row-major (read and written in place); e.stats_in + e.ln_gamma/
+//              e.ln_beta describe the LayerNorm of the residual (stats_in NULL: the residual is added as is); e.stats_out
+//              receives the partials of the new rows (N / 128 per row; must not alias stats_in: other tiles still read those).
+//   N % 256 == 0, K % 64 == 0; rows past M are neither read from out nor written.
 struct GemmEpi {
     const float* bias;        // [N]
     const float2* stats_in;   // [rows][parts_in]
@@ -48,8 +48,8 @@ struct GemmEpi {
     float2* stats_out;        // [rows][N / 128] EPI 2 (may be NULL)
     float eps;
 };
-cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const CUtensorMap* tlo,
-                        const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream);
+cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
+                        int K, int sm_count, cudaStream_t stream);
 
 // gamma != NULL: w_out[n,k] = fp16(w[n,k] gamma[k] - mean_k(w[n,:] gamma)), cvec[n] = sum_k w[n,k] beta[k] + bias[n]
 // gamma == NULL: w_out = fp16(w) (cvec untouched)
@@ -59,10 +59,8 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
 // Multi-head self-attention over a padded batch: qkv fp16 [B, S, 2304] (Q | K | V, head-major within each),
 // lens[B] valid keys per item, ctx fp16 [B*S, 768].  tq: 3D map over qkv {2304, S, B}, tctx: 3D map over ctx {768, S, B};
 // both box {64,128,1}, 128B swizzle.  Persistent: min(units, sm_count) CTAs walk the (item, head[, query tile]) units.
-// dbg: B200RT_DIAG builds only -- device buffer of 5*32*8 clock stamps written by CTA 0 (NULL in the product path)
-// pairs: launch the CTAs as clusters of 2 (no cooperation: only so that they occupy whole TPCs next to a CTA-pair GEMM)
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                             cudaStream_t stream, unsigned long long* dbg = nullptr, bool pairs = false);
+                             cudaStream_t stream);
 
 // word + position + token_type(0) embedding gather -> y = hi + lo (pre-LN residual stream) + the row's statistic partials.
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,

@@ -1,11 +1,10 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA, tcgen05 (MMA / TMEM), fences.
-// Everything here is hand-written for Blackwell; there is no fallback path.
+// Thin inline-PTX wrappers for sm_90a (Hopper): mbarrier, TMA, wgmma, fences.
+// Everything here is hand-written for Hopper; there is no fallback path.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <cstdio>
 
 namespace b200 {
 
@@ -41,7 +40,7 @@ __device__ __forceinline__ void fence_barrier_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 
-// make generic-proxy smem writes visible to the async proxy (TMA / tcgen05.mma operand reads)
+// make generic-proxy smem writes visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -69,17 +68,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 
-// Bounded wait: a protocol bug must trap (=> a CUDA error the host reports) instead of hanging the
-// GPU box.  try_wait suspends in hardware, so the poll count is small; the wall-clock bound is 4 s.
 __device__ __forceinline__ uint64_t global_timer_ns() {
     uint64_t t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
-
-#ifdef B200RT_DIAG
-__device__ uint32_t g_attn_prog = 0;  // shared-memory address of the attention kernel's per-role progress words (diagnostics)
-#endif
 
 // try_wait with a suspend-time hint: the waiting thread may stay suspended in hardware for up to `ns` nanoseconds (or until
 // the phase completes) instead of coming back after the default, much shorter, interval.
@@ -97,15 +90,13 @@ __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parit
     return ok != 0;
 }
 
-// Bounded wait: a protocol bug must trap (=> a CUDA error the host reports) instead of hanging the GPU box.  The retry loop
-// asks the hardware to keep the thread suspended for up to 20 us per attempt: ncu showed the single-thread roles' retry loops
-// (try_wait, counter, compare, branch -- ~7 instructions per wake-up at the default suspend time) taking ~20 % of the issue
-// slots of the attention kernel's SM sub-partitions, which they share with the exp warps.  The wall-clock bound is 4 s.
+// Bounded wait: a protocol bug must trap (=> a CUDA error the host reports) instead of hanging the GPU.  The retry loop asks
+// the hardware to keep the thread suspended for up to 20 us per attempt, so that waiting threads take few issue slots from
+// the warps that share their SM sub-partition.  The wall-clock bound is 4 s.  (No printf here: a function call anywhere in a
+// kernel makes ptxas serialise its wgmma pipeline.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
-    // retry loop: suspended in hardware for up to 20 us per attempt; the wall clock is only looked at every 256th wake-up
-    // (single-thread roles run this loop once per sub-block: ~15 instructions per wake-up for timer arithmetic were a
-    // measurable share of their instruction budget)
+    // the wall clock is only looked at every 256th wake-up
     uint64_t t0 = 0;
     uint32_t spins = 0;
     while (!mbar_try_wait_hint(bar, parity, 20000u)) {
@@ -116,46 +107,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             continue;
         }
         if (now - t0 > 4000000000ull) {
-            printf("b200rt: mbarrier wait timed out (block %d thread %d bar@%u parity %u)\n", (int)blockIdx.x,
-                   (int)threadIdx.x, smem_u32(bar), parity);
-#ifdef B200RT_DIAG
-            if (g_attn_prog != 0) {
-                for (int role = 0; role < 8; ++role) {
-                    uint32_t a, b, c;
-                    asm volatile("ld.volatile.shared.b32 %0, [%1];" : "=r"(a) : "r"(g_attn_prog + role * 16));
-                    asm volatile("ld.volatile.shared.b32 %0, [%1];" : "=r"(b) : "r"(g_attn_prog + role * 16 + 4));
-                    asm volatile("ld.volatile.shared.b32 %0, [%1];" : "=r"(c) : "r"(g_attn_prog + role * 16 + 8));
-                    printf("   block %d role %d: unit %u sub-block %u step %u\n", (int)blockIdx.x, role, a, b, c);
-                }
-            }
-#endif
             __trap();
         }
     }
-}
-
-// ------------------------------------------------------------------------------------ packed fp32 (sm_100: FFMA2 / FADD2)
-// Two IEEE fp32 operations per instruction -- same rounding as the scalar forms, half the issue slots.
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma2_f32(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ uint64_t mul2_f32(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ uint64_t add2_f32(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
 }
 
 // ------------------------------------------------------------------------------------ programmatic dependent launch
@@ -204,97 +158,6 @@ __device__ __forceinline__ void tma_store_wait_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-// ------------------------------------------------------------------------------------ tcgen05 / TMEM
-
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kCols) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], fp16 inputs, fp32 accumulate.  One thread issues.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M x 16 halves per instruction: lane = row, 8 consecutive 32-bit columns of
-// packed half2) is read from tensor memory
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread = lane = tile row)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// the store twin: 32 registers per thread -> 32 lanes x 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-        ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-          "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]),
-          "r"(taddr)
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t r4,
-                                                  uint32_t r5, uint32_t r6, uint32_t r7) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%8], {%0, %1, %2, %3, %4, %5, %6, %7};"
-                 ::"r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(r4), "r"(r5), "r"(r6), "r"(r7), "r"(taddr)
-                 : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // Warpgroup register re-allocation: every warp of an aligned group of four must execute the same one.
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() {
@@ -305,100 +168,80 @@ __device__ __forceinline__ void setmaxnreg_dec() {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 
-// ------------------------------------------------------------------------------------ CTA pair (cta_group::2)
+// ------------------------------------------------------------------------------------ wgmma
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// until at most N of this warpgroup's committed wgmma groups are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Pins accumulator registers in program order around wgmma issue / wait: the asynchronous MMA writes them behind the
+// compiler's back, so no read or write of them may be moved across the fence / wait.
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(cta)
-        : "memory");
-}
-
-// TMA load issued by either CTA of a pair; the transaction bytes land on the LEADER CTA's mbarrier
-// (bit 24 of a shared::cluster address selects the CTA of the pair).
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-        : "memory");
-}
-
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kCols) : "memory");
-}
-
-// D[tmem of both CTAs] (+)= A * B over the CTA pair (M = 256): issued by the leader CTA only.
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// commit of the pair's MMAs, arriving on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(cta_mask)
-        : "memory");
-}
-
-// ------------------------------------------------------------------------------------ descriptors
-
-// Shared-memory matrix descriptor for a 128B-swizzled tile whose rows are 128 bytes
-// (64 fp16) and whose 8-row groups are 1024 bytes apart (what a TMA box {64, rows} with
-// CU_TENSOR_MAP_SWIZZLE_128B writes).  Works for K-major operands (row = M/N index, the 128
-// bytes run along K) and for MN-major operands (row = K index, the 128 bytes run along N);
-// the major-ness itself is in the instruction descriptor.
-// bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2
-__host__ __device__ constexpr uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t lbo_bytes = 16,
-                                                       uint32_t sbo_bytes = 1024) {
+// Shared-memory matrix descriptor for a 128B-swizzled tile whose rows are 128 bytes (64 fp16) and whose 8-row groups are
+// 1024 bytes apart (what a TMA box {64, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes; the tile must be 1024-byte aligned).
+// K-major operand (row = M/N index, the 128 bytes run along K): SBO = 1024 is the stride between 8-row groups along M/N and
+// one k16 step is +32 bytes of start address.  MN-major operand (row = K index, the 128 bytes run along N = 64): SBO = 1024
+// is the stride between 8-row groups along K and one k16 step is +2048 bytes; LBO (the stride between 64-wide atoms along
+// N) is never used by an N = 64 operand.
+// bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 1 (128B swizzle)
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= 1ull << 46;
-    d |= 2ull << 61;
+    d |= static_cast<uint64_t>(1024 >> 4) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= 1ull << 62;
     return d;
 }
 
-// Instruction descriptor, kind::f16: fp16 A/B, fp32 D.  a_mn / b_mn = 1 for MN-major operands.
-// bits [4,6) c_format=1(F32) | [7,10) a_fmt=0(F16) | [10,13) b_fmt=0 | 15 a_major | 16 b_major |
-// [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n, int a_mn = 0, int b_mn = 0) {
-    return (1u << 4) | (static_cast<uint32_t>(a_mn) << 15) | (static_cast<uint32_t>(b_mn) << 16) |
-           (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
+// D (+)= A[smem] . B[smem]^T, m64n256k16, fp16 in, fp32 accumulate; both operands K-major.  Issued by a whole warpgroup.
+__device__ __forceinline__ void wgmma_m64n256k16_ss(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D (+)= A[smem] . B[smem]^T, m64n64k16, fp16 in, fp32 accumulate; both operands K-major.  Issued by a whole warpgroup.
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D (+)= A[registers] . B[smem], m64n64k16, fp16 in, fp32 accumulate; B is MN-major (rows of B run along N).  A is the
+// warpgroup's fragment of a 64 x 16 tile in the mma.m16n8k16 A layout (warp w holds rows 16w .. 16w+15).
+__device__ __forceinline__ void wgmma_m64n64k16_rs_mn(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
 }
 
 // ------------------------------------------------------------------------------------ shared-memory accessors

@@ -1,4 +1,4 @@
-// HBM-bound row-wise kernels (sm_100a): embedding gather into the split residual stream, CLS pooling + final LayerNorm +
+// HBM-bound row-wise kernels (sm_90a): embedding gather into the split residual stream, CLS pooling + final LayerNorm +
 // L2 normalise with the store aimed at the root GPU's gather buffer, the root-side scatter of token ids into (peer) shard
 // inputs, the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns), and a debug-only
 // LayerNorm materialisation.
@@ -371,7 +371,7 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
 
 cudaError_t launch_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t stream) {
     if (n % 4 != 0) return cudaErrorInvalidValue;
-    rw::f32_to_f16_kernel<<<148 * 8, 256, 0, stream>>>(src, dst, n / 4);
+    rw::f32_to_f16_kernel<<<132 * 8, 256, 0, stream>>>(src, dst, n / 4);
     return cudaGetLastError();
 }
 
@@ -383,7 +383,7 @@ cudaError_t launch_scatter(const int32_t* src_ids, const int32_t* src_lens, cons
     if (max_cnt == 0) return cudaSuccess;
     const size_t n4 = (static_cast<size_t>(max_cnt) * plan.S + 3) / 4;
     int gx = static_cast<int>((n4 + 255) / 256);
-    gx = gx < 1 ? 1 : (gx > 148 * 4 ? 148 * 4 : gx);
+    gx = gx < 1 ? 1 : (gx > 132 * 4 ? 132 * 4 : gx);
     rw::scatter_kernel<<<dim3(gx, plan.n_shards), 256, 0, stream>>>(src_ids, src_lens, plan);
     return cudaGetLastError();
 }

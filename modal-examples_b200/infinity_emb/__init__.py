@@ -4,7 +4,7 @@ EngineArgs(model_name_or_path="openai/clip-vit-base-patch16", engine=torch, dtyp
 ``await engine.astart()``, ``embeddings, usage = await engine.image_embed(images=[PIL images])``, ``await engine.astop()``.
 
 Like ``text-embeddings-router`` (tei_router/), it is the boundary the reference script already talks to, re-implemented
-over the b200rt C ABI: the CLIP ViT-B/16 image tower runs on the hand-written sm_100a kernels (kind "vit"), preprocessing
+over the b200rt C ABI: the CLIP ViT-B/16 image tower runs on the hand-written sm_90a kernels (kind "vit"), preprocessing
 is preprocess.clip_preprocess.  The reference starts one engine per concurrent input to pack a GPU with model copies
 (``n_engines``, :283-306); here every engine object of a process shares ONE loaded model and the scheduler's replica pool --
 concurrency comes from tickets in flight, not from model copies.  There is no CPU path: without the CUDA library (or a
@@ -115,7 +115,7 @@ class AsyncEmbeddingEngine:
         a = self._args
         dev = a.device.value if isinstance(a.device, Device) else str(a.device)
         if dev not in ("cuda", "auto"):
-            raise ValueError(f"infinity_emb/b200rt: device={dev!r} is not available: the engine runs on B200 GPUs only")
+            raise ValueError(f"infinity_emb/b200rt: device={dev!r} is not available: the engine runs on H100 GPUs only")
         with _lock:
             if _runtime_refs == 0:
                 _owns_runtime = not b200rt._initialised  # an application may already run the pool for its text models

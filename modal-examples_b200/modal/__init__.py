@@ -1,5 +1,5 @@
 """In-box ``modal``: the Python surface the reference scripts are written against (``modal-labs/modal-examples``,
-census in SURVEY.md §2.2), executing on the local 8xB200 host instead of the Modal cloud.  GPU work goes through
+census in SURVEY.md §2.2), executing on the local multi-H100 host instead of the Modal cloud.  GPU work goes through
 ``b200rt`` (ctypes over ``libb200rt.so``); everything that only makes sense in the cloud (images, secrets stores,
 web endpoints, schedules) is accepted and inert so that scripts import and run unchanged."""
 from . import config, exception, experimental, gpu  # noqa: F401

@@ -1,6 +1,6 @@
 """``modal.App``: registry + decorators.  ``@app.function`` / ``@app.cls`` / ``@app.local_entrypoint`` with the
 keyword census of SURVEY.md §2.2; unknown keywords are accepted and recorded (cloud-only knobs have no in-box
-meaning), ``gpu=`` is parsed to a local B200 count."""
+meaning), ``gpu=`` is parsed to a local H100 count."""
 from __future__ import annotations
 
 import contextlib

@@ -1,5 +1,5 @@
 """``gpu=`` grammar (SURVEY.md §2.2): "H100", "a10g", "A100-80GB", "H100:2", f"B200:{N}", "H100!", "any",
-lists of fallbacks, ``modal.gpu.L40S(count=N)``, None/False.  In-box every value means "N of the local B200s"."""
+lists of fallbacks, ``modal.gpu.L40S(count=N)``, None/False.  In-box every value means "N of the local H100s"."""
 from __future__ import annotations
 
 

@@ -303,6 +303,6 @@ class Sandbox:
 
     @staticmethod
     def create(*_a, **_k):
-        raise NotImplementedError("modal.Sandbox is outside the in-box B200 runtime's scope")
+        raise NotImplementedError("modal.Sandbox is outside the in-box H100 runtime's scope")
 
     from_id = from_name = create

@@ -1,7 +1,7 @@
 """BERT uncased tokenisation (BasicTokenizer + greedy WordPiece), restated from the published algorithm that
 ``transformers.BertTokenizer`` implements (tests/test_tokenizer.py checks this file against it on the same
-vocabulary).  TEI tokenises with the model repo's ``tokenizer.json``; no BERT vocabulary exists offline
-(SURVEY.md §7.4.5), so a real ``vocab.txt`` is optional (``--tokenizer-vocab`` / ``B200RT_VOCAB``) and the
+vocabulary).  TEI tokenises with the model repo's ``tokenizer.json``; no BERT vocabulary exists offline,
+so a real ``vocab.txt`` is optional (``--tokenizer-vocab`` / ``B200RT_VOCAB``) and the
 fallback is a deterministic SYNTHETIC vocabulary -- the server says so at start-up; embeddings of strings are
 then not comparable with the real model's (token-id inputs are unaffected)."""
 from __future__ import annotations

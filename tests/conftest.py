@@ -11,7 +11,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run under gpurun); everything else runs on CPU")
+    config.addinivalue_line("markers", "gpu: needs an H100; everything else runs on CPU")
 
 
 def _has_gpu():

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, exports every symbol include/*.h declares, and fails
+"""CPU: the C-ABI library builds for sm_90a, loads, exports every symbol include/*.h declares, and fails
 loudly (no CPU fallback) when there is no GPU.  No compute calls here."""
 import ctypes
 import os
@@ -28,17 +28,17 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in include/ but not exported"
 
 
-def test_library_is_blackwell_native():
-    """SASS must carry the tcgen05 / TMA / TMEM mnemonics (B200_PROFILING.md) and only sm_100a code."""
+def test_library_is_hopper_native():
+    """SASS must carry the wgmma / TMA mnemonics and only sm_90a code."""
     import b200rt
 
     cuobjdump = "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     elf = subprocess.run([cuobjdump, "-lelf", b200rt.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in elf and not re.search(r"sm_(7|8|9)\d", elf)
+    assert "sm_90a" in elf and not re.search(r"sm_(7\d|8\d|10\d|12\d)", elf)
     sass = subprocess.run([cuobjdump, "-sass", b200rt.LIB_PATH], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "LDTM", "UTMALDG"):
+    for mnem in ("HGMMA", "UTMALDG", "UTMASTG"):
         assert mnem in sass, f"{mnem} missing from SASS"
     assert "HMMA.16816" not in sass, "legacy mma.sync path found"
 

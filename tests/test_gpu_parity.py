@@ -175,16 +175,16 @@ def _ref_attention(qkv, lens, B, S):
 
 @pytest.mark.parametrize("B,S,lens", [(2, 512, [512, 300]), (13, 512, [512] * 12 + [77])])
 def test_attention_running_max_rescale(rt, B, S, lens):
-    """Scores that climb by more than the kernel's 2^8 lazy-rescale threshold from one 64-key sub-block to the next
-    (for the rows whose query points along u; they fall for the others), so that the in-TMEM accumulator rescale runs at
-    every sub-block for part of each warp.  B = 2 takes the query-tile-split launch, B = 13 the one-CTA-per-head launch."""
+    """Scores that climb steeply from one 64-key sub-block to the next (raw q.k steps by 48 for the rows whose query points
+    along u; they fall for the others), so that the running maximum moves and the online softmax rescales the output
+    accumulator and the row sum at every sub-block for part of each warp.  B = 2 takes the query-tile-split launch, B = 13 the one-CTA-per-head launch."""
     rng = np.random.default_rng(7 * B + S)
     x = rng.standard_normal((B, S, 3, 12, 64)) * 0.5
     u = rng.standard_normal(64)
     u /= np.linalg.norm(u)
     sign = np.where(rng.random((B, S, 12, 1)) < 0.6, 1.0, -1.0)
     x[:, :, 0] += 4.0 * sign * u                                          # q . u = +-4
-    x[:, :, 1] += (12.0 * (np.arange(S) // 64))[None, :, None, None] * u  # k . u = 12 * sub-block: raw q.k steps by 48 > 44.4
+    x[:, :, 1] += (12.0 * (np.arange(S) // 64))[None, :, None, None] * u  # k . u = 12 * sub-block: raw q.k steps by 48
     qkv = x.reshape(B * S, 2304).astype(np.float16)
     ctx, _ = rt.debug_attention(qkv, np.array(lens, np.int32), B, S)
     ref = _ref_attention(qkv, lens, B, S)

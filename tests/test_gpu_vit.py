@@ -106,7 +106,7 @@ def test_scheduler_waves_pool_and_text_model_side_by_side(rt):
 def test_infinity_emb_adapter_matches_the_oracle_on_pil_images(rt, tmp_path):
     """The product's `infinity_emb` stand-in (what image_embeddings_infinity.py:296-306, 340-350 drives): engines started the
     reference's way -- several per process, one per concurrent input -- share one loaded model; PIL images go through
-    preprocess.clip_preprocess and the sm_100a tower; vectors equal the oracle's on HF-CLIPImageProcessor pixels.  Weights
+    preprocess.clip_preprocess and the sm_90a tower; vectors equal the oracle's on HF-CLIPImageProcessor pixels.  Weights
     come from a .safetensors checkpoint in HF CLIP naming (the real-checkpoint path)."""
     import asyncio
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Diagnostics: where one 512-token item's ~1 ms goes -- per-kernel device times of a 1-item forward (events between
+"""Diagnostics: where one 512-token item's time goes -- per-kernel device times of a 1-item forward (events between
 launches, no graph), the graph-replayed forward end to end, and the host path around it."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
