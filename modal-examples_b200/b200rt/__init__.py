@@ -28,7 +28,13 @@ ABI_SYMBOLS = [
     "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items",
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
-DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_hidden", "b200rt_debug_vit_hidden", "b200rt_debug_profile_forward"]
+DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_hidden", "b200rt_debug_vit_hidden", "b200rt_debug_profile_forward",
+                 "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_vit_pool", "b200rt_debug_fold_ln"]
+
+
+def SPLIT_SMS(k: int) -> int:
+    """``init`` flag (B200RT_INIT_SPLIT_SMS): two replicas per GPU, each replica's GEMMs on all but k SMs, its attention on k."""
+    return (k & 0xFF) << 16
 
 
 class B200RTError(RuntimeError):
@@ -95,8 +101,15 @@ def load_library():
         lib.b200rt_shutdown.restype = None
         lib.b200rt_debug_gemm.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p, ctypes.c_void_p,
-                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p]
-        lib.b200rt_debug_attention.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p]
+                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_int]
+        lib.b200rt_debug_attention.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p,
+                                               ctypes.c_int]
+        vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
+        lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp]
+        lib.b200rt_debug_vit_embed.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, vp, vp]
+        lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp]
+        lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
+        lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
         lib.b200rt_debug_hidden.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                      f32p, i32p, ctypes.c_int]
@@ -356,9 +369,10 @@ def device_sync(gpu: int = 0):
 
 
 def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, resid=None, iters: int = 1, ln_stats=None,
-               ln_gamma=None, ln_beta=None, eps: float = 1e-12, want_stats: bool = False):
+               ln_gamma=None, ln_beta=None, eps: float = 1e-12, want_stats: bool = False, sms: int = 0):
     """a16 [M,K], w16 [N,K] float16; returns (out, ms) -- or (out, ms, stats_out [M, N/128, 2]) with ``want_stats`` (epi 2).
-    ``ln_stats`` [M, parts, 2] (sum, M2) partials switch the LayerNorm epilogues on (see include/b200rt_debug.h)."""
+    ``ln_stats`` [M, parts, 2] (sum, M2) partials switch the LayerNorm epilogues on (see include/b200rt_debug.h).
+    ``sms``: CTAs of the persistent launch (0 = every SM)."""
     a16 = np.ascontiguousarray(a16, dtype=np.float16)
     w16 = np.ascontiguousarray(w16, dtype=np.float16)
     bias = np.ascontiguousarray(bias, dtype=np.float32)
@@ -371,14 +385,75 @@ def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, res
     p = lambda v: _ptr(v) if v is not None else None  # noqa: E731
     ms = ctypes.c_float(0)
     _check(load_library().b200rt_debug_gemm(epi, _ptr(a16), _ptr(w16), _ptr(bias), p(r), _ptr(out), M, N, K, iters, ctypes.byref(ms),
-                                            p(st), p(lg), p(lb), eps, p(so)))
+                                            p(st), p(lg), p(lb), eps, p(so), sms))
     return (out, ms.value, so) if want_stats else (out, ms.value)
 
 
-def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1):
+def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0):
     qkv16 = np.ascontiguousarray(qkv16, dtype=np.float16)
     lens = np.ascontiguousarray(lens, dtype=np.int32)
     ctx = np.empty((B * S, 768), np.float16)
     ms = ctypes.c_float(0)
-    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms)))
+    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms))
     return ctx, ms.value
+
+
+# Row kernels behind host buffers (include/b200rt_debug.h).  hi / lo are float16 arrays [rows, 768]; stats [rows, 6, 2].
+def _f32(v):
+    return np.ascontiguousarray(v, dtype=np.float32)
+
+
+def _f16(v):
+    return np.ascontiguousarray(v, dtype=np.float16)
+
+
+def debug_embed(ids: np.ndarray, word: np.ndarray, pos: np.ndarray, type0: np.ndarray, S: int):
+    """ids [n_tokens] (token t sits at position t % S); returns (hi, lo, stats)."""
+    ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+    word, pos, type0 = _f32(word), _f32(pos), _f32(type0)
+    n = ids.size
+    hi, lo = np.empty((n, 768), np.float16), np.empty((n, 768), np.float16)
+    st = np.empty((n, 6, 2), np.float32)
+    _check(load_library().b200rt_debug_embed(_ptr(ids), _ptr(word), _ptr(pos), _ptr(type0), n, S, word.shape[0], _ptr(hi), _ptr(lo), _ptr(st)))
+    return hi, lo, st
+
+
+def debug_vit_embed(patch_out: np.ndarray, cls: np.ndarray, pos: np.ndarray, gamma: np.ndarray, beta: np.ndarray, T: int, eps: float):
+    """patch_out [rows, 768] float16 (row t is token t % T); returns (hi, lo, stats)."""
+    patch_out, cls, pos, gamma, beta = _f16(patch_out), _f32(cls), _f32(pos), _f32(gamma), _f32(beta)
+    n = patch_out.shape[0]
+    hi, lo = np.empty((n, 768), np.float16), np.empty((n, 768), np.float16)
+    st = np.empty((n, 6, 2), np.float32)
+    _check(load_library().b200rt_debug_vit_embed(_ptr(patch_out), _ptr(cls), _ptr(pos), _ptr(gamma), _ptr(beta), n, T, eps,
+                                                 _ptr(hi), _ptr(lo), _ptr(st)))
+    return hi, lo, st
+
+
+def debug_pool_normalize(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta: np.ndarray, S: int, eps: float):
+    """hi, lo [n_items * S, 768]: the LayerNorm'd, L2-normalised row i * S of every item, [n_items, 768]."""
+    hi, lo, gamma, beta = _f16(hi), _f16(lo), _f32(gamma), _f32(beta)
+    n = hi.shape[0] // S
+    out = np.empty((n, 768), np.float32)
+    _check(load_library().b200rt_debug_pool_normalize(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), n, S, eps, _ptr(out)))
+    return out
+
+
+def debug_vit_pool(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta: np.ndarray, proj: np.ndarray, T: int, eps: float):
+    """hi, lo [n_items * T, 768], proj [P, 768]: normalise(proj . LayerNorm(row i * T)), [n_items, P]."""
+    hi, lo, gamma, beta, proj = _f16(hi), _f16(lo), _f32(gamma), _f32(beta), _f32(proj)
+    n, P = hi.shape[0] // T, proj.shape[0]
+    out = np.empty((n, max(P, 1)), np.float32)
+    _check(load_library().b200rt_debug_vit_pool(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), _ptr(proj), n, T, P, eps, _ptr(out)))
+    return out
+
+
+def debug_fold_ln(w: np.ndarray, gamma=None, beta=None, bias=None):
+    """w [N, K] float32; returns (w_out float16 [N, K], cvec [N] or None when gamma is None)."""
+    w = _f32(w)
+    N, K = w.shape
+    p = lambda v: _ptr(v) if v is not None else None  # noqa: E731
+    g, b, bs = (_f32(v) if v is not None else None for v in (gamma, beta, bias))
+    w_out = np.empty((N, K), np.float16)
+    cvec = np.empty(N, np.float32) if gamma is not None else None
+    _check(load_library().b200rt_debug_fold_ln(_ptr(w), p(g), p(b), p(bs), N, K, _ptr(w_out), p(cvec)))
+    return w_out, cvec

@@ -1327,6 +1327,33 @@ int check_ids(const b200rt_bert_config& c, const int32_t* ids, const int32_t* le
     return 0;
 }
 
+// Device buffers of one row-kernel debug entry (b200rt_debug_embed & co.): filled from the host (or zeroed) in stream order on
+// allocation, and all freed when the entry returns, on success or on error.
+struct DebugBuffers {
+    cudaStream_t stream;
+    std::vector<void*> ptrs;
+    explicit DebugBuffers(cudaStream_t s) : stream(s) {}
+    DebugBuffers(const DebugBuffers&) = delete;
+    DebugBuffers& operator=(const DebugBuffers&) = delete;
+    ~DebugBuffers() {
+        cudaStreamSynchronize(stream);
+        for (void* p : ptrs) cudaFree(p);
+    }
+    template <typename T>
+    cudaError_t upload(T** dp, const void* host, size_t bytes) {  // host NULL: zeros
+        void* p = nullptr;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) return e;
+        ptrs.push_back(p);
+        *dp = static_cast<T*>(p);
+        return host ? cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, stream) : cudaMemsetAsync(p, 0, bytes, stream);
+    }
+    cudaError_t download(void* host, const void* dev, size_t bytes) {
+        cudaError_t e = cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, stream);
+        return e != cudaSuccess ? e : cudaStreamSynchronize(stream);
+    }
+};
+
 }  // namespace
 
 // ============================================================================================ C ABI
@@ -1664,13 +1691,15 @@ void b200rt_shutdown(void) {
 
 int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid, void* out,
                       int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
-                      const float* ln_gamma, const float* ln_beta, float eps, float* stats_out) {
+                      const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!a || !w || !bias || !out || M < 1 || N % 256 || K % 64 || epi < 0 || epi > 2) return fail(B200RT_E_INVALID, "bad gemm arguments");
-    if (ln_stats && epi != 2 && K % 128) return fail(B200RT_E_INVALID, "LayerNorm fold needs K % 128 == 0");
+    if (!a || !w || !bias || !out || M < 1 || N % 256 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
+    if (ln_stats && (epi == 2 ? N : K) != HIDDEN) return fail(B200RT_E_INVALID, "the LayerNorm'd width must be %d", HIDDEN);
     if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
     Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    const int grid_sms = sms ? sms : d.sm_count;
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
     const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256;
@@ -1735,10 +1764,10 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     cudaEventCreate(&e1);
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, d.sm_count, d.compute));  // timing (values drift in place)
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(reload());
-    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, d.sm_count, d.compute));  // the result that is returned
+    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // the result that is returned
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
@@ -1758,11 +1787,13 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     return 0;
 }
 
-int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out) {
+int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!qkv || !lens || !ctx || B < 1 || S < 1 || S > MAX_SEQ) return fail(B200RT_E_INVALID, "bad attention arguments");
     Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    const int grid_sms = sms ? sms : d.sm_count;
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
     const size_t M = static_cast<size_t>(B) * S;
@@ -1781,9 +1812,9 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
     if (iters < 1) iters = 1;
-    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, d.sm_count, d.compute));
+    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute));
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, d.sm_count, d.compute));
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute));
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
@@ -1792,6 +1823,137 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     CUDA_TRY(cudaMemcpy(ctx, dc, M * HIDDEN * 2, cudaMemcpyDeviceToHost));
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     cudaFree(dq); cudaFree(dc); cudaFree(dl_);
+    return 0;
+}
+
+int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, int n_tokens, int S, int vocab,
+                       uint16_t* hi_out, uint16_t* lo_out, float* stats_out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!ids || !word || !pos || !type0 || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1)
+        return fail(B200RT_E_INVALID, "bad embed arguments");
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_tokens);
+    DebugBuffers b(d.compute);
+    int32_t* dids;
+    float *dw, *dp, *dt;
+    __half *dhi, *dlo;
+    float2* dst;
+    CUDA_TRY(b.upload(&dids, ids, rows * 4));
+    CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * HIDDEN * 4));
+    CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * HIDDEN * 4));
+    CUDA_TRY(b.upload(&dt, type0, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dhi, nullptr, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dlo, nullptr, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dst, nullptr, rows * STAT_PARTS * sizeof(float2)));
+    CUDA_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, d.compute));
+    CUDA_TRY(b.download(hi_out, dhi, rows * HIDDEN * 2));
+    CUDA_TRY(b.download(lo_out, dlo, rows * HIDDEN * 2));
+    CUDA_TRY(b.download(stats_out, dst, rows * STAT_PARTS * sizeof(float2)));
+    return 0;
+}
+
+int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
+                           int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!patch_out || !cls || !pos || !gamma || !beta || !hi_out || !lo_out || !stats_out || n_rows < 1 || T < 1)
+        return fail(B200RT_E_INVALID, "bad vit_embed arguments");
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_rows);
+    DebugBuffers b(d.compute);
+    __half *dpatch, *dhi, *dlo;
+    float *dcls, *dpos, *dg, *dbt;
+    float2* dst;
+    CUDA_TRY(b.upload(&dpatch, patch_out, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dcls, cls, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dpos, pos, static_cast<size_t>(T) * HIDDEN * 4));
+    CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dhi, nullptr, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dlo, nullptr, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dst, nullptr, rows * STAT_PARTS * sizeof(float2)));
+    CUDA_TRY(launch_vit_embed(dpatch, dcls, dpos, dg, dbt, dhi, dlo, dst, n_rows, T, eps, d.compute));
+    CUDA_TRY(b.download(hi_out, dhi, rows * HIDDEN * 2));
+    CUDA_TRY(b.download(lo_out, dlo, rows * HIDDEN * 2));
+    CUDA_TRY(b.download(stats_out, dst, rows * STAT_PARTS * sizeof(float2)));
+    return 0;
+}
+
+int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
+                                float eps, float* out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!hi || !lo || !gamma || !beta || !out || n_items < 1 || S < 1) return fail(B200RT_E_INVALID, "bad pool_normalize arguments");
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_items) * S;
+    DebugBuffers b(d.compute);
+    __half *dhi, *dlo;
+    float *dg, *dbt, *dout;
+    CUDA_TRY(b.upload(&dhi, hi, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dlo, lo, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * HIDDEN * 4));
+    CUDA_TRY(launch_pool_normalize(dhi, dlo, dg, dbt, dout, n_items, S, eps, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * HIDDEN * 4));
+    return 0;
+}
+
+int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* proj, int n_items,
+                          int T, int P, float eps, float* out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!hi || !lo || !gamma || !beta || !proj || !out || n_items < 1 || T < 1) return fail(B200RT_E_INVALID, "bad vit_pool arguments");
+    if (P < 1 || P > 1024) return fail(B200RT_E_INVALID, "projection width %d outside [1, 1024]", P);
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_items) * T;
+    DebugBuffers b(d.compute);
+    __half *dhi, *dlo;
+    float *dg, *dbt, *dproj, *dout;
+    CUDA_TRY(b.upload(&dhi, hi, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dlo, lo, rows * HIDDEN * 2));
+    CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
+    CUDA_TRY(b.upload(&dproj, proj, static_cast<size_t>(P) * HIDDEN * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * P * 4));
+    CUDA_TRY(launch_vit_pool(dhi, dlo, dg, dbt, dproj, dout, n_items, T, P, eps, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * P * 4));
+    return 0;
+}
+
+int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,
+                         float* cvec_out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!w || !w_out || N < 1 || K < 64 || K % 64) return fail(B200RT_E_INVALID, "bad fold_ln arguments (K must be a multiple of 64)");
+    if (gamma && (!beta || !cvec_out)) return fail(B200RT_E_INVALID, "a LayerNorm fold needs beta and cvec_out");
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t n = static_cast<size_t>(N) * K;
+    DebugBuffers b(d.compute);
+    float *dw, *dg = nullptr, *dbt = nullptr, *dbias = nullptr, *dc = nullptr;
+    __half* dout;
+    CUDA_TRY(b.upload(&dw, w, n * 4));
+    if (gamma) {
+        CUDA_TRY(b.upload(&dg, gamma, static_cast<size_t>(K) * 4));
+        CUDA_TRY(b.upload(&dbt, beta, static_cast<size_t>(K) * 4));
+        if (bias) CUDA_TRY(b.upload(&dbias, bias, static_cast<size_t>(N) * 4));
+        CUDA_TRY(b.upload(&dc, nullptr, static_cast<size_t>(N) * 4));
+    }
+    CUDA_TRY(b.upload(&dout, nullptr, n * 2));
+    CUDA_TRY(launch_fold_ln(dw, dg, dbt, dbias, dout, dc, N, K, d.compute));
+    CUDA_TRY(b.download(w_out, dout, n * 2));
+    if (gamma) CUDA_TRY(b.download(cvec_out, dc, static_cast<size_t>(N) * 4));
     return 0;
 }
 

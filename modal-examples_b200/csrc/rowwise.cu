@@ -35,7 +35,10 @@ __device__ __forceinline__ float2 ln_inplace(float4 (&x)[V4], const float* __res
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < V4; ++i) s += (x[i].x + x[i].y) + (x[i].z + x[i].w);
-    const float mean = warp_sum(s) * (1.0f / H);
+    // __fmul_rn: the rounded mean itself is subtracted.  A plain product would be contracted into the subtractions below
+    // (fma(-s, 1/768, x)), which see the unrounded s * fl(1/768): a constant row then centres to -x * 2^-25 instead of 0,
+    // and rstd = eps^-1/2 blows that up into a unit vector where LayerNorm + F.normalize give zeros.
+    const float mean = __fmul_rn(warp_sum(s), 1.0f / H);
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < V4; ++i) {

@@ -8,6 +8,7 @@ import os
 import numpy as np
 import pytest
 
+import kernel_refs as KR
 from oracle import bge_ref as R
 
 pytestmark = pytest.mark.gpu
@@ -46,20 +47,13 @@ def get_model(rt, layers, style, seed):
     return _models[key]
 
 
-def ref_gemm(a16, w16, bias, epi, resid=None):
-    from scipy.special import erf
-
-    acc = a16.astype(np.float32) @ w16.astype(np.float32).T + bias
-    if epi == 1:
-        a64 = acc.astype(np.float64)
-        acc = (a64 * 0.5 * (1.0 + erf(a64 / np.sqrt(2.0)))).astype(np.float32)
-    if epi == 2:
-        acc = acc + resid
-    return acc
-
-
 @pytest.mark.parametrize("M,N,K,epi", [(128, 256, 64, 0), (384, 768, 768, 0), (384, 768, 768, 1), (384, 768, 768, 2),
-                                       (1000, 768, 3072, 2), (4133, 3072, 768, 1), (148 * 128 + 5, 2304, 768, 0)])
+                                       (1000, 768, 3072, 2), (4133, 3072, 768, 1), (148 * 128 + 5, 2304, 768, 0),
+                                       # M around the 64-row halves and 128-row tiles; K = 128 / 192 (fewer k-blocks than the
+                                       # 4 ring stages), 256 (exactly 4); the quick-GELU epilogue
+                                       (1, 256, 128, 0), (8, 512, 192, 1), (9, 256, 256, 3), (63, 768, 128, 2), (65, 256, 192, 0),
+                                       (127, 512, 256, 3), (129, 256, 128, 1), (255, 768, 256, 2), (257, 512, 64, 3),
+                                       (384, 768, 768, 3), (4133, 3072, 768, 3)])
 def test_gemm_kernel_vs_numpy(rt, M, N, K, epi):
     rng = np.random.default_rng(M + N + K + epi)
     a = rng.standard_normal((M, K)).astype(np.float16)
@@ -67,27 +61,14 @@ def test_gemm_kernel_vs_numpy(rt, M, N, K, epi):
     bias = rng.standard_normal(N).astype(np.float32)
     resid = rng.standard_normal((M, N)).astype(np.float32) if epi == 2 else None
     out, _ = rt.debug_gemm(epi, a, w, bias, resid)
-    ref = ref_gemm(a, w, bias, epi, resid)
-    err = np.abs(out.astype(np.float32) - ref)
-    # epi 2: the residual stream is fp16 hi + fp16 lo (22 mantissa bits): 2^-21 relative on top of fp32 accumulation order
-    tol = 2e-3 * np.abs(ref) + 2e-3 if epi != 2 else 1e-4 * np.abs(ref) + 1e-4
-    assert (err <= tol).all(), (float(err.max()), np.argwhere(err > tol)[:4])
+    KR.check_gemm(f"gemm M={M} N={N} K={K} epi {epi}", out, epi, a, w, bias, resid=resid)
 
 
-def _partials(y):
-    """(sum, M2 about the slice mean) per 128-column slice: the form row statistics travel in (kernels.h)."""
-    M, W = y.shape
-    sl = y.astype(np.float64).reshape(M, W // 128, 128)
-    s = sl.sum(-1)
-    m2 = ((sl - sl.mean(-1, keepdims=True)) ** 2).sum(-1)
-    return np.stack([s, m2], -1).astype(np.float32)
-
-
-@pytest.mark.parametrize("M,N,epi", [(300, 2304, 0), (300, 3072, 1), (2 * 148 * 128 + 77, 2304, 0)])
+@pytest.mark.parametrize("M,N,epi", [(300, 2304, 0), (300, 3072, 1), (2 * 148 * 128 + 77, 2304, 0), (300, 3072, 3)])
 def test_gemm_folded_layernorm_epilogue(rt, M, N, epi):
     """QKV / FFN1 consume the raw pre-LayerNorm residual (its fp16 hi part) against fp16(gamma o W, rows centred so that the
     LayerNorm's mean subtraction happens inside the GEMM); the epilogue applies rstd * acc + (W beta + b).
-    Reference: LayerNorm in fp64 on the same fp16-rounded operands."""
+    Reference: the same operands in fp64, rstd from the same partials (kernel_refs.gemm_ref)."""
     K, eps = 768, 1e-12
     rng = np.random.default_rng(M + N)
     y = (rng.standard_normal((M, K)) * 1.7 + 0.3).astype(np.float32)
@@ -100,20 +81,12 @@ def test_gemm_folded_layernorm_epilogue(rt, M, N, epi):
     wg = W * gamma[None, :]
     wp = (wg - wg.mean(1, keepdims=True)).astype(np.float16)
     cvec = (W.astype(np.float64) @ beta.astype(np.float64) + b).astype(np.float32)
-    out, _ = rt.debug_gemm(epi, y16, wp, cvec, ln_stats=_partials(y), eps=eps)
-    # what the kernel is meant to equal: LN (statistics of the fp32 row) applied to the fp16-rounded row, folded weights
+    st = KR.partials(y).astype(np.float32)
+    out, _ = rt.debug_gemm(epi, y16, wp, cvec, ln_stats=st, eps=eps)
+    KR.check_gemm(f"folded LayerNorm M={M} N={N} epi {epi}", out, epi, y16, wp, cvec, ln_stats=st, eps=eps)
+    # and it is a faithful LayerNorm + projection: against the unrounded computation
     y64 = y.astype(np.float64)
     mu, var = y64.mean(1, keepdims=True), y64.var(1, keepdims=True)
-    z = (y16.astype(np.float64) - mu) / np.sqrt(var + eps)
-    ref = z @ (W * gamma[None, :]).astype(np.float16).astype(np.float64).T + cvec
-    if epi == 1:
-        from scipy.special import erf
-
-        ref = ref * 0.5 * (1.0 + erf(ref / np.sqrt(2.0)))
-    err = np.abs(out.astype(np.float64) - ref)
-    tol = 2e-3 * np.abs(ref) + 3e-3
-    assert (err <= tol).all(), (float(err.max()), np.argwhere(err > tol)[:4])
-    # and it is a faithful LayerNorm + projection: against the unrounded computation
     full = ((y64 - mu) / np.sqrt(var + eps) * gamma + beta) @ W.astype(np.float64).T + b
     if epi == 0:
         assert np.abs(out.astype(np.float64) - full).max() < 0.05 * np.abs(full).max()
@@ -131,46 +104,25 @@ def test_gemm_residual_layernorm_epilogue_and_row_statistics(rt, M, K):
     resid = (rng.standard_normal((M, N)) * 2.0 - 0.5).astype(np.float32)
     resid[:, 381] -= 55.0
     # the kernel sees the residual as fp16 hi + fp16 lo
-    hi = resid.astype(np.float16)
-    res22 = hi.astype(np.float32) + (resid - hi.astype(np.float32)).astype(np.float16).astype(np.float32)
+    st_in = KR.partials(KR.hilo64(*KR.split_hilo(resid))).astype(np.float32)
     gamma = (1.5 + 0.4 * rng.standard_normal(N)).astype(np.float32)
     beta = (0.3 * rng.standard_normal(N)).astype(np.float32)
-    out, _, st = rt.debug_gemm(2, a, w, bias, resid, ln_stats=_partials(res22), ln_gamma=gamma, ln_beta=beta, eps=eps, want_stats=True)
-    r64 = res22.astype(np.float64)
-    ln = (r64 - r64.mean(1, keepdims=True)) / np.sqrt(r64.var(1, keepdims=True) + eps) * gamma + beta
-    ref = a.astype(np.float64) @ w.astype(np.float64).T + bias + ln
-    err = np.abs(out - ref)
-    tol = 1e-4 * np.abs(ref) + 2e-4
-    assert (err <= tol).all(), (float(err.max()), np.argwhere(err > tol)[:4])
-    want = _partials(ref.astype(np.float32))
-    assert np.allclose(st[..., 0], want[..., 0], rtol=1e-4, atol=2e-2), float(np.abs(st[..., 0] - want[..., 0]).max())
-    assert np.allclose(st[..., 1], want[..., 1], rtol=2e-4, atol=1e-2), float(np.abs(st[..., 1] - want[..., 1]).max())
+    kw = dict(resid=resid, ln_stats=st_in, ln_gamma=gamma, ln_beta=beta, eps=eps)
+    out, _, st = rt.debug_gemm(2, a, w, bias, want_stats=True, **kw)
+    KR.check_gemm(f"residual LayerNorm M={M} K={K}", out, 2, a, w, bias, **kw)
+    KR.check_gemm_stats(f"residual LayerNorm M={M} K={K}: stats_out", st, (a, w, bias), **kw)
 
 
 @pytest.mark.parametrize("B,S,lens", [(1, 128, [128]), (2, 512, [512, 512]), (3, 300, [300, 17, 129]), (4, 512, [512, 1, 128, 385]),
-                                      (2, 7, [7, 3]), (1, 1, [1])])
+                                      (2, 7, [7, 3]), (1, 1, [1]),
+                                      # lens on and next to the 64-key sub-blocks, odd S
+                                      (2, 63, [63, 1]), (2, 65, [65, 64]), (3, 127, [127, 64, 63]), (3, 129, [129, 128, 65]),
+                                      (2, 449, [449, 193]), (3, 511, [511, 256, 257])])
 def test_attention_kernel_vs_numpy(rt, B, S, lens):
     rng = np.random.default_rng(B * 1000 + S)
     qkv = (rng.standard_normal((B * S, 2304)) * 2.0).astype(np.float16)
     ctx, _ = rt.debug_attention(qkv, np.array(lens, np.int32), B, S)
-    q = qkv.astype(np.float64).reshape(B, S, 3, 12, 64)
-    qq, kk, vv = (q[:, :, j].transpose(0, 2, 1, 3) for j in range(3))
-    s = (qq @ kk.transpose(0, 1, 3, 2)) * 0.125
-    s = np.where((np.arange(S)[None, :] >= np.array(lens)[:, None])[:, None, None, :], -np.inf, s)
-    e = np.exp(s - s.max(-1, keepdims=True))
-    ref = ((e / e.sum(-1, keepdims=True)) @ vv).transpose(0, 2, 1, 3).reshape(B * S, 768)
-    got = ctx.astype(np.float64)
-    assert np.isfinite(got).all(), "padded query rows must stay finite"
-    assert (np.abs(got - ref) <= 4e-3 * np.abs(ref) + 4e-3).all()  # P and ctx are rounded to fp16
-
-
-def _ref_attention(qkv, lens, B, S):
-    q = qkv.astype(np.float64).reshape(B, S, 3, 12, 64)
-    qq, kk, vv = (q[:, :, j].transpose(0, 2, 1, 3) for j in range(3))
-    s = (qq @ kk.transpose(0, 1, 3, 2)) * 0.125
-    s = np.where((np.arange(S)[None, :] >= np.array(lens)[:, None])[:, None, None, :], -np.inf, s)
-    e = np.exp(s - s.max(-1, keepdims=True))
-    return ((e / e.sum(-1, keepdims=True)) @ vv).transpose(0, 2, 1, 3).reshape(B * S, 768)
+    KR.check_attention(f"attention B={B} S={S}", ctx, qkv, lens, B, S)
 
 
 @pytest.mark.parametrize("B,S,lens", [(2, 512, [512, 300]), (13, 512, [512] * 12 + [77])])
@@ -187,10 +139,7 @@ def test_attention_running_max_rescale(rt, B, S, lens):
     x[:, :, 1] += (12.0 * (np.arange(S) // 64))[None, :, None, None] * u  # k . u = 12 * sub-block: raw q.k steps by 48
     qkv = x.reshape(B * S, 2304).astype(np.float16)
     ctx, _ = rt.debug_attention(qkv, np.array(lens, np.int32), B, S)
-    ref = _ref_attention(qkv, lens, B, S)
-    got = ctx.astype(np.float64)
-    assert np.isfinite(got).all()
-    assert (np.abs(got - ref) <= 4e-3 * np.abs(ref) + 4e-3).all()
+    KR.check_attention(f"running-max rescale B={B}", ctx, qkv, lens, B, S)
 
 
 def test_hidden_states_layer_by_layer(rt):
