@@ -24,10 +24,11 @@ extern "C" {
 #define B200RT_E_STATE (-2)     /* not initialised / already initialised / shut down */
 #define B200RT_E_CUDA (-3)      /* CUDA error; the context is poisoned and every later call fails fast */
 #define B200RT_E_NOMEM (-4)
-#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is not BERT-base */
+#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is neither bge-base nor bge-small */
 
-/* Geometry of a BERT encoder (HF BertConfig fields).  The sm_90a kernels are specialised for the
- * BGE-base geometry (hidden 768, 12 heads of 64, inter 3072, max_pos <= 512); `layers` is free.   */
+/* Geometry of a BERT encoder (HF BertConfig fields).  The sm_90a kernels cover two geometries: bge-base (hidden 768,
+ * 12 heads of 64, inter 3072) and bge-small (hidden 384, 12 heads of 32, inter 1536), with max_pos <= 512; `layers` is
+ * free.  A model's results are `hidden` floats per item.                                                              */
 typedef struct b200rt_bert_config {
     int32_t vocab, hidden, layers, heads, inter, max_pos, type_vocab;
     float eps;

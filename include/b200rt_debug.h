@@ -10,13 +10,13 @@
 extern "C" {
 #endif
 
-/* out[M,N] = epi(A[M,K] . W[N,K]^T + bias (+ resid)) on replica 0.  a, w: fp16 bit patterns (uint16),
+/* out[M,N] = epi(A[M,K] . W[N,K]^T + bias (+ resid)) on replica 0, N % 128 == 0, K % 64 == 0.  a, w: fp16 bit patterns (uint16),
  * bias fp32 [N], resid fp32 [M,N] or NULL.  epi: 0 bias->fp16 out, 1 bias+gelu->fp16 out, 2 bias+resid->fp32
  * out (the residual travels through the kernel as fp16 hi + fp16 lo; out = hi + lo), 3 bias+quick_gelu->fp16 out.
  * out is uint16 [M,N] for epi 0/1/3 and float [M,N] for epi 2.  ms_out (optional): device time of `iters` back-to-back
  * launches divided by iters.
  * LayerNorm in the epilogue (optional; all NULL = none): ln_stats = [M][parts] (sum, M2) float pairs, one per 128 columns
- * of the LayerNorm'd row (parts = K/128 for epi 0/1/3, N/128 for epi 2; that width must be 768).
+ * of the LayerNorm'd row (parts = K/128 for epi 0/1/3, N/128 for epi 2; that width must be 768 or 384).
  *   epi 0/1/3: `a` is the PRE-LayerNorm row in fp16, `w` = fp16(gamma o W with every row centred: sum_k w[n,k] = 0),
  *            bias = W beta + b:  out = epi(rstd * acc + bias)
  *   epi 2  : out = acc + bias + ((resid - mean) * rstd * ln_gamma + ln_beta) (ln_stats NULL: acc + bias + resid);
@@ -27,27 +27,29 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
                       void* out, int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
                       const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms);
 
-/* ctx[B*S,768] (fp16 bits) = multi-head attention over qkv[B*S,2304] (fp16 bits), lens[B].  sms as for
- * b200rt_debug_gemm (it also decides whether units are split by query tile).                          */
+/* ctx[B*S,H] (fp16 bits) = multi-head attention of 12 heads of head_dim over qkv[B*S,3H] (fp16 bits), lens[B],
+ * H = 12 head_dim; head_dim 64 or 32 (0 = 64).  sms as for b200rt_debug_gemm (it also decides whether units are split
+ * by query tile).                                                                                                    */
 int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters,
-                           float* ms_out, int sms);
+                           float* ms_out, int sms, int head_dim);
 
-/* Row kernels, one launch each behind host buffers.  hi/lo: fp16 bit patterns [rows, 768]; stats: [rows][6] (sum, M2)
- * float pairs, one per 128-column slice, M2 about the slice's own mean.
+/* Row kernels, one launch each behind host buffers.  hi/lo: fp16 bit patterns [rows, W]; stats: [rows][W/128] (sum, M2)
+ * float pairs, one per 128-column slice, M2 about the slice's own mean.  W = 768, except for embed and pool_normalize,
+ * whose trailing `hidden` sets it: 768 or 384 (0 = 768).
  *   embed:          x = (word[ids[t]] + type0) + pos[t % S] -> hi = fp16(x), lo = fp16(x - hi), stats of x.
- *                   word [vocab, 768], pos [S, 768], type0 [768].
+ *                   word [vocab, W], pos [S, W], type0 [W].
  *   vit_embed:      x = pre_layrnorm((t % T == 0 ? cls : patch_out[t]) + pos[t % T]) -> hi, lo, stats of x.
- *   pool_normalize: out[i] = L2-normalise(LayerNorm(hi + lo of row i * S)), out fp32 [n_items, 768].
+ *   pool_normalize: out[i] = L2-normalise(LayerNorm(hi + lo of row i * S)), out fp32 [n_items, W].
  *   vit_pool:       out[i] = L2-normalise(proj . LayerNorm(hi + lo of row i * T)), proj fp32 [P, 768], 1 <= P <= 1024,
  *                   out fp32 [n_items, P].
  *   fold_ln:        w_out = fp16(w o gamma - rowmean(w o gamma)), cvec_out = w beta + bias (bias may be NULL);
  *                   gamma NULL: w_out = fp16(w) and cvec_out is not written.  w fp32 [N, K], K % 64 == 0.    */
 int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, int n_tokens, int S, int vocab,
-                       uint16_t* hi_out, uint16_t* lo_out, float* stats_out);
+                       uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden);
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out);
 int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
-                                float eps, float* out);
+                                float eps, float* out, int hidden);
 int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* proj, int n_items,
                           int T, int P, float eps, float* out);
 int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,

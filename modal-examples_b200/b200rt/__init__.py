@@ -103,11 +103,11 @@ def load_library():
                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_int]
         lib.b200rt_debug_attention.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p,
-                                               ctypes.c_int]
+                                               ctypes.c_int, ctypes.c_int]
         vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-        lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp]
+        lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp, ci]
         lib.b200rt_debug_vit_embed.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, vp, vp]
-        lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp]
+        lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
         lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
         lib.b200rt_debug_hidden.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
@@ -389,16 +389,21 @@ def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, res
     return (out, ms.value, so) if want_stats else (out, ms.value)
 
 
-def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0):
+def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0, head_dim: int = 64):
+    """qkv16 [B*S, 3H] float16 with H = 12 head_dim (head_dim 64: bge-base, 32: bge-small); returns (ctx [B*S, H], ms)."""
+    H = 12 * head_dim
     qkv16 = np.ascontiguousarray(qkv16, dtype=np.float16)
+    if qkv16.size != B * S * 3 * H:
+        raise B200RTError(E_INVALID, f"qkv must be [{B * S}, {3 * H}] for head_dim {head_dim}, got shape {qkv16.shape}")
     lens = np.ascontiguousarray(lens, dtype=np.int32)
-    ctx = np.empty((B * S, 768), np.float16)
+    ctx = np.empty((B * S, H), np.float16)
     ms = ctypes.c_float(0)
-    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms))
+    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms, head_dim))
     return ctx, ms.value
 
 
-# Row kernels behind host buffers (include/b200rt_debug.h).  hi / lo are float16 arrays [rows, 768]; stats [rows, 6, 2].
+# Row kernels behind host buffers (include/b200rt_debug.h).  hi / lo are float16 arrays [rows, W]; stats [rows, W / 128, 2];
+# W = 768, or ``hidden`` (768 or 384) where a wrapper takes it.
 def _f32(v):
     return np.ascontiguousarray(v, dtype=np.float32)
 
@@ -407,14 +412,17 @@ def _f16(v):
     return np.ascontiguousarray(v, dtype=np.float16)
 
 
-def debug_embed(ids: np.ndarray, word: np.ndarray, pos: np.ndarray, type0: np.ndarray, S: int):
-    """ids [n_tokens] (token t sits at position t % S); returns (hi, lo, stats)."""
+def debug_embed(ids: np.ndarray, word: np.ndarray, pos: np.ndarray, type0: np.ndarray, S: int, hidden: int = 768):
+    """ids [n_tokens] (token t sits at position t % S), word [vocab, hidden], pos [S, hidden]; returns (hi, lo, stats)."""
     ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
     word, pos, type0 = _f32(word), _f32(pos), _f32(type0)
+    if word.shape[1] != hidden or pos.shape[1] != hidden or type0.size != hidden:
+        raise B200RTError(E_INVALID, f"embedding tables must be {hidden} wide")
     n = ids.size
-    hi, lo = np.empty((n, 768), np.float16), np.empty((n, 768), np.float16)
-    st = np.empty((n, 6, 2), np.float32)
-    _check(load_library().b200rt_debug_embed(_ptr(ids), _ptr(word), _ptr(pos), _ptr(type0), n, S, word.shape[0], _ptr(hi), _ptr(lo), _ptr(st)))
+    hi, lo = np.empty((n, hidden), np.float16), np.empty((n, hidden), np.float16)
+    st = np.empty((n, hidden // 128, 2), np.float32)
+    _check(load_library().b200rt_debug_embed(_ptr(ids), _ptr(word), _ptr(pos), _ptr(type0), n, S, word.shape[0], _ptr(hi), _ptr(lo), _ptr(st),
+                                             hidden))
     return hi, lo, st
 
 
@@ -429,12 +437,14 @@ def debug_vit_embed(patch_out: np.ndarray, cls: np.ndarray, pos: np.ndarray, gam
     return hi, lo, st
 
 
-def debug_pool_normalize(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta: np.ndarray, S: int, eps: float):
-    """hi, lo [n_items * S, 768]: the LayerNorm'd, L2-normalised row i * S of every item, [n_items, 768]."""
+def debug_pool_normalize(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta: np.ndarray, S: int, eps: float, hidden: int = 768):
+    """hi, lo [n_items * S, hidden]: the LayerNorm'd, L2-normalised row i * S of every item, [n_items, hidden]."""
     hi, lo, gamma, beta = _f16(hi), _f16(lo), _f32(gamma), _f32(beta)
+    if hi.shape[1] != hidden or lo.shape[1] != hidden or gamma.size != hidden or beta.size != hidden:
+        raise B200RTError(E_INVALID, f"rows and LayerNorm parameters must be {hidden} wide")
     n = hi.shape[0] // S
-    out = np.empty((n, 768), np.float32)
-    _check(load_library().b200rt_debug_pool_normalize(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), n, S, eps, _ptr(out)))
+    out = np.empty((n, hidden), np.float32)
+    _check(load_library().b200rt_debug_pool_normalize(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), n, S, eps, _ptr(out), hidden))
     return out
 
 

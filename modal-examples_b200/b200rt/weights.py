@@ -19,6 +19,8 @@ import struct
 import numpy as np
 
 BGE_BASE_GEOMETRY = dict(vocab=30522, hidden=768, layers=12, heads=12, inter=3072, max_pos=512, type_vocab=2, eps=1e-12)
+# BAAI/bge-small-en-v1.5: 12 heads of 32 -- the head count is not implied by the tensor shapes (384 // 64 would be 6)
+BGE_SMALL_GEOMETRY = dict(vocab=30522, hidden=384, layers=12, heads=12, inter=1536, max_pos=512, type_vocab=2, eps=1e-12)
 
 
 def blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
@@ -66,8 +68,14 @@ def _strip_prefix(sd: dict) -> dict:
 
 
 def geometry_from_state_dict(sd: dict, eps: float = 1e-12, heads: int | None = None) -> dict:
+    """``heads``: ``num_attention_heads`` from the checkpoint's config.json.  Without it the head count is guessed as
+    hidden // 64, which is right for bge-base; for hidden 384 that guess (6 heads of 64) is not bge-small's 12 heads of 32,
+    so it raises instead."""
     sd = _strip_prefix(sd)
     vocab, hidden = sd["embeddings.word_embeddings.weight"].shape
+    if heads is None and hidden == 384:
+        raise ValueError("hidden 384 without num_attention_heads: bge-small has 12 heads of 32, not 384 // 64 = 6; "
+                         "put the checkpoint's config.json next to its weights")
     layers = 0
     while f"encoder.layer.{layers}.attention.self.query.weight" in sd:
         layers += 1

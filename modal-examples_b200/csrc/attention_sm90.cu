@@ -1,4 +1,5 @@
-// Multi-head self-attention for S <= 512, d = 64, on wgmma (sm_90a): persistent CTAs.
+// Multi-head self-attention for S <= 512, 12 heads of d = 64 (bge-base) or d = 32 (bge-small), on wgmma (sm_90a):
+// persistent CTAs.  The kernel is a template on d; the comments below give the d = 64 figures, d = 32 differences follow.
 //
 // A work unit is one (item, head) -- or, for batches with fewer units than SMs, one (item, head, query tile).  Each CTA walks
 // the units u = blockIdx.x, blockIdx.x + gridDim.x, ...  For the unit in hand one thread TMA-loads the head's K and V
@@ -13,6 +14,9 @@
 //   O  += P . V_c        four wgmma.m64n64k16 with A = P (fp16) straight from the registers -- the S accumulator fragment
 //                        is already the A-operand fragment of the same rows -- and B = V_c (MN-major) from shared memory.
 // The tile's output ctx = O / l is staged in the tile's own (now idle) query buffer and leaves with one TMA store.
+//
+// d = 32: a row of Q, K or V is 64 bytes, so every tile is 64B-swizzled (TMA box {32, 128, 1}, 8 KB per 128 rows); S = Q . K^T
+// is two k-steps of m64n64k16 and O += P . V four m64n32k16 (16 fp32 O registers per thread); the softmax scale is 1/sqrt(32).
 //
 // Keys >= len are masked to -inf before the max (exactly P = 0, matching HF's additive -inf mask); sub-blocks wholly past
 // len are skipped.  Every query tile is computed the same way whether the item travels as one unit or split by query tile,
@@ -30,19 +34,32 @@ namespace attn {
 constexpr int QT = 128;      // query rows per tile
 constexpr int KB = 128;      // keys per K/V smem tile (TMA box)
 constexpr int SB = 64;       // keys per sub-block
-constexpr int D = HEAD_DIM;  // 64
 constexpr int MAX_KB = 4;    // S <= 512
-constexpr int TILE_BYTES = 128 * D * 2;              // 16 KB: 128 rows x 128 B
-constexpr int OFF_Q = 0;                             // 2 x 16 KB (double buffered across tiles), also the output staging tile
-constexpr int OFF_K = OFF_Q + 2 * TILE_BYTES;        // 4 x 16 KB
-constexpr int OFF_V = OFF_K + MAX_KB * TILE_BYTES;   // 4 x 16 KB
-constexpr int OFF_BAR = OFF_V + MAX_KB * TILE_BYTES;
-constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 constexpr int NUM_THREADS = 256;
-static_assert(SMEM_BYTES <= 232448, "shared memory");
 
-// softmax_scale * log2(e) with softmax_scale = 1/sqrt(64)
-constexpr float kScaleLog2e = 0.125f * 1.4426950408889634f;
+// Shared-memory layout of the head-dim-D kernel: rows of RB = 2D bytes (128 or 64), each tile 128 rows.
+template <int D>
+struct Layout {
+    static constexpr int RB = 2 * D;                                // bytes per row
+    static constexpr int TILE_BYTES = 128 * RB;                     // 16 KB (d = 64) / 8 KB (d = 32)
+    static constexpr int OFF_Q = 0;                                 // 2 tiles (double buffered across tiles), also the output staging
+    static constexpr int OFF_K = OFF_Q + 2 * TILE_BYTES;            // MAX_KB tiles
+    static constexpr int OFF_V = OFF_K + MAX_KB * TILE_BYTES;       // MAX_KB tiles
+    static constexpr int OFF_BAR = OFF_V + MAX_KB * TILE_BYTES;
+    static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+    static_assert(SMEM_BYTES <= 232448, "shared memory");
+};
+
+// softmax_scale * log2(e) with softmax_scale = 1/sqrt(D)
+template <int D>
+constexpr float scale_log2e() { return (D == 64 ? 0.125f : 0.17677669529663687f) * 1.4426950408889634f; }
+
+// descriptor of a K-major (Q, K) or MN-major (V) operand tile of the head-dim-D layout
+template <int D>
+__device__ __forceinline__ uint64_t make_desc(uint32_t addr) {
+    if constexpr (D == 64) return make_sw128_desc(addr);
+    else return make_sw64_desc(addr);
+}
 
 struct Unit {
     int b, h, t0, nq;  // item, head, first query tile, query tiles
@@ -68,9 +85,15 @@ __device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const 
     return U;
 }
 
+template <int D>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tctx,
                  const int32_t* __restrict__ lens, int S, int split, int n_units) {
+    using L = Layout<D>;
+    constexpr int RB = L::RB, TILE_BYTES = L::TILE_BYTES, OFF_Q = L::OFF_Q, OFF_K = L::OFF_K, OFF_V = L::OFF_V, OFF_BAR = L::OFF_BAR;
+    constexpr int HID = HEADS * D;     // ctx width; qkv rows are 3 HID wide (Q | K | V)
+    constexpr int NO = D / 2;          // O accumulators per thread
+    constexpr float kScaleLog2e = scale_log2e<D>();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -94,8 +117,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
     __syncthreads();
     griddep_wait();  // the prologue above overlapped the previous kernel's tail; nothing it wrote (qkv, lens) has been read yet
 
-    // this thread's rows of a tile (first and +8) and their 16-byte chunk in a 128B-swizzled row: dims 8j .. 8j+7 of row r
-    // sit in chunk j ^ (r & 7)
+    // this thread's rows of a tile (first and +8) and their 16-byte chunk in a swizzled row: dims 8j .. 8j+7 of row r
+    // sit in chunk j ^ (r & 7) (128-byte rows) or j ^ ((r >> 1) & 3) (64-byte rows)
     const int rr = wg * 64 + w4 * 16 + (lane >> 2);
     const uint32_t cq = 4 * (lane & 3);  // byte offset of this thread's two dims inside a chunk
     uint32_t kv_par = 0;                 // bit j: parity of the number of loads of K/V tile j so far
@@ -110,8 +133,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
             load_q(gt, 0);
             for (int j = 0; j < U.nkb; ++j) {
                 mbar_arrive_expect_tx(&kv_full[j], 2 * TILE_BYTES);
-                tma_load_3d(smem + OFF_K + j * TILE_BYTES, &tq, &kv_full[j], HIDDEN + U.h * D, j * KB, U.b);
-                tma_load_3d(smem + OFF_V + j * TILE_BYTES, &tq, &kv_full[j], 2 * HIDDEN + U.h * D, j * KB, U.b);
+                tma_load_3d(smem + OFF_K + j * TILE_BYTES, &tq, &kv_full[j], HID + U.h * D, j * KB, U.b);
+                tma_load_3d(smem + OFF_V + j * TILE_BYTES, &tq, &kv_full[j], 2 * HID + U.h * D, j * KB, U.b);
             }
             if (U.nq > 1) load_q(gt + 1, 1);
         }
@@ -119,21 +142,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
             const uint32_t g = gt + t;
             const uint32_t q_buf = smem_u32(smem + OFF_Q + (g & 1) * TILE_BYTES);
             mbar_wait(&q_full[g & 1], (g >> 1) & 1);
-            float o[32];
+            float o[NO];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = 0.f;
+            for (int i = 0; i < NO; ++i) o[i] = 0.f;
             float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-            const uint32_t q_addr = q_buf + wg * (64 * 128);
+            const uint32_t q_addr = q_buf + wg * (64 * RB);
 #pragma unroll 1
             for (int sb = 0; sb < U.nsb; ++sb) {
                 if ((sb & 1) == 0) mbar_wait(&kv_full[sb >> 1], (kv_par >> (sb >> 1)) & 1);
-                const uint32_t k_addr = smem_u32(smem + OFF_K) + sb * (SB * 128);
+                const uint32_t k_addr = smem_u32(smem + OFF_K) + sb * (SB * RB);
                 float s[32];
                 wgmma_fence();
                 fence_operands(s);
 #pragma unroll
                 for (int k = 0; k < D / 16; ++k)
-                    wgmma_m64n64k16_ss(s, make_sw128_desc(q_addr + k * 32), make_sw128_desc(k_addr + k * 32), k != 0);
+                    wgmma_m64n64k16_ss(s, make_desc<D>(q_addr + k * 32), make_desc<D>(k_addr + k * 32), k != 0);
                 wgmma_commit();
                 wgmma_wait<0>();
                 fence_operands(s);
@@ -163,16 +186,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
                         ls += p0 + p1;
                         // keys 8j .. 8j+7: k-step j/2, register 2 (j odd) + h
                         pa[j >> 1][2 * (j & 1) + h] = pack_half2(p0, p1);
-                        o[4 * j + 2 * h] *= alpha;
-                        o[4 * j + 2 * h + 1] *= alpha;
+                        if (j < D / 8) {  // O has D / 8 column groups
+                            o[4 * j + 2 * h] *= alpha;
+                            o[4 * j + 2 * h + 1] *= alpha;
+                        }
                     }
                     l_run[h] = fmaf(l_run[h], alpha, ls);
                 }
-                const uint32_t v_addr = smem_u32(smem + OFF_V) + sb * (SB * 128);
+                const uint32_t v_addr = smem_u32(smem + OFF_V) + sb * (SB * RB);
                 wgmma_fence();
                 fence_operands(o);
 #pragma unroll
-                for (int kk = 0; kk < SB / 16; ++kk) wgmma_m64n64k16_rs_mn(o, pa[kk], make_sw128_desc(v_addr + kk * (16 * 128)), 1);
+                for (int kk = 0; kk < SB / 16; ++kk) {
+                    if constexpr (D == 64) wgmma_m64n64k16_rs_mn(o, pa[kk], make_desc<D>(v_addr + kk * (16 * RB)), 1);
+                    else wgmma_m64n32k16_rs_mn(o, pa[kk], make_desc<D>(v_addr + kk * (16 * RB)), 1);
+                }
                 wgmma_commit();
                 wgmma_wait<0>();
                 fence_operands(o);
@@ -185,10 +213,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
                 l += __shfl_xor_sync(0xffffffff, l, 2);
                 const float inv_l = 1.0f / l;
                 const int r = rr + 8 * h;
-                const uint32_t row = q_buf + r * 128 + cq;
+                const uint32_t row = q_buf + r * RB + cq;
+                const uint32_t sw = (static_cast<uint32_t>(r) * RB >> 7) & (RB / 16 - 1);  // the row's chunk swizzle
 #pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(row + ((static_cast<uint32_t>(j) ^ (r & 7)) << 4)),
+                for (int j = 0; j < D / 8; ++j)
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(row + ((static_cast<uint32_t>(j) ^ sw) << 4)),
                                  "r"(pack_half2(o[4 * j + 2 * h] * inv_l, o[4 * j + 2 * h + 1] * inv_l))
                                  : "memory");
             }
@@ -211,19 +240,25 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
 }  // namespace attn
 
 cudaError_t attention_init_device() {
-    return cudaFuncSetAttribute(attn::attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(attn::attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<64>::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(attn::attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<32>::SMEM_BYTES);
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                             cudaStream_t stream) {
-    if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1) return cudaErrorInvalidValue;
+                             cudaStream_t stream, int head_dim) {
+    if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1 || (head_dim != 64 && head_dim != 32)) return cudaErrorInvalidValue;
     // fewer (item, head) units than SMs: split them by query tile (K and V are then loaded once per tile, but a single item
     // spreads over 48 SMs instead of 12)
     const int nq = (S + attn::QT - 1) / attn::QT;
     const int split = (B * HEADS < sm_count && nq > 1) ? 1 : 0;
     const int n_units = B * HEADS * (split ? nq : 1);
     const int grid = n_units < sm_count ? n_units : sm_count;
-    return launch_pdl(attn::attention_kernel, dim3(grid), dim3(attn::NUM_THREADS), attn::SMEM_BYTES, stream, tq, tctx, lens, S, split, n_units);
+    if (head_dim == 64)
+        return launch_pdl(attn::attention_kernel<64>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<64>::SMEM_BYTES, stream, tq, tctx, lens, S,
+                          split, n_units);
+    return launch_pdl(attn::attention_kernel<32>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<32>::SMEM_BYTES, stream, tq, tctx, lens, S,
+                      split, n_units);
 }
 
 }  // namespace b200

@@ -98,15 +98,16 @@ int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, 
     return 0;
 }
 
-// fp16 [B, S, width] (qkv: width 2304, ctx: width 768) -> box {64, 128, 1}, 128B swizzle (rows past S are zero-filled
-// on load and clipped on store)
-int make_map_qkv(CUtensorMap* m, const void* base, uint64_t B, uint64_t S, uint64_t width = QKV_DIM) {
+// fp16 [B, S, width] (qkv: width 3H, ctx: width H, H = 12 head_dim) -> box {head_dim, 128, 1}: one head's 128 rows, 128B
+// swizzle for head_dim 64, 64B for head_dim 32 (rows past S are zero-filled on load and clipped on store)
+int make_map_qkv(CUtensorMap* m, const void* base, uint64_t B, uint64_t S, uint64_t width, uint32_t head_dim) {
     cuuint64_t dims[3] = {width, S, B};
     cuuint64_t strides[2] = {width * 2, S * width * 2};
-    cuuint32_t box[3] = {64, 128, 1};
+    cuuint32_t box[3] = {head_dim, 128, 1};
     cuuint32_t es[3] = {1, 1, 1};
     CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, head_dim == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(B200RT_E_CUDA, "cuTensorMapEncodeTiled(qkv B=%llu S=%llu) -> %d",
                                        (unsigned long long)B, (unsigned long long)S, (int)r);
@@ -119,6 +120,13 @@ constexpr int NSLOT = 4;
 constexpr int MIN_ITEMS_PER_REPLICA = 8;  // a wave uses fewer replicas rather than giving one fewer items than this
 constexpr int MAX_SEQ = 512;
 constexpr int VIT_WAVE_ITEMS = 64;  // images one replica takes per wave (64 x 197 tokens; 38.5 MB of pixels per wave slot)
+
+// The text geometries the kernels cover (hidden, heads, inter): bge-base and bge-small.  The ViT tower is bge-base-wide.
+struct TextGeometry {
+    int hidden, heads, inter;
+};
+constexpr TextGeometry TEXT_GEOMETRIES[2] = {{768, 12, 3072}, {384, 12, 1536}};
+inline int geometry_index(int hidden) { return hidden == 768 ? 0 : 1; }
 
 struct LayerW {
     __half *qkv_w, *ao_w, *ff1_w, *ff2_w;
@@ -165,8 +173,12 @@ struct Dev {
     float2* pstats[2] = {nullptr, nullptr};  // [rows][STAT_PARTS] (sum, M2) partials: [0] embedding LN / LN2 inputs, [1] LN1 inputs
     float* x32_dbg = nullptr;    // tests only (b200rt_debug_hidden): normalised fp32 rows, allocated on first use
     __half *qkv = nullptr, *ctx = nullptr, *ffn = nullptr;
-    CUtensorMap m_yhi, m_ctx, m_ffn;      // fp16 [rows,*] box {64,128}: GEMM A operands (m_ffn is also FFN1's output map)
-    std::unordered_map<int, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per padded length
+    // fp16 [rows, *] box {64,128}: GEMM A operands, per TEXT_GEOMETRIES entry (a narrower model reads the same buffers densely
+    // at its own widths)
+    struct ActMaps {
+        CUtensorMap yhi, ctx, ffn;
+    } act[2];
+    std::map<std::pair<int, int>, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per (padded length, hidden)
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
     int32_t* ids_in[NSLOT] = {};
     int32_t* lens_in[NSLOT] = {};
@@ -282,23 +294,26 @@ struct Prof {
     std::vector<cudaEvent_t> evs;
 };
 
-int get_qkv_map(Dev& d, int S, const CUtensorMap** out, const CUtensorMap** out_ctx) {
-    auto it = d.m_qkv_by_S.find(S);
+int get_qkv_map(Dev& d, int S, int hidden, const CUtensorMap** out, const CUtensorMap** out_ctx) {
+    const auto key = std::make_pair(S, hidden);
+    auto it = d.m_qkv_by_S.find(key);
     if (it == d.m_qkv_by_S.end()) {
         CUtensorMap m, mc;
         const uint64_t B = static_cast<uint64_t>(g_rt->cap_rows) / S;
-        int rc = make_map_qkv(&m, d.qkv, B, S);
+        const uint32_t head_dim = hidden / HEADS;
+        int rc = make_map_qkv(&m, d.qkv, B, S, 3 * hidden, head_dim);
         if (rc) return rc;
-        rc = make_map_qkv(&mc, d.ctx, B, S, HIDDEN);
+        rc = make_map_qkv(&mc, d.ctx, B, S, hidden, head_dim);
         if (rc) return rc;
-        it = d.m_qkv_by_S.emplace(S, std::make_pair(m, mc)).first;
+        it = d.m_qkv_by_S.emplace(key, std::make_pair(m, mc)).first;
     }
     *out = &it->second.first;
     *out_ctx = &it->second.second;
     return 0;
 }
 
-// Enqueue the forward of one padded batch [B, S] on `stream`.  out: fp32 [B, 768], may be peer memory.
+// Enqueue the forward of one padded batch [B, S] on `stream`.  out: fp32 [B, hidden], may be peer memory.  Widths, statistic
+// partials and the attention head size follow the model's geometry.
 // n_layers >= 0 (debug): stop early and materialise the post-LN hidden state in d.x32_dbg.
 int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int32_t* lens, int B, int S, float* out,
                     cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr) {
@@ -308,8 +323,10 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, c
     const bool full = n_layers < 0;
     const int M = B * S;
     if (M > g_rt->cap_rows) return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds wave capacity %d rows", B, S, g_rt->cap_rows);
+    const int H = c.hidden, I = c.inter, P = H / 128, HD = H / c.heads;
+    const Dev::ActMaps& am = d.act[geometry_index(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
-    if (int rc = get_qkv_map(d, S, &mq, &mc)) return rc;
+    if (int rc = get_qkv_map(d, S, H, &mq, &mc)) return rc;
     uint64_t nl = 0;
     auto mark = [&](const char* name) {
         if (prof) {
@@ -322,36 +339,36 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, c
     };
     mark("begin");
     float* const dbg = full ? nullptr : d.x32_dbg;
-    CUDA_TRY(launch_embed(ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, c.vocab, stream));
+    CUDA_TRY(launch_embed(ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, c.vocab, H, stream));
     ++nl; mark("embed");
     const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // the LayerNorm that applies to the current residual rows
     for (int l = 0; l < L; ++l) {
         const LayerW& lw = w.layers[l];
         // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
-        GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
+        GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, c.eps};
+        CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
         ++nl; mark("gemm_qkv");
-        CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream));
+        CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, HD));
         ++nl; mark("attention");
         // y <- ctx Wao^T + b + LN_prev(y); new row statistics (LN1's) into pstats[1]
-        GemmEpi e_ao{lw.ao_b, d.pstats[0], STAT_PARTS, prev_g, prev_b, d.pstats[1], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
+        GemmEpi e_ao{lw.ao_b, d.pstats[0], P, prev_g, prev_b, d.pstats[1], c.eps};
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
         ++nl; mark("gemm_attn_out");
-        GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, d.m_yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
+        GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, c.eps};
+        CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
         ++nl; mark("gemm_ffn1_gelu");
         // y <- ffn W2^T + b + LN1(y); LN2's statistics into pstats[0]
-        GemmEpi e_ff2{lw.ff2_b, d.pstats[1], STAT_PARTS, lw.ln1_g, lw.ln1_b, d.pstats[0], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
+        GemmEpi e_ff2{lw.ff2_b, d.pstats[1], P, lw.ln1_g, lw.ln1_b, d.pstats[0], c.eps};
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
         ++nl; mark("gemm_ffn2");
         prev_g = lw.ln2_g;
         prev_b = lw.ln2_b;
     }
     if (full) {
-        CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, c.eps, stream));
+        CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, c.eps, H, stream));
         ++nl; mark("pool_normalize");
     } else {  // debug: materialise the post-LayerNorm hidden state
-        CUDA_TRY(launch_ln_materialize(d.yhi, d.ylo, prev_g, prev_b, dbg, M, c.eps, stream));
+        CUDA_TRY(launch_ln_materialize(d.yhi, d.ylo, prev_g, prev_b, dbg, M, c.eps, H, stream));
         ++nl;
     }
     if (launches) *launches += nl;
@@ -370,7 +387,8 @@ int forward_enqueue_vit(Dev& d, const Model& m, int dev_index, const float* pixe
     const int L = n_layers < 0 ? c.layers : n_layers;
     if (M > g_rt->cap_rows || B > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "batch of %d images exceeds the wave capacity (%d)", B, VIT_WAVE_ITEMS);
     const CUtensorMap *mq = nullptr, *mc = nullptr;
-    if (int rc = get_qkv_map(d, T, &mq, &mc)) return rc;
+    if (int rc = get_qkv_map(d, T, HIDDEN, &mq, &mc)) return rc;
+    const Dev::ActMaps& am = d.act[0];
     uint64_t nl = 0;
     // patches -> im2col rows in the (idle) ffn buffer -> patch projection into the (idle) ctx buffer -> + class / position
     // embeddings, pre_layrnorm -> residual stream + statistics
@@ -382,14 +400,14 @@ int forward_enqueue_vit(Dev& d, const Model& m, int dev_index, const float* pixe
     for (int l = 0; l < L; ++l) {
         const LayerW& lw = w.layers[l];
         GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
-        CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream, HIDDEN / HEADS));
         GemmEpi e_ao{lw.ao_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[1], c.eps};  // h += ctx Wo^T + b (raw residual)
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
         GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, d.m_yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
         GemmEpi e_ff2{lw.ff2_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[0], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, d.m_ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
+        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
         nl += 5;
     }
     if (n_layers < 0) {
@@ -469,7 +487,7 @@ int forward(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int
                 cache.entries.erase(victim);
             }
             const CUtensorMap *mq = nullptr, *mc = nullptr;
-            if (int r2 = get_qkv_map(d, S, &mq, &mc)) return r2;  // host-side map creation happens outside the capture
+            if (int r2 = get_qkv_map(d, S, m.cfg.hidden, &mq, &mc)) return r2;  // host-side map creation happens outside the capture
             uint64_t nl = 0;
             CUDA_TRY(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
             rc = forward_enqueue(d, m, dev_index, ids, lens, B, S, out, stream, -1, nullptr, &nl);
@@ -936,9 +954,12 @@ int alloc_dev(Runtime& rt, Dev& d) {
     CUDA_TRY(cudaMemset(d.qkv, 0, R * QKV_DIM * 2));
     CUDA_TRY(cudaMemset(d.ctx, 0, R * HIDDEN * 2));
     CUDA_TRY(cudaMemset(d.ffn, 0, R * 3072 * 2));
-    if (int rc = make_map_2d(&d.m_yhi, d.yhi, R, HIDDEN, 128)) return rc;
-    if (int rc = make_map_2d(&d.m_ctx, d.ctx, R, HIDDEN, 128)) return rc;
-    if (int rc = make_map_2d(&d.m_ffn, d.ffn, R, 3072, 128)) return rc;
+    for (int g = 0; g < 2; ++g) {
+        const TextGeometry& tg = TEXT_GEOMETRIES[g];
+        if (int rc = make_map_2d(&d.act[g].yhi, d.yhi, R, tg.hidden, 128)) return rc;
+        if (int rc = make_map_2d(&d.act[g].ctx, d.ctx, R, tg.hidden, 128)) return rc;
+        if (int rc = make_map_2d(&d.act[g].ffn, d.ffn, R, tg.inter, 128)) return rc;
+    }
     for (int s = 0; s < NSLOT; ++s) {
         CUDA_TRY(cudaMalloc(&d.ids_in[s], R * 4));
         CUDA_TRY(cudaMalloc(&d.lens_in[s], R * 4));
@@ -1034,12 +1055,13 @@ struct BlobCursor {
 
 int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, int* model_out) {
     Runtime& rt = *g_rt;
-    if (c.hidden != HIDDEN || c.heads != HEADS || c.inter != 3072 || c.max_pos > MAX_SEQ || c.max_pos < 1 ||
-        c.layers < 1 || c.vocab < 1 || c.type_vocab < 1)
+    bool known = false;
+    for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
+    if (!known || c.max_pos > MAX_SEQ || c.max_pos < 1 || c.layers < 1 || c.vocab < 1 || c.type_vocab < 1)
         return fail(B200RT_E_UNSUPPORTED,
-                    "kernels are specialised for hidden=768 heads=12 inter=3072 max_pos<=512 (got %d/%d/%d/%d)", c.hidden,
-                    c.heads, c.inter, c.max_pos);
-    const size_t H = HIDDEN, I = 3072;
+                    "kernels cover two geometries, bge-base (hidden=768 heads=12 inter=3072) and bge-small (hidden=384 heads=12 "
+                    "inter=1536), with max_pos<=512 (got hidden %d heads %d inter %d max_pos %d)", c.hidden, c.heads, c.inter, c.max_pos);
+    const size_t H = c.hidden, I = c.inter;
     const size_t emb = (static_cast<size_t>(c.vocab) + c.max_pos + c.type_vocab) * H + 2 * H;
     const size_t per_layer_w = 3 * H * H + H * H + I * H + H * I;
     const size_t per_layer_p = 3 * H + H + 2 * H + I + H + 2 * H;
@@ -1048,6 +1070,7 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, in
 
     auto m = std::make_unique<Model>();
     m->cfg = c;
+    m->out_dim = c.hidden;
     const size_t per_layer_x = 3 * H + I;  // derived vectors: qkv_c, ff1_c
     const size_t blob_f32 = emb + static_cast<size_t>(c.layers) * per_layer_p;
     m->f32_elems = blob_f32 + static_cast<size_t>(c.layers) * per_layer_x;
@@ -1409,7 +1432,7 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     } else {
         t->ids.assign(ids, ids + static_cast<size_t>(n_items) * max_len);
     }
-    t->out_pinned = is_pinned(out, static_cast<size_t>(n_items) * HIDDEN * 4);
+    t->out_pinned = is_pinned(out, static_cast<size_t>(n_items) * m->out_dim * 4);
     if (lens) t->lens.assign(lens, lens + n_items);
     else t->lens.assign(n_items, max_len);
     // runs of items per 64-token length bucket (TEI batches by token budget, un-padded; here every bucket is padded to its
@@ -1694,8 +1717,9 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
                       const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!a || !w || !bias || !out || M < 1 || N % 256 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
-    if (ln_stats && (epi == 2 ? N : K) != HIDDEN) return fail(B200RT_E_INVALID, "the LayerNorm'd width must be %d", HIDDEN);
+    if (!a || !w || !bias || !out || M < 1 || N % 128 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
+    if (ln_stats && (epi == 2 ? N : K) != 768 && (epi == 2 ? N : K) != 384)
+        return fail(B200RT_E_INVALID, "the LayerNorm'd width must be 768 or 384");
     if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
     Dev& d = *rt->devs[0];
     if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
@@ -1787,10 +1811,14 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     return 0;
 }
 
-int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms) {
+int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms,
+                           int head_dim) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!qkv || !lens || !ctx || B < 1 || S < 1 || S > MAX_SEQ) return fail(B200RT_E_INVALID, "bad attention arguments");
+    if (head_dim == 0) head_dim = 64;
+    if (head_dim != 64 && head_dim != 32) return fail(B200RT_E_INVALID, "head_dim must be 64 or 32 (0 = 64), got %d", head_dim);
+    const size_t H = static_cast<size_t>(HEADS) * head_dim;
     Dev& d = *rt->devs[0];
     if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
     const int grid_sms = sms ? sms : d.sm_count;
@@ -1799,39 +1827,42 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     const size_t M = static_cast<size_t>(B) * S;
     __half *dq = nullptr, *dc = nullptr;
     int32_t* dl_ = nullptr;
-    CUDA_TRY(cudaMalloc(&dq, M * QKV_DIM * 2));
-    CUDA_TRY(cudaMalloc(&dc, M * HIDDEN * 2));
+    CUDA_TRY(cudaMalloc(&dq, M * 3 * H * 2));
+    CUDA_TRY(cudaMalloc(&dc, M * H * 2));
     CUDA_TRY(cudaMalloc(&dl_, static_cast<size_t>(B) * 4));
-    CUDA_TRY(cudaMemset(dc, 0xFF, M * HIDDEN * 2));
-    CUDA_TRY(cudaMemcpy(dq, qkv, M * QKV_DIM * 2, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemset(dc, 0xFF, M * H * 2));
+    CUDA_TRY(cudaMemcpy(dq, qkv, M * 3 * H * 2, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(dl_, lens, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice));
     CUtensorMap tq, tc;
-    if (int rc = make_map_qkv(&tq, dq, B, S)) return rc;
-    if (int rc = make_map_qkv(&tc, dc, B, S, HIDDEN)) return rc;
+    if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, head_dim)) return rc;
+    if (int rc = make_map_qkv(&tc, dc, B, S, H, head_dim)) return rc;
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
     if (iters < 1) iters = 1;
-    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute));
+    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim));
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute));
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim));
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
     if (ms_out) *ms_out = ms / iters;
-    CUDA_TRY(cudaMemcpy(ctx, dc, M * HIDDEN * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(ctx, dc, M * H * 2, cudaMemcpyDeviceToHost));
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     cudaFree(dq); cudaFree(dc); cudaFree(dl_);
     return 0;
 }
 
 int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, int n_tokens, int S, int vocab,
-                       uint16_t* hi_out, uint16_t* lo_out, float* stats_out) {
+                       uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!ids || !word || !pos || !type0 || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1)
         return fail(B200RT_E_INVALID, "bad embed arguments");
+    if (hidden == 0) hidden = 768;
+    if (hidden != 768 && hidden != 384) return fail(B200RT_E_INVALID, "row width must be 768 or 384 (0 = 768), got %d", hidden);
+    const size_t H = hidden, P = H / 128;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
@@ -1842,16 +1873,16 @@ int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, 
     __half *dhi, *dlo;
     float2* dst;
     CUDA_TRY(b.upload(&dids, ids, rows * 4));
-    CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * HIDDEN * 4));
-    CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * HIDDEN * 4));
-    CUDA_TRY(b.upload(&dt, type0, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dhi, nullptr, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dlo, nullptr, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dst, nullptr, rows * STAT_PARTS * sizeof(float2)));
-    CUDA_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, d.compute));
-    CUDA_TRY(b.download(hi_out, dhi, rows * HIDDEN * 2));
-    CUDA_TRY(b.download(lo_out, dlo, rows * HIDDEN * 2));
-    CUDA_TRY(b.download(stats_out, dst, rows * STAT_PARTS * sizeof(float2)));
+    CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * H * 4));
+    CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * H * 4));
+    CUDA_TRY(b.upload(&dt, type0, H * 4));
+    CUDA_TRY(b.upload(&dhi, nullptr, rows * H * 2));
+    CUDA_TRY(b.upload(&dlo, nullptr, rows * H * 2));
+    CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
+    CUDA_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, hidden, d.compute));
+    CUDA_TRY(b.download(hi_out, dhi, rows * H * 2));
+    CUDA_TRY(b.download(lo_out, dlo, rows * H * 2));
+    CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
     return 0;
 }
 
@@ -1885,10 +1916,13 @@ int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const fl
 }
 
 int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
-                                float eps, float* out) {
+                                float eps, float* out, int hidden) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!hi || !lo || !gamma || !beta || !out || n_items < 1 || S < 1) return fail(B200RT_E_INVALID, "bad pool_normalize arguments");
+    if (hidden == 0) hidden = 768;
+    if (hidden != 768 && hidden != 384) return fail(B200RT_E_INVALID, "row width must be 768 or 384 (0 = 768), got %d", hidden);
+    const size_t H = hidden;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
@@ -1896,13 +1930,13 @@ int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const fl
     DebugBuffers b(d.compute);
     __half *dhi, *dlo;
     float *dg, *dbt, *dout;
-    CUDA_TRY(b.upload(&dhi, hi, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dlo, lo, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * HIDDEN * 4));
-    CUDA_TRY(launch_pool_normalize(dhi, dlo, dg, dbt, dout, n_items, S, eps, d.compute));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * HIDDEN * 4));
+    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+    CUDA_TRY(b.upload(&dg, gamma, H * 4));
+    CUDA_TRY(b.upload(&dbt, beta, H * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * H * 4));
+    CUDA_TRY(launch_pool_normalize(dhi, dlo, dg, dbt, dout, n_items, S, eps, hidden, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * H * 4));
     return 0;
 }
 
@@ -1982,7 +2016,7 @@ int b200rt_debug_hidden(int model, const int32_t* ids, const int32_t* lens, int 
     int rc = forward(d, *m, 0, dids, dlens, n_items, max_len, nullptr, d.compute, n_layers);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(d.compute));
-    CUDA_TRY(cudaMemcpy(hidden_out, d.x32_dbg, M * HIDDEN * 4, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(hidden_out, d.x32_dbg, M * m->cfg.hidden * 4, cudaMemcpyDeviceToHost));
     cudaFree(dids); cudaFree(dlens);
     return 0;
 }

@@ -1,6 +1,7 @@
 // Warp-specialised wgmma GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] . W[N,K]^T + bias)
 //
-// Persistent CTAs walk 128 x 256 output tiles (tile = blockIdx.x, blockIdx.x + gridDim.x, ...).  Three warpgroups:
+// Persistent CTAs walk 128 x BN output tiles, BN = 256, or 128 where N % 256 != 0 (bge-small's 384 / 1152-wide projections;
+// the figures below are BN = 256's, BN = 128 halves the W box, the stage and the accumulators) (tile = blockIdx.x, blockIdx.x + gridDim.x, ...).  Three warpgroups:
 //   warpgroup 0  : one thread TMA-loads A [128 x 64] and W [256 x 64] per 64-wide k-block into a STAGES-deep ring
 //                  (48 KB per stage, 128B-swizzled), running ahead across tiles while the consumers are in their epilogue;
 //   warpgroups 1-2: consumer c owns rows 64c .. 64c+63 of the tile and all 256 columns: four wgmma.m64n256k16 per k-block
@@ -28,15 +29,19 @@ namespace b200 {
 namespace gemm {
 
 constexpr int BM = 128;  // rows per tile (two consumer warpgroups of 64)
-constexpr int BN = 256;  // columns per tile
 constexpr int BK = 64, STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2;            // 16 KB
-constexpr int B_BYTES = BN * BK * 2;            // 32 KB (two TMA boxes of 128 rows)
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // 48 KB
-constexpr int OFF_BAR = STAGES * STAGE_BYTES;
 constexpr int NUM_THREADS = 384;
-constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-static_assert(SMEM_BYTES <= 232448, "shared memory");
+
+// ring layout of the BN-column kernel
+template <int BN>
+struct Tiles {
+    static constexpr int B_BYTES = BN * BK * 2;            // 32 KB (two TMA boxes of 128 rows) / 16 KB (one)
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // 48 KB / 32 KB
+    static constexpr int OFF_BAR = STAGES * STAGE_BYTES;
+    static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+    static_assert(SMEM_BYTES <= 232448, "shared memory");
+};
 
 // erf-GELU x * Phi(x), erf by Abramowitz-Stegun 7.1.26 (abs err <= 1.5e-7): 2 MUFU (rcp, ex2) per value
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -59,27 +64,47 @@ __device__ __forceinline__ float gelu_quick(float x) {
     return x * r;
 }
 
-// LayerNorm statistics of a row from its STAT_PARTS (sum, M2) partials (Chan et al.)
+// LayerNorm statistics of a row from its PARTS (sum, M2) partials (Chan et al.): 6 for a 768-wide row, 3 for a 384-wide one
+template <int PARTS>
 __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float eps, float& mean, float& rstd) {
-    const float4* __restrict__ pp = reinterpret_cast<const float4*>(st);
-    const float4 a = __ldg(pp), b = __ldg(pp + 1), c = __ldg(pp + 2);
-    const float2 p[STAT_PARTS] = {make_float2(a.x, a.y), make_float2(a.z, a.w), make_float2(b.x, b.y),
-                                  make_float2(b.z, b.w), make_float2(c.x, c.y), make_float2(c.z, c.w)};
-    constexpr float inv_n = 1.0f / (128.0f * STAT_PARTS);
-    mean = (((p[0].x + p[1].x) + (p[2].x + p[3].x)) + (p[4].x + p[5].x)) * inv_n;
-    float m2[STAT_PARTS];
+    static_assert(PARTS == 6 || PARTS == 3, "LayerNorm width 768 or 384");
+    constexpr float inv_n = 1.0f / (128.0f * PARTS);
+    if constexpr (PARTS == 6) {
+        const float4* __restrict__ pp = reinterpret_cast<const float4*>(st);
+        const float4 a = __ldg(pp), b = __ldg(pp + 1), c = __ldg(pp + 2);
+        const float2 p[PARTS] = {make_float2(a.x, a.y), make_float2(a.z, a.w), make_float2(b.x, b.y),
+                                 make_float2(b.z, b.w), make_float2(c.x, c.y), make_float2(c.z, c.w)};
+        mean = (((p[0].x + p[1].x) + (p[2].x + p[3].x)) + (p[4].x + p[5].x)) * inv_n;
+        float m2[PARTS];
 #pragma unroll
-    for (int i = 0; i < STAT_PARTS; ++i) {
-        const float d = p[i].x * (1.0f / 128.0f) - mean;
-        m2[i] = fmaf(128.0f * d, d, p[i].y);
+        for (int i = 0; i < PARTS; ++i) {
+            const float d = p[i].x * (1.0f / 128.0f) - mean;
+            m2[i] = fmaf(128.0f * d, d, p[i].y);
+        }
+        rstd = rsqrtf((((m2[0] + m2[1]) + (m2[2] + m2[3])) + (m2[4] + m2[5])) * inv_n + eps);
+    } else {
+        // a row's three partials are 24 bytes: 8-byte loads
+        const float2 p[PARTS] = {__ldg(st), __ldg(st + 1), __ldg(st + 2)};
+        mean = ((p[0].x + p[1].x) + p[2].x) * inv_n;
+        float m2[PARTS];
+#pragma unroll
+        for (int i = 0; i < PARTS; ++i) {
+            const float d = p[i].x * (1.0f / 128.0f) - mean;
+            m2[i] = fmaf(128.0f * d, d, p[i].y);
+        }
+        rstd = rsqrtf(((m2[0] + m2[1]) + m2[2]) * inv_n + eps);
     }
-    rstd = rsqrtf((((m2[0] + m2[1]) + (m2[2] + m2[3])) + (m2[4] + m2[5])) * inv_n + eps);
 }
 
-template <int EPI>
+// BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128)
+template <int EPI, int BN, int PARTS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
             __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K) {
+    static_assert(BN == 256 || BN == 128, "tile width");
+    constexpr int B_BYTES = Tiles<BN>::B_BYTES, STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
+    constexpr int NACC = BN / 2;     // fp32 accumulators per consumer thread
+    constexpr int NSLICE = BN / 128; // 128-column statistic slices per tile
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -119,7 +144,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
                     mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
                     tma_load_2d(sa, &tma_a, &full[stage], kb * BK, m0);
                     tma_load_2d(sa + A_BYTES, &tma_b, &full[stage], kb * BK, n0);
-                    tma_load_2d(sa + A_BYTES + B_BYTES / 2, &tma_b, &full[stage], kb * BK, n0 + BN / 2);
+                    if constexpr (BN == 256) tma_load_2d(sa + A_BYTES + B_BYTES / 2, &tma_b, &full[stage], kb * BK, n0 + BN / 2);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -137,9 +162,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m0 = (tile / num_n) * BM, n_blk = tile % num_n, n0 = n_blk * BN;
-        float acc[128];
+        float acc[NACC];
 #pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
         int prev = -1;
         for (int kb = 0; kb < kblocks; ++kb) {
             mbar_wait(&full[stage], phase);
@@ -148,8 +173,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             wgmma_fence();
             fence_operands(acc);
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-                wgmma_m64n256k16_ss(acc, make_sw128_desc(a_addr + k * 32), make_sw128_desc(b_addr + k * 32), (kb | k) != 0);
+            for (int k = 0; k < BK / 16; ++k) {
+                if constexpr (BN == 256) wgmma_m64n256k16_ss(acc, make_sw128_desc(a_addr + k * 32), make_sw128_desc(b_addr + k * 32), (kb | k) != 0);
+                else wgmma_m64n128k16_ss(acc, make_sw128_desc(a_addr + k * 32), make_sw128_desc(b_addr + k * 32), (kb | k) != 0);
+            }
             wgmma_commit();
             fence_operands(acc);
             if (prev >= 0) {
@@ -170,11 +197,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
         if (has_ln) {
 #pragma unroll
             for (int h = 0; h < 2; ++h)
-                if (r0 + 8 * h < M) row_stats(ep.stats_in + static_cast<size_t>(r0 + 8 * h) * STAT_PARTS, ep.eps, mean[h], rstd[h]);
+                if (r0 + 8 * h < M) row_stats<PARTS>(ep.stats_in + static_cast<size_t>(r0 + 8 * h) * PARTS, ep.eps, mean[h], rstd[h]);
         }
         if constexpr (EPI != EPI_BIAS_RES_SPLIT) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
+            for (int j = 0; j < BN / 8; ++j) {
                 const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -190,9 +217,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             }
         } else {
             // y' = acc + bias + LN(y); LN(y) = fmaf((y - mean) * rstd, gamma, beta) (stats_in NULL: the residual is added as is)
-            float csum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // [row][128-column half of the tile]
+            float csum[2][NSLICE] = {};  // [row][128-column slice of the tile]
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
+            for (int j = 0; j < BN / 8; ++j) {
                 const int col = c0 + 8 * j;
                 const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + col));
                 float2 gm = make_float2(1.f, 1.f), bt = make_float2(0.f, 0.f);
@@ -225,7 +252,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
 #pragma unroll
-                    for (int half = 0; half < 2; ++half) {
+                    for (int half = 0; half < NSLICE; ++half) {
                         float s = csum[h][half];
                         s += __shfl_xor_sync(0xffffffff, s, 1);
                         s += __shfl_xor_sync(0xffffffff, s, 2);
@@ -240,7 +267,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
                         m2 += __shfl_xor_sync(0xffffffff, m2, 2);
                         const int row = r0 + 8 * h;
                         if ((lane & 3) == 0 && row < M)
-                            ep.stats_out[static_cast<size_t>(row) * (N / 128) + n_blk * 2 + half] = make_float2(s, m2);
+                            ep.stats_out[static_cast<size_t>(row) * (N / 128) + n_blk * NSLICE + half] = make_float2(s, m2);
                     }
                 }
             }
@@ -250,37 +277,62 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
 
 }  // namespace gemm
 
-template <int EPI>
+template <int EPI, int BN, int PARTS>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                               int K, int sm_count, cudaStream_t stream) {
-    const int tiles = ((M + gemm::BM - 1) / gemm::BM) * (N / gemm::BN);
+    const int tiles = ((M + gemm::BM - 1) / gemm::BM) * (N / BN);
     const int grid = tiles < sm_count ? tiles : sm_count;
-    return launch_pdl(gemm::gemm_kernel<EPI>, dim3(grid), dim3(gemm::NUM_THREADS), gemm::SMEM_BYTES, stream, ta, tb, e, out, out_lo, M, N, K);
+    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(grid), dim3(gemm::NUM_THREADS), gemm::Tiles<BN>::SMEM_BYTES, stream, ta, tb, e,
+                      out, out_lo, M, N, K);
+}
+
+// the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / ViT launch), else 128
+template <int EPI>
+static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
+                              int K, int sm_count, cudaStream_t stream) {
+    const bool wide = N % 256 == 0;
+    const bool six = e.stats_in == nullptr || e.parts_in == 6;
+    if (wide) return six ? launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream)
+                         : launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
+    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream)
+               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
+}
+
+template <int EPI, int BN, int PARTS>
+static cudaError_t set_smem() {
+    return cudaFuncSetAttribute(gemm::gemm_kernel<EPI, BN, PARTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::Tiles<BN>::SMEM_BYTES);
+}
+template <int EPI>
+static cudaError_t set_smem_epi() {
+    cudaError_t e;
+    if ((e = set_smem<EPI, 256, 6>()) != cudaSuccess) return e;
+    if ((e = set_smem<EPI, 256, 3>()) != cudaSuccess) return e;
+    if ((e = set_smem<EPI, 128, 6>()) != cudaSuccess) return e;
+    return set_smem<EPI, 128, 3>();
 }
 
 cudaError_t gemm_init_device() {
     cudaError_t e;
-    e = cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_GELU_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_QGELU_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(gemm::gemm_kernel<EPI_BIAS_RES_SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::SMEM_BYTES);
+    if ((e = set_smem_epi<EPI_BIAS_F16>()) != cudaSuccess) return e;
+    if ((e = set_smem_epi<EPI_BIAS_GELU_F16>()) != cudaSuccess) return e;
+    if ((e = set_smem_epi<EPI_BIAS_QGELU_F16>()) != cudaSuccess) return e;
+    return set_smem_epi<EPI_BIAS_RES_SPLIT>();
 }
 
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                         int K, int sm_count, cudaStream_t stream) {
-    if (N % gemm::BN != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
-    if (e.stats_in != nullptr && e.parts_in != STAT_PARTS) return cudaErrorInvalidValue;  // the LayerNorm'd width is HIDDEN
+    if (N % 128 != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
+    // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 768 or 384
+    const int ln_width = epi == EPI_BIAS_RES_SPLIT ? N : K;
+    if (e.stats_in != nullptr && ((e.parts_in != 6 && e.parts_in != 3) || e.parts_in * 128 != ln_width)) return cudaErrorInvalidValue;
     switch (epi) {
-        case EPI_BIAS_F16: return launch_one<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
-        case EPI_BIAS_GELU_F16: return launch_one<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
-        case EPI_BIAS_QGELU_F16: return launch_one<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
         case EPI_BIAS_RES_SPLIT:
             if (out_lo == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr))) return cudaErrorInvalidValue;
             if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
-            return launch_one<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
+            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
     }
     return cudaErrorInvalidValue;
 }

@@ -14,17 +14,19 @@ enum GemmEpilogue : int {
     EPI_BIAS_QGELU_F16 = 3, // out fp16 = quick_gelu(LNfold(acc) + bias), x * sigmoid(1.702 x)   (CLIP MLP up-projection)
 };
 
+// Two text geometries: bge-base (hidden 768, 12 heads of 64, inter 3072) and bge-small (hidden 384, 12 heads of 32,
+// inter 1536); the ViT tower is 768 wide.  The constants below are the widest geometry's: workspaces are sized by them, and a
+// narrower model uses the same buffers densely at its own widths.
 constexpr int HIDDEN = 768;
-constexpr int HEADS = 12;
-constexpr int HEAD_DIM = 64;
+constexpr int HEADS = 12;  // both text geometries
 constexpr int QKV_DIM = 3 * HIDDEN;
-constexpr int STAT_PARTS = HIDDEN / 128;  // row statistics travel as one (sum, M2) partial per 128 columns
+constexpr int STAT_PARTS = HIDDEN / 128;  // row statistics travel as one (sum, M2) partial per 128 columns: 6 (768) or 3 (384)
 
 // One-time per-device setup (dynamic shared memory opt-in for every kernel). Call with the device current.
 cudaError_t kernels_init_device();
 
 // The residual stream lives in HBM as y = hi + lo (two fp16 arrays, 22 mantissa bits together), stored PRE-LayerNorm, with
-// the row statistics of the LayerNorm that applies to it as STAT_PARTS partials per row: (sum, M2 about the partial's own
+// the row statistics of the LayerNorm that applies to it as width / 128 partials per row: (sum, M2 about the partial's own
 // mean) over each 128-column slice, written by whoever produced the row (embedding kernel or a residual GEMM epilogue).
 // No kernel ever materialises LN(y):
 //   * a GEMM that consumes LN(y) reads `hi` as its fp16 A operand against W'' = fp16(gamma o W - rowmean(gamma o W)): gamma folded
@@ -38,7 +40,9 @@ cudaError_t kernels_init_device();
 //   EPI 2    : out = hi, out_lo = lo, both fp16 [M, N] row-major (read and written in place); e.stats_in + e.ln_gamma/
 //              e.ln_beta describe the LayerNorm of the residual (stats_in NULL: the residual is added as is); e.stats_out
 //              receives the partials of the new rows (N / 128 per row; must not alias stats_in: other tiles still read those).
-//   N % 256 == 0, K % 64 == 0; rows past M are neither read from out nor written.
+//   N % 128 == 0, K % 64 == 0; rows past M are neither read from out nor written.  Tiles are 128 x 256 when N % 256 == 0,
+//   else 128 x 128.  e.parts_in (with stats_in) must be the LayerNorm'd width / 128, that width being 768 or 384 (K for
+//   EPI 0/1/3, N for EPI 2).
 struct GemmEpi {
     const float* bias;        // [N]
     const float2* stats_in;   // [rows][parts_in]
@@ -56,24 +60,26 @@ cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, _
 cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, __half* w_out, float* cvec,
                            int N, int K, cudaStream_t stream);
 
-// Multi-head self-attention over a padded batch: qkv fp16 [B, S, 2304] (Q | K | V, head-major within each),
-// lens[B] valid keys per item, ctx fp16 [B*S, 768].  tq: 3D map over qkv {2304, S, B}, tctx: 3D map over ctx {768, S, B};
-// both box {64,128,1}, 128B swizzle.  Persistent: min(units, sm_count) CTAs walk the (item, head[, query tile]) units.
+// Multi-head self-attention over a padded batch of 12 heads of head_dim (64 or 32), H = 12 head_dim: qkv fp16 [B, S, 3H]
+// (Q | K | V, head-major within each), lens[B] valid keys per item, ctx fp16 [B*S, H].  tq: 3D map over qkv {3H, S, B},
+// tctx: 3D map over ctx {H, S, B}; both box {head_dim, 128, 1}, 128B (d = 64) or 64B (d = 32) swizzle.  Persistent:
+// min(units, sm_count) CTAs walk the (item, head[, query tile]) units.
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                             cudaStream_t stream);
+                             cudaStream_t stream, int head_dim);
 
+// Text row kernels on rows of `width` (768 or 384) columns.
 // word + position + token_type(0) embedding gather -> y = hi + lo (pre-LN residual stream) + the row's statistic partials.
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,
-                         float2* stats, int n_tokens, int S, int vocab, cudaStream_t stream);
+                         float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream);
 
 // debug only: x32[row] = LN(hi + lo) with the row's own statistics (the product path never materialises this)
 cudaError_t launch_ln_materialize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* x32,
-                                  int n_rows, float eps, cudaStream_t stream);
+                                  int n_rows, float eps, int width, cudaStream_t stream);
 
-// final LayerNorm of the CLS row of every item + L2 normalise; row i is stored at out + i * 768,
+// final LayerNorm of the CLS row of every item + L2 normalise; row i is stored at out + i * width,
 // where `out` may be a peer-mapped pointer into the root GPU's gather buffer (the fused gather).
 cudaError_t launch_pool_normalize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* out,
-                                  int n_items, int S, float eps, cudaStream_t stream);
+                                  int n_items, int S, float eps, int width, cudaStream_t stream);
 
 // ViT image tower (CLIP): pixels fp32 [n, 3, img, img] -> im2col A fp16 [n*T, 3 p p] (class-token rows zero); patch GEMM output +
 // class / position embeddings + pre_layrnorm -> residual stream + statistics; pooled head: post_layernorm(class token) ->

@@ -3,11 +3,11 @@
 // inputs, the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns), and a debug-only
 // LayerNorm materialisation.
 //
-// Row kernels: one warp per 768-wide row, 128-bit accesses, statistics by warp shuffle in fp32, two-pass variance on
-// register-resident data (no E[x^2]-E[x]^2 cancellation).
+// Row kernels: one warp per row (768 wide, or 384 for bge-small's embed / pool / LayerNorm), 128-bit accesses, statistics
+// by warp shuffle in fp32, two-pass variance on register-resident data (no E[x^2]-E[x]^2 cancellation).
 //
-// The residual stream is stored PRE-LayerNorm as y = hi + lo (fp16 + fp16) together with STAT_PARTS (sum, M2) partials per
-// row; there is no LayerNorm kernel in the product path -- the consuming GEMM folds it into its epilogue (kernels.h).
+// The residual stream is stored PRE-LayerNorm as y = hi + lo (fp16 + fp16) together with one (sum, M2) partial per 128
+// columns of each row; there is no LayerNorm kernel in the product path -- the consuming GEMM folds it into its epilogue (kernels.h).
 //
 // Restates BertEmbeddings.forward (HF modeling_bert.py:72-111), the LayerNorm halves of
 // BertSelfOutput :287-298 / BertOutput :345-356, and sentence-transformers' CLS pooling + Normalize
@@ -18,10 +18,16 @@
 namespace b200 {
 namespace rw {
 
-constexpr int H = HIDDEN;          // 768
-constexpr int V4 = H / 4 / 32;     // float4 per lane = 6: float4 i of lane l holds columns [128 i + 4 l, +4)
+// Row width W: float4 i of lane l holds columns [128 i + 4 l, +4), i < W / 128 -- so float4 i of every lane covers exactly the
+// i-th 128-column statistic slice.  The ViT kernels are 768 wide only.
+constexpr int H = HIDDEN;  // 768
+template <int W>
+struct Row {
+    static_assert(W == 768 || W == 384, "row width");
+    static constexpr int V4 = W / 128;  // float4 per lane: 6 or 3
+};
+constexpr int V4 = Row<H>::V4;
 constexpr int WARPS_PER_BLOCK = 8;
-static_assert(V4 == STAT_PARTS, "float4 i of every lane covers exactly the i-th 128-column slice");
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -29,23 +35,25 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-// normalise the 24 register-resident values of this lane in place; returns (mean, rstd) of the row
-__device__ __forceinline__ float2 ln_inplace(float4 (&x)[V4], const float* __restrict__ gamma,
+// normalise the 4 W / 128 register-resident values of this lane in place; returns (mean, rstd) of the row
+template <int W = H>
+__device__ __forceinline__ float2 ln_inplace(float4 (&x)[Row<W>::V4], const float* __restrict__ gamma,
                                              const float* __restrict__ beta, float eps, int lane) {
+    constexpr int V4 = Row<W>::V4;
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < V4; ++i) s += (x[i].x + x[i].y) + (x[i].z + x[i].w);
     // __fmul_rn: the rounded mean itself is subtracted.  A plain product would be contracted into the subtractions below
     // (fma(-s, 1/768, x)), which see the unrounded s * fl(1/768): a constant row then centres to -x * 2^-25 instead of 0,
     // and rstd = eps^-1/2 blows that up into a unit vector where LayerNorm + F.normalize give zeros.
-    const float mean = __fmul_rn(warp_sum(s), 1.0f / H);
+    const float mean = __fmul_rn(warp_sum(s), 1.0f / W);
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < V4; ++i) {
         x[i].x -= mean; x[i].y -= mean; x[i].z -= mean; x[i].w -= mean;
         q += (x[i].x * x[i].x + x[i].y * x[i].y) + (x[i].z * x[i].z + x[i].w * x[i].w);
     }
-    const float rstd = rsqrtf(warp_sum(q) * (1.0f / H) + eps);
+    const float rstd = rsqrtf(warp_sum(q) * (1.0f / W) + eps);
     const float4* g4 = reinterpret_cast<const float4*>(gamma);
     const float4* b4 = reinterpret_cast<const float4*>(beta);
 #pragma unroll
@@ -60,11 +68,13 @@ __device__ __forceinline__ float2 ln_inplace(float4 (&x)[V4], const float* __res
     return make_float2(mean, rstd);
 }
 
-// y = hi + lo of one row -> 24 fp32 values per lane (same column mapping as a float4 row)
+// y = hi + lo of one row -> 4 W / 128 fp32 values per lane (same column mapping as a float4 row)
+template <int W = H>
 __device__ __forceinline__ void load_split_row(const __half* __restrict__ yhi, const __half* __restrict__ ylo, size_t row, int lane,
-                                               float4 (&x)[V4]) {
-    const uint2* h2 = reinterpret_cast<const uint2*>(yhi + row * H);
-    const uint2* l2 = reinterpret_cast<const uint2*>(ylo + row * H);
+                                               float4 (&x)[Row<W>::V4]) {
+    constexpr int V4 = Row<W>::V4;
+    const uint2* h2 = reinterpret_cast<const uint2*>(yhi + row * W);
+    const uint2* l2 = reinterpret_cast<const uint2*>(ylo + row * W);
 #pragma unroll
     for (int i = 0; i < V4; ++i) {
         const uint2 hv = h2[i * 32 + lane], lv = l2[i * 32 + lane];
@@ -74,22 +84,24 @@ __device__ __forceinline__ void load_split_row(const __half* __restrict__ yhi, c
     }
 }
 
+template <int W>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ word, const float* __restrict__ pos,
              const float* __restrict__ type0, __half* __restrict__ yhi, __half* __restrict__ ylo, float2* __restrict__ stats,
              int n_tokens, int S, int vocab) {
+    constexpr int V4 = Row<W>::V4;
     const int lane = threadIdx.x & 31;
     const int tok = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
     if (tok >= n_tokens) return;
     int id = ids[tok];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);  // submit() rejects out-of-range ids; never read OOB
     const int p = tok % S;
-    const float4* w4 = reinterpret_cast<const float4*>(word + static_cast<size_t>(id) * H);
-    const float4* p4 = reinterpret_cast<const float4*>(pos + static_cast<size_t>(p) * H);
+    const float4* w4 = reinterpret_cast<const float4*>(word + static_cast<size_t>(id) * W);
+    const float4* p4 = reinterpret_cast<const float4*>(pos + static_cast<size_t>(p) * W);
     const float4* t4 = reinterpret_cast<const float4*>(type0);
-    uint2* oh = reinterpret_cast<uint2*>(yhi + static_cast<size_t>(tok) * H);
-    uint2* ol = reinterpret_cast<uint2*>(ylo + static_cast<size_t>(tok) * H);
-    float ps = 0.f, pq = 0.f;  // lane i < STAT_PARTS keeps partial i
+    uint2* oh = reinterpret_cast<uint2*>(yhi + static_cast<size_t>(tok) * W);
+    uint2* ol = reinterpret_cast<uint2*>(ylo + static_cast<size_t>(tok) * W);
+    float ps = 0.f, pq = 0.f;  // lane i < V4 keeps partial i
 #pragma unroll
     for (int i = 0; i < V4; ++i) {
         const float4 a = __ldg(w4 + i * 32 + lane);
@@ -109,38 +121,42 @@ embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ word, co
         const float q = warp_sum((dx * dx + dy * dy) + (dz * dz + dw * dw));
         if (lane == i) { ps = s; pq = q; }
     }
-    if (lane < STAT_PARTS) stats[static_cast<size_t>(tok) * STAT_PARTS + lane] = make_float2(ps, pq);
+    if (lane < V4) stats[static_cast<size_t>(tok) * V4 + lane] = make_float2(ps, pq);
 }
 
 // debug only (b200rt_debug_hidden): materialise LN(hi + lo) in fp32
+template <int W>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 ln_materialize_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, const float* __restrict__ gamma,
                       const float* __restrict__ beta, float* __restrict__ x32, int n_rows, float eps) {
+    constexpr int V4 = Row<W>::V4;
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
     if (row >= n_rows) return;
     float4 x[V4];
-    load_split_row(yhi, ylo, row, lane, x);
-    ln_inplace(x, gamma, beta, eps, lane);
-    float4* o32 = reinterpret_cast<float4*>(x32 + static_cast<size_t>(row) * H);
+    load_split_row<W>(yhi, ylo, row, lane, x);
+    ln_inplace<W>(x, gamma, beta, eps, lane);
+    float4* o32 = reinterpret_cast<float4*>(x32 + static_cast<size_t>(row) * W);
 #pragma unroll
     for (int i = 0; i < V4; ++i) o32[i * 32 + lane] = x[i];
 }
 
+template <int W>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 pool_normalize_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, const float* __restrict__ gamma,
                       const float* __restrict__ beta, float* __restrict__ out, int n_items, int S, float eps) {
+    constexpr int V4 = Row<W>::V4;
     const int lane = threadIdx.x & 31;
     const int item = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
     if (item >= n_items) return;
     float4 x[V4];
-    load_split_row(yhi, ylo, static_cast<size_t>(item) * S, lane, x);  // CLS row
-    ln_inplace(x, gamma, beta, eps, lane);
+    load_split_row<W>(yhi, ylo, static_cast<size_t>(item) * S, lane, x);  // CLS row
+    ln_inplace<W>(x, gamma, beta, eps, lane);
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < V4; ++i) q += (x[i].x * x[i].x + x[i].y * x[i].y) + (x[i].z * x[i].z + x[i].w * x[i].w);
     const float inv = 1.0f / fmaxf(sqrtf(warp_sum(q)), 1e-12f);  // torch.nn.functional.normalize eps
-    float4* o4 = reinterpret_cast<float4*>(out + static_cast<size_t>(item) * H);  // may be peer memory
+    float4* o4 = reinterpret_cast<float4*>(out + static_cast<size_t>(item) * W);  // may be peer memory
 #pragma unroll
     for (int i = 0; i < V4; ++i)
         o4[i * 32 + lane] = make_float4(x[i].x * inv, x[i].y * inv, x[i].z * inv, x[i].w * inv);
@@ -217,7 +233,7 @@ vit_embed_kernel(const __half* __restrict__ patch_out, const float* __restrict__
         const float q = warp_sum((dx * dx + dy * dy) + (dz * dz + dw * dw));
         if (lane == i) { ps = sm; pq = q; }
     }
-    if (lane < STAT_PARTS) stats[static_cast<size_t>(row) * STAT_PARTS + lane] = make_float2(ps, pq);
+    if (lane < V4) stats[static_cast<size_t>(row) * V4 + lane] = make_float2(ps, pq);
 }
 
 // One block per image: post_layernorm of the class-token row, visual projection [P, H], L2 normalise; row i is stored at
@@ -322,23 +338,29 @@ scatter_kernel(const int32_t* __restrict__ src_ids, const int32_t* __restrict__ 
 }  // namespace rw
 
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,
-                         float2* stats, int n_tokens, int S, int vocab, cudaStream_t stream) {
+                         float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream) {
     const int grid = (n_tokens + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
-    rw::embed_kernel<<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
+    if (width == 768) rw::embed_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
+    else if (width == 384) rw::embed_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
+    else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 
 cudaError_t launch_ln_materialize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* x32,
-                                  int n_rows, float eps, cudaStream_t stream) {
+                                  int n_rows, float eps, int width, cudaStream_t stream) {
     const int grid = (n_rows + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
-    rw::ln_materialize_kernel<<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, x32, n_rows, eps);
+    if (width == 768) rw::ln_materialize_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, x32, n_rows, eps);
+    else if (width == 384) rw::ln_materialize_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, x32, n_rows, eps);
+    else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 
 cudaError_t launch_pool_normalize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* out,
-                                  int n_items, int S, float eps, cudaStream_t stream) {
+                                  int n_items, int S, float eps, int width, cudaStream_t stream) {
     const int grid = (n_items + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
-    rw::pool_normalize_kernel<<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
+    if (width == 768) rw::pool_normalize_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
+    else if (width == 384) rw::pool_normalize_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
+    else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 

@@ -13,6 +13,16 @@ import threading
 from http.server import BaseHTTPRequestHandler, ThreadingHTTPServer
 
 GEOMETRY = dict(vocab=30522, hidden=768, layers=12, heads=12, inter=3072, max_pos=512, type_vocab=2, eps=1e-12)
+BGE_SMALL_ID = "BAAI/bge-small-en-v1.5"
+
+
+def geometry_for_model_id(model_id: str) -> dict:
+    """Geometry of the offline seeded fallback and of a raw --weights blob (which carries no shapes): bge-small's for
+    BAAI/bge-small-en-v1.5, bge-base's for BAAI/bge-base-en-v1.5 and for any id this table does not know."""
+    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_SMALL_GEOMETRY
+
+    known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY}
+    return dict(known.get(model_id, BGE_BASE_GEOMETRY))
 
 
 def parse_args(argv):
@@ -37,11 +47,11 @@ def parse_args(argv):
     return args
 
 
-def random_blob(seed=0):
-    """Seeded BGE-base-geometry weights (the one definition lives in b200rt.weights)."""
+def random_blob(seed=0, geometry=None):
+    """Seeded weights of `geometry` (default BGE-base; the one definition lives in b200rt.weights)."""
     from b200rt.weights import random_blob as rb
 
-    return rb(GEOMETRY, seed)
+    return rb(geometry or GEOMETRY, seed)
 
 
 def load_weights(args):
@@ -56,13 +66,14 @@ def load_weights(args):
             return W.load_safetensors(args.weights) + (f"safetensors {args.weights}",)
         if os.path.isdir(args.weights):
             return W.load_hf_dir(args.weights) + (f"HF directory {args.weights}",)
-        return dict(GEOMETRY), np.fromfile(args.weights, np.float32), f"flat blob {args.weights}"
+        return geometry_for_model_id(args.model_id), np.fromfile(args.weights, np.float32), f"flat blob {args.weights}"
     cache = args.huggingface_hub_cache or os.environ.get("HUGGINGFACE_HUB_CACHE") or os.environ.get("HF_HUB_CACHE")
     if cache:
         snap = W.resolve_hub_snapshot(cache, args.model_id)
         if snap:
             return W.load_hf_dir(snap) + (f"hub snapshot {snap}",)
-    return dict(GEOMETRY), random_blob(), None
+    g = geometry_for_model_id(args.model_id)
+    return g, random_blob(geometry=g), None
 
 
 class Engine:

@@ -7,7 +7,9 @@ written as CUDA.
   mode "fold"   : y16 = fp16(y) (the raw pre-LayerNorm residual) feeds QKV / FFN1 with gamma folded into the weight columns;
                   and the weight rows centred; the epilogue applies rstd * acc + (W beta + b)   (round-2 design, no LN kernels)
 
-    python tools/emulate_numerics.py [--style hf|trained|hard] [--layers 12] [--items 4] [--seq 512]
+    python tools/emulate_numerics.py [--geometry base|small] [--style hf|trained|hard] [--layers 12] [--items 4] [--seq 512]
+
+--geometry small: bge-small (hidden 384, 12 heads of 32, inter 1536) instead of bge-base.
 """
 import argparse
 import math
@@ -19,6 +21,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import bge_ref as R  # noqa: E402
+
+GEOMETRIES = {"base": {}, "small": dict(hidden=384, heads=12, inter=1536)}
 
 f16 = lambda a: a.astype(np.float16).astype(np.float32)  # noqa: E731
 
@@ -45,7 +49,7 @@ def emulate(flat, ids, lens, g, mode="current", p_sum="exact", keep=()):
     y = (W["emb.word"][ids] + W["emb.type"][0]) + W["emb.pos"][:S][None]
     ln = ("emb.ln.g", "emb.ln.b")
     keymask = np.arange(S)[None, :] >= np.asarray(lens)[:, None]
-    k2 = np.float32(0.125 * 1.4426950408889634)
+    k2 = np.float32(1.4426950408889634 / math.sqrt(dh))  # softmax scale 1 / sqrt(d) in base 2
 
     def ln_apply(y, ln):
         mu, rstd = stats(y, g.eps)
@@ -85,6 +89,7 @@ def emulate(flat, ids, lens, g, mode="current", p_sum="exact", keep=()):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--geometry", choices=("base", "small"), default="base")
     ap.add_argument("--style", default="hf")
     ap.add_argument("--layers", type=int, default=12)
     ap.add_argument("--items", type=int, default=4)
@@ -92,12 +97,12 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--ablate", action="store_true")
     a = ap.parse_args()
-    g = R.BertGeometry(layers=a.layers)
+    g = R.BertGeometry(layers=a.layers, **GEOMETRIES[a.geometry])
     flat = R.make_weights(g, a.seed, a.style)
     ids, lens = R.synth_ragged(a.items, a.seq, seed=1, min_len=max(1, a.seq // 4))
     ref = R.forward_np(flat, ids, lens, g, dtype=np.float64)
     hf = R.forward_hf(R.build_hf_model(flat, g), ids, lens)
-    print(f"style {a.style} layers {a.layers} items {a.items} x {a.seq}")
+    print(f"geometry {a.geometry} style {a.style} layers {a.layers} items {a.items} x {a.seq}")
     print("  HF fp32 vs numpy fp64     :", R.rel_l2(hf, ref).max())
     for mode in ("current", "fold"):
         for ps in ("exact", "p16"):
