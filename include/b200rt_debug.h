@@ -21,11 +21,13 @@ extern "C" {
  *            bias = W beta + b:  out = epi(rstd * acc + bias)
  *   epi 2  : out = acc + bias + ((resid - mean) * rstd * ln_gamma + ln_beta) (ln_stats NULL: acc + bias + resid);
  *            stats_out (optional) receives [M][N/128] (sum, M2) partials of the new rows.
- * sms: CTAs the persistent kernel is launched with (0 = the device's SM count, else 1..SM count; anything else is
- * B200RT_E_INVALID) -- the result must not depend on it.                                                          */
+ * sms: the most CTAs the persistent kernel is launched with (0 = the device's SM count, else 1..SM count; anything else
+ * is B200RT_E_INVALID).  The kernel runs as clusters of 2 CTAs: sms is rounded down to whole clusters, at least one, and
+ * capped by the clusters that fit on the device at once -- the result must not depend on it.  ctas_out (optional)
+ * receives the number of CTAs launched.                                                                           */
 int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid,
                       void* out, int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
-                      const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms);
+                      const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out);
 
 /* ctx[B*S,H] (fp16 bits) = multi-head attention of 12 heads of head_dim over qkv[B*S,3H] (fp16 bits), lens[B],
  * H = 12 head_dim; head_dim 64 or 32 (0 = 64).  sms as for b200rt_debug_gemm (it also decides whether units are split

@@ -101,7 +101,8 @@ def load_library():
         lib.b200rt_shutdown.restype = None
         lib.b200rt_debug_gemm.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p, ctypes.c_void_p,
-                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_int]
+                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_int,
+                                          ctypes.POINTER(ctypes.c_int)]
         lib.b200rt_debug_attention.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p,
                                                ctypes.c_int, ctypes.c_int]
         vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
@@ -369,10 +370,11 @@ def device_sync(gpu: int = 0):
 
 
 def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, resid=None, iters: int = 1, ln_stats=None,
-               ln_gamma=None, ln_beta=None, eps: float = 1e-12, want_stats: bool = False, sms: int = 0):
-    """a16 [M,K], w16 [N,K] float16; returns (out, ms) -- or (out, ms, stats_out [M, N/128, 2]) with ``want_stats`` (epi 2).
+               ln_gamma=None, ln_beta=None, eps: float = 1e-12, want_stats: bool = False, sms: int = 0, want_ctas: bool = False):
+    """a16 [M,K], w16 [N,K] float16; returns (out, ms) -- or (out, ms, stats_out [M, N/128, 2]) with ``want_stats`` (epi 2),
+    and with ``want_ctas`` the number of CTAs launched appended.
     ``ln_stats`` [M, parts, 2] (sum, M2) partials switch the LayerNorm epilogues on (see include/b200rt_debug.h).
-    ``sms``: CTAs of the persistent launch (0 = every SM)."""
+    ``sms``: the most CTAs of the persistent launch (0 = every SM), rounded down to whole 2-CTA clusters, at least one."""
     a16 = np.ascontiguousarray(a16, dtype=np.float16)
     w16 = np.ascontiguousarray(w16, dtype=np.float16)
     bias = np.ascontiguousarray(bias, dtype=np.float32)
@@ -384,9 +386,11 @@ def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, res
     so = np.zeros((M, N // 128, 2), np.float32) if want_stats else None
     p = lambda v: _ptr(v) if v is not None else None  # noqa: E731
     ms = ctypes.c_float(0)
+    ctas = ctypes.c_int(0)
     _check(load_library().b200rt_debug_gemm(epi, _ptr(a16), _ptr(w16), _ptr(bias), p(r), _ptr(out), M, N, K, iters, ctypes.byref(ms),
-                                            p(st), p(lg), p(lb), eps, p(so), sms))
-    return (out, ms.value, so) if want_stats else (out, ms.value)
+                                            p(st), p(lg), p(lb), eps, p(so), sms, ctypes.byref(ctas)))
+    res = (out, ms.value, so) if want_stats else (out, ms.value)
+    return res + (ctas.value,) if want_ctas else res
 
 
 def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0, head_dim: int = 64):

@@ -1714,7 +1714,7 @@ void b200rt_shutdown(void) {
 
 int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid, void* out,
                       int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
-                      const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms) {
+                      const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!a || !w || !bias || !out || M < 1 || N % 128 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
@@ -1791,7 +1791,7 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(reload());
-    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // the result that is returned
+    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute, ctas_out));  // the result that is returned
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);

@@ -1,15 +1,25 @@
 // Warp-specialised wgmma GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] . W[N,K]^T + bias)
 //
-// Persistent CTAs walk 128 x BN output tiles, BN = 256, or 128 where N % 256 != 0 (bge-small's 384 / 1152-wide projections;
-// the figures below are BN = 256's, BN = 128 halves the W box, the stage and the accumulators) (tile = blockIdx.x, blockIdx.x + gridDim.x, ...).  Three warpgroups:
-//   warpgroup 0  : one thread TMA-loads A [128 x 64] and W [256 x 64] per 64-wide k-block into a STAGES-deep ring
-//                  (48 KB per stage, 128B-swizzled), running ahead across tiles while the consumers are in their epilogue;
+// Persistent clusters of CM = 2 CTAs walk pairs of 128 x BN output tiles that share their columns, BN = 256, or 128 where
+// N % 256 != 0 (bge-small's 384 / 1152-wide projections; the figures below are BN = 256's, BN = 128 halves the W box, the
+// stage and the accumulators).  Pair p = (m-pair p / num_n, n-block p % num_n), n fastest; CTA rank r of the cluster takes
+// m-tile CM (p / num_n) + r; cluster c walks p = c, c + clusters, ..., its two CTAs in step.  Three warpgroups per CTA:
+//   warpgroup 0  : one thread TMA-loads its own A [128 x 64] per 64-wide k-block into a STAGES-deep ring (48 KB per stage,
+//                  128B-swizzled), plus its share of the pair's W [256 x 64] -- 128-row box b is loaded by rank b % CM and
+//                  multicast into the same stage of every CTA of the cluster, so the pair reads W from L2 once instead of
+//                  twice (2 A + W = 64 KB per k-block-pair instead of 96 KB).  It runs ahead across tiles while the
+//                  consumers are in their epilogue;
 //   warpgroups 1-2: consumer c owns rows 64c .. 64c+63 of the tile and all 256 columns: four wgmma.m64n256k16 per k-block
 //                  into 128 fp32 accumulator registers per thread, one k-block's MMAs kept in flight while the previous
-//                  stage is handed back to the producer; then the epilogue runs straight from the registers.
+//                  stage is handed back to the producers; then the epilogue runs straight from the registers.
 //
-//   full[s]  : producer arrive.expect_tx(48 KB); the TMA loads complete_tx on it
-//   empty[s] : one arrival per consumer warp once the wgmma that read stage s have completed
+//   full[s]  : own producer arrive.expect_tx(48 KB); own A, own W share and the peer's W share complete_tx on it
+//   empty[s] : one arrival per consumer warp of EVERY CTA of the cluster once the wgmma that read stage s have completed
+//              (8 CM arrivals): a producer refills a stage -- its multicast writes the peer's copy too -- only once the
+//              consumers of both CTAs are done with it.  Both CTAs walk the same pairs and k-blocks, so the rings run in
+//              lockstep.  A rank whose m-tile lies past M still loads and arrives; its epilogue stores nothing (row < M).
+// A cluster barrier after the barrier init (before any remote arrive or multicast) and one before exit (so that no CTA leaves
+// while the peer may still arrive on its barriers) bracket the protocol; every thread of both warpgroups takes both.
 //
 // Epilogues (see kernels.h for the residual-stream format):
 //   EPI_BIAS(_GELU / _QGELU)_F16 : folded LayerNorm  rstd * acc + c  (c = W beta + b), optional GELU, fp16 out;
@@ -22,6 +32,8 @@
 // Replaces (inside TEI, un-vendored; restated from HF modeling_bert.py): the Linear layers of
 // BertSelfAttention :143-207 (fused QKV), BertSelfOutput.dense :287-298, BertIntermediate :330-342
 // (dense + GELU) and BertOutput.dense :345-356.
+#include <algorithm>
+
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -31,7 +43,9 @@ namespace gemm {
 constexpr int BM = 128;  // rows per tile (two consumer warpgroups of 64)
 constexpr int BK = 64, STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2;            // 16 KB
+constexpr int W_BOX_BYTES = 128 * BK * 2;       // one 128-row TMA box of W: 16 KB
 constexpr int NUM_THREADS = 384;
+constexpr int CM = 2;  // CTAs per cluster, along M, sharing every W tile
 
 // ring layout of the BN-column kernel
 template <int BN>
@@ -98,13 +112,13 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float e
 
 // BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128)
 template <int EPI, int BN, int PARTS>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __cluster_dims__(CM, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
             __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K) {
     static_assert(BN == 256 || BN == 128, "tile width");
-    constexpr int B_BYTES = Tiles<BN>::B_BYTES, STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
+    constexpr int STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
     constexpr int NACC = BN / 2;     // fp32 accumulators per consumer thread
-    constexpr int NSLICE = BN / 128; // 128-column statistic slices per tile
+    constexpr int NSLICE = BN / 128; // 128-column statistic slices per tile, and 128-row W boxes per stage
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -115,7 +129,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
     const int lane = lane_id();
     const int num_n = N / BN;
-    const int num_tiles = ((M + BM - 1) / BM) * num_n;
+    // Slot t = CM p + r is rank r's tile of pair p.  A 1-D grid of (CM, 1, 1) clusters numbers its CTAs blockIdx.x =
+    // CM cluster + rank, so t = blockIdx.x, blockIdx.x + gridDim.x, ... walks pairs cluster, cluster + clusters, ... with both
+    // ranks in step (and keeps the loop state of an unclustered walk: two more live registers spill the epilogue).
+    const int num_slots = ((M + CM * BM - 1) / (CM * BM)) * num_n * CM;
     const int kblocks = K / BK;
 
     if (threadIdx.x == 0) {
@@ -123,11 +140,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
         prefetch_tmap(&tma_b);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 8);  // the 8 consumer warps
+            mbar_init(&empty[s], 8 * CM);  // the 8 consumer warps of every CTA of the cluster
         }
         fence_barrier_init();
     }
-    __syncthreads();
+    cluster_sync();  // the peer's barriers are initialised before anything arrives on them or multicasts into its ring
     griddep_wait();  // everything above overlapped the previous kernel's tail; nothing it wrote has been read yet
 
     if (warp < 4) {
@@ -136,19 +153,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
         if (warp == 0 && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
+            for (int t = blockIdx.x; t < num_slots; t += gridDim.x) {
+                const int p = t / CM, rank = t % CM;
+                const int m0 = ((p / num_n) * CM + rank) * BM, n0 = (p % num_n) * BN;
                 for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(&empty[stage], phase ^ 1);
+                    mbar_wait(&empty[stage], phase ^ 1);  // the consumers of every CTA of the cluster have freed the stage
                     uint8_t* sa = smem + stage * STAGE_BYTES;
-                    mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
+                    mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);  // own A + all of W, whichever CTA loads each box
                     tma_load_2d(sa, &tma_a, &full[stage], kb * BK, m0);
-                    tma_load_2d(sa + A_BYTES, &tma_b, &full[stage], kb * BK, n0);
-                    if constexpr (BN == 256) tma_load_2d(sa + A_BYTES + B_BYTES / 2, &tma_b, &full[stage], kb * BK, n0 + BN / 2);
+                    for (int b = rank; b < NSLICE; b += CM)
+                        tma_load_2d_multicast(sa + A_BYTES + b * W_BOX_BYTES, &tma_b, &full[stage], kb * BK, n0 + 128 * b,
+                                              (1u << CM) - 1);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
+        __syncwarp();
+        cluster_sync();
         return;
     }
 
@@ -160,8 +181,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     const bool has_ln = ep.stats_in != nullptr;
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n) * BM, n_blk = tile % num_n, n0 = n_blk * BN;
+    for (int t = blockIdx.x; t < num_slots; t += gridDim.x) {
+        const int p = t / CM;
+        const int m0 = ((p / num_n) * CM + t % CM) * BM, n_blk = p % num_n, n0 = n_blk * BN;
         float acc[NACC];
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
@@ -181,14 +203,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             fence_operands(acc);
             if (prev >= 0) {
                 wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
-                if (lane == 0) mbar_arrive(&empty[prev]);
+                if (lane < CM) mbar_arrive_cluster(&empty[prev], lane);  // lane r frees it in CTA r's producer's eyes
             }
             prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         wgmma_wait<0>();
         fence_operands(acc);
-        if (lane == 0) mbar_arrive(&empty[prev]);
+        if (lane < CM) mbar_arrive_cluster(&empty[prev], lane);
 
         // -------------------------------------------------------------------- epilogue, straight from the registers
         const int r0 = m0 + cw * 64 + w4 * 16 + (lane >> 2);  // this thread's rows r0 and r0 + 8
@@ -273,66 +295,89 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             }
         }
     }
+    cluster_sync();  // the peer's consumers have made their last arrival on this CTA's barriers
 }
 
 }  // namespace gemm
 
+// Clusters of this instantiation that fit on the GPU at once (cudaOccupancyMaxActiveClusters at set-up; the least over the
+// devices set up).  Not assumed to be SM count / CM: a cluster must sit within one GPC, and GPCs differ in size.
+template <int EPI, int BN, int PARTS>
+static int& max_clusters() {
+    static int n = 0;
+    return n;
+}
+
 template <int EPI, int BN, int PARTS>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                              int K, int sm_count, cudaStream_t stream) {
-    const int tiles = ((M + gemm::BM - 1) / gemm::BM) * (N / BN);
-    const int grid = tiles < sm_count ? tiles : sm_count;
-    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(grid), dim3(gemm::NUM_THREADS), gemm::Tiles<BN>::SMEM_BYTES, stream, ta, tb, e,
-                      out, out_lo, M, N, K);
+                              int K, int sm_count, cudaStream_t stream, int* ctas) {
+    const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
+    int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
+    if (clusters < 1) clusters = 1;
+    if (ctas) *ctas = clusters * gemm::CM;
+    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::Tiles<BN>::SMEM_BYTES,
+                      stream, ta, tb, e, out, out_lo, M, N, K);
 }
 
 // the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / ViT launch), else 128
 template <int EPI>
 static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                              int K, int sm_count, cudaStream_t stream) {
+                              int K, int sm_count, cudaStream_t stream, int* ctas) {
     const bool wide = N % 256 == 0;
     const bool six = e.stats_in == nullptr || e.parts_in == 6;
-    if (wide) return six ? launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream)
-                         : launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
-    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream)
-               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
+    if (wide) return six ? launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas)
+                         : launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas)
+               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
 }
 
 template <int EPI, int BN, int PARTS>
-static cudaError_t set_smem() {
-    return cudaFuncSetAttribute(gemm::gemm_kernel<EPI, BN, PARTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::Tiles<BN>::SMEM_BYTES);
+static cudaError_t setup() {
+    auto kernel = gemm::gemm_kernel<EPI, BN, PARTS>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::Tiles<BN>::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    cudaLaunchConfig_t cfg = {};  // the cluster shape comes from the kernel's __cluster_dims__
+    cfg.gridDim = dim3(gemm::CM);
+    cfg.blockDim = dim3(gemm::NUM_THREADS);
+    cfg.dynamicSmemBytes = gemm::Tiles<BN>::SMEM_BYTES;
+    int n = 0;
+    if ((e = cudaOccupancyMaxActiveClusters(&n, kernel, &cfg)) != cudaSuccess) return e;
+    if (n < 1) return cudaErrorInvalidConfiguration;
+    int& m = max_clusters<EPI, BN, PARTS>();
+    m = m == 0 ? n : std::min(m, n);
+    return cudaSuccess;
 }
 template <int EPI>
-static cudaError_t set_smem_epi() {
+static cudaError_t setup_epi() {
     cudaError_t e;
-    if ((e = set_smem<EPI, 256, 6>()) != cudaSuccess) return e;
-    if ((e = set_smem<EPI, 256, 3>()) != cudaSuccess) return e;
-    if ((e = set_smem<EPI, 128, 6>()) != cudaSuccess) return e;
-    return set_smem<EPI, 128, 3>();
+    if ((e = setup<EPI, 256, 6>()) != cudaSuccess) return e;
+    if ((e = setup<EPI, 256, 3>()) != cudaSuccess) return e;
+    if ((e = setup<EPI, 128, 6>()) != cudaSuccess) return e;
+    return setup<EPI, 128, 3>();
 }
 
 cudaError_t gemm_init_device() {
     cudaError_t e;
-    if ((e = set_smem_epi<EPI_BIAS_F16>()) != cudaSuccess) return e;
-    if ((e = set_smem_epi<EPI_BIAS_GELU_F16>()) != cudaSuccess) return e;
-    if ((e = set_smem_epi<EPI_BIAS_QGELU_F16>()) != cudaSuccess) return e;
-    return set_smem_epi<EPI_BIAS_RES_SPLIT>();
+    if ((e = setup_epi<EPI_BIAS_F16>()) != cudaSuccess) return e;
+    if ((e = setup_epi<EPI_BIAS_GELU_F16>()) != cudaSuccess) return e;
+    if ((e = setup_epi<EPI_BIAS_QGELU_F16>()) != cudaSuccess) return e;
+    return setup_epi<EPI_BIAS_RES_SPLIT>();
 }
 
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                        int K, int sm_count, cudaStream_t stream) {
+                        int K, int sm_count, cudaStream_t stream, int* ctas) {
     if (N % 128 != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
     // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 768 or 384
     const int ln_width = epi == EPI_BIAS_RES_SPLIT ? N : K;
     if (e.stats_in != nullptr && ((e.parts_in != 6 && e.parts_in != 3) || e.parts_in * 128 != ln_width)) return cudaErrorInvalidValue;
     switch (epi) {
-        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
-        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
-        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream);
+        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
         case EPI_BIAS_RES_SPLIT:
             if (out_lo == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr))) return cudaErrorInvalidValue;
             if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
-            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream);
+            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
     }
     return cudaErrorInvalidValue;
 }

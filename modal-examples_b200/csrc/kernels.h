@@ -42,7 +42,12 @@ cudaError_t kernels_init_device();
 //              receives the partials of the new rows (N / 128 per row; must not alias stats_in: other tiles still read those).
 //   N % 128 == 0, K % 64 == 0; rows past M are neither read from out nor written.  Tiles are 128 x 256 when N % 256 == 0,
 //   else 128 x 128.  e.parts_in (with stats_in) must be the LayerNorm'd width / 128, that width being 768 or 384 (K for
-//   EPI 0/1/3, N for EPI 2).
+//   EPI 0/1/3, N for EPI 2).  ta's map may end at M rows or run past them: a tile's A rows past M only feed rows no store
+//   reaches.
+//   The kernel runs as 2-CTA clusters (two m-tiles sharing one W tile):  min(tile pairs, sm_count / 2, the clusters that
+//   fit at once) clusters, at least one -- sm_count bounds the CTAs from above, rounded down to whole clusters, except that
+//   sm_count = 1 still launches one cluster of 2.  The result does not depend on sm_count.  ctas (optional) receives the
+//   number of CTAs launched.
 struct GemmEpi {
     const float* bias;        // [N]
     const float2* stats_in;   // [rows][parts_in]
@@ -53,7 +58,7 @@ struct GemmEpi {
     float eps;
 };
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                        int K, int sm_count, cudaStream_t stream);
+                        int K, int sm_count, cudaStream_t stream, int* ctas = nullptr);
 
 // gamma != NULL: w_out[n,k] = fp16(w[n,k] gamma[k] - mean_k(w[n,:] gamma)), cvec[n] = sum_k w[n,k] beta[k] + bias[n]
 // gamma == NULL: w_out = fp16(w) (cvec untouched)
@@ -112,7 +117,8 @@ cudaError_t launch_scatter(const int32_t* src_ids, const int32_t* src_lens, cons
 #include <utility>
 // Launch with programmatic stream serialisation: the kernel's CTAs may be scheduled while the previous kernel of the
 // stream drains (see ptx.cuh: griddep_launch_dependents / griddep_wait); the kernel itself waits before it reads anything
-// the previous kernel wrote.
+// the previous kernel wrote.  A kernel declared with __cluster_dims__ (the GEMM) is launched in clusters of that shape; the
+// grid must then be a whole number of clusters.
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     cudaLaunchConfig_t cfg = {};

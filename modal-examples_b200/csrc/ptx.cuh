@@ -54,6 +54,21 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
+// Arrive on the barrier at `bar`'s offset in the shared memory of CTA `cta` of the cluster (this CTA's own rank included).
+// Default .release.cta semantics: enough to hand a ring stage back once the wgmma that read it have been waited for, and
+// cheap -- .release.cluster would put a GPU-wide memory barrier (MEMBAR.ALL.GPU) in front of every arrival, which also
+// waits for the previous tile's epilogue stores.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+    asm volatile(
+        "{\n\t"
+        ".reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
+        "}\n"
+        ::"r"(smem_u32(bar)), "r"(cta)
+        : "memory");
+}
+
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -129,6 +144,17 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+        : "memory");
+}
+
+// The same box, written to `smem_dst`'s offset in every CTA of the cluster whose bit is set in `cta_mask`; each of those
+// CTAs' barrier at `bar`'s offset receives the complete_tx of its copy.  One L2 read serves all of them.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
 
@@ -304,6 +330,14 @@ __device__ __forceinline__ float4 lds128f(uint32_t addr) {
 }
 __device__ __forceinline__ void sts32f(uint32_t addr, float a) {
     asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(a) : "memory");
+}
+
+// ------------------------------------------------------------------------------------ thread-block clusters
+
+// Every non-exited thread of every CTA of the cluster: what each did before its arrive (barrier inits, remote arrivals) is
+// visible to all after the wait.  Not .aligned: the threads of a warp may reach it apart.
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
 
 // ------------------------------------------------------------------------------------ misc
