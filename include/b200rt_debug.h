@@ -66,6 +66,24 @@ int b200rt_debug_hidden(int model, const int32_t* ids, const int32_t* lens, int 
  * image], hidden_out fp32 [n_items * tokens, hidden] on the host (pre-LN architecture: the stream itself, not a LayerNorm of it). */
 int b200rt_debug_vit_hidden(int model, const float* pixels, int n_items, int n_layers, float* hidden_out);
 
+/* Trace of the product forward on replica 0: the workspace is set to 0xFF bytes (NaN in fp16 and fp32), then the first
+ * n_launches launches of the forward of this batch run exactly as the product enqueues them (same kernels, buffers and stream,
+ * no sync or copy between them), and the workspace is copied out once they finish.  n_launches is in [0, n_total], n_total =
+ * 5 layers + 2 (text: embed, 5 per layer, pool_normalize) or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer,
+ * vit_pool).  Every buffer comes back for rows = min(M + 256, 512 b200rt_wave_capacity_items()) rows, M = n_items * max_len
+ * (text) or n_items * tokens (vit), at the model's widths (H = hidden, I = inter, P = H / 128):
+ *   yhi, ylo, ctx: fp16 bits [rows, H]; qkv: fp16 bits [rows, 3H]; ffn: fp16 bits [rows, I] (vit: the im2col matrix
+ *   [M, 3 p p] is its start until FFN1 overwrites it); pstats0, pstats1: (sum, M2) float pairs [rows, P];
+ *   out: fp32 [n_items, out_dim], poisoned too, written by the pool launch.
+ * names_out receives the names of the launches run, NUL-terminated and packed (up to names_cap bytes); n_total (optional)
+ * the launch count of the whole forward.                                                                                 */
+int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_launches,
+                               uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx,
+                               uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total);
+int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
+                                   float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx, uint16_t* ffn, float* out,
+                                   char* names_out, size_t names_cap, int* n_total);
+
 /* Per-kernel device times (ms, CUDA events on the compute stream) of one forward of a resident batch:
  * names_out receives up to cap NUL-terminated names packed in a char buffer, ms_out the times.        */
 int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters, char* names_out, size_t names_cap,

@@ -29,7 +29,8 @@ ABI_SYMBOLS = [
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
 DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_hidden", "b200rt_debug_vit_hidden", "b200rt_debug_profile_forward",
-                 "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_vit_pool", "b200rt_debug_fold_ln"]
+                 "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_vit_pool", "b200rt_debug_fold_ln",
+                 "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace"]
 
 
 def SPLIT_SMS(k: int) -> int:
@@ -112,6 +113,8 @@ def load_library():
         lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
         lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
         lib.b200rt_debug_hidden.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
+        lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
+        lib.b200rt_debug_vit_forward_trace.argtypes = [ci, vp, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                      f32p, i32p, ctypes.c_int]
         _lib = lib
@@ -242,7 +245,7 @@ class EmbedModel:
         blob = np.ascontiguousarray(blob, dtype=np.float32)
         self.cfg = BertConfig(geometry["vocab"], geometry["hidden"], geometry["layers"], geometry["heads"], geometry["inter"],
                               geometry["max_pos"], geometry["type_vocab"], geometry["eps"])
-        self.hidden = geometry["hidden"]
+        self.hidden, self.inter = geometry["hidden"], geometry["inter"]
         h = ctypes.c_int32(-1)
         _check(lib.b200rt_model_load(b"bert", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
         self.handle = h.value
@@ -306,6 +309,15 @@ class EmbedModel:
         _check(self._lib.b200rt_debug_hidden(self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_layers, _ptr(out)))
         return out.reshape(n, S, self.hidden)
 
+    def debug_trace(self, ids: np.ndarray, lens, n_launches: int) -> dict:
+        """The workspace after the first ``n_launches`` launches of this batch's forward (see :func:`_debug_trace`)."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        n, S = ids.shape
+        lens_a = np.ascontiguousarray(lens, dtype=np.int32) if lens is not None else None
+        return _debug_trace(lambda *bufs: self._lib.b200rt_debug_forward_trace(
+            self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_launches, *bufs),
+            n * S, n, self.hidden, self.inter, self.hidden, n_launches)
+
     def profile_forward(self, n_items: int, max_len: int, iters: int = 3) -> dict:
         names = ctypes.create_string_buffer(4096)
         ms = (ctypes.c_float * 64)()
@@ -327,7 +339,7 @@ class ImageEmbedModel:
         self.cfg = VitConfig(g["image"], g["patch"], g["hidden"], g["layers"], g["heads"], g["inter"], g["proj"], g["eps"])
         self.image, self.proj = g["image"], g["proj"]
         self.tokens = (g["image"] // g["patch"]) ** 2 + 1
-        self.hidden = g["hidden"]
+        self.hidden, self.inter = g["hidden"], g["inter"]
         h = ctypes.c_int32(-1)
         _check(lib.b200rt_model_load(b"vit", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
         self.handle = h.value
@@ -363,6 +375,36 @@ class ImageEmbedModel:
         out = np.empty((n * self.tokens, self.hidden), np.float32)
         _check(self._lib.b200rt_debug_vit_hidden(self.handle, _ptr(pixels), n, n_layers, _ptr(out)))
         return out.reshape(n, self.tokens, self.hidden)
+
+    def debug_trace(self, pixels: np.ndarray, n_launches: int) -> dict:
+        """The workspace after the first ``n_launches`` launches of this batch's forward (see :func:`_debug_trace`)."""
+        pixels = np.ascontiguousarray(pixels, dtype=np.float32)
+        n = pixels.shape[0]
+        return _debug_trace(lambda *bufs: self._lib.b200rt_debug_vit_forward_trace(self.handle, _ptr(pixels), n, n_launches, *bufs),
+                            n * self.tokens, n, self.hidden, self.inter, self.proj, n_launches)
+
+
+_TRACE_NAMES_CAP = 8192
+
+
+def _debug_trace(call, M: int, n_items: int, H: int, I: int, out_dim: int, n_launches: int) -> dict:
+    """One b200rt_debug_*forward_trace call (include/b200rt_debug.h).  Returns the workspace, each buffer for
+    ``rows = min(M + 256, capacity)`` rows: yhi, ylo, ctx float16 [rows, H]; qkv float16 [rows, 3H]; ffn float16 [rows, I];
+    pstats0, pstats1 float32 [rows, H / 128, 2]; ``out`` [n_items, out_dim] once the pool launch has run (else None);
+    ``names`` of the launches run, ``n_total`` launches in the whole forward, ``M`` and ``rows``."""
+    rows = min(M + 256, wave_capacity_items() * 512)
+    P = H // 128
+    bufs = dict(yhi=np.empty((rows, H), np.float16), ylo=np.empty((rows, H), np.float16),
+                pstats0=np.empty((rows, P, 2), np.float32), pstats1=np.empty((rows, P, 2), np.float32),
+                qkv=np.empty((rows, 3 * H), np.float16), ctx=np.empty((rows, H), np.float16), ffn=np.empty((rows, I), np.float16))
+    out = np.empty((n_items, out_dim), np.float32)
+    names = ctypes.create_string_buffer(_TRACE_NAMES_CAP)
+    total = ctypes.c_int32(0)
+    order = ("yhi", "ylo", "pstats0", "pstats1", "qkv", "ctx", "ffn")
+    _check(call(*(_ptr(bufs[k]) for k in order), _ptr(out), names, _TRACE_NAMES_CAP, ctypes.byref(total)))
+    bufs.update(out=out if n_launches == total.value else None, names=[s.decode() for s in names.raw.split(b"\0")[:n_launches]],
+                n_total=total.value, M=M, rows=rows)
+    return bufs
 
 
 def device_sync(gpu: int = 0):

@@ -315,8 +315,11 @@ int get_qkv_map(Dev& d, int S, int hidden, const CUtensorMap** out, const CUtens
 // Enqueue the forward of one padded batch [B, S] on `stream`.  out: fp32 [B, hidden], may be peer memory.  Widths, statistic
 // partials and the attention head size follow the model's geometry.
 // n_layers >= 0 (debug): stop early and materialise the post-LN hidden state in d.x32_dbg.
+// stop_after >= 0 (debug trace): enqueue only the first stop_after launches of the forward; `names` (optional) receives the
+// name of every launch enqueued.
 int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int32_t* lens, int B, int S, float* out,
-                    cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr) {
+                    cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr, int stop_after = -1,
+                    std::vector<std::string>* names = nullptr) {
     const DevWeights& w = m.per_dev[dev_index];
     const b200rt_bert_config& c = m.cfg;
     const int L = n_layers < 0 ? c.layers : n_layers;
@@ -337,50 +340,63 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, c
             prof->evs.push_back(e);
         }
     };
-    mark("begin");
-    float* const dbg = full ? nullptr : d.x32_dbg;
-    CUDA_TRY(launch_embed(ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, c.vocab, H, stream));
-    ++nl; mark("embed");
-    const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // the LayerNorm that applies to the current residual rows
-    for (int l = 0; l < L; ++l) {
-        const LayerW& lw = w.layers[l];
-        // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
-        GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
-        ++nl; mark("gemm_qkv");
-        CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, HD));
-        ++nl; mark("attention");
-        // y <- ctx Wao^T + b + LN_prev(y); new row statistics (LN1's) into pstats[1]
-        GemmEpi e_ao{lw.ao_b, d.pstats[0], P, prev_g, prev_b, d.pstats[1], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
-        ++nl; mark("gemm_attn_out");
-        GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
-        ++nl; mark("gemm_ffn1_gelu");
-        // y <- ffn W2^T + b + LN1(y); LN2's statistics into pstats[0]
-        GemmEpi e_ff2{lw.ff2_b, d.pstats[1], P, lw.ln1_g, lw.ln1_b, d.pstats[0], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
-        ++nl; mark("gemm_ffn2");
-        prev_g = lw.ln2_g;
-        prev_b = lw.ln2_b;
-    }
-    if (full) {
-        CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, c.eps, H, stream));
-        ++nl; mark("pool_normalize");
-    } else {  // debug: materialise the post-LayerNorm hidden state
-        CUDA_TRY(launch_ln_materialize(d.yhi, d.ylo, prev_g, prev_b, dbg, M, c.eps, H, stream));
+    // counts the launch just enqueued; true once the trace has all it asked for
+    auto step = [&](const char* name) {
         ++nl;
-    }
+        mark(name);
+        if (names) names->push_back(name);
+        return stop_after >= 0 && nl >= static_cast<uint64_t>(stop_after);
+    };
+    auto enqueue = [&]() -> int {
+        if (stop_after == 0) return 0;
+        mark("begin");
+        float* const dbg = full ? nullptr : d.x32_dbg;
+        CUDA_TRY(launch_embed(ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, c.vocab, H, stream));
+        if (step("embed")) return 0;
+        const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // the LayerNorm that applies to the current residual rows
+        for (int l = 0; l < L; ++l) {
+            const LayerW& lw = w.layers[l];
+            // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
+            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
+            if (step("gemm_qkv")) return 0;
+            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, HD));
+            if (step("attention")) return 0;
+            // y <- ctx Wao^T + b + LN_prev(y); new row statistics (LN1's) into pstats[1]
+            GemmEpi e_ao{lw.ao_b, d.pstats[0], P, prev_g, prev_b, d.pstats[1], c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
+            if (step("gemm_attn_out")) return 0;
+            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+            if (step("gemm_ffn1_gelu")) return 0;
+            // y <- ffn W2^T + b + LN1(y); LN2's statistics into pstats[0]
+            GemmEpi e_ff2{lw.ff2_b, d.pstats[1], P, lw.ln1_g, lw.ln1_b, d.pstats[0], c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
+            if (step("gemm_ffn2")) return 0;
+            prev_g = lw.ln2_g;
+            prev_b = lw.ln2_b;
+        }
+        if (full) {
+            CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, c.eps, H, stream));
+            step("pool_normalize");
+        } else {  // debug: materialise the post-LayerNorm hidden state
+            CUDA_TRY(launch_ln_materialize(d.yhi, d.ylo, prev_g, prev_b, dbg, M, c.eps, H, stream));
+            ++nl;
+        }
+        return 0;
+    };
+    if (int rc = enqueue()) return rc;
     if (launches) *launches += nl;
     return 0;
 }
 
 // Forward of one batch of images on `stream`: pixels fp32 [B, 3, image, image] in this replica's HBM; out fp32 [B, proj],
 // may be peer memory.  n_layers >= 0 (debug): stop after that many layers (the residual stream stays in yhi / ylo).
+// stop_after / names (debug trace) as for forward_enqueue.
 // CLIPVisionTransformer is pre-LN: LayerNorm1 / LayerNorm2 are folded into QKV / FFN1, the residual GEMMs add the raw
 // stream (no LayerNorm re-applied) and emit the statistics the next fold needs.
 int forward_enqueue_vit(Dev& d, const Model& m, int dev_index, const float* pixels, int B, float* out, cudaStream_t stream,
-                        int n_layers = -1, uint64_t* launches = nullptr) {
+                        int n_layers = -1, uint64_t* launches = nullptr, int stop_after = -1, std::vector<std::string>* names = nullptr) {
     const DevWeights& w = m.per_dev[dev_index];
     const b200rt_vit_config& c = m.vcfg;
     const int T = m.tokens, M = B * T;
@@ -390,39 +406,55 @@ int forward_enqueue_vit(Dev& d, const Model& m, int dev_index, const float* pixe
     if (int rc = get_qkv_map(d, T, HIDDEN, &mq, &mc)) return rc;
     const Dev::ActMaps& am = d.act[0];
     uint64_t nl = 0;
-    // patches -> im2col rows in the (idle) ffn buffer -> patch projection into the (idle) ctx buffer -> + class / position
-    // embeddings, pre_layrnorm -> residual stream + statistics
-    CUDA_TRY(launch_im2col(pixels, d.ffn, B, c.image, c.patch, stream));
-    GemmEpi e_patch{w.zero_bias, nullptr, STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-    CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, e_patch, M, HIDDEN, 3 * c.patch * c.patch, d.sm_gemm, stream));
-    CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, T, c.eps, stream));
-    nl += 3;
-    for (int l = 0; l < L; ++l) {
-        const LayerW& lw = w.layers[l];
-        GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
-        CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream, HIDDEN / HEADS));
-        GemmEpi e_ao{lw.ao_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[1], c.eps};  // h += ctx Wo^T + b (raw residual)
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
-        GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
-        GemmEpi e_ff2{lw.ff2_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[0], c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
-        nl += 5;
-    }
-    if (n_layers < 0) {
-        CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, T, c.proj, c.eps, stream));
+    auto step = [&](const char* name) {
         ++nl;
-    }
+        if (names) names->push_back(name);
+        return stop_after >= 0 && nl >= static_cast<uint64_t>(stop_after);
+    };
+    auto enqueue = [&]() -> int {
+        if (stop_after == 0) return 0;
+        // patches -> im2col rows in the (idle) ffn buffer -> patch projection into the (idle) ctx buffer -> + class / position
+        // embeddings, pre_layrnorm -> residual stream + statistics
+        CUDA_TRY(launch_im2col(pixels, d.ffn, B, c.image, c.patch, stream));
+        if (step("im2col")) return 0;
+        GemmEpi e_patch{w.zero_bias, nullptr, STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
+        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, e_patch, M, HIDDEN, 3 * c.patch * c.patch, d.sm_gemm, stream));
+        if (step("gemm_patch")) return 0;
+        CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, T, c.eps, stream));
+        if (step("vit_embed")) return 0;
+        for (int l = 0; l < L; ++l) {
+            const LayerW& lw = w.layers[l];
+            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
+            if (step("gemm_qkv")) return 0;
+            CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream, HIDDEN / HEADS));
+            if (step("attention")) return 0;
+            GemmEpi e_ao{lw.ao_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[1], c.eps};  // h += ctx Wo^T + b (raw residual)
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
+            if (step("gemm_attn_out")) return 0;
+            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
+            if (step("gemm_ffn1_qgelu")) return 0;
+            GemmEpi e_ff2{lw.ff2_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[0], c.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
+            if (step("gemm_ffn2")) return 0;
+        }
+        if (n_layers < 0) {
+            CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, T, c.proj, c.eps, stream));
+            step("vit_pool");
+        }
+        return 0;
+    };
+    if (int rc = enqueue()) return rc;
     if (launches) *launches += nl;
     return 0;
 }
 
 // Orders a ViT forward behind the previous forward on the replica's workspace, like forward() does (caller holds d.mu).
 int forward_vit(Dev& d, const Model& m, int dev_index, const float* pixels, int B, float* out, cudaStream_t stream, int n_layers = -1,
-                uint64_t* launches = nullptr) {
+                uint64_t* launches = nullptr, int stop_after = -1, std::vector<std::string>* names = nullptr) {
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(stream, d.ev_ws, 0));
-    if (int rc = forward_enqueue_vit(d, m, dev_index, pixels, B, out, stream, n_layers, launches)) return rc;
+    if (int rc = forward_enqueue_vit(d, m, dev_index, pixels, B, out, stream, n_layers, launches, stop_after, names)) return rc;
     CUDA_TRY(cudaEventRecord(d.ev_ws, stream));
     d.ev_ws_armed = true;
     return 0;
@@ -468,12 +500,13 @@ void drop_graphs(Dev& d) {  // the replica is going away: its cached launches po
 
 // The caller holds d.mu.  Orders this forward behind the previous one on the replica's workspace (see Dev::ev_ws).
 int forward(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int32_t* lens, int B, int S, float* out,
-            cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr) {
+            cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr, int stop_after = -1,
+            std::vector<std::string>* names = nullptr) {
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(stream, d.ev_ws, 0));
     int rc = 0;
-    const bool use_graph = !(n_layers >= 0 || prof || B * S > GRAPH_MAX_ROWS);
+    const bool use_graph = !(n_layers >= 0 || prof || stop_after >= 0 || B * S > GRAPH_MAX_ROWS);
     if (!use_graph) {
-        rc = forward_enqueue(d, m, dev_index, ids, lens, B, S, out, stream, n_layers, prof, launches);
+        rc = forward_enqueue(d, m, dev_index, ids, lens, B, S, out, stream, n_layers, prof, launches, stop_after, names);
     } else {
         GraphCache& cache = graph_cache(d);
         const GraphKey key{&m, ids, lens, out, stream, B, S};
@@ -1377,6 +1410,55 @@ struct DebugBuffers {
     }
 };
 
+// Host buffers of a forward trace (b200rt_debug_forward_trace / b200rt_debug_vit_forward_trace, include/b200rt_debug.h).
+struct TraceOut {
+    uint16_t *yhi, *ylo, *qkv, *ctx, *ffn;
+    float *pstats0, *pstats1, *out;
+    char* names;
+    size_t names_cap;
+};
+
+// Rows a trace returns per buffer: the batch's M rows and a guard band of 256, within the workspace.
+size_t trace_rows(size_t M) { return std::min(M + 256, static_cast<size_t>(g_rt->cap_rows)); }
+
+// Runs a traced forward on replica d (the caller holds d.mu): every workspace buffer is set to 0xFF bytes (NaN in fp16 and
+// fp32) behind the previous forward, `run` enqueues the first launches of the forward on d.compute through forward() /
+// forward_vit(), and once the stream has drained the first `rows` rows of every buffer, at the model's widths (the buffers
+// are used densely at those widths), and the pooled output are copied out.
+int trace_forward(Dev& d, int H, int I, size_t rows, const float* dout, size_t out_floats, const TraceOut& o,
+                  const std::function<int(std::vector<std::string>*)>& run) {
+    const size_t R = g_rt->cap_rows;
+    if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(d.compute, d.ev_ws, 0));
+    for (int i = 0; i < 2; ++i) CUDA_TRY(cudaMemsetAsync(d.pstats[i], 0xFF, R * STAT_PARTS * sizeof(float2), d.compute));
+    CUDA_TRY(cudaMemsetAsync(d.yhi, 0xFF, R * HIDDEN * 2, d.compute));
+    CUDA_TRY(cudaMemsetAsync(d.ylo, 0xFF, R * HIDDEN * 2, d.compute));
+    CUDA_TRY(cudaMemsetAsync(d.qkv, 0xFF, R * QKV_DIM * 2, d.compute));
+    CUDA_TRY(cudaMemsetAsync(d.ctx, 0xFF, R * HIDDEN * 2, d.compute));
+    CUDA_TRY(cudaMemsetAsync(d.ffn, 0xFF, R * 3072 * 2, d.compute));
+    std::vector<std::string> names;
+    if (int rc = run(&names)) return rc;
+    CUDA_TRY(cudaStreamSynchronize(d.compute));
+    const size_t P = H / 128;
+    CUDA_TRY(cudaMemcpy(o.yhi, d.yhi, rows * H * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.ylo, d.ylo, rows * H * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.pstats0, d.pstats[0], rows * P * sizeof(float2), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.pstats1, d.pstats[1], rows * P * sizeof(float2), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.qkv, d.qkv, rows * 3 * H * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.ctx, d.ctx, rows * H * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.ffn, d.ffn, rows * I * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(o.out, dout, out_floats * 4, cudaMemcpyDeviceToHost));
+    if (o.names && o.names_cap) {
+        size_t off = 0;
+        for (const auto& n : names) {
+            if (off + n.size() + 1 > o.names_cap) break;
+            memcpy(o.names + off, n.c_str(), n.size() + 1);
+            off += n.size() + 1;
+        }
+        if (off < o.names_cap) o.names[off] = '\0';
+    }
+    return 0;
+}
+
 }  // namespace
 
 // ============================================================================================ C ABI
@@ -2007,18 +2089,77 @@ int b200rt_debug_hidden(int model, const int32_t* ids, const int32_t* lens, int 
     if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
     std::vector<int32_t> l(n_items, max_len);
     if (lens) l.assign(lens, lens + n_items);
+    DebugBuffers b(d.compute);
     int32_t *dids = nullptr, *dlens = nullptr;
-    CUDA_TRY(cudaMalloc(&dids, M * 4));
-    CUDA_TRY(cudaMalloc(&dlens, static_cast<size_t>(n_items) * 4));
-    CUDA_TRY(cudaMemcpy(dids, ids, M * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(dlens, l.data(), static_cast<size_t>(n_items) * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(b.upload(&dids, ids, M * 4));
+    CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
     if (!d.x32_dbg) CUDA_TRY(cudaMalloc(&d.x32_dbg, static_cast<size_t>(rt->cap_rows) * HIDDEN * 4));
     int rc = forward(d, *m, 0, dids, dlens, n_items, max_len, nullptr, d.compute, n_layers);
     if (rc) return rc;
-    CUDA_TRY(cudaStreamSynchronize(d.compute));
-    CUDA_TRY(cudaMemcpy(hidden_out, d.x32_dbg, M * m->cfg.hidden * 4, cudaMemcpyDeviceToHost));
-    cudaFree(dids); cudaFree(dlens);
+    CUDA_TRY(b.download(hidden_out, d.x32_dbg, M * m->cfg.hidden * 4));
     return 0;
+}
+
+int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_launches,
+                               uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx,
+                               uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    const Model* m = get_model(*rt, model);
+    if (!m) return B200RT_E_INVALID;
+    if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+    if (int rc = check_ids(m->cfg, ids, lens, n_items, max_len)) return rc;
+    const int total = 5 * m->cfg.layers + 2;
+    if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
+    if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
+    const size_t M = static_cast<size_t>(n_items) * max_len;
+    if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
+    if (n_total) *n_total = total;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    std::vector<int32_t> l(n_items, max_len);
+    if (lens) l.assign(lens, lens + n_items);
+    const size_t out_floats = static_cast<size_t>(n_items) * m->out_dim;
+    DebugBuffers b(d.compute);
+    int32_t *dids = nullptr, *dlens = nullptr;
+    float* dout = nullptr;
+    CUDA_TRY(b.upload(&dids, ids, M * 4));
+    CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, out_floats * 4, d.compute));
+    const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
+    return trace_forward(d, m->cfg.hidden, m->cfg.inter, trace_rows(M), dout, out_floats, o, [&](std::vector<std::string>* names) {
+        return forward(d, *m, 0, dids, dlens, n_items, max_len, dout, d.compute, -1, nullptr, nullptr, n_launches, names);
+    });
+}
+
+int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
+                                   float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx, uint16_t* ffn, float* out,
+                                   char* names_out, size_t names_cap, int* n_total) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    const Model* m = get_model(*rt, model);
+    if (!m) return B200RT_E_INVALID;
+    if (m->kind != KIND_VIT || !pixels || n_items < 1 || n_items > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "bad arguments");
+    const int total = 5 * m->vcfg.layers + 4;
+    if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
+    if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
+    if (n_total) *n_total = total;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t M = static_cast<size_t>(n_items) * m->tokens;
+    const size_t out_floats = static_cast<size_t>(n_items) * m->out_dim;
+    DebugBuffers b(d.compute);
+    float *dpix = nullptr, *dout = nullptr;
+    CUDA_TRY(b.upload(&dpix, pixels, static_cast<size_t>(n_items) * m->item_bytes));
+    CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, out_floats * 4, d.compute));
+    const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
+    return trace_forward(d, HIDDEN, m->vcfg.inter, trace_rows(M), dout, out_floats, o, [&](std::vector<std::string>* names) {
+        return forward_vit(d, *m, 0, dpix, n_items, dout, d.compute, -1, nullptr, n_launches, names);
+    });
 }
 
 int b200rt_debug_vit_hidden(int model, const float* pixels, int n_items, int n_layers, float* hidden_out) {

@@ -135,9 +135,12 @@ GELU_SLOPE = 1.13  # max |d gelu / dx| of both GELUs (erf: 1.129 at x = 1.5; qui
 GELU_ULPS = 8      # the kernels' GELUs: erf by Abramowitz-Stegun 7.1.26 (1.5e-7 absolute), rcp / ex2 .approx (2 ulp each)
 
 
-def gemm_ref(epi, a16, w16, bias, resid=None, ln_stats=None, ln_gamma=None, ln_beta=None, eps=1e-12):
+def gemm_ref(epi, a16, w16, bias, resid=None, ln_stats=None, ln_gamma=None, ln_beta=None, eps=1e-12, resid_hilo=None):
     """What b200rt_debug_gemm returns, in fp64, and its elementwise tolerance: (ref, tol, v_tol), v_tol being the bound
-    on the kernel's fp32 epilogue value before its output rounding (what the emitted row statistics are taken of)."""
+    on the kernel's fp32 epilogue value before its output rounding (what the emitted row statistics are taken of).
+    epi 2 takes the residual either as fp32 `resid`, split here as the debug entry splits it, or as the (hi, lo) fp16 pair
+    `resid_hilo` the kernel read in place (a residual stream traced out of a forward: re-splitting hi + lo can move hi when
+    lo sits exactly on half an ulp)."""
     a = np.asarray(a16, np.float16).astype(np.float64)
     w = np.asarray(w16, np.float16).astype(np.float64)
     K = a.shape[1]
@@ -157,8 +160,8 @@ def gemm_ref(epi, a16, w16, bias, resid=None, ln_stats=None, ln_gamma=None, ln_b
         elif epi == 3:
             v, v_tol = gelu_quick(v), GELU_SLOPE * v_tol + GELU_ULPS * U32 * np.abs(v)
         return v, v_tol + fp16_round_tol(np.abs(v) + v_tol), v_tol
-    hi, lo = split_hilo(resid)
-    r = hilo64(hi, lo)  # the residual as the kernel holds it
+    hi, lo = resid_hilo if resid_hilo is not None else split_hilo(resid)
+    r = hilo64(np.asarray(hi, np.float16), np.asarray(lo, np.float16))  # the residual as the kernel holds it
     if ln_stats is not None:
         mean, rstd, mean_tol, rstd_rel = (x[:, None] for x in stats_from_partials(ln_stats, eps))
         g = np.asarray(ln_gamma, np.float32).astype(np.float64)

@@ -8,6 +8,7 @@ mask or position, a missing rescale, the wrong pooled row -- fails it."""
 import numpy as np
 import pytest
 
+import kernel_emul as KE
 import kernel_refs as KR
 
 gpu = pytest.mark.gpu
@@ -329,63 +330,6 @@ def test_attention_lens_on_every_sub_block_boundary(rt, S):
 
 # ================================================================================================ CPU: the checks discriminate
 
-def _row_stats32(p, eps):
-    """gemm_sm90.cu row_stats in fp32."""
-    p = p.astype(np.float32)
-    s, m2 = p[..., 0], p[..., 1]
-    mean = ((s[:, 0] + s[:, 1]) + (s[:, 2] + s[:, 3])) + (s[:, 4] + s[:, 5])
-    mean = mean * np.float32(1.0 / 768.0)
-    d = s * np.float32(1.0 / 128.0) - mean[:, None]
-    m = np.float32(128.0) * d * d + m2
-    var = (((m[:, 0] + m[:, 1]) + (m[:, 2] + m[:, 3])) + (m[:, 4] + m[:, 5])) * np.float32(1.0 / 768.0)
-    return mean, (np.float32(1.0) / np.sqrt(var + np.float32(eps))).astype(np.float32)
-
-
-def _emulate_gemm(epi, a16, w16, bias, resid=None, ln_stats=None, ln_gamma=None, ln_beta=None, eps=1e-12, mutant=None):
-    """The kernel's rounding in numpy: fp16 operands, fp32 accumulation (k-blocks of 64 in reverse order), fp32 epilogue,
-    fp16 or hi + lo out."""
-    from scipy.special import erf
-
-    K = a16.shape[1]
-    a32, w32 = a16.astype(np.float32), w16.astype(np.float32)
-    blocks = list(range(K // 64))[::-1]
-    if mutant == "drop_kblock":
-        blocks = blocks[1:]
-    acc = np.zeros((a16.shape[0], w16.shape[0]), np.float32)
-    for kb in blocks:
-        acc += a32[:, kb * 64:(kb + 1) * 64] @ w32[:, kb * 64:(kb + 1) * 64].T
-    bias = np.asarray(bias, np.float32)
-    if mutant == "bias_shift":
-        bias = np.roll(bias, 1)
-    if epi != 2:
-        v = acc + bias
-        if ln_stats is not None:
-            _, rstd = _row_stats32(ln_stats, eps)
-            v = rstd[:, None] * acc + bias
-        gelu = {1: "erf", 3: "quick"}.get(epi)
-        if mutant == "gelu_swap":
-            gelu = {"erf": "quick", "quick": "erf"}[gelu]
-        if gelu == "erf":
-            v = (v * np.float32(0.5) * (np.float32(1.0) + erf(v / np.float32(np.sqrt(2.0))))).astype(np.float32)
-        elif gelu == "quick":
-            v = (v / (np.float32(1.0) + np.exp(np.float32(-1.702) * v))).astype(np.float32)
-        out = v.astype(np.float16)
-    else:
-        hi, lo = KR.split_hilo(resid)
-        r = hi.astype(np.float32) + lo.astype(np.float32)
-        if ln_stats is not None:
-            mean, rstd = _row_stats32(ln_stats, eps)
-            r = ((r - mean[:, None]) * rstd[:, None]) * np.asarray(ln_gamma, np.float32) + np.asarray(ln_beta, np.float32)
-        v = acc + bias + r
-        h2, l2 = KR.split_hilo(v)
-        out = h2.astype(np.float32) + (0 if mutant == "lo_dropped" else l2.astype(np.float32))
-    if mutant == "swap_halves":  # the two consumer warpgroups' 64-row halves of every 128-row tile exchanged
-        out = out.reshape(-1, 2, 64, out.shape[1])[:, ::-1].reshape(out.shape)
-    if mutant == "permute_fragments":  # 8-column fragments j and j + 1 exchanged inside every 256-column tile
-        out = out.reshape(out.shape[0], -1, 16, 2, 8)[:, :, :, ::-1].reshape(out.shape)
-    return out
-
-
 GEMM_MUTANTS = {0: ["drop_kblock", "swap_halves", "permute_fragments", "bias_shift"],
                 1: ["drop_kblock", "swap_halves", "permute_fragments", "bias_shift", "gelu_swap"],
                 2: ["drop_kblock", "swap_halves", "permute_fragments", "bias_shift", "lo_dropped"],
@@ -400,48 +344,21 @@ def test_gemm_check_accepts_emulation_and_rejects_mutants(epi, N, K):
         kw["resid"] = kw["resid"] * np.float32(30.0)
         if "ln_stats" in kw:
             kw["ln_stats"] = KR.partials(KR.hilo64(*KR.split_hilo(kw["resid"]))).astype(np.float32)
-    KR.check_gemm(f"epi {epi} emulation", _emulate_gemm(epi, *args, **kw), epi, *args, **kw)
+    KR.check_gemm(f"epi {epi} emulation", KE.emulate_gemm(epi, *args, **kw), epi, *args, **kw)
     for m in GEMM_MUTANTS[epi]:
         with pytest.raises(AssertionError):
-            KR.check_gemm(f"epi {epi} mutant {m}", _emulate_gemm(epi, *args, mutant=m, **kw), epi, *args, **kw)
+            KR.check_gemm(f"epi {epi} mutant {m}", KE.emulate_gemm(epi, *args, mutant=m, **kw), epi, *args, **kw)
 
 
 def test_gemm_stats_check_rejects_a_partial_about_the_row_mean():
     args, kw = _gemm_case(2, 128, 768, 128, seed=3, ln=False)
-    v = _emulate_gemm(2, *args, **kw).astype(np.float64)
+    v = KE.emulate_gemm(2, *args, **kw).astype(np.float64)
     sl = v.reshape(v.shape[0], -1, 128)
     good = np.stack([sl.sum(-1), ((sl - sl.mean(-1, keepdims=True)) ** 2).sum(-1)], -1).astype(np.float32)
     bad = np.stack([sl.sum(-1), ((sl - v.mean(-1)[:, None, None]) ** 2).sum(-1)], -1).astype(np.float32)
     KR.check_gemm_stats("stats emulation", good, args, **kw)
     with pytest.raises(AssertionError):
         KR.check_gemm_stats("stats mutant: row mean", bad, args, **kw)
-
-
-def _emulate_attention(qkv16, lens, B, S, mutant=None):
-    """attention_sm90.cu's rounding: fp32 scores, online softmax over 64-key sub-blocks with exp2, P rounded to fp16, fp32
-    P.V, ctx = fp16(O / l)."""
-    c = np.float32(0.125 * 1.4426950408889634)
-    q = qkv16.reshape(B, S, 3, 12, 64).astype(np.float32)
-    ctx = np.zeros((B, S, 12, 64), np.float16)
-    for b in range(B):
-        n = int(min(max(lens[b], 1), S)) + {"mask_plus": 1, "mask_minus": -1}.get(mutant, 0)
-        qq, kk, vv = (q[b, :, j].transpose(1, 0, 2) for j in range(3))
-        o = np.zeros((12, S, 64), np.float32)
-        m = np.full((12, S, 1), -np.inf, np.float32)
-        l = np.zeros((12, S, 1), np.float32)
-        for k0 in range(0, n, 64):
-            s = qq @ kk[:, k0:k0 + 64].transpose(0, 2, 1)
-            s[:, :, max(n - k0, 0):] = -np.inf
-            m_new = np.maximum(m, s.max(-1, keepdims=True))
-            alpha = np.exp2((m - m_new) * c).astype(np.float32)
-            if mutant == "no_rescale":
-                alpha = np.where(np.isinf(m), 0.0, 1.0).astype(np.float32)
-            p = np.exp2(s * c - m_new * c).astype(np.float32)
-            l = l * alpha + p.sum(-1, keepdims=True)
-            o = o * alpha + p.astype(np.float16).astype(np.float32) @ vv[:, k0:k0 + 64]
-            m = m_new
-        ctx[b] = (o / l).astype(np.float16).transpose(1, 0, 2)
-    return ctx.reshape(B * S, 768)
 
 
 def test_attention_check_accepts_emulation_and_rejects_mutants():
@@ -455,24 +372,10 @@ def test_attention_check_accepts_emulation_and_rejects_mutants():
     x[:, :, 0] += 4.0 * np.where(rng.random((B, S, 12, 1)) < 0.6, 1.0, -1.0) * u
     x[:, :, 1] += (12.0 * (np.arange(S) // 64))[None, :, None, None] * u
     qkv = x.reshape(B * S, 2304).astype(np.float16)
-    KR.check_attention("attention emulation", _emulate_attention(qkv, lens, B, S), qkv, lens, B, S)
+    KR.check_attention("attention emulation", KE.emulate_attention(qkv, lens, B, S), qkv, lens, B, S)
     for m in ("mask_plus", "mask_minus", "no_rescale"):
         with pytest.raises(AssertionError):
-            KR.check_attention(f"attention mutant {m}", _emulate_attention(qkv, lens, B, S, m), qkv, lens, B, S)
-
-
-def _ln32(x, g, b, eps):
-    x = x.astype(np.float32)
-    mu = x.mean(-1, keepdims=True, dtype=np.float32)
-    d = x - mu
-    rstd = np.float32(1.0) / np.sqrt((d * d).mean(-1, keepdims=True, dtype=np.float32) + np.float32(eps))
-    return (d * rstd) * g + b
-
-
-def _partials32(x, about_row_mean=False):
-    sl = x.astype(np.float32).reshape(x.shape[0], -1, 128)
-    mu = x.astype(np.float32).mean(-1)[:, None, None] if about_row_mean else sl.mean(-1, keepdims=True)
-    return np.stack([sl.sum(-1, dtype=np.float32), ((sl - mu) ** 2).sum(-1, dtype=np.float32)], -1)
+            KR.check_attention(f"attention mutant {m}", KE.emulate_attention(qkv, lens, B, S, m), qkv, lens, B, S)
 
 
 def test_row_checks_accept_emulations_and_reject_mutants():
@@ -482,15 +385,15 @@ def test_row_checks_accept_emulations_and_reject_mutants():
     word, pos, type0 = _embed_tables(rng, vocab, S)
     ids = rng.integers(0, vocab, size=2 * S).astype(np.int32)
     hi, lo, x = KR.embed_exact(ids, word, pos, type0, S)
-    KR.check_embed("embed emulation", hi, lo, _partials32(x), ids, word, pos, type0, S)
+    KR.check_embed("embed emulation", hi, lo, KE.partials32(x), ids, word, pos, type0, S)
     hi_p, lo_p, x_p = KR.embed_exact(ids, word, np.roll(pos, -1, axis=0), type0, S)  # position t + 1
     with pytest.raises(AssertionError):
-        KR.check_embed("embed mutant: position off by one", hi_p, lo_p, _partials32(x_p), ids, word, pos, type0, S)
+        KR.check_embed("embed mutant: position off by one", hi_p, lo_p, KE.partials32(x_p), ids, word, pos, type0, S)
     with pytest.raises(AssertionError):
-        KR.check_embed("embed mutant: lo dropped", hi, np.zeros_like(lo), _partials32(x), ids, word, pos, type0, S)
+        KR.check_embed("embed mutant: lo dropped", hi, np.zeros_like(lo), KE.partials32(x), ids, word, pos, type0, S)
     fin = np.isfinite(x).all(-1)
     with pytest.raises(AssertionError):
-        KR.check_partials("embed mutant: partials about the row mean", _partials32(x[fin], True), x[fin].astype(np.float64))
+        KR.check_partials("embed mutant: partials about the row mean", KE.partials32(x[fin], True), x[fin].astype(np.float64))
     # vit_embed
     T = 197
     patch, cls, vpos, g, b = _vit_embed_inputs(rng, T, 2)
@@ -498,8 +401,8 @@ def test_row_checks_accept_emulations_and_reject_mutants():
 
     def vit_emul(shift):
         src = np.where((tk == 0)[:, None], cls[None, :], patch.astype(np.float32))
-        y = _ln32(src + vpos[(tk + shift) % T], g, b, 1e-5)
-        return (*KR.split_hilo(y), _partials32(y))
+        y = KE.ln32(src + vpos[(tk + shift) % T], g, b, 1e-5)
+        return (*KR.split_hilo(y), KE.partials32(y))
 
     KR.check_vit_embed("vit_embed emulation", *vit_emul(0), patch, cls, vpos, g, b, T, 1e-5)
     with pytest.raises(AssertionError):
@@ -511,7 +414,7 @@ def test_row_checks_accept_emulations_and_reject_mutants():
     proj = (rng.standard_normal((64, KR.H)) * 0.03).astype(np.float32)
 
     def pooled(row0, P=None):
-        z = _ln32(x[row0::S], g, b, 1e-12)
+        z = KE.ln32(x[row0::S], g, b, 1e-12)
         if P is not None:
             z = z @ P.T
         return z / np.maximum(np.linalg.norm(z, axis=-1, keepdims=True), np.float32(1e-12))
