@@ -57,15 +57,6 @@ int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* g
 int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,
                          float* cvec_out);
 
-/* Hidden state after `n_layers` encoder layers (0 = embedding LayerNorm output) of a loaded model,
- * hidden_out fp32 [n_items*max_len, hidden] on the host.                                              */
-int b200rt_debug_hidden(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_layers,
-                        float* hidden_out);
-
-/* ViT model: the residual stream after `n_layers` encoder layers (0 = pre_layrnorm output) for pixels [n_items, 3, image,
- * image], hidden_out fp32 [n_items * tokens, hidden] on the host (pre-LN architecture: the stream itself, not a LayerNorm of it). */
-int b200rt_debug_vit_hidden(int model, const float* pixels, int n_items, int n_layers, float* hidden_out);
-
 /* Trace of the product forward on replica 0: the workspace is set to 0xFF bytes (NaN in fp16 and fp32), then the first
  * n_launches launches of the forward of this batch run exactly as the product enqueues them (same kernels, buffers and stream,
  * no sync or copy between them), and the workspace is copied out once they finish.  n_launches is in [0, n_total], n_total =

@@ -28,7 +28,7 @@ ABI_SYMBOLS = [
     "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items",
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
-DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_hidden", "b200rt_debug_vit_hidden", "b200rt_debug_profile_forward",
+DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_profile_forward",
                  "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_vit_pool", "b200rt_debug_fold_ln",
                  "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace"]
 
@@ -88,7 +88,6 @@ def load_library():
         lib.b200rt_submit_ex.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.c_uint32, u64p]
         lib.b200rt_submit_pixels.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, u64p]
-        lib.b200rt_debug_vit_hidden.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         lib.b200rt_wait.argtypes = [ctypes.c_uint64, ctypes.c_int]
         lib.b200rt_poll_any.argtypes = [u64p, ctypes.c_int]
         lib.b200rt_embed_device.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
@@ -112,7 +111,6 @@ def load_library():
         lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
         lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
-        lib.b200rt_debug_hidden.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_vit_forward_trace.argtypes = [ci, vp, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
@@ -301,14 +299,6 @@ class EmbedModel:
         _check(self._lib.b200rt_embed_device(self.handle, gpu, d_ids, d_lens, n_items, max_len, d_out, stream or None))
 
     # ---- debug helpers (tests only)
-    def debug_hidden(self, ids: np.ndarray, lens, n_layers: int) -> np.ndarray:
-        ids = np.ascontiguousarray(ids, dtype=np.int32)
-        n, S = ids.shape
-        lens_a = np.ascontiguousarray(lens, dtype=np.int32) if lens is not None else None
-        out = np.empty((n * S, self.hidden), np.float32)
-        _check(self._lib.b200rt_debug_hidden(self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_layers, _ptr(out)))
-        return out.reshape(n, S, self.hidden)
-
     def debug_trace(self, ids: np.ndarray, lens, n_launches: int) -> dict:
         """The workspace after the first ``n_launches`` launches of this batch's forward (see :func:`_debug_trace`)."""
         ids = np.ascontiguousarray(ids, dtype=np.int32)
@@ -317,6 +307,11 @@ class EmbedModel:
         return _debug_trace(lambda *bufs: self._lib.b200rt_debug_forward_trace(
             self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_launches, *bufs),
             n * S, n, self.hidden, self.inter, self.hidden, n_launches)
+
+    def debug_residual(self, ids: np.ndarray, lens, n_layers: int) -> np.ndarray:
+        """The residual stream after ``n_layers`` encoder layers (0: the embedding sum), pre-LayerNorm as the forward carries
+        it: hi + lo, float32 [n_items, max_len, hidden].  The launches before it are embed and 5 per layer."""
+        return _residual(self.debug_trace(ids, lens, 1 + 5 * n_layers), len(ids))
 
     def profile_forward(self, n_items: int, max_len: int, iters: int = 3) -> dict:
         names = ctypes.create_string_buffer(4096)
@@ -369,19 +364,17 @@ class ImageEmbedModel:
     def embed(self, pixels: np.ndarray) -> np.ndarray:
         return self.wait(self.submit(pixels))
 
-    def debug_hidden(self, pixels: np.ndarray, n_layers: int) -> np.ndarray:
-        pixels = np.ascontiguousarray(pixels, dtype=np.float32)
-        n = pixels.shape[0]
-        out = np.empty((n * self.tokens, self.hidden), np.float32)
-        _check(self._lib.b200rt_debug_vit_hidden(self.handle, _ptr(pixels), n, n_layers, _ptr(out)))
-        return out.reshape(n, self.tokens, self.hidden)
-
     def debug_trace(self, pixels: np.ndarray, n_launches: int) -> dict:
         """The workspace after the first ``n_launches`` launches of this batch's forward (see :func:`_debug_trace`)."""
         pixels = np.ascontiguousarray(pixels, dtype=np.float32)
         n = pixels.shape[0]
         return _debug_trace(lambda *bufs: self._lib.b200rt_debug_vit_forward_trace(self.handle, _ptr(pixels), n, n_launches, *bufs),
                             n * self.tokens, n, self.hidden, self.inter, self.proj, n_launches)
+
+    def debug_residual(self, pixels: np.ndarray, n_layers: int) -> np.ndarray:
+        """The residual stream after ``n_layers`` encoder layers (0: the pre_layrnorm output): hi + lo, float32
+        [n_items, tokens, hidden].  The launches before it are im2col, gemm_patch, vit_embed and 5 per layer."""
+        return _residual(self.debug_trace(pixels, 3 + 5 * n_layers), len(pixels))
 
 
 _TRACE_NAMES_CAP = 8192
@@ -405,6 +398,12 @@ def _debug_trace(call, M: int, n_items: int, H: int, I: int, out_dim: int, n_lau
     bufs.update(out=out if n_launches == total.value else None, names=[s.decode() for s in names.raw.split(b"\0")[:n_launches]],
                 n_total=total.value, M=M, rows=rows)
     return bufs
+
+
+def _residual(trace: dict, n_items: int) -> np.ndarray:
+    """hi + lo of a trace's M rows, [n_items, M / n_items, hidden] float32 (the sum the row kernels form)."""
+    M = trace["M"]
+    return (trace["yhi"][:M].astype(np.float32) + trace["ylo"][:M].astype(np.float32)).reshape(n_items, M // n_items, -1)
 
 
 def device_sync(gpu: int = 0):

@@ -140,7 +140,7 @@ struct LayerW {
 struct DevWeights {
     float* f32_arena = nullptr;  // embeddings, biases, LayerNorm params
     __half* f16_arena = nullptr; // GEMM weights
-    float *word, *pos, *type, *emb_g, *emb_b;
+    float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;
     std::vector<LayerW> layers;
     // ViT (kind "vit"): patch projection (fp16, the stride-p convolution as a [H, 3 p p] matrix), class / position embeddings,
     // pre / post LayerNorm, visual projection; `pos` above holds the position table.  For a ViT layer, LayerW::ln1_* is the
@@ -156,6 +156,8 @@ struct Model {
     ModelKind kind = KIND_BERT;
     b200rt_bert_config cfg{};
     b200rt_vit_config vcfg{};
+    int hidden = 0, inter = 0, heads = 0, layers = 0;  // encoder geometry, from whichever config the kind has
+    float eps = 0.f;
     int tokens = 0;          // vit: (image / patch)^2 + 1
     int out_dim = HIDDEN;    // floats per item in the result
     size_t item_bytes = 0;   // vit: bytes of one item's pixels
@@ -171,7 +173,6 @@ struct Dev {
     // workspace (capacity cap_rows rows)
     __half *yhi = nullptr, *ylo = nullptr;  // residual stream y = hi + lo, PRE-LayerNorm; hi doubles as the GEMM A operand
     float2* pstats[2] = {nullptr, nullptr};  // [rows][STAT_PARTS] (sum, M2) partials: [0] embedding LN / LN2 inputs, [1] LN1 inputs
-    float* x32_dbg = nullptr;    // tests only (b200rt_debug_hidden): normalised fp32 rows, allocated on first use
     __half *qkv = nullptr, *ctx = nullptr, *ffn = nullptr;
     // fp16 [rows, *] box {64,128}: GEMM A operands, per TEXT_GEOMETRIES entry (a narrower model reads the same buffers densely
     // at its own widths)
@@ -289,9 +290,43 @@ Runtime* g_rt = nullptr;
 
 // ------------------------------------------------------------------------------------------ forward
 
-struct Prof {
+// One forward's input, in the replica's HBM: token ids [B, S] and valid lengths [B] (text), or pixels [B, 3, image, image]
+// (vit, S = the model's token count).
+struct Input {
+    const int32_t* ids;
+    const int32_t* lens;
+    const float* pixels;
+    int B, S;
+};
+
+// A debug view of one forward; the product path passes none.  The forward calls at() ahead of its first launch (name NULL)
+// and behind every launch.  The hook keeps the launch names, records a timing event at each call when `timing` is set
+// (evs[0] ahead of the first launch, evs[i] behind launch i), and ends the enqueue once `stop_after` launches are in (-1: the
+// whole forward).  The events belong to the hook and go with it, whatever the forward returned.
+struct LaunchHook {
+    int stop_after = -1;
+    bool timing = false;
     std::vector<std::string> names;
     std::vector<cudaEvent_t> evs;
+    cudaError_t error = cudaSuccess;  // of the first timing event that could not be created or recorded (ends the enqueue)
+    LaunchHook() = default;
+    LaunchHook(const LaunchHook&) = delete;
+    LaunchHook& operator=(const LaunchHook&) = delete;
+    ~LaunchHook() {
+        for (cudaEvent_t e : evs) cudaEventDestroy(e);
+    }
+    bool at(const char* name, cudaStream_t stream) {  // true: enqueue nothing more
+        if (name) names.push_back(name);
+        if (timing && error == cudaSuccess) {
+            cudaEvent_t e;
+            error = cudaEventCreate(&e);
+            if (error == cudaSuccess) {
+                evs.push_back(e);
+                error = cudaEventRecord(e, stream);
+            }
+        }
+        return error != cudaSuccess || (stop_after >= 0 && names.size() >= static_cast<size_t>(stop_after));
+    }
 };
 
 int get_qkv_map(Dev& d, int S, int hidden, const CUtensorMap** out, const CUtensorMap** out_ctx) {
@@ -312,151 +347,81 @@ int get_qkv_map(Dev& d, int S, int hidden, const CUtensorMap** out, const CUtens
     return 0;
 }
 
-// Enqueue the forward of one padded batch [B, S] on `stream`.  out: fp32 [B, hidden], may be peer memory.  Widths, statistic
-// partials and the attention head size follow the model's geometry.
-// n_layers >= 0 (debug): stop early and materialise the post-LN hidden state in d.x32_dbg.
-// stop_after >= 0 (debug trace): enqueue only the first stop_after launches of the forward; `names` (optional) receives the
-// name of every launch enqueued.
-int forward_enqueue(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int32_t* lens, int B, int S, float* out,
-                    cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr, int stop_after = -1,
-                    std::vector<std::string>* names = nullptr) {
+// Enqueue the forward of one padded batch on `stream` and add the launches it enqueued to `launches`.  out: fp32 [B, out_dim],
+// may be peer memory.  Widths, statistic partials and the attention head size follow the model's geometry.
+// BERT is post-LN: a residual epilogue re-applies the LayerNorm of the rows it adds to (the embedding LN or LN2 of the layer
+// before, then LN1).  CLIPVisionTransformer is pre-LN: LayerNorm1 / LayerNorm2 are folded into QKV / FFN1, the residual
+// epilogues add the raw stream and emit the statistics the next fold needs.
+int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
+                    LaunchHook* hook) {
     const DevWeights& w = m.per_dev[dev_index];
-    const b200rt_bert_config& c = m.cfg;
-    const int L = n_layers < 0 ? c.layers : n_layers;
-    const bool full = n_layers < 0;
-    const int M = B * S;
-    if (M > g_rt->cap_rows) return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds wave capacity %d rows", B, S, g_rt->cap_rows);
-    const int H = c.hidden, I = c.inter, P = H / 128, HD = H / c.heads;
+    const bool vit = m.kind == KIND_VIT;
+    const int B = in.B, S = in.S, M = B * S;
+    if (M > g_rt->cap_rows || (vit && B > VIT_WAVE_ITEMS))
+        return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the wave capacity (%d rows)", B, S, g_rt->cap_rows);
+    const int H = m.hidden, I = m.inter, P = H / 128;
     const Dev::ActMaps& am = d.act[geometry_index(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
     if (int rc = get_qkv_map(d, S, H, &mq, &mc)) return rc;
-    uint64_t nl = 0;
-    auto mark = [&](const char* name) {
-        if (prof) {
-            cudaEvent_t e;
-            cudaEventCreate(&e);
-            cudaEventRecord(e, stream);
-            prof->names.push_back(name);
-            prof->evs.push_back(e);
-        }
+    const int32_t* lens = vit ? d.lens_const : in.lens;
+    // residual epilogue: y <- acc + bias + LN(y), LN given by (stats, gamma, beta) -- or + y (pre-LN); new statistics to stats_out
+    auto residual = [&](const float* bias, const float2* stats, const float* gamma, const float* beta, float2* stats_out) {
+        return vit ? GemmEpi{bias, nullptr, P, nullptr, nullptr, stats_out, m.eps} : GemmEpi{bias, stats, P, gamma, beta, stats_out, m.eps};
     };
-    // counts the launch just enqueued; true once the trace has all it asked for
+    uint64_t nl = 0;
+    // counts the launch just enqueued; true once the hook wants no more
     auto step = [&](const char* name) {
         ++nl;
-        mark(name);
-        if (names) names->push_back(name);
-        return stop_after >= 0 && nl >= static_cast<uint64_t>(stop_after);
+        return hook && hook->at(name, stream);
     };
     auto enqueue = [&]() -> int {
-        if (stop_after == 0) return 0;
-        mark("begin");
-        float* const dbg = full ? nullptr : d.x32_dbg;
-        CUDA_TRY(launch_embed(ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, c.vocab, H, stream));
-        if (step("embed")) return 0;
-        const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // the LayerNorm that applies to the current residual rows
-        for (int l = 0; l < L; ++l) {
+        if (hook && hook->at(nullptr, stream)) return 0;
+        if (vit) {
+            // patches -> im2col rows in the (idle) ffn buffer -> patch projection into the (idle) ctx buffer -> + class / position
+            // embeddings, pre_layrnorm -> residual stream + statistics
+            const b200rt_vit_config& c = m.vcfg;
+            CUDA_TRY(launch_im2col(in.pixels, d.ffn, B, c.image, c.patch, stream));
+            if (step("im2col")) return 0;
+            GemmEpi e_patch{w.zero_bias, nullptr, P, nullptr, nullptr, nullptr, m.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
+            if (step("gemm_patch")) return 0;
+            CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, S, m.eps, stream));
+            if (step("vit_embed")) return 0;
+        } else {
+            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, m.cfg.vocab, H, stream));
+            if (step("embed")) return 0;
+        }
+        const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // BERT: the LayerNorm that applies to the current residual rows
+        for (int l = 0; l < m.layers; ++l) {
             const LayerW& lw = w.layers[l];
             // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
-            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, c.eps};
+            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
             CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
             if (step("gemm_qkv")) return 0;
-            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, HD));
+            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads));
             if (step("attention")) return 0;
-            // y <- ctx Wao^T + b + LN_prev(y); new row statistics (LN1's) into pstats[1]
-            GemmEpi e_ao{lw.ao_b, d.pstats[0], P, prev_g, prev_b, d.pstats[1], c.eps};
+            // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
+            const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
             CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
             if (step("gemm_attn_out")) return 0;
-            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, c.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
-            if (step("gemm_ffn1_gelu")) return 0;
-            // y <- ffn W2^T + b + LN1(y); LN2's statistics into pstats[0]
-            GemmEpi e_ff2{lw.ff2_b, d.pstats[1], P, lw.ln1_g, lw.ln1_b, d.pstats[0], c.eps};
+            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
+            CUDA_TRY(launch_gemm(vit ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+            if (step(vit ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
+            // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
+            const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
             CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
             if (step("gemm_ffn2")) return 0;
             prev_g = lw.ln2_g;
             prev_b = lw.ln2_b;
         }
-        if (full) {
-            CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, c.eps, H, stream));
-            step("pool_normalize");
-        } else {  // debug: materialise the post-LayerNorm hidden state
-            CUDA_TRY(launch_ln_materialize(d.yhi, d.ylo, prev_g, prev_b, dbg, M, c.eps, H, stream));
-            ++nl;
-        }
+        if (vit) CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
+        else CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
+        step(vit ? "vit_pool" : "pool_normalize");
         return 0;
     };
     if (int rc = enqueue()) return rc;
-    if (launches) *launches += nl;
-    return 0;
-}
-
-// Forward of one batch of images on `stream`: pixels fp32 [B, 3, image, image] in this replica's HBM; out fp32 [B, proj],
-// may be peer memory.  n_layers >= 0 (debug): stop after that many layers (the residual stream stays in yhi / ylo).
-// stop_after / names (debug trace) as for forward_enqueue.
-// CLIPVisionTransformer is pre-LN: LayerNorm1 / LayerNorm2 are folded into QKV / FFN1, the residual GEMMs add the raw
-// stream (no LayerNorm re-applied) and emit the statistics the next fold needs.
-int forward_enqueue_vit(Dev& d, const Model& m, int dev_index, const float* pixels, int B, float* out, cudaStream_t stream,
-                        int n_layers = -1, uint64_t* launches = nullptr, int stop_after = -1, std::vector<std::string>* names = nullptr) {
-    const DevWeights& w = m.per_dev[dev_index];
-    const b200rt_vit_config& c = m.vcfg;
-    const int T = m.tokens, M = B * T;
-    const int L = n_layers < 0 ? c.layers : n_layers;
-    if (M > g_rt->cap_rows || B > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "batch of %d images exceeds the wave capacity (%d)", B, VIT_WAVE_ITEMS);
-    const CUtensorMap *mq = nullptr, *mc = nullptr;
-    if (int rc = get_qkv_map(d, T, HIDDEN, &mq, &mc)) return rc;
-    const Dev::ActMaps& am = d.act[0];
-    uint64_t nl = 0;
-    auto step = [&](const char* name) {
-        ++nl;
-        if (names) names->push_back(name);
-        return stop_after >= 0 && nl >= static_cast<uint64_t>(stop_after);
-    };
-    auto enqueue = [&]() -> int {
-        if (stop_after == 0) return 0;
-        // patches -> im2col rows in the (idle) ffn buffer -> patch projection into the (idle) ctx buffer -> + class / position
-        // embeddings, pre_layrnorm -> residual stream + statistics
-        CUDA_TRY(launch_im2col(pixels, d.ffn, B, c.image, c.patch, stream));
-        if (step("im2col")) return 0;
-        GemmEpi e_patch{w.zero_bias, nullptr, STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-        CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, e_patch, M, HIDDEN, 3 * c.patch * c.patch, d.sm_gemm, stream));
-        if (step("gemm_patch")) return 0;
-        CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, T, c.eps, stream));
-        if (step("vit_embed")) return 0;
-        for (int l = 0; l < L; ++l) {
-            const LayerW& lw = w.layers[l];
-            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, QKV_DIM, HIDDEN, d.sm_gemm, stream));
-            if (step("gemm_qkv")) return 0;
-            CUDA_TRY(launch_attention(*mq, *mc, d.lens_const, B, T, d.sm_attn, stream, HIDDEN / HEADS));
-            if (step("attention")) return 0;
-            GemmEpi e_ao{lw.ao_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[1], c.eps};  // h += ctx Wo^T + b (raw residual)
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, HIDDEN, HIDDEN, d.sm_gemm, stream));
-            if (step("gemm_attn_out")) return 0;
-            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], STAT_PARTS, nullptr, nullptr, nullptr, c.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_QGELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, c.inter, HIDDEN, d.sm_gemm, stream));
-            if (step("gemm_ffn1_qgelu")) return 0;
-            GemmEpi e_ff2{lw.ff2_b, nullptr, STAT_PARTS, nullptr, nullptr, d.pstats[0], c.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, HIDDEN, c.inter, d.sm_gemm, stream));
-            if (step("gemm_ffn2")) return 0;
-        }
-        if (n_layers < 0) {
-            CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, T, c.proj, c.eps, stream));
-            step("vit_pool");
-        }
-        return 0;
-    };
-    if (int rc = enqueue()) return rc;
-    if (launches) *launches += nl;
-    return 0;
-}
-
-// Orders a ViT forward behind the previous forward on the replica's workspace, like forward() does (caller holds d.mu).
-int forward_vit(Dev& d, const Model& m, int dev_index, const float* pixels, int B, float* out, cudaStream_t stream, int n_layers = -1,
-                uint64_t* launches = nullptr, int stop_after = -1, std::vector<std::string>* names = nullptr) {
-    if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(stream, d.ev_ws, 0));
-    if (int rc = forward_enqueue_vit(d, m, dev_index, pixels, B, out, stream, n_layers, launches, stop_after, names)) return rc;
-    CUDA_TRY(cudaEventRecord(d.ev_ws, stream));
-    d.ev_ws_armed = true;
+    if (hook) CUDA_TRY(hook->error);
+    launches += nl;
     return 0;
 }
 
@@ -498,18 +463,16 @@ void drop_graphs(Dev& d) {  // the replica is going away: its cached launches po
     g_graphs.erase(it);
 }
 
-// The caller holds d.mu.  Orders this forward behind the previous one on the replica's workspace (see Dev::ev_ws).
-int forward(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int32_t* lens, int B, int S, float* out,
-            cudaStream_t stream, int n_layers = -1, Prof* prof = nullptr, uint64_t* launches = nullptr, int stop_after = -1,
-            std::vector<std::string>* names = nullptr) {
+// The caller holds d.mu.  Orders this forward behind the previous one on the replica's workspace (see Dev::ev_ws) and adds
+// its launches to `launches`.  Text batches of at most GRAPH_MAX_ROWS rows without a hook replay their CUDA graph.
+int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
+            LaunchHook* hook = nullptr) {
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(stream, d.ev_ws, 0));
-    int rc = 0;
-    const bool use_graph = !(n_layers >= 0 || prof || stop_after >= 0 || B * S > GRAPH_MAX_ROWS);
-    if (!use_graph) {
-        rc = forward_enqueue(d, m, dev_index, ids, lens, B, S, out, stream, n_layers, prof, launches, stop_after, names);
+    if (hook || m.kind == KIND_VIT || in.B * in.S > GRAPH_MAX_ROWS) {
+        if (int rc = forward_enqueue(d, m, dev_index, in, out, stream, launches, hook)) return rc;
     } else {
         GraphCache& cache = graph_cache(d);
-        const GraphKey key{&m, ids, lens, out, stream, B, S};
+        const GraphKey key{&m, in.ids, in.lens, out, stream, in.B, in.S};
         auto it = cache.entries.find(key);
         if (it == cache.entries.end()) {
             if (cache.entries.size() >= GRAPH_CACHE_MAX) {  // evict the least recently replayed graph
@@ -520,10 +483,10 @@ int forward(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int
                 cache.entries.erase(victim);
             }
             const CUtensorMap *mq = nullptr, *mc = nullptr;
-            if (int r2 = get_qkv_map(d, S, m.cfg.hidden, &mq, &mc)) return r2;  // host-side map creation happens outside the capture
+            if (int rc = get_qkv_map(d, in.S, m.hidden, &mq, &mc)) return rc;  // host-side map creation happens outside the capture
             uint64_t nl = 0;
             CUDA_TRY(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-            rc = forward_enqueue(d, m, dev_index, ids, lens, B, S, out, stream, -1, nullptr, &nl);
+            const int rc = forward_enqueue(d, m, dev_index, in, out, stream, nl, nullptr);
             cudaGraph_t graph = nullptr;
             const cudaError_t ce = cudaStreamEndCapture(stream, &graph);
             if (rc) {
@@ -538,9 +501,8 @@ int forward(Dev& d, const Model& m, int dev_index, const int32_t* ids, const int
         }
         it->second.last_use = ++cache.tick;
         CUDA_TRY(cudaGraphLaunch(it->second.exec, stream));
-        if (launches) *launches += it->second.launches;
+        launches += it->second.launches;
     }
-    if (rc) return rc;
     CUDA_TRY(cudaEventRecord(d.ev_ws, stream));
     d.ev_ws_armed = true;
     return 0;
@@ -798,9 +760,11 @@ void dispatcher_main(Runtime* rtp) {
                             }
                             if (e.empty() && ck(cudaEventRecord(dd.ev_pix[slot], dd.copy), "cudaEventRecord") &&
                                 ck(cudaStreamWaitEvent(dd.compute, dd.ev_pix[slot], 0), "cudaStreamWaitEvent"))
-                                rc = forward_vit(dd, model, g, dd.pix_in[slot], plan.item_count[g], dst, dd.compute, -1, &nl);
+                                rc = forward(dd, model, g, Input{nullptr, nullptr, dd.pix_in[slot], plan.item_count[g], model.tokens}, dst,
+                                             dd.compute, nl);
                         } else {
-                            rc = forward(dd, model, g, dd.ids_in[slot], dd.lens_in[slot], plan.item_count[g], S, dst, dd.compute, -1, nullptr, &nl);
+                            rc = forward(dd, model, g, Input{dd.ids_in[slot], dd.lens_in[slot], nullptr, plan.item_count[g], S}, dst,
+                                         dd.compute, nl);
                         }
                         if (rc) { e = t_last_error; code = rc; }
                         else {
@@ -1103,6 +1067,7 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, in
 
     auto m = std::make_unique<Model>();
     m->cfg = c;
+    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->out_dim = c.hidden;
     const size_t per_layer_x = 3 * H + I;  // derived vectors: qkv_c, ff1_c
     const size_t blob_f32 = emb + static_cast<size_t>(c.layers) * per_layer_p;
@@ -1221,6 +1186,7 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
     auto m = std::make_unique<Model>();
     m->kind = KIND_VIT;
     m->vcfg = c;
+    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->tokens = T;
     m->out_dim = c.proj;
     m->item_bytes = static_cast<size_t>(3) * c.image * c.image * 4;
@@ -1383,17 +1349,19 @@ int check_ids(const b200rt_bert_config& c, const int32_t* ids, const int32_t* le
     return 0;
 }
 
-// Device buffers of one row-kernel debug entry (b200rt_debug_embed & co.): filled from the host (or zeroed) in stream order on
-// allocation, and all freed when the entry returns, on success or on error.
+// Device buffers and timing events of one debug entry (b200rt_debug_embed & co.): buffers are filled from the host (or
+// zeroed) in stream order on allocation, and everything is freed when the entry returns, on success or on error.
 struct DebugBuffers {
     cudaStream_t stream;
     std::vector<void*> ptrs;
+    std::vector<cudaEvent_t> evs;
     explicit DebugBuffers(cudaStream_t s) : stream(s) {}
     DebugBuffers(const DebugBuffers&) = delete;
     DebugBuffers& operator=(const DebugBuffers&) = delete;
     ~DebugBuffers() {
         cudaStreamSynchronize(stream);
         for (void* p : ptrs) cudaFree(p);
+        for (cudaEvent_t e : evs) cudaEventDestroy(e);
     }
     template <typename T>
     cudaError_t upload(T** dp, const void* host, size_t bytes) {  // host NULL: zeros
@@ -1408,6 +1376,11 @@ struct DebugBuffers {
         cudaError_t e = cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, stream);
         return e != cudaSuccess ? e : cudaStreamSynchronize(stream);
     }
+    cudaError_t event(cudaEvent_t* ev) {
+        cudaError_t e = cudaEventCreate(ev);
+        if (e == cudaSuccess) evs.push_back(*ev);
+        return e;
+    }
 };
 
 // Host buffers of a forward trace (b200rt_debug_forward_trace / b200rt_debug_vit_forward_trace, include/b200rt_debug.h).
@@ -1418,16 +1391,16 @@ struct TraceOut {
     size_t names_cap;
 };
 
-// Rows a trace returns per buffer: the batch's M rows and a guard band of 256, within the workspace.
-size_t trace_rows(size_t M) { return std::min(M + 256, static_cast<size_t>(g_rt->cap_rows)); }
-
-// Runs a traced forward on replica d (the caller holds d.mu): every workspace buffer is set to 0xFF bytes (NaN in fp16 and
-// fp32) behind the previous forward, `run` enqueues the first launches of the forward on d.compute through forward() /
-// forward_vit(), and once the stream has drained the first `rows` rows of every buffer, at the model's widths (the buffers
-// are used densely at those widths), and the pooled output are copied out.
-int trace_forward(Dev& d, int H, int I, size_t rows, const float* dout, size_t out_floats, const TraceOut& o,
-                  const std::function<int(std::vector<std::string>*)>& run) {
-    const size_t R = g_rt->cap_rows;
+// Runs the first n_launches launches of the forward of `in` on replica d (the caller holds d.mu): every workspace buffer and
+// the pooled output are set to 0xFF bytes (NaN in fp16 and fp32) behind the previous forward, the launches run on d.compute
+// through forward(), and once the stream has drained, rows = min(M + 256, workspace rows) rows of every buffer, at the
+// model's widths (the buffers are used densely at those widths), and the pooled output are copied out.
+int trace_forward(DebugBuffers& b, Dev& d, const Model& m, const Input& in, int n_launches, const TraceOut& o) {
+    const size_t R = g_rt->cap_rows, rows = std::min(static_cast<size_t>(in.B) * in.S + 256, R);
+    const size_t H = m.hidden, I = m.inter, P = H / 128, out_floats = static_cast<size_t>(in.B) * m.out_dim;
+    float* dout = nullptr;
+    CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, out_floats * 4, d.compute));
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(d.compute, d.ev_ws, 0));
     for (int i = 0; i < 2; ++i) CUDA_TRY(cudaMemsetAsync(d.pstats[i], 0xFF, R * STAT_PARTS * sizeof(float2), d.compute));
     CUDA_TRY(cudaMemsetAsync(d.yhi, 0xFF, R * HIDDEN * 2, d.compute));
@@ -1435,10 +1408,11 @@ int trace_forward(Dev& d, int H, int I, size_t rows, const float* dout, size_t o
     CUDA_TRY(cudaMemsetAsync(d.qkv, 0xFF, R * QKV_DIM * 2, d.compute));
     CUDA_TRY(cudaMemsetAsync(d.ctx, 0xFF, R * HIDDEN * 2, d.compute));
     CUDA_TRY(cudaMemsetAsync(d.ffn, 0xFF, R * 3072 * 2, d.compute));
-    std::vector<std::string> names;
-    if (int rc = run(&names)) return rc;
+    LaunchHook hook;
+    hook.stop_after = n_launches;
+    uint64_t launches = 0;
+    if (int rc = forward(d, m, 0, in, dout, d.compute, launches, &hook)) return rc;
     CUDA_TRY(cudaStreamSynchronize(d.compute));
-    const size_t P = H / 128;
     CUDA_TRY(cudaMemcpy(o.yhi, d.yhi, rows * H * 2, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(o.ylo, d.ylo, rows * H * 2, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(o.pstats0, d.pstats[0], rows * P * sizeof(float2), cudaMemcpyDeviceToHost));
@@ -1449,7 +1423,7 @@ int trace_forward(Dev& d, int H, int I, size_t rows, const float* dout, size_t o
     CUDA_TRY(cudaMemcpy(o.out, dout, out_floats * 4, cudaMemcpyDeviceToHost));
     if (o.names && o.names_cap) {
         size_t off = 0;
-        for (const auto& n : names) {
+        for (const auto& n : hook.names) {
             if (off + n.size() + 1 > o.names_cap) break;
             memcpy(o.names + off, n.c_str(), n.size() + 1);
             off += n.size() + 1;
@@ -1679,8 +1653,8 @@ int b200rt_embed_device(int model, int gpu, const int32_t* d_ids, const int32_t*
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
     uint64_t launches = 0;
-    int rc = forward(d, *m, gpu, d_ids, d_lens, n_items, max_len, d_out, stream ? static_cast<cudaStream_t>(stream) : d.compute,
-                     -1, nullptr, &launches);
+    int rc = forward(d, *m, gpu, Input{d_ids, d_lens, nullptr, n_items, max_len}, d_out,
+                     stream ? static_cast<cudaStream_t>(stream) : d.compute, launches);
     std::lock_guard<std::mutex> sl(rt->stats_mu);
     rt->stats.kernel_launches += launches;
     return rc;
@@ -1772,7 +1746,7 @@ void b200rt_shutdown(void) {
     for (auto& d : rt->devs) {
         cudaSetDevice(d->id);
         drop_graphs(*d);
-        cudaFree(d->x32_dbg); cudaFree(d->pstats[0]); cudaFree(d->pstats[1]); cudaFree(d->yhi); cudaFree(d->ylo); cudaFree(d->qkv); cudaFree(d->ctx); cudaFree(d->ffn);
+        cudaFree(d->pstats[0]); cudaFree(d->pstats[1]); cudaFree(d->yhi); cudaFree(d->ylo); cudaFree(d->qkv); cudaFree(d->ctx); cudaFree(d->ffn);
         cudaFree(d->lens_const);
         if (d->copy) cudaStreamDestroy(d->copy);
         for (int s = 0; s < NSLOT; ++s) if (d->ev_pix[s]) cudaEventDestroy(d->ev_pix[s]);
@@ -1800,6 +1774,7 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!a || !w || !bias || !out || M < 1 || N % 128 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
+    if (epi == 2 && !resid) return fail(B200RT_E_INVALID, "epi 2 needs resid");
     if (ln_stats && (epi == 2 ? N : K) != 768 && (epi == 2 ? N : K) != 384)
         return fail(B200RT_E_INVALID, "the LayerNorm'd width must be 768 or 384");
     if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
@@ -1811,35 +1786,25 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256;
     const int parts_in = epi == 2 ? N / 128 : K / 128;
     const int parts_out = N / 128;
-    __half *da = nullptr, *dw = nullptr, *dhi = nullptr, *dlo = nullptr, *dhi0 = nullptr, *dlo0 = nullptr;
-    float *db = nullptr, *dg = nullptr, *dbt = nullptr;
+    DebugBuffers b(d.compute);
+    __half *da, *dw, *dhi = nullptr, *dlo = nullptr, *dhi0 = nullptr, *dlo0 = nullptr, *dout = nullptr;
+    float *db, *dg = nullptr, *dbt = nullptr;
     float2 *dsi = nullptr, *dso = nullptr;
-    void* dout = nullptr;
-    CUDA_TRY(cudaMalloc(&da, Mp * K * 2));
-    CUDA_TRY(cudaMemset(da, 0, Mp * K * 2));
-    CUDA_TRY(cudaMalloc(&dw, static_cast<size_t>(N) * K * 2));
-    CUDA_TRY(cudaMalloc(&db, static_cast<size_t>(N) * 4));
-    CUDA_TRY(cudaMemcpy(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(dw, w, static_cast<size_t>(N) * K * 2, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(db, bias, static_cast<size_t>(N) * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));  // rows past M stay zero
+    CUDA_TRY(cudaMemcpyAsync(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, d.compute));
+    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
+    CUDA_TRY(b.upload(&db, bias, static_cast<size_t>(N) * 4));
     if (ln_stats) {
-        CUDA_TRY(cudaMalloc(&dsi, Mp * parts_in * sizeof(float2)));
-        CUDA_TRY(cudaMemset(dsi, 0, Mp * parts_in * sizeof(float2)));
-        CUDA_TRY(cudaMemcpy(dsi, ln_stats, static_cast<size_t>(M) * parts_in * sizeof(float2), cudaMemcpyHostToDevice));
+        CUDA_TRY(b.upload(&dsi, nullptr, Mp * parts_in * sizeof(float2)));
+        CUDA_TRY(cudaMemcpyAsync(dsi, ln_stats, static_cast<size_t>(M) * parts_in * sizeof(float2), cudaMemcpyHostToDevice, d.compute));
     }
-    auto up = [&](float** dp, const float* h) -> cudaError_t {
-        if (!h) return cudaSuccess;
-        cudaError_t e = cudaMalloc(dp, static_cast<size_t>(N) * 4);
-        return e != cudaSuccess ? e : cudaMemcpy(*dp, h, static_cast<size_t>(N) * 4, cudaMemcpyHostToDevice);
-    };
-    CUDA_TRY(up(&dg, ln_gamma));
-    CUDA_TRY(up(&dbt, ln_beta));
+    if (ln_gamma) CUDA_TRY(b.upload(&dg, ln_gamma, static_cast<size_t>(N) * 4));
+    if (ln_beta) CUDA_TRY(b.upload(&dbt, ln_beta, static_cast<size_t>(N) * 4));
     CUtensorMap ta, tb;
     if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
     if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
     std::vector<__half> hhi, hlo;
     if (epi == 2) {
-        if (!resid) return fail(B200RT_E_INVALID, "epi 2 needs resid");
         // the residual travels as hi + lo (fp16 + fp16): split on the host, keep a pristine copy for the final launch
         hhi.assign(Mp * N, __float2half_rn(0.f));
         hlo.assign(Mp * N, __float2half_rn(0.f));
@@ -1847,17 +1812,16 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
             hhi[i] = __float2half_rn(resid[i]);
             hlo[i] = __float2half_rn(resid[i] - __half2float(hhi[i]));
         }
-        for (__half** pp : {&dhi, &dlo, &dhi0, &dlo0}) CUDA_TRY(cudaMalloc(pp, Mp * N * 2));
-        CUDA_TRY(cudaMemcpy(dhi0, hhi.data(), Mp * N * 2, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(dlo0, hlo.data(), Mp * N * 2, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(dhi, dhi0, Mp * N * 2, cudaMemcpyDeviceToDevice));
-        CUDA_TRY(cudaMemcpy(dlo, dlo0, Mp * N * 2, cudaMemcpyDeviceToDevice));
-        CUDA_TRY(cudaMalloc(&dso, Mp * parts_out * sizeof(float2)));
+        CUDA_TRY(b.upload(&dhi0, hhi.data(), Mp * N * 2));
+        CUDA_TRY(b.upload(&dlo0, hlo.data(), Mp * N * 2));
+        CUDA_TRY(b.upload(&dhi, hhi.data(), Mp * N * 2));
+        CUDA_TRY(b.upload(&dlo, hlo.data(), Mp * N * 2));
+        CUDA_TRY(b.upload(&dso, nullptr, Mp * parts_out * sizeof(float2)));
     } else {
-        CUDA_TRY(cudaMalloc(&dout, Mp * N * 2));
-        CUDA_TRY(cudaMemset(dout, 0xFF, Mp * N * 2));
+        CUDA_TRY(b.upload(&dout, nullptr, Mp * N * 2));
+        CUDA_TRY(cudaMemsetAsync(dout, 0xFF, Mp * N * 2, d.compute));
     }
-    __half* const o_hi = epi == 2 ? dhi : static_cast<__half*>(dout);
+    __half* const o_hi = epi == 2 ? dhi : dout;
     GemmEpi e{db, dsi, parts_in, dg, dbt, dso, eps};
     // epi 2 updates hi / lo in place (y = acc + bias + LN(y)): reload the residual before the launch whose result is returned
     auto reload = [&]() -> cudaError_t {
@@ -1866,8 +1830,8 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
         return ce != cudaSuccess ? ce : cudaMemcpyAsync(dlo, dlo0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute);
     };
     cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    CUDA_TRY(b.event(&e0));
+    CUDA_TRY(b.event(&e1));
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
     for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
@@ -1879,17 +1843,14 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     cudaEventElapsedTime(&ms, e0, e1);
     if (ms_out) *ms_out = ms / iters;
     if (epi == 2) {
-        CUDA_TRY(cudaMemcpy(hhi.data(), dhi, Mp * N * 2, cudaMemcpyDeviceToHost));
-        CUDA_TRY(cudaMemcpy(hlo.data(), dlo, Mp * N * 2, cudaMemcpyDeviceToHost));
+        CUDA_TRY(b.download(hhi.data(), dhi, Mp * N * 2));
+        CUDA_TRY(b.download(hlo.data(), dlo, Mp * N * 2));
         float* o = static_cast<float*>(out);
         for (size_t i = 0; i < static_cast<size_t>(M) * N; ++i) o[i] = __half2float(hhi[i]) + __half2float(hlo[i]);
-        if (stats_out) CUDA_TRY(cudaMemcpy(stats_out, dso, static_cast<size_t>(M) * parts_out * sizeof(float2), cudaMemcpyDeviceToHost));
+        if (stats_out) CUDA_TRY(b.download(stats_out, dso, static_cast<size_t>(M) * parts_out * sizeof(float2)));
     } else {
-        CUDA_TRY(cudaMemcpy(out, dout, static_cast<size_t>(M) * N * 2, cudaMemcpyDeviceToHost));
+        CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * N * 2));
     }
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    cudaFree(da); cudaFree(dw); cudaFree(db); cudaFree(dg); cudaFree(dbt); cudaFree(dsi); cudaFree(dso);
-    cudaFree(dhi); cudaFree(dlo); cudaFree(dhi0); cudaFree(dlo0); cudaFree(dout);
     return 0;
 }
 
@@ -1907,20 +1868,19 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
     const size_t M = static_cast<size_t>(B) * S;
-    __half *dq = nullptr, *dc = nullptr;
-    int32_t* dl_ = nullptr;
-    CUDA_TRY(cudaMalloc(&dq, M * 3 * H * 2));
-    CUDA_TRY(cudaMalloc(&dc, M * H * 2));
-    CUDA_TRY(cudaMalloc(&dl_, static_cast<size_t>(B) * 4));
-    CUDA_TRY(cudaMemset(dc, 0xFF, M * H * 2));
-    CUDA_TRY(cudaMemcpy(dq, qkv, M * 3 * H * 2, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(dl_, lens, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice));
+    DebugBuffers b(d.compute);
+    __half *dq, *dc;
+    int32_t* dl_;
+    CUDA_TRY(b.upload(&dq, qkv, M * 3 * H * 2));
+    CUDA_TRY(b.upload(&dc, nullptr, M * H * 2));
+    CUDA_TRY(cudaMemsetAsync(dc, 0xFF, M * H * 2, d.compute));
+    CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));
     CUtensorMap tq, tc;
     if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, head_dim)) return rc;
     if (int rc = make_map_qkv(&tc, dc, B, S, H, head_dim)) return rc;
     cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    CUDA_TRY(b.event(&e0));
+    CUDA_TRY(b.event(&e1));
     if (iters < 1) iters = 1;
     CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim));
     CUDA_TRY(cudaEventRecord(e0, d.compute));
@@ -1930,9 +1890,7 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
     if (ms_out) *ms_out = ms / iters;
-    CUDA_TRY(cudaMemcpy(ctx, dc, M * H * 2, cudaMemcpyDeviceToHost));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    cudaFree(dq); cudaFree(dc); cudaFree(dl_);
+    CUDA_TRY(b.download(ctx, dc, M * H * 2));
     return 0;
 }
 
@@ -2073,33 +2031,6 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
     return 0;
 }
 
-int b200rt_debug_hidden(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_layers,
-                        float* hidden_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    const Model* m = get_model(*rt, model);
-    if (!m) return B200RT_E_INVALID;
-    if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
-    if (int rc = check_ids(m->cfg, ids, lens, n_items, max_len)) return rc;
-    if (n_layers < 0 || n_layers > m->cfg.layers || !hidden_out) return fail(B200RT_E_INVALID, "bad n_layers / hidden_out");
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t M = static_cast<size_t>(n_items) * max_len;
-    if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
-    std::vector<int32_t> l(n_items, max_len);
-    if (lens) l.assign(lens, lens + n_items);
-    DebugBuffers b(d.compute);
-    int32_t *dids = nullptr, *dlens = nullptr;
-    CUDA_TRY(b.upload(&dids, ids, M * 4));
-    CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
-    if (!d.x32_dbg) CUDA_TRY(cudaMalloc(&d.x32_dbg, static_cast<size_t>(rt->cap_rows) * HIDDEN * 4));
-    int rc = forward(d, *m, 0, dids, dlens, n_items, max_len, nullptr, d.compute, n_layers);
-    if (rc) return rc;
-    CUDA_TRY(b.download(hidden_out, d.x32_dbg, M * m->cfg.hidden * 4));
-    return 0;
-}
-
 int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_launches,
                                uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx,
                                uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total) {
@@ -2109,7 +2040,7 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
     if (!m) return B200RT_E_INVALID;
     if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (int rc = check_ids(m->cfg, ids, lens, n_items, max_len)) return rc;
-    const int total = 5 * m->cfg.layers + 2;
+    const int total = 5 * m->layers + 2;
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
     const size_t M = static_cast<size_t>(n_items) * max_len;
@@ -2120,18 +2051,12 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
     CUDA_TRY(cudaSetDevice(d.id));
     std::vector<int32_t> l(n_items, max_len);
     if (lens) l.assign(lens, lens + n_items);
-    const size_t out_floats = static_cast<size_t>(n_items) * m->out_dim;
     DebugBuffers b(d.compute);
     int32_t *dids = nullptr, *dlens = nullptr;
-    float* dout = nullptr;
     CUDA_TRY(b.upload(&dids, ids, M * 4));
     CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, out_floats * 4, d.compute));
     const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(d, m->cfg.hidden, m->cfg.inter, trace_rows(M), dout, out_floats, o, [&](std::vector<std::string>* names) {
-        return forward(d, *m, 0, dids, dlens, n_items, max_len, dout, d.compute, -1, nullptr, nullptr, n_launches, names);
-    });
+    return trace_forward(b, d, *m, Input{dids, dlens, nullptr, n_items, max_len}, n_launches, o);
 }
 
 int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
@@ -2142,45 +2067,18 @@ int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, 
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
     if (m->kind != KIND_VIT || !pixels || n_items < 1 || n_items > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "bad arguments");
-    const int total = 5 * m->vcfg.layers + 4;
+    const int total = 5 * m->layers + 4;
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
     if (n_total) *n_total = total;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
-    const size_t M = static_cast<size_t>(n_items) * m->tokens;
-    const size_t out_floats = static_cast<size_t>(n_items) * m->out_dim;
     DebugBuffers b(d.compute);
-    float *dpix = nullptr, *dout = nullptr;
+    float* dpix = nullptr;
     CUDA_TRY(b.upload(&dpix, pixels, static_cast<size_t>(n_items) * m->item_bytes));
-    CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, out_floats * 4, d.compute));
     const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(d, HIDDEN, m->vcfg.inter, trace_rows(M), dout, out_floats, o, [&](std::vector<std::string>* names) {
-        return forward_vit(d, *m, 0, dpix, n_items, dout, d.compute, -1, nullptr, n_launches, names);
-    });
-}
-
-int b200rt_debug_vit_hidden(int model, const float* pixels, int n_items, int n_layers, float* hidden_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    const Model* m = get_model(*rt, model);
-    if (!m) return B200RT_E_INVALID;
-    if (m->kind != KIND_VIT || !pixels || !hidden_out || n_items < 1 || n_items > VIT_WAVE_ITEMS || n_layers < 0 || n_layers > m->vcfg.layers)
-        return fail(B200RT_E_INVALID, "bad arguments");
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    CUDA_TRY(cudaMemcpy(d.pix_in[0], pixels, static_cast<size_t>(n_items) * m->item_bytes, cudaMemcpyHostToDevice));
-    if (int rc = forward_vit(d, *m, 0, d.pix_in[0], n_items, nullptr, d.compute, n_layers)) return rc;
-    CUDA_TRY(cudaStreamSynchronize(d.compute));
-    const size_t n = static_cast<size_t>(n_items) * m->tokens * HIDDEN;
-    std::vector<__half> hi(n), lo(n);
-    CUDA_TRY(cudaMemcpy(hi.data(), d.yhi, n * 2, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(lo.data(), d.ylo, n * 2, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < n; ++i) hidden_out[i] = __half2float(hi[i]) + __half2float(lo[i]);
-    return 0;
+    return trace_forward(b, d, *m, Input{nullptr, nullptr, dpix, n_items, m->tokens}, n_launches, o);
 }
 
 int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters, char* names_out, size_t names_cap,
@@ -2191,38 +2089,35 @@ int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters,
     if (!m) return B200RT_E_INVALID;
     if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > m->cfg.max_pos) return fail(B200RT_E_INVALID, "bad argument");
+    const size_t M = static_cast<size_t>(n_items) * max_len;
+    if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
-    const size_t M = static_cast<size_t>(n_items) * max_len;
-    if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
     std::vector<int32_t> ids(M), l(n_items, max_len);
     uint32_t x = 12345;
     for (auto& v : ids) { x = x * 1664525u + 1013904223u; v = 1000 + static_cast<int32_t>((x >> 8) % (m->cfg.vocab - 1000)); }
+    DebugBuffers b(d.compute);
     int32_t *dids = nullptr, *dlens = nullptr;
     float* dout = nullptr;
-    CUDA_TRY(cudaMalloc(&dids, M * 4));
-    CUDA_TRY(cudaMalloc(&dlens, static_cast<size_t>(n_items) * 4));
-    CUDA_TRY(cudaMalloc(&dout, static_cast<size_t>(n_items) * HIDDEN * 4));
-    CUDA_TRY(cudaMemcpy(dids, ids.data(), M * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(dlens, l.data(), static_cast<size_t>(n_items) * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(b.upload(&dids, ids.data(), M * 4));
+    CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * m->out_dim * 4));
     if (iters < 1) iters = 1;
     std::map<std::string, double> acc;
     std::vector<std::string> order;
     for (int it = 0; it < iters + 1; ++it) {
-        Prof prof;
-        int rc = forward(d, *m, 0, dids, dlens, n_items, max_len, dout, d.compute, -1, &prof);
-        if (rc) return rc;
+        LaunchHook hook;
+        hook.timing = true;
+        uint64_t launches = 0;
+        if (int rc = forward(d, *m, 0, Input{dids, dlens, nullptr, n_items, max_len}, dout, d.compute, launches, &hook)) return rc;
         CUDA_TRY(cudaStreamSynchronize(d.compute));
-        for (size_t i = 1; i < prof.evs.size(); ++i) {
+        for (size_t i = 0; it > 0 && i < hook.names.size(); ++i) {  // the first forward warms up
             float ms = 0;
-            cudaEventElapsedTime(&ms, prof.evs[i - 1], prof.evs[i]);
-            if (it > 0) {
-                if (!acc.count(prof.names[i])) order.push_back(prof.names[i]);
-                acc[prof.names[i]] += ms;
-            }
+            cudaEventElapsedTime(&ms, hook.evs[i], hook.evs[i + 1]);
+            if (!acc.count(hook.names[i])) order.push_back(hook.names[i]);
+            acc[hook.names[i]] += ms;
         }
-        for (auto e : prof.evs) cudaEventDestroy(e);
     }
     size_t off = 0;
     int n = 0;
@@ -2233,7 +2128,6 @@ int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters,
         ms_out[n++] = static_cast<float>(acc[name] / iters);
     }
     *n_out = n;
-    cudaFree(dids); cudaFree(dlens); cudaFree(dout);
     return 0;
 }
 

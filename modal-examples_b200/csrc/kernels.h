@@ -77,10 +77,6 @@ cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, con
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,
                          float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream);
 
-// debug only: x32[row] = LN(hi + lo) with the row's own statistics (the product path never materialises this)
-cudaError_t launch_ln_materialize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* x32,
-                                  int n_rows, float eps, int width, cudaStream_t stream);
-
 // final LayerNorm of the CLS row of every item + L2 normalise; row i is stored at out + i * width,
 // where `out` may be a peer-mapped pointer into the root GPU's gather buffer (the fused gather).
 cudaError_t launch_pool_normalize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* out,
@@ -94,9 +90,6 @@ cudaError_t launch_vit_embed(const __half* patch_out, const float* cls, const fl
                              __half* yhi, __half* ylo, float2* stats, int n_rows, int T, float eps, cudaStream_t stream);
 cudaError_t launch_vit_pool(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const float* proj, float* out,
                             int n_items, int T, int P, float eps, cudaStream_t stream);
-
-// fp32 -> fp16 (weight conversion at model load)
-cudaError_t launch_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t stream);
 
 // Root-side scatter of a wave's token ids / lengths into each shard's (possibly peer) input slot.
 struct ScatterPlan {

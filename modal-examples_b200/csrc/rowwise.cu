@@ -1,7 +1,6 @@
 // HBM-bound row-wise kernels (sm_90a): embedding gather into the split residual stream, CLS pooling + final LayerNorm +
 // L2 normalise with the store aimed at the root GPU's gather buffer, the root-side scatter of token ids into (peer) shard
-// inputs, the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns), and a debug-only
-// LayerNorm materialisation.
+// inputs, and the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns).
 //
 // Row kernels: one warp per row (768 wide, or 384 for bge-small's embed / pool / LayerNorm), 128-bit accesses, statistics
 // by warp shuffle in fp32, two-pass variance on register-resident data (no E[x^2]-E[x]^2 cancellation).
@@ -122,23 +121,6 @@ embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ word, co
         if (lane == i) { ps = s; pq = q; }
     }
     if (lane < V4) stats[static_cast<size_t>(tok) * V4 + lane] = make_float2(ps, pq);
-}
-
-// debug only (b200rt_debug_hidden): materialise LN(hi + lo) in fp32
-template <int W>
-__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
-ln_materialize_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, const float* __restrict__ gamma,
-                      const float* __restrict__ beta, float* __restrict__ x32, int n_rows, float eps) {
-    constexpr int V4 = Row<W>::V4;
-    const int lane = threadIdx.x & 31;
-    const int row = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
-    if (row >= n_rows) return;
-    float4 x[V4];
-    load_split_row<W>(yhi, ylo, row, lane, x);
-    ln_inplace<W>(x, gamma, beta, eps, lane);
-    float4* o32 = reinterpret_cast<float4*>(x32 + static_cast<size_t>(row) * W);
-#pragma unroll
-    for (int i = 0; i < V4; ++i) o32[i * 32 + lane] = x[i];
 }
 
 template <int W>
@@ -303,15 +285,6 @@ fold_ln_kernel(const float* __restrict__ w, const float* __restrict__ gamma, con
     }
 }
 
-__global__ void __launch_bounds__(256)
-f32_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n4) {
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4; i += stride) {
-        const float4 v = reinterpret_cast<const float4*>(src)[i];
-        reinterpret_cast<uint2*>(dst)[i] = make_uint2(pack_half2(v.x, v.y), pack_half2(v.z, v.w));
-    }
-}
-
 // blockIdx.y = shard.  Copies ids[item_begin*S .. (item_begin+item_count)*S) and the matching lens to the
 // shard's input slot; dst pointers of remote shards are peer-mapped, so the stores cross NVLink directly.
 __global__ void __launch_bounds__(256)
@@ -342,15 +315,6 @@ cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos
     const int grid = (n_tokens + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
     if (width == 768) rw::embed_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
     else if (width == 384) rw::embed_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
-    else return cudaErrorInvalidValue;
-    return cudaGetLastError();
-}
-
-cudaError_t launch_ln_materialize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* x32,
-                                  int n_rows, float eps, int width, cudaStream_t stream) {
-    const int grid = (n_rows + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
-    if (width == 768) rw::ln_materialize_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, x32, n_rows, eps);
-    else if (width == 384) rw::ln_materialize_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, x32, n_rows, eps);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
@@ -391,12 +355,6 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
     if (K % 64 != 0 || N < 1) return cudaErrorInvalidValue;
     const int grid = (N + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
     rw::fold_ln_kernel<<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(w, gamma, beta, bias, w_out, cvec, N, K);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_f32_to_f16(const float* src, __half* dst, size_t n, cudaStream_t stream) {
-    if (n % 4 != 0) return cudaErrorInvalidValue;
-    rw::f32_to_f16_kernel<<<132 * 8, 256, 0, stream>>>(src, dst, n / 4);
     return cudaGetLastError();
 }
 

@@ -270,7 +270,9 @@ def test_residual_stream_layer_by_layer(rt):
     ids, lens = R.synth_ragged(3, 160, seed=9, min_len=20)
     _, hidden = R.forward_np(flat, ids, lens, g, return_hidden=True)
     for L in (0, 1, 2, 6, 12):
-        h = model.debug_hidden(ids, lens, L)
+        # the oracle's hidden state: the LayerNorm that holds after layer L, applied in fp64 to the residual stream
+        ln = ("emb.ln.g", "emb.ln.b") if L == 0 else (f"l{L - 1}.ln2.g", f"l{L - 1}.ln2.b")
+        h = KR.layernorm_ref(model.debug_residual(ids, lens, L), flat[ln[0]], flat[ln[1]], g.eps)[0]
         assert h.shape == (3, 160, H)
         for i, n in enumerate(lens):
             d = h[i, :n] - hidden[L][i, :n]

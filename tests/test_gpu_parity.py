@@ -147,7 +147,9 @@ def test_hidden_states_layer_by_layer(rt):
     ids, lens = R.synth_ragged(3, 200, seed=5, min_len=3)
     _, hidden = R.forward_np(flat, ids, lens, g, dtype=np.float64, return_hidden=True)
     for L in range(3):
-        h = model.debug_hidden(ids, lens, L)
+        # the oracle's hidden state: the LayerNorm that holds after layer L, applied in fp64 to the residual stream
+        ln = ("emb.ln.g", "emb.ln.b") if L == 0 else (f"l{L - 1}.ln2.g", f"l{L - 1}.ln2.b")
+        h = KR.layernorm_ref(model.debug_residual(ids, lens, L), flat[ln[0]], flat[ln[1]], g.eps)[0]
         for i, n in enumerate(lens):
             d = h[i, :n] - hidden[L][i, :n]
             rel = np.sqrt((d ** 2).sum()) / np.sqrt((hidden[L][i, :n] ** 2).sum())

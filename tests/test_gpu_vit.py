@@ -51,7 +51,7 @@ def test_residual_stream_layer_by_layer(rt):
     px = C.synth_pixels(3, g, 2)
     _, hidden = C.forward_np(flat, px, g, return_hidden=True)
     for L in range(g.layers + 1):
-        got = model.debug_hidden(px, L)
+        got = model.debug_residual(px, L)
         rel = np.linalg.norm(got - hidden[L]) / np.linalg.norm(hidden[L])
         assert rel < (1e-3 if L else 6e-4), (L, rel)  # layer 0: fp16 pixels x fp16 patch weights, fp16 patch output, then pre_layrnorm
 

@@ -14,13 +14,13 @@ model = b200rt.EmbedModel(R.geometry_dict(g), R.pack_blob(flat, g))
 n, S = 45, 256
 ids, lens = R.synth_ragged(n, S, seed=11, min_len=2)
 for L in (0, 1, 2):
-    full = model.debug_hidden(ids, lens, L)
-    part = np.concatenate([model.debug_hidden(ids[i:i + 32], lens[i:i + 32], L) for i in range(0, n, 32)])
+    full = model.debug_residual(ids, lens, L)
+    part = np.concatenate([model.debug_residual(ids[i:i + 32], lens[i:i + 32], L) for i in range(0, n, 32)])
     d = full != part
     # only rows < len matter
     valid = np.arange(S)[None, :] < lens[:, None]
     dv = d & valid[:, :, None]
-    print(f"hidden after {L} layers: {int(dv.sum())} differing valid elements of {int(valid.sum()) * 768}; items affected {sorted(set(np.where(dv.any((1, 2)))[0].tolist()))[:20]}")
+    print(f"residual stream after {L} layers: {int(dv.sum())} differing valid elements of {int(valid.sum()) * 768}; items affected {sorted(set(np.where(dv.any((1, 2)))[0].tolist()))[:20]}")
     if dv.any():
         it = np.where(dv.any((1, 2)))[0][0]
         rows = np.where(dv[it].any(1))[0]
