@@ -71,6 +71,13 @@ int b200rt_num_gpus(void);
  * "vit" (cfg: b200rt_vit_config; the CLIP ViT-B/16 image tower behind 06_gpu_and_ml/embeddings/image_embeddings_infinity.py:76-77;
  * blob order: b200rt.weights.vit_blob_layout).                                                         */
 int b200rt_model_load(const char* kind, const void* cfg, const void* weights, size_t nbytes, int* model_out);
+/* b200rt_model_load with load flags (b200rt_model_load is this with flags = 0).  B200RT_LOAD_POOL_MEAN (kind "bert" only):
+ * pool each item as sentence-transformers' Pooling(mean) + Normalize does -- the mean over the item's lens[i] valid tokens
+ * ([CLS] and [SEP] included) of the final hidden states, then L2 normalise -- instead of taking the [CLS] row; the pooling of
+ * all-MiniLM-L6-v2, e5 and gte.  The forward before the pool, and its launch count, are the same either way.  With kind
+ * "vit", or with any other flag bit set, returns B200RT_E_INVALID.                                                       */
+#define B200RT_LOAD_POOL_MEAN 1u
+int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out);
 
 /* One .map() input.  Stands in for `TextEmbeddingsInference.embed` -> `POST /embed`
  * (text_embeddings_inference.py:97-104) with token ids instead of strings: ids is [n_items, max_len]

@@ -42,6 +42,9 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
  *                   word [vocab, W], pos [S, W], type0 [W].
  *   vit_embed:      x = pre_layrnorm((t % T == 0 ? cls : patch_out[t]) + pos[t % T]) -> hi, lo, stats of x.
  *   pool_normalize: out[i] = L2-normalise(LayerNorm(hi + lo of row i * S)), out fp32 [n_items, W].
+ *   mean_pool_normalize: out[i] = L2-normalise((1 / L) sum_{r < L} LayerNorm(hi + lo of row i * S + r)), L = lens[i] clamped
+ *                   to [1, S] on the device (lens is passed through unchecked); rows past L are never read.  out fp32
+ *                   [n_items, W]; W from the trailing `hidden` as for pool_normalize.
  *   vit_pool:       out[i] = L2-normalise(proj . LayerNorm(hi + lo of row i * T)), proj fp32 [P, 768], 1 <= P <= 1024,
  *                   out fp32 [n_items, P].
  *   fold_ln:        w_out = fp16(w o gamma - rowmean(w o gamma)), cvec_out = w beta + bias (bias may be NULL);
@@ -52,6 +55,8 @@ int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const fl
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out);
 int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
                                 float eps, float* out, int hidden);
+int b200rt_debug_mean_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const int32_t* lens,
+                                     int n_items, int S, float eps, float* out, int hidden);
 int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* proj, int n_items,
                           int T, int P, float eps, float* out);
 int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,
@@ -60,7 +65,7 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
 /* Trace of the product forward on replica 0: the workspace is set to 0xFF bytes (NaN in fp16 and fp32), then the first
  * n_launches launches of the forward of this batch run exactly as the product enqueues them (same kernels, buffers and stream,
  * no sync or copy between them), and the workspace is copied out once they finish.  n_launches is in [0, n_total], n_total =
- * 5 layers + 2 (text: embed, 5 per layer, pool_normalize) or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer,
+ * 5 layers + 2 (text: embed, 5 per layer, pool_normalize -- mean_pool_normalize for a B200RT_LOAD_POOL_MEAN model) or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer,
  * vit_pool).  Every buffer comes back for rows = min(M + 256, 512 b200rt_wave_capacity_items()) rows, M = n_items * max_len
  * (text) or n_items * tokens (vit), at the model's widths (H = hidden, I = inter, P = H / 128):
  *   yhi, ylo, ctx: fp16 bits [rows, H]; qkv: fp16 bits [rows, 3H]; ffn: fp16 bits [rows, I] (vit: the im2col matrix

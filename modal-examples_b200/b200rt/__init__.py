@@ -24,12 +24,13 @@ E_INVALID, E_STATE, E_CUDA, E_NOMEM, E_UNSUPPORTED = -1, -2, -3, -4, -5
 
 # every symbol include/b200rt.h and include/b200rt_debug.h declare (tests check the export list)
 ABI_SYMBOLS = [
-    "b200rt_init", "b200rt_init_devices", "b200rt_num_gpus", "b200rt_model_load", "b200rt_submit", "b200rt_submit_ex", "b200rt_submit_pixels", "b200rt_wait",
+    "b200rt_init", "b200rt_init_devices", "b200rt_num_gpus", "b200rt_model_load", "b200rt_model_load_ex", "b200rt_submit", "b200rt_submit_ex", "b200rt_submit_pixels", "b200rt_wait",
     "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items",
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
 DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_profile_forward",
-                 "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_vit_pool", "b200rt_debug_fold_ln",
+                 "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_mean_pool_normalize",
+                 "b200rt_debug_vit_pool", "b200rt_debug_fold_ln",
                  "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace"]
 
 
@@ -84,6 +85,7 @@ def load_library():
         lib.b200rt_init.argtypes = [ctypes.c_int, ctypes.c_uint32]
         lib.b200rt_init_devices.argtypes = [i32p, ctypes.c_int, ctypes.c_uint32]
         lib.b200rt_model_load.argtypes = [ctypes.c_char_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, i32p]
+        lib.b200rt_model_load_ex.argtypes = [ctypes.c_char_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_uint32, i32p]
         lib.b200rt_submit.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, u64p]
         lib.b200rt_submit_ex.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.c_uint32, u64p]
@@ -109,6 +111,7 @@ def load_library():
         lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp, ci]
         lib.b200rt_debug_vit_embed.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, vp, vp]
         lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp, ci]
+        lib.b200rt_debug_mean_pool_normalize.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
         lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
         lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
@@ -235,17 +238,27 @@ def poll_any(timeout_ms: int = -1) -> Ticket | None:
     return tk
 
 
-class EmbedModel:
-    """A loaded BERT-geometry encoder; ``submit``/``wait``/``poll_any`` are the .map() primitives."""
+LOAD_POOL_MEAN = 1
+POOLINGS = ("cls", "mean")
 
-    def __init__(self, geometry: dict, blob: np.ndarray):
+
+class EmbedModel:
+    """A loaded BERT-geometry encoder; ``submit``/``wait``/``poll_any`` are the .map() primitives.
+    ``pooling``: "cls" (the [CLS] row: bge) or "mean" (the mean of the valid tokens' final hidden states, as
+    sentence-transformers' Pooling(mean) computes it: all-MiniLM-L6-v2, e5, gte); either way the result is L2-normalised."""
+
+    def __init__(self, geometry: dict, blob: np.ndarray, pooling: str = "cls"):
+        if pooling not in POOLINGS:
+            raise B200RTError(E_INVALID, f"pooling must be one of {POOLINGS}, got {pooling!r}")
         lib = load_library()
         blob = np.ascontiguousarray(blob, dtype=np.float32)
         self.cfg = BertConfig(geometry["vocab"], geometry["hidden"], geometry["layers"], geometry["heads"], geometry["inter"],
                               geometry["max_pos"], geometry["type_vocab"], geometry["eps"])
         self.hidden, self.inter = geometry["hidden"], geometry["inter"]
+        self.pooling = pooling
         h = ctypes.c_int32(-1)
-        _check(lib.b200rt_model_load(b"bert", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
+        flags = LOAD_POOL_MEAN if pooling == "mean" else 0
+        _check(lib.b200rt_model_load_ex(b"bert", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, flags, ctypes.byref(h)))
         self.handle = h.value
         self._lib = lib
 
@@ -490,6 +503,23 @@ def debug_pool_normalize(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta
     n = hi.shape[0] // S
     out = np.empty((n, hidden), np.float32)
     _check(load_library().b200rt_debug_pool_normalize(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), n, S, eps, _ptr(out), hidden))
+    return out
+
+
+def debug_mean_pool_normalize(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta: np.ndarray, lens, S: int, eps: float,
+                              hidden: int = 768):
+    """hi, lo [n_items * S, hidden], lens [n_items] (passed to the device as given; the kernel clamps each to [1, S]): the
+    L2-normalised mean of the LayerNorm'd rows i * S + r, r < lens[i], of every item, [n_items, hidden]."""
+    hi, lo, gamma, beta = _f16(hi), _f16(lo), _f32(gamma), _f32(beta)
+    lens = np.ascontiguousarray(lens, dtype=np.int32)
+    if hi.shape[1] != hidden or lo.shape[1] != hidden or gamma.size != hidden or beta.size != hidden:
+        raise B200RTError(E_INVALID, f"rows and LayerNorm parameters must be {hidden} wide")
+    n = hi.shape[0] // S
+    if lens.shape != (n,):
+        raise B200RTError(E_INVALID, f"lens must have shape ({n},), got {lens.shape}")
+    out = np.empty((n, hidden), np.float32)
+    _check(load_library().b200rt_debug_mean_pool_normalize(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), _ptr(lens), n, S, eps, _ptr(out),
+                                                           hidden))
     return out
 
 

@@ -21,6 +21,40 @@ import numpy as np
 BGE_BASE_GEOMETRY = dict(vocab=30522, hidden=768, layers=12, heads=12, inter=3072, max_pos=512, type_vocab=2, eps=1e-12)
 # BAAI/bge-small-en-v1.5: 12 heads of 32 -- the head count is not implied by the tensor shapes (384 // 64 would be 6)
 BGE_SMALL_GEOMETRY = dict(vocab=30522, hidden=384, layers=12, heads=12, inter=1536, max_pos=512, type_vocab=2, eps=1e-12)
+# sentence-transformers/all-MiniLM-L6-v2: bge-small's geometry with 6 layers; mean-pooled (see pooling_from_dir)
+MINILM_L6_GEOMETRY = dict(vocab=30522, hidden=384, layers=6, heads=12, inter=1536, max_pos=512, type_vocab=2, eps=1e-12)
+
+_ST_POOLING_MODULE = "sentence_transformers.models.Pooling"
+_ST_POOLING_MODES = ("pooling_mode_cls_token", "pooling_mode_mean_tokens", "pooling_mode_max_tokens",
+                     "pooling_mode_mean_sqrt_len_tokens", "pooling_mode_weightedmean_tokens", "pooling_mode_lasttoken")
+
+
+def pooling_from_dir(path: str) -> str | None:
+    """The pooling a sentence-transformers snapshot declares: ``modules.json`` names the
+    ``sentence_transformers.models.Pooling`` module and its directory (``1_Pooling``), whose ``config.json`` switches the
+    modes on.  Returns "cls" or "mean"; None when the directory carries no such module (a plain HF checkpoint).  Any other
+    mode (max, mean_sqrt_len, weightedmean, lasttoken), or more than one at once, raises ValueError: the runtime pools the
+    two supported ways only, and serving such a model with either would return a different embedding."""
+    mod_path = os.path.join(path, "modules.json")
+    if not os.path.exists(mod_path):
+        return None
+    with open(mod_path) as f:
+        modules = json.load(f)
+    pool = next((m for m in modules if m.get("type") == _ST_POOLING_MODULE), None)
+    if pool is None:
+        return None
+    cfg_path = os.path.join(path, pool.get("path", ""), "config.json")
+    if not os.path.exists(cfg_path):
+        return None
+    with open(cfg_path) as f:
+        cfg = json.load(f)
+    on = [k for k in _ST_POOLING_MODES if cfg.get(k)]
+    if on == ["pooling_mode_cls_token"]:
+        return "cls"
+    if on == ["pooling_mode_mean_tokens"]:
+        return "mean"
+    raise ValueError(f"{cfg_path}: pooling modes {on or 'none'} enabled; the supported poolings are cls "
+                     "(pooling_mode_cls_token) and mean (pooling_mode_mean_tokens), one at a time")
 
 
 def blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:

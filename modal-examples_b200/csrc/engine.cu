@@ -154,6 +154,7 @@ enum ModelKind { KIND_BERT = 0, KIND_VIT = 1 };
 
 struct Model {
     ModelKind kind = KIND_BERT;
+    bool pool_mean = false;  // text: mean of the valid tokens' final hidden states (B200RT_LOAD_POOL_MEAN) instead of the CLS row
     b200rt_bert_config cfg{};
     b200rt_vit_config vcfg{};
     int hidden = 0, inter = 0, heads = 0, layers = 0;  // encoder geometry, from whichever config the kind has
@@ -415,8 +416,9 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             prev_b = lw.ln2_b;
         }
         if (vit) CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
+        else if (m.pool_mean) CUDA_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
         else CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
-        step(vit ? "vit_pool" : "pool_normalize");
+        step(vit ? "vit_pool" : (m.pool_mean ? "mean_pool_normalize" : "pool_normalize"));
         return 0;
     };
     if (int rc = enqueue()) return rc;
@@ -1050,7 +1052,7 @@ struct BlobCursor {
     size_t f32 = 0, f16 = 0;
 };
 
-int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, int* model_out) {
+int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out) {
     Runtime& rt = *g_rt;
     bool known = false;
     for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
@@ -1067,6 +1069,7 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, in
 
     auto m = std::make_unique<Model>();
     m->cfg = c;
+    m->pool_mean = pool_mean;
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->out_dim = c.hidden;
     const size_t per_layer_x = 3 * H + I;  // derived vectors: qkv_c, ff1_c
@@ -1453,14 +1456,22 @@ int b200rt_wave_capacity_items(void) {
 }
 
 int b200rt_model_load(const char* kind, const void* cfg, const void* weights, size_t nbytes, int* model_out) {
+    return b200rt_model_load_ex(kind, cfg, weights, nbytes, 0, model_out);
+}
+
+int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0))
         return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\" or \"vit\")", kind ? kind : "(null)");
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
-    if (strcmp(kind, "vit") == 0)
+    if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
+    const bool pool_mean = (flags & B200RT_LOAD_POOL_MEAN) != 0;
+    if (strcmp(kind, "vit") == 0) {
+        if (pool_mean) return fail(B200RT_E_INVALID, "B200RT_LOAD_POOL_MEAN applies to text encoders (kind \"bert\"), not \"vit\"");
         return model_load_vit(*static_cast<const b200rt_vit_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
-    return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
+    }
+    return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean, model_out);
 }
 
 static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, float* out,
@@ -1976,6 +1987,34 @@ int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const fl
     CUDA_TRY(b.upload(&dbt, beta, H * 4));
     CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * H * 4));
     CUDA_TRY(launch_pool_normalize(dhi, dlo, dg, dbt, dout, n_items, S, eps, hidden, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * H * 4));
+    return 0;
+}
+
+int b200rt_debug_mean_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const int32_t* lens,
+                                     int n_items, int S, float eps, float* out, int hidden) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!hi || !lo || !gamma || !beta || !lens || !out || n_items < 1 || S < 1)
+        return fail(B200RT_E_INVALID, "bad mean_pool_normalize arguments");
+    if (hidden == 0) hidden = 768;
+    if (hidden != 768 && hidden != 384) return fail(B200RT_E_INVALID, "row width must be 768 or 384 (0 = 768), got %d", hidden);
+    const size_t H = hidden;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_items) * S;
+    DebugBuffers b(d.compute);
+    __half *dhi, *dlo;
+    float *dg, *dbt, *dout;
+    int32_t* dlens;
+    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+    CUDA_TRY(b.upload(&dg, gamma, H * 4));
+    CUDA_TRY(b.upload(&dbt, beta, H * 4));
+    CUDA_TRY(b.upload(&dlens, lens, static_cast<size_t>(n_items) * 4));  // passed through unchecked: the kernel clamps to [1, S]
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * H * 4));
+    CUDA_TRY(launch_mean_pool_normalize(dhi, dlo, dg, dbt, dlens, dout, n_items, S, eps, hidden, d.compute));
     CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * H * 4));
     return 0;
 }

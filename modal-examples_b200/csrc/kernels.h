@@ -82,6 +82,12 @@ cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos
 cudaError_t launch_pool_normalize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, float* out,
                                   int n_items, int S, float eps, int width, cudaStream_t stream);
 
+// mean pooling (sentence-transformers Pooling(mean)) + L2 normalise: out + i * width = normalise((1 / len_i) sum over rows
+// i * S + r, r < len_i, of the final LayerNorm of hi + lo), len_i = lens[i] clamped to [1, S] (lens NULL: S).  Rows past
+// len_i are never read.  One block per item; the summation order depends on len_i only.  `out` may be peer memory.
+cudaError_t launch_mean_pool_normalize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const int32_t* lens,
+                                       float* out, int n_items, int S, float eps, int width, cudaStream_t stream);
+
 // ViT image tower (CLIP): pixels fp32 [n, 3, img, img] -> im2col A fp16 [n*T, 3 p p] (class-token rows zero); patch GEMM output +
 // class / position embeddings + pre_layrnorm -> residual stream + statistics; pooled head: post_layernorm(class token) ->
 // projection [P, 768] -> L2 normalise, stored at out + i * P (possibly peer memory).

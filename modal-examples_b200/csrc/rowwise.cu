@@ -1,4 +1,4 @@
-// HBM-bound row-wise kernels (sm_90a): embedding gather into the split residual stream, CLS pooling + final LayerNorm +
+// HBM-bound row-wise kernels (sm_90a): embedding gather into the split residual stream, CLS or mean pooling + final LayerNorm +
 // L2 normalise with the store aimed at the root GPU's gather buffer, the root-side scatter of token ids into (peer) shard
 // inputs, and the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns).
 //
@@ -142,6 +142,84 @@ pool_normalize_kernel(const __half* __restrict__ yhi, const __half* __restrict__
 #pragma unroll
     for (int i = 0; i < V4; ++i)
         o4[i * 32 + lane] = make_float4(x[i].x * inv, x[i].y * inv, x[i].z * inv, x[i].w * inv);
+}
+
+// sentence-transformers' Pooling(mean) + Normalize: out[i] = L2normalise((1 / len_i) sum_{r < len_i} LN(hi + lo of row i S + r)),
+// [CLS] and [SEP] included.  One block per item: warp w LayerNorms rows w, w + 8, w + 16, ... (the same load_split_row /
+// ln_inplace as the CLS pool) and sums them in fp32 registers; the 8 warp sums are then added in warp order through shared
+// memory.  The summation order is a function of len_i alone -- not of B, S, the grid or the replica -- so an item's embedding
+// is bit-identical in any batch.  Rows len_i <= r < S are padding and are never read; len_i is clamped to [1, S] (lens may be
+// a caller's unvalidated device array) and lens == NULL means every item is S long.
+template <int W>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
+mean_pool_normalize_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, const float* __restrict__ gamma,
+                           const float* __restrict__ beta, const int32_t* __restrict__ lens, float* __restrict__ out, int S, float eps) {
+    constexpr int V4 = Row<W>::V4;
+    __shared__ __align__(16) float s_sum[WARPS_PER_BLOCK][W];
+    __shared__ float s_red[WARPS_PER_BLOCK];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int item = blockIdx.x;
+    int L = lens ? lens[item] : S;
+    L = L < 1 ? 1 : (L > S ? S : L);
+    float4 acc[V4];
+#pragma unroll
+    for (int i = 0; i < V4; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    auto add = [&](float4 (&x)[V4]) {
+#pragma unroll
+        for (int i = 0; i < V4; ++i) {
+            acc[i].x += x[i].x; acc[i].y += x[i].y; acc[i].z += x[i].z; acc[i].w += x[i].w;
+        }
+    };
+    const size_t row0 = static_cast<size_t>(item) * S;
+    int r = warp;
+    // two rows in flight per warp (one block per item leaves few warps per SM to hide HBM latency); still added in row order
+    for (; r + WARPS_PER_BLOCK < L; r += 2 * WARPS_PER_BLOCK) {
+        float4 x[V4], x2[V4];
+        load_split_row<W>(yhi, ylo, row0 + r, lane, x);
+        load_split_row<W>(yhi, ylo, row0 + r + WARPS_PER_BLOCK, lane, x2);
+        ln_inplace<W>(x, gamma, beta, eps, lane);
+        add(x);
+        ln_inplace<W>(x2, gamma, beta, eps, lane);
+        add(x2);
+    }
+    if (r < L) {
+        float4 x[V4];
+        load_split_row<W>(yhi, ylo, row0 + r, lane, x);
+        ln_inplace<W>(x, gamma, beta, eps, lane);
+        add(x);
+    }
+#pragma unroll
+    for (int i = 0; i < V4; ++i) *reinterpret_cast<float4*>(&s_sum[warp][i * 128 + 4 * lane]) = acc[i];
+    __syncthreads();
+    // column c = threadIdx.x + k * 256: the warp sums in warp order, then / len_i (sum / count, as Pooling(mean) divides)
+    constexpr int PER_THREAD = (W + WARPS_PER_BLOCK * 32 - 1) / (WARPS_PER_BLOCK * 32);
+    float v[PER_THREAD];
+    float q = 0.f;
+#pragma unroll
+    for (int k = 0; k < PER_THREAD; ++k) {
+        const int c = threadIdx.x + k * WARPS_PER_BLOCK * 32;
+        v[k] = 0.f;
+        if (c < W) {
+            float s = s_sum[0][c];
+#pragma unroll
+            for (int w = 1; w < WARPS_PER_BLOCK; ++w) s += s_sum[w][c];
+            v[k] = s / static_cast<float>(L);
+            q = fmaf(v[k], v[k], q);
+        }
+    }
+    q = warp_sum(q);
+    if (lane == 0) s_red[warp] = q;
+    __syncthreads();
+    float tot = 0.f;
+#pragma unroll
+    for (int w = 0; w < WARPS_PER_BLOCK; ++w) tot += s_red[w];
+    const float inv = 1.0f / fmaxf(sqrtf(tot), 1e-12f);  // torch.nn.functional.normalize eps
+    float* o = out + static_cast<size_t>(item) * W;  // may be peer memory
+#pragma unroll
+    for (int k = 0; k < PER_THREAD; ++k) {
+        const int c = threadIdx.x + k * WARPS_PER_BLOCK * 32;
+        if (c < W) o[c] = v[k] * inv;
+    }
 }
 
 // ----------------------------------------------------------------------------------------------- ViT image tower (CLIP)
@@ -324,6 +402,16 @@ cudaError_t launch_pool_normalize(const __half* yhi, const __half* ylo, const fl
     const int grid = (n_items + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
     if (width == 768) rw::pool_normalize_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
     else if (width == 384) rw::pool_normalize_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
+    else return cudaErrorInvalidValue;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mean_pool_normalize(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const int32_t* lens,
+                                       float* out, int n_items, int S, float eps, int width, cudaStream_t stream) {
+    if (n_items < 1 || S < 1) return cudaErrorInvalidValue;
+    const int block = rw::WARPS_PER_BLOCK * 32;
+    if (width == 768) rw::mean_pool_normalize_kernel<768><<<n_items, block, 0, stream>>>(yhi, ylo, gamma, beta, lens, out, S, eps);
+    else if (width == 384) rw::mean_pool_normalize_kernel<384><<<n_items, block, 0, stream>>>(yhi, ylo, gamma, beta, lens, out, S, eps);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }

@@ -16,13 +16,36 @@ GEOMETRY = dict(vocab=30522, hidden=768, layers=12, heads=12, inter=3072, max_po
 BGE_SMALL_ID = "BAAI/bge-small-en-v1.5"
 
 
+MINILM_L6_ID = "sentence-transformers/all-MiniLM-L6-v2"
+POOLING_BY_MODEL_ID = {MINILM_L6_ID: "mean"}  # models whose sentence-transformers config pools other than by [CLS]
+POOLINGS = ("cls", "mean")  # TEI also knows splade and last-token; this runtime does not
+
+
 def geometry_for_model_id(model_id: str) -> dict:
     """Geometry of the offline seeded fallback and of a raw --weights blob (which carries no shapes): bge-small's for
-    BAAI/bge-small-en-v1.5, bge-base's for BAAI/bge-base-en-v1.5 and for any id this table does not know."""
-    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_SMALL_GEOMETRY
+    BAAI/bge-small-en-v1.5, MiniLM-L6's (bge-small's with 6 layers) for sentence-transformers/all-MiniLM-L6-v2, bge-base's
+    for BAAI/bge-base-en-v1.5 and for any id this table does not know."""
+    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY
 
-    known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY}
+    known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY, MINILM_L6_ID: MINILM_L6_GEOMETRY}
     return dict(known.get(model_id, BGE_BASE_GEOMETRY))
+
+
+def resolve_pooling(flag: str | None, snapshot_dir: str | None, model_id: str) -> str:
+    """The pooling to serve, resolved as TEI resolves it: --pooling when given; else the Pooling module of the snapshot's
+    sentence-transformers config (modules.json -> 1_Pooling/config.json); else the model-id table; else cls.  Raises
+    ValueError for a --pooling other than cls / mean and for a snapshot that declares a pooling other than those two."""
+    from b200rt.weights import pooling_from_dir
+
+    if flag is not None:
+        if flag not in POOLINGS:
+            raise ValueError(f"--pooling {flag!r} is not supported (supported: {', '.join(POOLINGS)})")
+        return flag
+    if snapshot_dir:
+        declared = pooling_from_dir(snapshot_dir)
+        if declared is not None:
+            return declared
+    return POOLING_BY_MODEL_ID.get(model_id, "cls")
 
 
 def parse_args(argv):
@@ -36,7 +59,7 @@ def parse_args(argv):
     ap.add_argument("--huggingface-hub-cache", default=None)
     ap.add_argument("--revision", default=None)
     ap.add_argument("--dtype", default="float16")
-    ap.add_argument("--pooling", default="cls")
+    ap.add_argument("--pooling", default=None, help="cls or mean; default: the snapshot's sentence-transformers Pooling config, else cls")
     ap.add_argument("--auto-truncate", action="store_true")
     ap.add_argument("--tokenizer-vocab", default=os.environ.get("B200RT_VOCAB"))
     ap.add_argument("--weights", default=os.environ.get("B200RT_WEIGHTS"), help="flat fp32 blob (DESIGN.md §3), a .safetensors checkpoint or an HF snapshot directory; default: the hub cache, else seeded random init")
@@ -52,6 +75,19 @@ def random_blob(seed=0, geometry=None):
     from b200rt.weights import random_blob as rb
 
     return rb(geometry or GEOMETRY, seed)
+
+
+def weights_dir(args) -> str | None:
+    """The directory the weights come from (an HF snapshot directory or the one holding a .safetensors checkpoint), which
+    is where a sentence-transformers model keeps modules.json; None for a flat blob or the seeded fallback."""
+    from b200rt import weights as W
+
+    if args.weights:
+        if os.path.isdir(args.weights):
+            return args.weights
+        return os.path.dirname(os.path.abspath(args.weights)) if args.weights.endswith(".safetensors") else None
+    cache = args.huggingface_hub_cache or os.environ.get("HUGGINGFACE_HUB_CACHE") or os.environ.get("HF_HUB_CACHE")
+    return W.resolve_hub_snapshot(cache, args.model_id) if cache else None
 
 
 def load_weights(args):
@@ -84,6 +120,7 @@ class Engine:
 
         self.np = np
         self.args = args
+        self.pooling = resolve_pooling(args.pooling, weights_dir(args), args.model_id)
         self.tok = WordPiece(load_vocab(args.tokenizer_vocab) if args.tokenizer_vocab else None)
         if self.tok.synthetic:
             print("[text-embeddings-router/b200] no BERT vocabulary available: SYNTHETIC WordPiece vocabulary, auto-truncate on "
@@ -100,8 +137,9 @@ class Engine:
             print(f"[text-embeddings-router/b200] no weights for {args.model_id!r} offline: seeded random init", file=sys.stderr)
         else:
             print(f"[text-embeddings-router/b200] weights: {source}", file=sys.stderr)
+        print(f"[text-embeddings-router/b200] pooling: {self.pooling}", file=sys.stderr)
         self.geometry = geometry
-        self.model = b200rt.EmbedModel(geometry, blob)
+        self.model = b200rt.EmbedModel(geometry, blob, pooling=self.pooling)
         self.n_gpus = n_gpus
 
     def embed(self, inputs):
@@ -134,7 +172,7 @@ def make_handler(engine: Engine):
                 self._send(200, {})
             elif self.path == "/info":
                 self._send(200, {"model_id": engine.args.model_id, "model_dtype": "float16", "max_client_batch_size": engine.args.max_client_batch_size,
-                                 "max_input_length": GEOMETRY["max_pos"], "backend": f"b200rt x{engine.n_gpus}", "pooling": "cls"})
+                                 "max_input_length": GEOMETRY["max_pos"], "backend": f"b200rt x{engine.n_gpus}", "pooling": engine.pooling})
             else:
                 self._send(404, {"error": "not found", "error_type": "NotFound"})
 

@@ -8,8 +8,11 @@ written as CUDA.
                   and the weight rows centred; the epilogue applies rstd * acc + (W beta + b)   (round-2 design, no LN kernels)
 
     python tools/emulate_numerics.py [--geometry base|small] [--style hf|trained|hard] [--layers 12] [--items 4] [--seq 512]
+                                     [--pooling cls|mean]
 
 --geometry small: bge-small (hidden 384, 12 heads of 32, inter 1536) instead of bge-base.
+--pooling mean: sentence-transformers' mean of the valid tokens' final hidden states (all-MiniLM-L6-v2, e5, gte) instead of
+the [CLS] row, against the fp64 oracle pooled the same way (tests/mean_pool_refs.py).
 """
 import argparse
 import math
@@ -20,7 +23,9 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import bge_ref as R  # noqa: E402
+import mean_pool_refs as MP  # noqa: E402
 
 GEOMETRIES = {"base": {}, "small": dict(hidden=384, heads=12, inter=1536)}
 
@@ -40,7 +45,7 @@ def stats(y, eps):
     return mu, (1.0 / np.sqrt(var + eps)).astype(np.float32)
 
 
-def emulate(flat, ids, lens, g, mode="current", p_sum="exact", keep=()):
+def emulate(flat, ids, lens, g, mode="current", p_sum="exact", keep=(), pooling="cls"):
     """keep: names of rounding points left in fp32 (ablation): x, w, qkv, p, ctx, ffn"""
     r = lambda name, a: a if name in keep else f16(a)  # noqa: E731
     B, S = ids.shape
@@ -83,8 +88,12 @@ def emulate(flat, ids, lens, g, mode="current", p_sum="exact", keep=()):
         x = ln_apply(y, ln)
         y = ffn @ r("w", W[p + "ff2.w"]).T + W[p + "ff2.b"] + x
         ln = (p + "ln2.g", p + "ln2.b")
-    cls = ln_apply(y[:, 0, :], ln)
-    return cls / np.maximum(np.sqrt((cls * cls).sum(-1, keepdims=True)), 1e-12)
+    if pooling == "mean":  # fp32 LayerNorm of every valid row, fp32 masked mean
+        h = ln_apply(y, ln) * (~keymask)[..., None]
+        pooled = (h.sum(1, dtype=np.float32) / np.asarray(lens, np.float32)[:, None]).astype(np.float32)
+    else:
+        pooled = ln_apply(y[:, 0, :], ln)
+    return pooled / np.maximum(np.sqrt((pooled * pooled).sum(-1, keepdims=True)), 1e-12)
 
 
 def main():
@@ -96,17 +105,22 @@ def main():
     ap.add_argument("--seq", type=int, default=512)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--ablate", action="store_true")
+    ap.add_argument("--pooling", choices=("cls", "mean"), default="cls")
     a = ap.parse_args()
     g = R.BertGeometry(layers=a.layers, **GEOMETRIES[a.geometry])
     flat = R.make_weights(g, a.seed, a.style)
     ids, lens = R.synth_ragged(a.items, a.seq, seed=1, min_len=max(1, a.seq // 4))
-    ref = R.forward_np(flat, ids, lens, g, dtype=np.float64)
-    hf = R.forward_hf(R.build_hf_model(flat, g), ids, lens)
-    print(f"geometry {a.geometry} style {a.style} layers {a.layers} items {a.items} x {a.seq}")
+    if a.pooling == "mean":
+        ref = MP.forward_np_mean(flat, ids, lens, g)
+        hf = MP.forward_hf_mean(R.build_hf_model(flat, g), ids, lens)
+    else:
+        ref = R.forward_np(flat, ids, lens, g, dtype=np.float64)
+        hf = R.forward_hf(R.build_hf_model(flat, g), ids, lens)
+    print(f"geometry {a.geometry} style {a.style} layers {a.layers} items {a.items} x {a.seq} pooling {a.pooling}")
     print("  HF fp32 vs numpy fp64     :", R.rel_l2(hf, ref).max())
     for mode in ("current", "fold"):
         for ps in ("exact", "p16"):
-            out = emulate(flat, ids, lens, g, mode, ps)
+            out = emulate(flat, ids, lens, g, mode, ps, pooling=a.pooling)
             print(f"  emulated {mode:8s} l={ps:5s} vs fp64: {R.rel_l2(out, ref).max():.3e}   vs HF fp32: {R.rel_l2(out, hf).max():.3e}")
     if a.ablate:
         for keep in (("x",), ("w",), ("qkv",), ("p",), ("ctx",), ("ffn",), ("x", "w"), ("qkv", "p", "ctx"), ("x", "w", "qkv", "p", "ctx", "ffn")):
