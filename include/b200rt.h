@@ -24,11 +24,13 @@ extern "C" {
 #define B200RT_E_STATE (-2)     /* not initialised / already initialised / shut down */
 #define B200RT_E_CUDA (-3)      /* CUDA error; the context is poisoned and every later call fails fast */
 #define B200RT_E_NOMEM (-4)
-#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is neither bge-base nor bge-small */
+#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is none of bge-base, bge-small, bge-large */
 
-/* Geometry of a BERT encoder (HF BertConfig fields).  The sm_90a kernels cover two geometries: bge-base (hidden 768,
- * 12 heads of 64, inter 3072) and bge-small (hidden 384, 12 heads of 32, inter 1536), with max_pos <= 512; `layers` is
- * free.  A model's results are `hidden` floats per item.                                                              */
+/* Geometry of a BERT encoder (HF BertConfig fields).  The sm_90a kernels cover three geometries: bge-base (hidden 768,
+ * 12 heads of 64, inter 3072), bge-small (hidden 384, 12 heads of 32, inter 1536) and bge-large (hidden 1024, 16 heads of
+ * 64, inter 4096), with max_pos <= 512; `layers` is free.  A model's results are `hidden` floats per item.  The workspace
+ * is sized for bge-base, so a bge-large wave holds 3/4 of the tokens (b200rt_model_wave_capacity_items); loading a
+ * bge-large model returns B200RT_E_INVALID when that is less than one 512-token item.                                */
 typedef struct b200rt_bert_config {
     int32_t vocab, hidden, layers, heads, inter, max_pos, type_vocab;
     float eps;
@@ -107,11 +109,16 @@ int b200rt_poll_any(uint64_t* ticket_out, int timeout_ms);
 
 /* Device-resident variant for callers that already hold the batch in HBM on replica `gpu` (index into
  * the pool): enqueues the forward of one batch on `stream` (a cudaStream_t; NULL = the replica's own
- * compute stream) and returns without synchronising.  n_items * max_len must fit the wave capacity.  */
+ * compute stream) and returns without synchronising.  n_items * max_len must fit the model's wave capacity
+ * (512 b200rt_model_wave_capacity_items(model) tokens, or B200RT_E_INVALID).                           */
 int b200rt_embed_device(int model, int gpu, const int32_t* d_ids, const int32_t* d_lens, int n_items, int max_len,
                         float* d_out, void* stream);
 int b200rt_device_sync(int gpu);
-int b200rt_wave_capacity_items(void); /* items of 512 tokens one replica takes per wave */
+int b200rt_wave_capacity_items(void); /* items of 512 tokens one replica takes per wave (bge-base, bge-small) */
+/* items of 512 tokens one replica takes per wave of this model: b200rt_wave_capacity_items() for bge-base and bge-small,
+ * 3/4 of it for bge-large (the rows of a 1024-wide model that the workspace holds, rounded down to 128: 99 on an H100 SXM);
+ * images per wave for kind "vit".                                                                                         */
+int b200rt_model_wave_capacity_items(int model);
 
 void* b200rt_alloc_pinned(size_t nbytes);
 void b200rt_free_pinned(void* p);

@@ -16,7 +16,8 @@ extern "C" {
  * out is uint16 [M,N] for epi 0/1/3 and float [M,N] for epi 2.  ms_out (optional): device time of `iters` back-to-back
  * launches divided by iters.
  * LayerNorm in the epilogue (optional; all NULL = none): ln_stats = [M][parts] (sum, M2) float pairs, one per 128 columns
- * of the LayerNorm'd row (parts = K/128 for epi 0/1/3, N/128 for epi 2; that width must be 768 or 384).
+ * of the LayerNorm'd row (parts = K/128 for epi 0/1/3, N/128 for epi 2; that width must be 768 or 384, or 1024 for epi 0/1/2
+ * with N % 256 == 0).
  *   epi 0/1/3: `a` is the PRE-LayerNorm row in fp16, `w` = fp16(gamma o W with every row centred: sum_k w[n,k] = 0),
  *            bias = W beta + b:  out = epi(rstd * acc + bias)
  *   epi 2  : out = acc + bias + ((resid - mean) * rstd * ln_gamma + ln_beta) (ln_stats NULL: acc + bias + resid);
@@ -29,15 +30,15 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
                       void* out, int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
                       const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out);
 
-/* ctx[B*S,H] (fp16 bits) = multi-head attention of 12 heads of head_dim over qkv[B*S,3H] (fp16 bits), lens[B],
- * H = 12 head_dim; head_dim 64 or 32 (0 = 64).  sms as for b200rt_debug_gemm (it also decides whether units are split
- * by query tile).                                                                                                    */
+/* ctx[B*S,H] (fp16 bits) = multi-head attention of `heads` heads of head_dim over qkv[B*S,3H] (fp16 bits), lens[B],
+ * H = heads head_dim; (head_dim, heads) is (64, 12), (32, 12) or (64, 16), 0 meaning 64 and 12.  sms as for
+ * b200rt_debug_gemm (it also decides whether units are split by query tile).                                        */
 int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters,
-                           float* ms_out, int sms, int head_dim);
+                           float* ms_out, int sms, int head_dim, int heads);
 
 /* Row kernels, one launch each behind host buffers.  hi/lo: fp16 bit patterns [rows, W]; stats: [rows][W/128] (sum, M2)
  * float pairs, one per 128-column slice, M2 about the slice's own mean.  W = 768, except for embed and pool_normalize,
- * whose trailing `hidden` sets it: 768 or 384 (0 = 768).
+ * whose trailing `hidden` sets it: 768, 384 or 1024 (0 = 768).
  *   embed:          x = (word[ids[t]] + type0) + pos[t % S] -> hi = fp16(x), lo = fp16(x - hi), stats of x.
  *                   word [vocab, W], pos [S, W], type0 [W].
  *   vit_embed:      x = pre_layrnorm((t % T == 0 ? cls : patch_out[t]) + pos[t % T]) -> hi, lo, stats of x.
@@ -66,7 +67,8 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
  * n_launches launches of the forward of this batch run exactly as the product enqueues them (same kernels, buffers and stream,
  * no sync or copy between them), and the workspace is copied out once they finish.  n_launches is in [0, n_total], n_total =
  * 5 layers + 2 (text: embed, 5 per layer, pool_normalize -- mean_pool_normalize for a B200RT_LOAD_POOL_MEAN model) or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer,
- * vit_pool).  Every buffer comes back for rows = min(M + 256, 512 b200rt_wave_capacity_items()) rows, M = n_items * max_len
+ * vit_pool).  Every buffer comes back for rows = min(M + 256, R) rows, R = b200rt_debug_model_cap_rows(model) (512
+ * b200rt_wave_capacity_items(), or 3/4 of that rounded down to 128 for bge-large), M = n_items * max_len
  * (text) or n_items * tokens (vit), at the model's widths (H = hidden, I = inter, P = H / 128):
  *   yhi, ylo, ctx: fp16 bits [rows, H]; qkv: fp16 bits [rows, 3H]; ffn: fp16 bits [rows, I] (vit: the im2col matrix
  *   [M, 3 p p] is its start until FFN1 overwrites it); pstats0, pstats1: (sum, M2) float pairs [rows, P];
@@ -79,6 +81,11 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
 int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
                                    float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx, uint16_t* ffn, float* out,
                                    char* names_out, size_t names_cap, int* n_total);
+
+/* Rows of this model that one replica's workspace holds, the bound of its waves and of a trace: 512
+ * b200rt_wave_capacity_items() for bge-base, bge-small and vit; cap_rows * 768 / hidden rounded down to 128 for a wider
+ * model (bge-large: 3/4).                                                                                            */
+int b200rt_debug_model_cap_rows(int model);
 
 /* Per-kernel device times (ms, CUDA events on the compute stream) of one forward of a resident batch:
  * names_out receives up to cap NUL-terminated names packed in a char buffer, ms_out the times.        */

@@ -25,13 +25,13 @@ E_INVALID, E_STATE, E_CUDA, E_NOMEM, E_UNSUPPORTED = -1, -2, -3, -4, -5
 # every symbol include/b200rt.h and include/b200rt_debug.h declare (tests check the export list)
 ABI_SYMBOLS = [
     "b200rt_init", "b200rt_init_devices", "b200rt_num_gpus", "b200rt_model_load", "b200rt_model_load_ex", "b200rt_submit", "b200rt_submit_ex", "b200rt_submit_pixels", "b200rt_wait",
-    "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items",
+    "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items", "b200rt_model_wave_capacity_items",
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
 DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_profile_forward",
                  "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_mean_pool_normalize",
                  "b200rt_debug_vit_pool", "b200rt_debug_fold_ln",
-                 "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace"]
+                 "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace", "b200rt_debug_model_cap_rows"]
 
 
 def SPLIT_SMS(k: int) -> int:
@@ -94,6 +94,8 @@ def load_library():
         lib.b200rt_poll_any.argtypes = [u64p, ctypes.c_int]
         lib.b200rt_embed_device.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
         lib.b200rt_device_sync.argtypes = [ctypes.c_int]
+        lib.b200rt_model_wave_capacity_items.argtypes = [ctypes.c_int]
+        lib.b200rt_debug_model_cap_rows.argtypes = [ctypes.c_int]
         lib.b200rt_alloc_pinned.argtypes = [ctypes.c_size_t]
         lib.b200rt_alloc_pinned.restype = ctypes.c_void_p
         lib.b200rt_free_pinned.argtypes = [ctypes.c_void_p]
@@ -106,7 +108,7 @@ def load_library():
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_int,
                                           ctypes.POINTER(ctypes.c_int)]
         lib.b200rt_debug_attention.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p,
-                                               ctypes.c_int, ctypes.c_int]
+                                               ctypes.c_int, ctypes.c_int, ctypes.c_int]
         vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
         lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp, ci]
         lib.b200rt_debug_vit_embed.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, vp, vp]
@@ -166,6 +168,7 @@ def num_gpus() -> int:
 
 
 def wave_capacity_items() -> int:
+    """Items of 512 tokens one replica takes per wave of a bge-base or bge-small model (see EmbedModel.wave_capacity_items)."""
     return _check(load_library().b200rt_wave_capacity_items())
 
 
@@ -307,6 +310,16 @@ class EmbedModel:
         lend = isinstance(ids, np.ndarray) and ids.dtype == np.int32 and ids.flags.c_contiguous
         return self.wait(self.submit(ids, lens, borrow_ids=lend))
 
+    def wave_capacity_items(self) -> int:
+        """Items of 512 tokens one replica takes per wave of this model: :func:`wave_capacity_items` for bge-base and
+        bge-small, 3/4 of it for bge-large (99 on an H100 SXM), whose 1024-wide rows fill the same workspace sooner."""
+        return _check(self._lib.b200rt_model_wave_capacity_items(self.handle))
+
+    def debug_cap_rows(self) -> int:
+        """Rows of this model one replica's workspace holds, as the engine records them (b200rt_debug_model_cap_rows): 512
+        :func:`wave_capacity_items` for bge-base and bge-small, 3/4 of that rounded down to 128 for bge-large."""
+        return _check(self._lib.b200rt_debug_model_cap_rows(self.handle))
+
     def embed_device(self, gpu: int, d_ids: int, d_lens: int, n_items: int, max_len: int, d_out: int, stream: int = 0):
         """Device-resident forward (raw device addresses); asynchronous on ``stream``."""
         _check(self._lib.b200rt_embed_device(self.handle, gpu, d_ids, d_lens, n_items, max_len, d_out, stream or None))
@@ -319,7 +332,7 @@ class EmbedModel:
         lens_a = np.ascontiguousarray(lens, dtype=np.int32) if lens is not None else None
         return _debug_trace(lambda *bufs: self._lib.b200rt_debug_forward_trace(
             self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_launches, *bufs),
-            n * S, n, self.hidden, self.inter, self.hidden, n_launches)
+            n * S, n, self.hidden, self.inter, self.hidden, n_launches, self.debug_cap_rows())
 
     def debug_residual(self, ids: np.ndarray, lens, n_layers: int) -> np.ndarray:
         """The residual stream after ``n_layers`` encoder layers (0: the embedding sum), pre-LayerNorm as the forward carries
@@ -393,12 +406,14 @@ class ImageEmbedModel:
 _TRACE_NAMES_CAP = 8192
 
 
-def _debug_trace(call, M: int, n_items: int, H: int, I: int, out_dim: int, n_launches: int) -> dict:
+def _debug_trace(call, M: int, n_items: int, H: int, I: int, out_dim: int, n_launches: int, cap_rows: int | None = None) -> dict:
     """One b200rt_debug_*forward_trace call (include/b200rt_debug.h).  Returns the workspace, each buffer for
-    ``rows = min(M + 256, capacity)`` rows: yhi, ylo, ctx float16 [rows, H]; qkv float16 [rows, 3H]; ffn float16 [rows, I];
+    ``rows = min(M + 256, cap_rows)`` rows (cap_rows: the model's workspace rows as the engine reports them; by default the
+    runtime's):
+    yhi, ylo, ctx float16 [rows, H]; qkv float16 [rows, 3H]; ffn float16 [rows, I];
     pstats0, pstats1 float32 [rows, H / 128, 2]; ``out`` [n_items, out_dim] once the pool launch has run (else None);
     ``names`` of the launches run, ``n_total`` launches in the whole forward, ``M`` and ``rows``."""
-    rows = min(M + 256, wave_capacity_items() * 512)
+    rows = min(M + 256, cap_rows if cap_rows is not None else wave_capacity_items() * 512)
     P = H // 128
     bufs = dict(yhi=np.empty((rows, H), np.float16), ylo=np.empty((rows, H), np.float16),
                 pstats0=np.empty((rows, P, 2), np.float32), pstats1=np.empty((rows, P, 2), np.float32),
@@ -447,21 +462,23 @@ def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, res
     return res + (ctas.value,) if want_ctas else res
 
 
-def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0, head_dim: int = 64):
-    """qkv16 [B*S, 3H] float16 with H = 12 head_dim (head_dim 64: bge-base, 32: bge-small); returns (ctx [B*S, H], ms)."""
-    H = 12 * head_dim
+def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0, head_dim: int = 64,
+                    heads: int = 12):
+    """qkv16 [B*S, 3H] float16 with H = heads head_dim ((64, 12): bge-base, (32, 12): bge-small, (64, 16): bge-large);
+    returns (ctx [B*S, H], ms)."""
+    H = heads * head_dim
     qkv16 = np.ascontiguousarray(qkv16, dtype=np.float16)
     if qkv16.size != B * S * 3 * H:
-        raise B200RTError(E_INVALID, f"qkv must be [{B * S}, {3 * H}] for head_dim {head_dim}, got shape {qkv16.shape}")
+        raise B200RTError(E_INVALID, f"qkv must be [{B * S}, {3 * H}] for {heads} heads of {head_dim}, got shape {qkv16.shape}")
     lens = np.ascontiguousarray(lens, dtype=np.int32)
     ctx = np.empty((B * S, H), np.float16)
     ms = ctypes.c_float(0)
-    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms, head_dim))
+    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms, head_dim, heads))
     return ctx, ms.value
 
 
 # Row kernels behind host buffers (include/b200rt_debug.h).  hi / lo are float16 arrays [rows, W]; stats [rows, W / 128, 2];
-# W = 768, or ``hidden`` (768 or 384) where a wrapper takes it.
+# W = 768, or ``hidden`` (768, 384 or 1024) where a wrapper takes it.
 def _f32(v):
     return np.ascontiguousarray(v, dtype=np.float32)
 

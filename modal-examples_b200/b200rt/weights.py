@@ -23,6 +23,8 @@ BGE_BASE_GEOMETRY = dict(vocab=30522, hidden=768, layers=12, heads=12, inter=307
 BGE_SMALL_GEOMETRY = dict(vocab=30522, hidden=384, layers=12, heads=12, inter=1536, max_pos=512, type_vocab=2, eps=1e-12)
 # sentence-transformers/all-MiniLM-L6-v2: bge-small's geometry with 6 layers; mean-pooled (see pooling_from_dir)
 MINILM_L6_GEOMETRY = dict(vocab=30522, hidden=384, layers=6, heads=12, inter=1536, max_pos=512, type_vocab=2, eps=1e-12)
+# BAAI/bge-large-en-v1.5 (BERT-large): 16 heads of 64, 24 layers; also the shape of e5-large-v2, gte-large, mxbai-embed-large-v1
+BGE_LARGE_GEOMETRY = dict(vocab=30522, hidden=1024, layers=24, heads=16, inter=4096, max_pos=512, type_vocab=2, eps=1e-12)
 
 _ST_POOLING_MODULE = "sentence_transformers.models.Pooling"
 _ST_POOLING_MODES = ("pooling_mode_cls_token", "pooling_mode_mean_tokens", "pooling_mode_max_tokens",

@@ -1,5 +1,6 @@
-// Multi-head self-attention for S <= 512, 12 heads of d = 64 (bge-base) or d = 32 (bge-small), on wgmma (sm_90a):
-// persistent CTAs.  The kernel is a template on d; the comments below give the d = 64 figures, d = 32 differences follow.
+// Multi-head self-attention for S <= 512, NH heads of d: 12 of 64 (bge-base), 12 of 32 (bge-small) or 16 of 64 (bge-large),
+// on wgmma (sm_90a): persistent CTAs.  The kernel is a template on (d, NH); the comments below give the d = 64 figures, d = 32
+// differences follow.  NH only sets the unit decode and the column offsets of K and V.
 //
 // A work unit is one (item, head) -- or, for batches with fewer units than SMs, one (item, head, query tile).  Each CTA walks
 // the units u = blockIdx.x, blockIdx.x + gridDim.x, ...  For the unit in hand one thread TMA-loads the head's K and V
@@ -66,6 +67,7 @@ struct Unit {
     int len, nsb, nkb; // valid keys, 64-key sub-blocks, 128-key K/V tiles
 };
 
+template <int NH>
 __device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const int32_t* __restrict__ lens, int S) {
     Unit U;
     int unit = u;
@@ -74,8 +76,8 @@ __device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const 
         U.t0 = unit % nq_all;
         unit /= nq_all;
     }
-    U.b = unit / HEADS;
-    U.h = unit % HEADS;
+    U.b = unit / NH;
+    U.h = unit % NH;
     int len = __ldg(lens + U.b);
     len = len < 1 ? 1 : (len > S ? S : len);
     U.len = len;
@@ -85,13 +87,13 @@ __device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const 
     return U;
 }
 
-template <int D>
+template <int D, int NH>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tctx,
                  const int32_t* __restrict__ lens, int S, int split, int n_units) {
     using L = Layout<D>;
     constexpr int RB = L::RB, TILE_BYTES = L::TILE_BYTES, OFF_Q = L::OFF_Q, OFF_K = L::OFF_K, OFF_V = L::OFF_V, OFF_BAR = L::OFF_BAR;
-    constexpr int HID = HEADS * D;     // ctx width; qkv rows are 3 HID wide (Q | K | V)
+    constexpr int HID = NH * D;        // ctx width; qkv rows are 3 HID wide (Q | K | V)
     constexpr int NO = D / 2;          // O accumulators per thread
     constexpr float kScaleLog2e = scale_log2e<D>();
     extern __shared__ uint8_t smem_raw[];
@@ -124,7 +126,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
     uint32_t kv_par = 0;                 // bit j: parity of the number of loads of K/V tile j so far
     uint32_t gt = 0;                     // the CTA's running query-tile index
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        const Unit U = decode_unit(u, nq_all, split, lens, S);
+        const Unit U = decode_unit<NH>(u, nq_all, split, lens, S);
         auto load_q = [&](uint32_t g, int t) {
             mbar_arrive_expect_tx(&q_full[g & 1], TILE_BYTES);
             tma_load_3d(smem + OFF_Q + (g & 1) * TILE_BYTES, &tq, &q_full[g & 1], U.h * D, (U.t0 + t) * QT, U.b);
@@ -239,26 +241,38 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
 
 }  // namespace attn
 
+template <int D, int NH>
+static cudaError_t setup() {
+    return cudaFuncSetAttribute(attn::attention_kernel<D, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<D>::SMEM_BYTES);
+}
+
+template <int D, int NH>
+static cudaError_t launch_one(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
+                              cudaStream_t stream) {
+    // fewer (item, head) units than SMs: split them by query tile (K and V are then loaded once per tile, but a single item
+    // spreads over 4 NH SMs instead of NH)
+    const int nq = (S + attn::QT - 1) / attn::QT;
+    const int split = (B * NH < sm_count && nq > 1) ? 1 : 0;
+    const int n_units = B * NH * (split ? nq : 1);
+    const int grid = n_units < sm_count ? n_units : sm_count;
+    return launch_pdl(attn::attention_kernel<D, NH>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<D>::SMEM_BYTES, stream, tq, tctx, lens,
+                      S, split, n_units);
+}
+
 cudaError_t attention_init_device() {
-    cudaError_t e = cudaFuncSetAttribute(attn::attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<64>::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(attn::attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<32>::SMEM_BYTES);
+    cudaError_t e;
+    if ((e = setup<64, 12>()) != cudaSuccess) return e;
+    if ((e = setup<32, 12>()) != cudaSuccess) return e;
+    return setup<64, 16>();
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                             cudaStream_t stream, int head_dim) {
-    if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1 || (head_dim != 64 && head_dim != 32)) return cudaErrorInvalidValue;
-    // fewer (item, head) units than SMs: split them by query tile (K and V are then loaded once per tile, but a single item
-    // spreads over 48 SMs instead of 12)
-    const int nq = (S + attn::QT - 1) / attn::QT;
-    const int split = (B * HEADS < sm_count && nq > 1) ? 1 : 0;
-    const int n_units = B * HEADS * (split ? nq : 1);
-    const int grid = n_units < sm_count ? n_units : sm_count;
-    if (head_dim == 64)
-        return launch_pdl(attn::attention_kernel<64>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<64>::SMEM_BYTES, stream, tq, tctx, lens, S,
-                          split, n_units);
-    return launch_pdl(attn::attention_kernel<32>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<32>::SMEM_BYTES, stream, tq, tctx, lens, S,
-                      split, n_units);
+                             cudaStream_t stream, int head_dim, int heads) {
+    if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1) return cudaErrorInvalidValue;
+    if (head_dim == 64 && heads == 12) return launch_one<64, 12>(tq, tctx, lens, B, S, sm_count, stream);
+    if (head_dim == 32 && heads == 12) return launch_one<32, 12>(tq, tctx, lens, B, S, sm_count, stream);
+    if (head_dim == 64 && heads == 16) return launch_one<64, 16>(tq, tctx, lens, B, S, sm_count, stream);
+    return cudaErrorInvalidValue;
 }
 
 }  // namespace b200

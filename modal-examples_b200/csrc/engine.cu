@@ -121,12 +121,27 @@ constexpr int MIN_ITEMS_PER_REPLICA = 8;  // a wave uses fewer replicas rather t
 constexpr int MAX_SEQ = 512;
 constexpr int VIT_WAVE_ITEMS = 64;  // images one replica takes per wave (64 x 197 tokens; 38.5 MB of pixels per wave slot)
 
-// The text geometries the kernels cover (hidden, heads, inter): bge-base and bge-small.  The ViT tower is bge-base-wide.
+// The text geometries the kernels cover (hidden, heads, inter): bge-base, bge-small and bge-large.  The ViT tower is
+// bge-base-wide.
 struct TextGeometry {
     int hidden, heads, inter;
 };
-constexpr TextGeometry TEXT_GEOMETRIES[2] = {{768, 12, 3072}, {384, 12, 1536}};
-inline int geometry_index(int hidden) { return hidden == 768 ? 0 : 1; }
+constexpr int N_TEXT_GEOMETRIES = 3;
+constexpr TextGeometry TEXT_GEOMETRIES[N_TEXT_GEOMETRIES] = {{768, 12, 3072}, {384, 12, 1536}, {1024, 16, 4096}};
+// index into TEXT_GEOMETRIES of the geometry `hidden` wide (-1: none); the hidden widths are distinct
+inline int text_geometry(int hidden) {
+    for (int g = 0; g < N_TEXT_GEOMETRIES; ++g)
+        if (TEXT_GEOMETRIES[g].hidden == hidden) return g;
+    return -1;
+}
+// Rows of a `hidden`-wide model that the workspace holds: the buffers are sized for bge-base (HIDDEN, QKV_DIM, 3072,
+// STAT_PARTS) at the runtime's cap_rows, so a wider model gets cap_rows * 768 / hidden rows, rounded down to a multiple of
+// 128 (bge-large: 3/4).  Every width of bge-large is 4/3 of bge-base's, so each of its buffers is then full; bge-base and
+// bge-small keep cap_rows.
+inline int model_cap_rows(int rt_cap_rows, int hidden) {
+    const int64_t r = static_cast<int64_t>(rt_cap_rows) * HIDDEN / hidden;
+    return r >= rt_cap_rows ? rt_cap_rows : static_cast<int>(r / 128 * 128);
+}
 
 struct LayerW {
     __half *qkv_w, *ao_w, *ff1_w, *ff2_w;
@@ -158,6 +173,7 @@ struct Model {
     b200rt_bert_config cfg{};
     b200rt_vit_config vcfg{};
     int hidden = 0, inter = 0, heads = 0, layers = 0;  // encoder geometry, from whichever config the kind has
+    int cap_rows = 0;        // rows of this model one replica's workspace holds (model_cap_rows): bounds every wave of it
     float eps = 0.f;
     int tokens = 0;          // vit: (image / patch)^2 + 1
     int out_dim = HIDDEN;    // floats per item in the result
@@ -175,11 +191,11 @@ struct Dev {
     __half *yhi = nullptr, *ylo = nullptr;  // residual stream y = hi + lo, PRE-LayerNorm; hi doubles as the GEMM A operand
     float2* pstats[2] = {nullptr, nullptr};  // [rows][STAT_PARTS] (sum, M2) partials: [0] embedding LN / LN2 inputs, [1] LN1 inputs
     __half *qkv = nullptr, *ctx = nullptr, *ffn = nullptr;
-    // fp16 [rows, *] box {64,128}: GEMM A operands, per TEXT_GEOMETRIES entry (a narrower model reads the same buffers densely
-    // at its own widths)
+    // fp16 [rows, *] box {64,128}: GEMM A operands, per TEXT_GEOMETRIES entry, each over that geometry's model_cap_rows rows
+    // (a model reads the same buffers densely at its own widths)
     struct ActMaps {
         CUtensorMap yhi, ctx, ffn;
-    } act[2];
+    } act[N_TEXT_GEOMETRIES];
     std::map<std::pair<int, int>, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per (padded length, hidden)
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
     int32_t* ids_in[NSLOT] = {};
@@ -330,13 +346,14 @@ struct LaunchHook {
     }
 };
 
-int get_qkv_map(Dev& d, int S, int hidden, const CUtensorMap** out, const CUtensorMap** out_ctx) {
+int get_qkv_map(Dev& d, const Model& model, int S, const CUtensorMap** out, const CUtensorMap** out_ctx) {
+    const int hidden = model.hidden;
     const auto key = std::make_pair(S, hidden);
     auto it = d.m_qkv_by_S.find(key);
     if (it == d.m_qkv_by_S.end()) {
         CUtensorMap m, mc;
-        const uint64_t B = static_cast<uint64_t>(g_rt->cap_rows) / S;
-        const uint32_t head_dim = hidden / HEADS;
+        const uint64_t B = static_cast<uint64_t>(model.cap_rows) / S;  // the maps end inside the allocations at any width
+        const uint32_t head_dim = hidden / model.heads;
         int rc = make_map_qkv(&m, d.qkv, B, S, 3 * hidden, head_dim);
         if (rc) return rc;
         rc = make_map_qkv(&mc, d.ctx, B, S, hidden, head_dim);
@@ -358,12 +375,12 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
     const DevWeights& w = m.per_dev[dev_index];
     const bool vit = m.kind == KIND_VIT;
     const int B = in.B, S = in.S, M = B * S;
-    if (M > g_rt->cap_rows || (vit && B > VIT_WAVE_ITEMS))
-        return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the wave capacity (%d rows)", B, S, g_rt->cap_rows);
+    if (M > m.cap_rows || (vit && B > VIT_WAVE_ITEMS))
+        return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the model's wave capacity (%d rows)", B, S, m.cap_rows);
     const int H = m.hidden, I = m.inter, P = H / 128;
-    const Dev::ActMaps& am = d.act[geometry_index(H)];
+    const Dev::ActMaps& am = d.act[text_geometry(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
-    if (int rc = get_qkv_map(d, S, H, &mq, &mc)) return rc;
+    if (int rc = get_qkv_map(d, m, S, &mq, &mc)) return rc;
     const int32_t* lens = vit ? d.lens_const : in.lens;
     // residual epilogue: y <- acc + bias + LN(y), LN given by (stats, gamma, beta) -- or + y (pre-LN); new statistics to stats_out
     auto residual = [&](const float* bias, const float2* stats, const float* gamma, const float* beta, float2* stats_out) {
@@ -399,7 +416,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
             CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
             if (step("gemm_qkv")) return 0;
-            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads));
+            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads));
             if (step("attention")) return 0;
             // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
             const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
@@ -485,7 +502,7 @@ int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, 
                 cache.entries.erase(victim);
             }
             const CUtensorMap *mq = nullptr, *mc = nullptr;
-            if (int rc = get_qkv_map(d, in.S, m.hidden, &mq, &mc)) return rc;  // host-side map creation happens outside the capture
+            if (int rc = get_qkv_map(d, m, in.S, &mq, &mc)) return rc;  // host-side map creation happens outside the capture
             uint64_t nl = 0;
             CUDA_TRY(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
             const int rc = forward_enqueue(d, m, dev_index, in, out, stream, nl, nullptr);
@@ -595,7 +612,7 @@ void dispatcher_main(Runtime* rtp) {
             {
                 const int S0 = rt.pending.front().bucket;
                 const Model* m0 = rt.pending.front().t->mp;
-                const int cap0 = (m0->kind == KIND_VIT ? VIT_WAVE_ITEMS : rt.cap_rows / S0) * G;
+                const int cap0 = (m0->kind == KIND_VIT ? VIT_WAVE_ITEMS : m0->cap_rows / S0) * G;
                 auto queued = [&] {
                     int n = 0;
                     for (auto& r : rt.pending)
@@ -621,8 +638,8 @@ void dispatcher_main(Runtime* rtp) {
             wv.S = rt.pending.front().bucket;
             wv.n_items = 0;
             const Model* model = rt.pending.front().t->mp;
-            // token capacity scales with 512/S: a wave holds cap_rows tokens per replica
-            const int cap_items_S = (model->kind == KIND_VIT ? VIT_WAVE_ITEMS : rt.cap_rows / wv.S) * G;
+            // token capacity scales with 512/S: a wave holds the model's cap_rows tokens per replica
+            const int cap_items_S = (model->kind == KIND_VIT ? VIT_WAVE_ITEMS : model->cap_rows / wv.S) * G;
             for (auto it = rt.pending.begin(); it != rt.pending.end() && wv.n_items < cap_items_S;) {
                 if (it->bucket != wv.S || it->t->mp != model) {
                     ++it;
@@ -953,11 +970,13 @@ int alloc_dev(Runtime& rt, Dev& d) {
     CUDA_TRY(cudaMemset(d.qkv, 0, R * QKV_DIM * 2));
     CUDA_TRY(cudaMemset(d.ctx, 0, R * HIDDEN * 2));
     CUDA_TRY(cudaMemset(d.ffn, 0, R * 3072 * 2));
-    for (int g = 0; g < 2; ++g) {
+    for (int g = 0; g < N_TEXT_GEOMETRIES; ++g) {
         const TextGeometry& tg = TEXT_GEOMETRIES[g];
-        if (int rc = make_map_2d(&d.act[g].yhi, d.yhi, R, tg.hidden, 128)) return rc;
-        if (int rc = make_map_2d(&d.act[g].ctx, d.ctx, R, tg.hidden, 128)) return rc;
-        if (int rc = make_map_2d(&d.act[g].ffn, d.ffn, R, tg.inter, 128)) return rc;
+        const size_t rows = model_cap_rows(rt.cap_rows, tg.hidden);
+        if (rows < 128) continue;  // no model of this width can be loaded (model_load refuses it)
+        if (int rc = make_map_2d(&d.act[g].yhi, d.yhi, rows, tg.hidden, 128)) return rc;
+        if (int rc = make_map_2d(&d.act[g].ctx, d.ctx, rows, tg.hidden, 128)) return rc;
+        if (int rc = make_map_2d(&d.act[g].ffn, d.ffn, rows, tg.inter, 128)) return rc;
     }
     for (int s = 0; s < NSLOT; ++s) {
         CUDA_TRY(cudaMalloc(&d.ids_in[s], R * 4));
@@ -1058,8 +1077,14 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
     for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
     if (!known || c.max_pos > MAX_SEQ || c.max_pos < 1 || c.layers < 1 || c.vocab < 1 || c.type_vocab < 1)
         return fail(B200RT_E_UNSUPPORTED,
-                    "kernels cover two geometries, bge-base (hidden=768 heads=12 inter=3072) and bge-small (hidden=384 heads=12 "
-                    "inter=1536), with max_pos<=512 (got hidden %d heads %d inter %d max_pos %d)", c.hidden, c.heads, c.inter, c.max_pos);
+                    "kernels cover three geometries, bge-base (hidden=768 heads=12 inter=3072), bge-small (hidden=384 heads=12 "
+                    "inter=1536) and bge-large (hidden=1024 heads=16 inter=4096), with max_pos<=512 (got hidden %d heads %d inter %d "
+                    "max_pos %d)", c.hidden, c.heads, c.inter, c.max_pos);
+    const int cap_rows = model_cap_rows(rt.cap_rows, c.hidden);
+    if (cap_rows < MAX_SEQ)
+        return fail(B200RT_E_INVALID,
+                    "a hidden=%d model needs room for one %d-token item, and the workspace holds %d of its rows: initialise with a "
+                    "larger B200RT_INIT_WAVE_ITEMS (now %d)", c.hidden, MAX_SEQ, cap_rows, rt.cap_items);
     const size_t H = c.hidden, I = c.inter;
     const size_t emb = (static_cast<size_t>(c.vocab) + c.max_pos + c.type_vocab) * H + 2 * H;
     const size_t per_layer_w = 3 * H * H + H * H + I * H + H * I;
@@ -1071,6 +1096,7 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
     m->cfg = c;
     m->pool_mean = pool_mean;
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
+    m->cap_rows = cap_rows;
     m->out_dim = c.hidden;
     const size_t per_layer_x = 3 * H + I;  // derived vectors: qkv_c, ff1_c
     const size_t blob_f32 = emb + static_cast<size_t>(c.layers) * per_layer_p;
@@ -1190,6 +1216,7 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
     m->kind = KIND_VIT;
     m->vcfg = c;
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
+    m->cap_rows = rt.cap_rows;
     m->tokens = T;
     m->out_dim = c.proj;
     m->item_bytes = static_cast<size_t>(3) * c.image * c.image * 4;
@@ -1396,10 +1423,10 @@ struct TraceOut {
 
 // Runs the first n_launches launches of the forward of `in` on replica d (the caller holds d.mu): every workspace buffer and
 // the pooled output are set to 0xFF bytes (NaN in fp16 and fp32) behind the previous forward, the launches run on d.compute
-// through forward(), and once the stream has drained, rows = min(M + 256, workspace rows) rows of every buffer, at the
+// through forward(), and once the stream has drained, rows = min(M + 256, the model's cap_rows) rows of every buffer, at the
 // model's widths (the buffers are used densely at those widths), and the pooled output are copied out.
 int trace_forward(DebugBuffers& b, Dev& d, const Model& m, const Input& in, int n_launches, const TraceOut& o) {
-    const size_t R = g_rt->cap_rows, rows = std::min(static_cast<size_t>(in.B) * in.S + 256, R);
+    const size_t R = g_rt->cap_rows, rows = std::min(static_cast<size_t>(in.B) * in.S + 256, static_cast<size_t>(m.cap_rows));
     const size_t H = m.hidden, I = m.inter, P = H / 128, out_floats = static_cast<size_t>(in.B) * m.out_dim;
     float* dout = nullptr;
     CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
@@ -1453,6 +1480,14 @@ int b200rt_num_gpus(void) {
 int b200rt_wave_capacity_items(void) {
     Runtime* rt = live_rt();
     return rt ? rt->cap_rows / MAX_SEQ : B200RT_E_STATE;
+}
+
+int b200rt_model_wave_capacity_items(int model) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    const Model* m = get_model(*rt, model);
+    if (!m) return B200RT_E_INVALID;
+    return m->kind == KIND_VIT ? VIT_WAVE_ITEMS : m->cap_rows / MAX_SEQ;
 }
 
 int b200rt_model_load(const char* kind, const void* cfg, const void* weights, size_t nbytes, int* model_out) {
@@ -1786,8 +1821,11 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!a || !w || !bias || !out || M < 1 || N % 128 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
     if (epi == 2 && !resid) return fail(B200RT_E_INVALID, "epi 2 needs resid");
-    if (ln_stats && (epi == 2 ? N : K) != 768 && (epi == 2 ? N : K) != 384)
-        return fail(B200RT_E_INVALID, "the LayerNorm'd width must be 768 or 384");
+    const int ln_w = epi == 2 ? N : K;
+    if (ln_stats && ln_w != 768 && ln_w != 384 && ln_w != 1024)
+        return fail(B200RT_E_INVALID, "the LayerNorm'd width must be 768, 384 or 1024");
+    if (ln_stats && ln_w == 1024 && (epi == 3 || N % 256 != 0))
+        return fail(B200RT_E_INVALID, "a 1024-wide LayerNorm needs epi 0, 1 or 2 and N %% 256 == 0");
     if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
     Dev& d = *rt->devs[0];
     if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
@@ -1866,13 +1904,15 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
 }
 
 int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms,
-                           int head_dim) {
+                           int head_dim, int heads) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!qkv || !lens || !ctx || B < 1 || S < 1 || S > MAX_SEQ) return fail(B200RT_E_INVALID, "bad attention arguments");
     if (head_dim == 0) head_dim = 64;
-    if (head_dim != 64 && head_dim != 32) return fail(B200RT_E_INVALID, "head_dim must be 64 or 32 (0 = 64), got %d", head_dim);
-    const size_t H = static_cast<size_t>(HEADS) * head_dim;
+    if (heads == 0) heads = HEADS;
+    if (!((head_dim == 64 && heads == 12) || (head_dim == 32 && heads == 12) || (head_dim == 64 && heads == 16)))
+        return fail(B200RT_E_INVALID, "(head_dim, heads) must be (64, 12), (32, 12) or (64, 16) (0 = 64, 12), got (%d, %d)", head_dim, heads);
+    const size_t H = static_cast<size_t>(heads) * head_dim;
     Dev& d = *rt->devs[0];
     if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
     const int grid_sms = sms ? sms : d.sm_count;
@@ -1893,9 +1933,9 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     CUDA_TRY(b.event(&e0));
     CUDA_TRY(b.event(&e1));
     if (iters < 1) iters = 1;
-    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim));
+    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads));
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim));
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads));
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
@@ -1912,7 +1952,8 @@ int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, 
     if (!ids || !word || !pos || !type0 || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1)
         return fail(B200RT_E_INVALID, "bad embed arguments");
     if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384) return fail(B200RT_E_INVALID, "row width must be 768 or 384 (0 = 768), got %d", hidden);
+    if (hidden != 768 && hidden != 384 && hidden != 1024)
+        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024 (0 = 768), got %d", hidden);
     const size_t H = hidden, P = H / 128;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
@@ -1972,7 +2013,8 @@ int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const fl
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!hi || !lo || !gamma || !beta || !out || n_items < 1 || S < 1) return fail(B200RT_E_INVALID, "bad pool_normalize arguments");
     if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384) return fail(B200RT_E_INVALID, "row width must be 768 or 384 (0 = 768), got %d", hidden);
+    if (hidden != 768 && hidden != 384 && hidden != 1024)
+        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024 (0 = 768), got %d", hidden);
     const size_t H = hidden;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
@@ -1998,7 +2040,8 @@ int b200rt_debug_mean_pool_normalize(const uint16_t* hi, const uint16_t* lo, con
     if (!hi || !lo || !gamma || !beta || !lens || !out || n_items < 1 || S < 1)
         return fail(B200RT_E_INVALID, "bad mean_pool_normalize arguments");
     if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384) return fail(B200RT_E_INVALID, "row width must be 768 or 384 (0 = 768), got %d", hidden);
+    if (hidden != 768 && hidden != 384 && hidden != 1024)
+        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024 (0 = 768), got %d", hidden);
     const size_t H = hidden;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
@@ -2083,7 +2126,7 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
     const size_t M = static_cast<size_t>(n_items) * max_len;
-    if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
+    if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
     if (n_total) *n_total = total;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
@@ -2120,6 +2163,14 @@ int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, 
     return trace_forward(b, d, *m, Input{nullptr, nullptr, dpix, n_items, m->tokens}, n_launches, o);
 }
 
+int b200rt_debug_model_cap_rows(int model) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    const Model* m = get_model(*rt, model);
+    if (!m) return B200RT_E_INVALID;
+    return m->cap_rows;
+}
+
 int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters, char* names_out, size_t names_cap,
                                  float* ms_out, int* n_out, int cap) {
     Runtime* rt = live_rt();
@@ -2129,7 +2180,7 @@ int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters,
     if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > m->cfg.max_pos) return fail(B200RT_E_INVALID, "bad argument");
     const size_t M = static_cast<size_t>(n_items) * max_len;
-    if (M > static_cast<size_t>(rt->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds wave capacity");
+    if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));

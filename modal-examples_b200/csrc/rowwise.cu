@@ -2,7 +2,7 @@
 // L2 normalise with the store aimed at the root GPU's gather buffer, the root-side scatter of token ids into (peer) shard
 // inputs, and the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns).
 //
-// Row kernels: one warp per row (768 wide, or 384 for bge-small's embed / pool / LayerNorm), 128-bit accesses, statistics
+// Row kernels: one warp per row (768 wide, or 384 / 1024 for bge-small's / bge-large's embed / pool / LayerNorm), 128-bit accesses, statistics
 // by warp shuffle in fp32, two-pass variance on register-resident data (no E[x^2]-E[x]^2 cancellation).
 //
 // The residual stream is stored PRE-LayerNorm as y = hi + lo (fp16 + fp16) together with one (sum, M2) partial per 128
@@ -22,8 +22,8 @@ namespace rw {
 constexpr int H = HIDDEN;  // 768
 template <int W>
 struct Row {
-    static_assert(W == 768 || W == 384, "row width");
-    static constexpr int V4 = W / 128;  // float4 per lane: 6 or 3
+    static_assert(W == 768 || W == 384 || W == 1024, "row width");
+    static constexpr int V4 = W / 128;  // float4 per lane: 6, 3 or 8
 };
 constexpr int V4 = Row<H>::V4;
 constexpr int WARPS_PER_BLOCK = 8;
@@ -393,6 +393,7 @@ cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos
     const int grid = (n_tokens + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
     if (width == 768) rw::embed_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
     else if (width == 384) rw::embed_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
+    else if (width == 1024) rw::embed_kernel<1024><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
@@ -402,6 +403,7 @@ cudaError_t launch_pool_normalize(const __half* yhi, const __half* ylo, const fl
     const int grid = (n_items + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
     if (width == 768) rw::pool_normalize_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
     else if (width == 384) rw::pool_normalize_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
+    else if (width == 1024) rw::pool_normalize_kernel<1024><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, out, n_items, S, eps);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
@@ -412,6 +414,7 @@ cudaError_t launch_mean_pool_normalize(const __half* yhi, const __half* ylo, con
     const int block = rw::WARPS_PER_BLOCK * 32;
     if (width == 768) rw::mean_pool_normalize_kernel<768><<<n_items, block, 0, stream>>>(yhi, ylo, gamma, beta, lens, out, S, eps);
     else if (width == 384) rw::mean_pool_normalize_kernel<384><<<n_items, block, 0, stream>>>(yhi, ylo, gamma, beta, lens, out, S, eps);
+    else if (width == 1024) rw::mean_pool_normalize_kernel<1024><<<n_items, block, 0, stream>>>(yhi, ylo, gamma, beta, lens, out, S, eps);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }

@@ -14,6 +14,7 @@ from http.server import BaseHTTPRequestHandler, ThreadingHTTPServer
 
 GEOMETRY = dict(vocab=30522, hidden=768, layers=12, heads=12, inter=3072, max_pos=512, type_vocab=2, eps=1e-12)
 BGE_SMALL_ID = "BAAI/bge-small-en-v1.5"
+BGE_LARGE_ID = "BAAI/bge-large-en-v1.5"
 
 
 MINILM_L6_ID = "sentence-transformers/all-MiniLM-L6-v2"
@@ -23,11 +24,13 @@ POOLINGS = ("cls", "mean")  # TEI also knows splade and last-token; this runtime
 
 def geometry_for_model_id(model_id: str) -> dict:
     """Geometry of the offline seeded fallback and of a raw --weights blob (which carries no shapes): bge-small's for
-    BAAI/bge-small-en-v1.5, MiniLM-L6's (bge-small's with 6 layers) for sentence-transformers/all-MiniLM-L6-v2, bge-base's
-    for BAAI/bge-base-en-v1.5 and for any id this table does not know."""
-    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY
+    BAAI/bge-small-en-v1.5, bge-large's for BAAI/bge-large-en-v1.5, MiniLM-L6's (bge-small's with 6 layers) for
+    sentence-transformers/all-MiniLM-L6-v2, bge-base's for BAAI/bge-base-en-v1.5 and for any id this table does not know.
+    A hub snapshot takes its geometry from its own config.json instead."""
+    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_LARGE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY
 
-    known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY, MINILM_L6_ID: MINILM_L6_GEOMETRY}
+    known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY, BGE_LARGE_ID: BGE_LARGE_GEOMETRY,
+             MINILM_L6_ID: MINILM_L6_GEOMETRY}
     return dict(known.get(model_id, BGE_BASE_GEOMETRY))
 
 

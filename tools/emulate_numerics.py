@@ -7,10 +7,11 @@ written as CUDA.
   mode "fold"   : y16 = fp16(y) (the raw pre-LayerNorm residual) feeds QKV / FFN1 with gamma folded into the weight columns;
                   and the weight rows centred; the epilogue applies rstd * acc + (W beta + b)   (round-2 design, no LN kernels)
 
-    python tools/emulate_numerics.py [--geometry base|small] [--style hf|trained|hard] [--layers 12] [--items 4] [--seq 512]
+    python tools/emulate_numerics.py [--geometry base|small|large] [--style hf|trained|hard] [--layers 12] [--items 4] [--seq 512]
                                      [--pooling cls|mean]
 
---geometry small: bge-small (hidden 384, 12 heads of 32, inter 1536) instead of bge-base.
+--geometry small: bge-small (hidden 384, 12 heads of 32, inter 1536) instead of bge-base; --geometry large: bge-large
+(hidden 1024, 16 heads of 64, inter 4096).
 --pooling mean: sentence-transformers' mean of the valid tokens' final hidden states (all-MiniLM-L6-v2, e5, gte) instead of
 the [CLS] row, against the fp64 oracle pooled the same way (tests/mean_pool_refs.py).
 """
@@ -27,7 +28,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import bge_ref as R  # noqa: E402
 import mean_pool_refs as MP  # noqa: E402
 
-GEOMETRIES = {"base": {}, "small": dict(hidden=384, heads=12, inter=1536)}
+GEOMETRIES = {"base": {}, "small": dict(hidden=384, heads=12, inter=1536), "large": dict(hidden=1024, heads=16, inter=4096)}
 
 f16 = lambda a: a.astype(np.float16).astype(np.float32)  # noqa: E731
 
@@ -98,7 +99,7 @@ def emulate(flat, ids, lens, g, mode="current", p_sum="exact", keep=(), pooling=
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--geometry", choices=("base", "small"), default="base")
+    ap.add_argument("--geometry", choices=tuple(GEOMETRIES), default="base")
     ap.add_argument("--style", default="hf")
     ap.add_argument("--layers", type=int, default=12)
     ap.add_argument("--items", type=int, default=4)
