@@ -24,7 +24,7 @@ extern "C" {
 #define B200RT_E_STATE (-2)     /* not initialised / already initialised / shut down */
 #define B200RT_E_CUDA (-3)      /* CUDA error; the context is poisoned and every later call fails fast */
 #define B200RT_E_NOMEM (-4)
-#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is none of bge-base, bge-small, bge-large */
+#define B200RT_E_UNSUPPORTED (-5) /* e.g. device is not sm_90, or geometry is none the kernels cover */
 
 /* Geometry of a BERT encoder (HF BertConfig fields).  The sm_90a kernels cover three geometries: bge-base (hidden 768,
  * 12 heads of 64, inter 3072), bge-small (hidden 384, 12 heads of 32, inter 1536) and bge-large (hidden 1024, 16 heads of
@@ -42,6 +42,18 @@ typedef struct b200rt_vit_config {
     int32_t image, patch, hidden, layers, heads, inter, proj;
     float eps;
 } b200rt_vit_config;
+
+/* Geometry of a CLIP text tower (HF CLIPTextConfig fields + projection_dim + eos_token_id): the text half of the CLIP model
+ * the reference's image example serves (image_embeddings_infinity.py:298-306, where infinity's `engine.embed(sentences=...)`
+ * runs it).  The kernels cover the tower of openai/clip-vit-base-patch16 (and -patch32): hidden 512, 8 heads of 64, inter
+ * 2048, max_pos <= 128 (77 in the checkpoint), proj <= 1024; `layers` and `vocab` are free.  Causal self-attention, pre-LN
+ * layers with quick-GELU MLPs; the pooled row of item i is chosen from its ids: eos_id == 2 (HF's legacy branch, the original
+ * openai configs) the first position of the largest id, otherwise the first position equal to eos_id (0 when there is none);
+ * then final_layer_norm, text_projection [proj, hidden] (no bias) and L2 normalisation.  Results are `proj` floats per item. */
+typedef struct b200rt_clip_text_config {
+    int32_t vocab, hidden, layers, heads, inter, max_pos, proj, eos_id;
+    float eps;
+} b200rt_clip_text_config;
 
 typedef struct b200rt_stats_t {
     uint64_t items, waves, tickets;     /* completed so far */
@@ -69,15 +81,20 @@ int b200rt_num_gpus(void);
 
 /* Cold start.  Stands in for `download_model` / `spawn_server` (text_embeddings_inference.py:37-56):
  * one host->root-GPU copy of the fp32 weight blob, fp16 conversion on the GPU, then a peer broadcast
- * over NVLink to the other replicas.  kind = "bert" (cfg: b200rt_bert_config; blob order: b200rt.weights.blob_layout) or
+ * over NVLink to the other replicas.  kind = "bert" (cfg: b200rt_bert_config; blob order: b200rt.weights.blob_layout),
  * "vit" (cfg: b200rt_vit_config; the CLIP ViT-B/16 image tower behind 06_gpu_and_ml/embeddings/image_embeddings_infinity.py:76-77;
- * blob order: b200rt.weights.vit_blob_layout).                                                         */
+ * blob order: b200rt.weights.vit_blob_layout) or "clip_text" (cfg: b200rt_clip_text_config; the same model's text tower, which
+ * infinity's `embed(sentences=...)` runs -- image_embeddings_infinity.py:298-306; blob order:
+ * b200rt.weights.clip_text_blob_layout).  A "clip_text" model takes token ids through b200rt_submit[_ex] (max_len <= max_pos,
+ * ids < vocab; items travel in the 64- or 128-token bucket) and b200rt_embed_device (max_len <= 128, the longest wave the
+ * scheduler forms for it: device-resident callers can run the bucket the scheduler would), and is refused by
+ * b200rt_submit_pixels.                                                                                              */
 int b200rt_model_load(const char* kind, const void* cfg, const void* weights, size_t nbytes, int* model_out);
 /* b200rt_model_load with load flags (b200rt_model_load is this with flags = 0).  B200RT_LOAD_POOL_MEAN (kind "bert" only):
  * pool each item as sentence-transformers' Pooling(mean) + Normalize does -- the mean over the item's lens[i] valid tokens
  * ([CLS] and [SEP] included) of the final hidden states, then L2 normalise -- instead of taking the [CLS] row; the pooling of
  * all-MiniLM-L6-v2, e5 and gte.  The forward before the pool, and its launch count, are the same either way.  With kind
- * "vit", or with any other flag bit set, returns B200RT_E_INVALID.                                                       */
+ * "vit" or "clip_text", or with any other flag bit set, returns B200RT_E_INVALID.                                                       */
 #define B200RT_LOAD_POOL_MEAN 1u
 int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out);
 

@@ -17,7 +17,7 @@ extern "C" {
  * launches divided by iters.
  * LayerNorm in the epilogue (optional; all NULL = none): ln_stats = [M][parts] (sum, M2) float pairs, one per 128 columns
  * of the LayerNorm'd row (parts = K/128 for epi 0/1/3, N/128 for epi 2; that width must be 768 or 384, or 1024 for epi 0/1/2
- * with N % 256 == 0).
+ * with N % 256 == 0; see b200rt_debug_gemm_ex for 512).
  *   epi 0/1/3: `a` is the PRE-LayerNorm row in fp16, `w` = fp16(gamma o W with every row centred: sum_k w[n,k] = 0),
  *            bias = W beta + b:  out = epi(rstd * acc + bias)
  *   epi 2  : out = acc + bias + ((resid - mean) * rstd * ln_gamma + ln_beta) (ln_stats NULL: acc + bias + resid);
@@ -29,16 +29,28 @@ extern "C" {
 int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid,
                       void* out, int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
                       const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out);
+/* b200rt_debug_gemm with flags (b200rt_debug_gemm is this with flags = 0).  B200RT_DEBUG_GEMM_LN512: the LayerNorm'd width may
+ * also be 512 -- the CLIP text tower's 4-partial epilogues, epi 0 or 3 with N % 256 == 0.                                  */
+#define B200RT_DEBUG_GEMM_LN512 1u
+int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid,
+                         void* out, int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
+                         const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out, uint32_t flags);
 
 /* ctx[B*S,H] (fp16 bits) = multi-head attention of `heads` heads of head_dim over qkv[B*S,3H] (fp16 bits), lens[B],
  * H = heads head_dim; (head_dim, heads) is (64, 12), (32, 12) or (64, 16), 0 meaning 64 and 12.  sms as for
  * b200rt_debug_gemm (it also decides whether units are split by query tile).                                        */
 int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters,
                            float* ms_out, int sms, int head_dim, int heads);
+/* b200rt_debug_attention with flags (b200rt_debug_attention is this with flags = 0).  B200RT_DEBUG_ATTN_CAUSAL: key k is also
+ * masked for query row q when k > q (the CLIP text tower's attention); (head_dim, heads) must then be (64, 8).          */
+#define B200RT_DEBUG_ATTN_CAUSAL 1u
+int b200rt_debug_attention_ex(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters,
+                              float* ms_out, int sms, int head_dim, int heads, uint32_t flags);
 
 /* Row kernels, one launch each behind host buffers.  hi/lo: fp16 bit patterns [rows, W]; stats: [rows][W/128] (sum, M2)
  * float pairs, one per 128-column slice, M2 about the slice's own mean.  W = 768, except for embed and pool_normalize,
- * whose trailing `hidden` sets it: 768, 384 or 1024 (0 = 768).
+ * whose trailing `hidden` sets it: 768, 384 or 1024 (0 = 768), for embed also 512 (the CLIP text tower, with a zero type0),
+ * and for clip_text_pool, which is 512 wide.
  *   embed:          x = (word[ids[t]] + type0) + pos[t % S] -> hi = fp16(x), lo = fp16(x - hi), stats of x.
  *                   word [vocab, W], pos [S, W], type0 [W].
  *   vit_embed:      x = pre_layrnorm((t % T == 0 ? cls : patch_out[t]) + pos[t % T]) -> hi, lo, stats of x.
@@ -48,6 +60,10 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
  *                   [n_items, W]; W from the trailing `hidden` as for pool_normalize.
  *   vit_pool:       out[i] = L2-normalise(proj . LayerNorm(hi + lo of row i * T)), proj fp32 [P, 768], 1 <= P <= 1024,
  *                   out fp32 [n_items, P].
+ *   clip_text_pool: out[i] = L2-normalise(proj . LayerNorm(hi + lo of row i * S + p_i)), p_i the pooled position of item i
+ *                   chosen from ids[i * S .. + L) (L = lens[i] clamped to [1, S] on the device; ids past L are never read):
+ *                   eos_id == 2, the first position of the largest id; otherwise the first position equal to eos_id, 0
+ *                   when there is none.  ids int32 [n_items * S], proj fp32 [P, 512], 1 <= P <= 1024, out fp32 [n_items, P].
  *   fold_ln:        w_out = fp16(w o gamma - rowmean(w o gamma)), cvec_out = w beta + bias (bias may be NULL);
  *                   gamma NULL: w_out = fp16(w) and cvec_out is not written.  w fp32 [N, K], K % 64 == 0.    */
 int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, int n_tokens, int S, int vocab,
@@ -60,14 +76,18 @@ int b200rt_debug_mean_pool_normalize(const uint16_t* hi, const uint16_t* lo, con
                                      int n_items, int S, float eps, float* out, int hidden);
 int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* proj, int n_items,
                           int T, int P, float eps, float* out);
+int b200rt_debug_clip_text_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* ids, const int32_t* lens, const float* gamma,
+                                const float* beta, const float* proj, int n_items, int S, int P, float eps, int eos_id, float* out);
 int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,
                          float* cvec_out);
 
 /* Trace of the product forward on replica 0: the workspace is set to 0xFF bytes (NaN in fp16 and fp32), then the first
  * n_launches launches of the forward of this batch run exactly as the product enqueues them (same kernels, buffers and stream,
  * no sync or copy between them), and the workspace is copied out once they finish.  n_launches is in [0, n_total], n_total =
- * 5 layers + 2 (text: embed, 5 per layer, pool_normalize -- mean_pool_normalize for a B200RT_LOAD_POOL_MEAN model) or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer,
- * vit_pool).  Every buffer comes back for rows = min(M + 256, R) rows, R = b200rt_debug_model_cap_rows(model) (512
+ * 5 layers + 2 (text: embed, 5 per layer, pool_normalize -- mean_pool_normalize for a B200RT_LOAD_POOL_MEAN model,
+ * clip_text_pool for kind "clip_text") or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer, vit_pool).
+ * max_len may be up to the longest wave the model runs (kind "clip_text": 128, its bucket for items of 65-77 tokens; the
+ * lengths stay <= max_pos), as for b200rt_debug_profile_forward.  Every buffer comes back for rows = min(M + 256, R) rows, R = b200rt_debug_model_cap_rows(model) (512
  * b200rt_wave_capacity_items(), or 3/4 of that rounded down to 128 for bge-large), M = n_items * max_len
  * (text) or n_items * tokens (vit), at the model's widths (H = hidden, I = inter, P = H / 128):
  *   yhi, ylo, ctx: fp16 bits [rows, H]; qkv: fp16 bits [rows, 3H]; ffn: fp16 bits [rows, I] (vit: the im2col matrix

@@ -28,9 +28,9 @@ ABI_SYMBOLS = [
     "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items", "b200rt_model_wave_capacity_items",
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
-DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_attention", "b200rt_debug_profile_forward",
+DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_gemm_ex", "b200rt_debug_attention", "b200rt_debug_attention_ex", "b200rt_debug_profile_forward",
                  "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_mean_pool_normalize",
-                 "b200rt_debug_vit_pool", "b200rt_debug_fold_ln",
+                 "b200rt_debug_vit_pool", "b200rt_debug_clip_text_pool", "b200rt_debug_fold_ln",
                  "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace", "b200rt_debug_model_cap_rows"]
 
 
@@ -53,6 +53,12 @@ class BertConfig(ctypes.Structure):
 
 class VitConfig(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("image", "patch", "hidden", "layers", "heads", "inter", "proj")] + [("eps", ctypes.c_float)]
+
+
+class ClipTextConfig(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("vocab", "hidden", "layers", "heads", "inter", "max_pos", "proj", "eos_id")] + [
+        ("eps", ctypes.c_float)
+    ]
 
 
 class Stats(ctypes.Structure):
@@ -107,14 +113,17 @@ def load_library():
                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_int,
                                           ctypes.POINTER(ctypes.c_int)]
+        lib.b200rt_debug_gemm_ex.argtypes = lib.b200rt_debug_gemm.argtypes + [ctypes.c_uint32]
         lib.b200rt_debug_attention.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, f32p,
                                                ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        lib.b200rt_debug_attention_ex.argtypes = lib.b200rt_debug_attention.argtypes + [ctypes.c_uint32]
         vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
         lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp, ci]
         lib.b200rt_debug_vit_embed.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, vp, vp]
         lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_mean_pool_normalize.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
+        lib.b200rt_debug_clip_text_pool.argtypes = [vp] * 7 + [ci, ci, ci, cf, ci, vp]
         lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
         lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_vit_forward_trace.argtypes = [ci, vp, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
@@ -258,6 +267,7 @@ class EmbedModel:
         self.cfg = BertConfig(geometry["vocab"], geometry["hidden"], geometry["layers"], geometry["heads"], geometry["inter"],
                               geometry["max_pos"], geometry["type_vocab"], geometry["eps"])
         self.hidden, self.inter = geometry["hidden"], geometry["inter"]
+        self.out_dim = self.hidden
         self.pooling = pooling
         h = ctypes.c_int32(-1)
         flags = LOAD_POOL_MEAN if pooling == "mean" else 0
@@ -279,9 +289,9 @@ class EmbedModel:
             if lens.shape != (n,):
                 raise B200RTError(E_INVALID, f"lens must have shape ({n},), got {lens.shape}")
         if out is None:
-            out = np.empty((n, self.hidden), np.float32)
-        elif out.dtype != np.float32 or not out.flags.c_contiguous or out.shape != (n, self.hidden):
-            raise B200RTError(E_INVALID, "out must be a C-contiguous float32 [n_items, hidden] array")
+            out = np.empty((n, self.out_dim), np.float32)
+        elif out.dtype != np.float32 or not out.flags.c_contiguous or out.shape != (n, self.out_dim):
+            raise B200RTError(E_INVALID, f"out must be a C-contiguous float32 [n_items, {self.out_dim}] array")
         t = ctypes.c_uint64(0)
         with _live_lock:
             _check(self._lib.b200rt_submit_ex(self.handle, _ptr(ids), _ptr(lens) if lens is not None else None, n, S, _ptr(out),
@@ -332,7 +342,7 @@ class EmbedModel:
         lens_a = np.ascontiguousarray(lens, dtype=np.int32) if lens is not None else None
         return _debug_trace(lambda *bufs: self._lib.b200rt_debug_forward_trace(
             self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_launches, *bufs),
-            n * S, n, self.hidden, self.inter, self.hidden, n_launches, self.debug_cap_rows())
+            n * S, n, self.hidden, self.inter, self.out_dim, n_launches, self.debug_cap_rows())
 
     def debug_residual(self, ids: np.ndarray, lens, n_layers: int) -> np.ndarray:
         """The residual stream after ``n_layers`` encoder layers (0: the embedding sum), pre-LayerNorm as the forward carries
@@ -346,6 +356,26 @@ class EmbedModel:
         _check(self._lib.b200rt_debug_profile_forward(self.handle, n_items, max_len, iters, names, 4096, ms, ctypes.byref(n), 64))
         parts = names.raw.split(b"\0")
         return {parts[i].decode(): float(ms[i]) for i in range(n.value)}
+
+
+class ClipTextModel(EmbedModel):
+    """A loaded CLIP text tower (kind "clip_text"): token ids in, ``[n, proj]`` unit-norm embeddings out -- the in-box
+    stand-in for infinity's ``engine.embed(sentences=...)`` on the reference's CLIP model (image_embeddings_infinity.py:298-306).
+    ``submit``/``wait``/``embed``/``debug_trace`` are :class:`EmbedModel`'s: same tickets, same scheduler, width ``proj``.
+    Token ids come from infinity_emb.clip_tokenizer (``<|startoftext|>`` ... ``<|endoftext|>``, at most ``max_pos``)."""
+
+    def __init__(self, geometry: dict, blob: np.ndarray):
+        lib = load_library()
+        blob = np.ascontiguousarray(blob, dtype=np.float32)
+        g = geometry
+        self.cfg = ClipTextConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["proj"], g["eos_id"], g["eps"])
+        self.hidden, self.inter, self.proj = g["hidden"], g["inter"], g["proj"]
+        self.out_dim = self.proj
+        self.pooling = "eos"
+        h = ctypes.c_int32(-1)
+        _check(lib.b200rt_model_load(b"clip_text", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
+        self.handle = h.value
+        self._lib = lib
 
 
 class ImageEmbedModel:
@@ -439,11 +469,13 @@ def device_sync(gpu: int = 0):
 
 
 def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, resid=None, iters: int = 1, ln_stats=None,
-               ln_gamma=None, ln_beta=None, eps: float = 1e-12, want_stats: bool = False, sms: int = 0, want_ctas: bool = False):
+               ln_gamma=None, ln_beta=None, eps: float = 1e-12, want_stats: bool = False, sms: int = 0, want_ctas: bool = False,
+               ln512: bool = False):
     """a16 [M,K], w16 [N,K] float16; returns (out, ms) -- or (out, ms, stats_out [M, N/128, 2]) with ``want_stats`` (epi 2),
     and with ``want_ctas`` the number of CTAs launched appended.
     ``ln_stats`` [M, parts, 2] (sum, M2) partials switch the LayerNorm epilogues on (see include/b200rt_debug.h).
-    ``sms``: the most CTAs of the persistent launch (0 = every SM), rounded down to whole 2-CTA clusters, at least one."""
+    ``sms``: the most CTAs of the persistent launch (0 = every SM), rounded down to whole 2-CTA clusters, at least one.
+    ``ln512``: also accept a 512-wide LayerNorm (the CLIP text tower's 4-partial epilogues; b200rt_debug_gemm_ex)."""
     a16 = np.ascontiguousarray(a16, dtype=np.float16)
     w16 = np.ascontiguousarray(w16, dtype=np.float16)
     bias = np.ascontiguousarray(bias, dtype=np.float32)
@@ -456,16 +488,20 @@ def debug_gemm(epi: int, a16: np.ndarray, w16: np.ndarray, bias: np.ndarray, res
     p = lambda v: _ptr(v) if v is not None else None  # noqa: E731
     ms = ctypes.c_float(0)
     ctas = ctypes.c_int(0)
-    _check(load_library().b200rt_debug_gemm(epi, _ptr(a16), _ptr(w16), _ptr(bias), p(r), _ptr(out), M, N, K, iters, ctypes.byref(ms),
-                                            p(st), p(lg), p(lb), eps, p(so), sms, ctypes.byref(ctas)))
+    _check(load_library().b200rt_debug_gemm_ex(epi, _ptr(a16), _ptr(w16), _ptr(bias), p(r), _ptr(out), M, N, K, iters, ctypes.byref(ms),
+                                               p(st), p(lg), p(lb), eps, p(so), sms, ctypes.byref(ctas), DEBUG_GEMM_LN512 if ln512 else 0))
     res = (out, ms.value, so) if want_stats else (out, ms.value)
     return res + (ctas.value,) if want_ctas else res
 
 
+DEBUG_ATTN_CAUSAL = 1
+DEBUG_GEMM_LN512 = 1
+
+
 def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: int = 1, sms: int = 0, head_dim: int = 64,
-                    heads: int = 12):
-    """qkv16 [B*S, 3H] float16 with H = heads head_dim ((64, 12): bge-base, (32, 12): bge-small, (64, 16): bge-large);
-    returns (ctx [B*S, H], ms)."""
+                    heads: int = 12, causal: bool = False):
+    """qkv16 [B*S, 3H] float16 with H = heads head_dim ((64, 12): bge-base, (32, 12): bge-small, (64, 16): bge-large;
+    causal (64, 8): the CLIP text tower); returns (ctx [B*S, H], ms)."""
     H = heads * head_dim
     qkv16 = np.ascontiguousarray(qkv16, dtype=np.float16)
     if qkv16.size != B * S * 3 * H:
@@ -473,7 +509,8 @@ def debug_attention(qkv16: np.ndarray, lens: np.ndarray, B: int, S: int, iters: 
     lens = np.ascontiguousarray(lens, dtype=np.int32)
     ctx = np.empty((B * S, H), np.float16)
     ms = ctypes.c_float(0)
-    _check(load_library().b200rt_debug_attention(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms, head_dim, heads))
+    _check(load_library().b200rt_debug_attention_ex(_ptr(qkv16), _ptr(lens), _ptr(ctx), B, S, iters, ctypes.byref(ms), sms, head_dim, heads,
+                                                 DEBUG_ATTN_CAUSAL if causal else 0))
     return ctx, ms.value
 
 
@@ -546,6 +583,22 @@ def debug_vit_pool(hi: np.ndarray, lo: np.ndarray, gamma: np.ndarray, beta: np.n
     n, P = hi.shape[0] // T, proj.shape[0]
     out = np.empty((n, max(P, 1)), np.float32)
     _check(load_library().b200rt_debug_vit_pool(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), _ptr(proj), n, T, P, eps, _ptr(out)))
+    return out
+
+
+def debug_clip_text_pool(hi: np.ndarray, lo: np.ndarray, ids: np.ndarray, lens, gamma: np.ndarray, beta: np.ndarray, proj: np.ndarray,
+                         S: int, eps: float, eos_id: int):
+    """hi, lo [n_items * S, 512], ids [n_items, S], lens [n_items] (clamped to [1, S] on the device), proj [P, 512]:
+    normalise(proj . LayerNorm(row i * S + p_i)) with p_i the item's pooled position, [n_items, P]."""
+    hi, lo, gamma, beta, proj = _f16(hi), _f16(lo), _f32(gamma), _f32(beta), _f32(proj)
+    ids = np.ascontiguousarray(ids, dtype=np.int32)
+    lens = np.ascontiguousarray(lens, dtype=np.int32)
+    n, P = hi.shape[0] // S, proj.shape[0]
+    if ids.size != n * S or lens.shape != (n,):
+        raise B200RTError(E_INVALID, f"ids must be [{n}, {S}] and lens [{n}]")
+    out = np.empty((n, max(P, 1)), np.float32)
+    _check(load_library().b200rt_debug_clip_text_pool(_ptr(hi), _ptr(lo), _ptr(ids), _ptr(lens), _ptr(gamma), _ptr(beta), _ptr(proj), n, S, P,
+                                                      eps, eos_id, _ptr(out)))
     return out
 
 

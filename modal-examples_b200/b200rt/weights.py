@@ -352,3 +352,116 @@ def load_clip_vision_state_dict(sd: dict, eps: float = 1e-5, heads: int | None =
     put(sd["visual_projection.weight"], (g["proj"], h))
     assert o == out.size
     return g, out
+
+
+# ----------------------------------------------------------------------------------------------- CLIP text tower
+# The other half of the same CLIP checkpoint: openai/clip-vit-base-patch16's (and -patch32's) text tower, which infinity's
+# `embed(sentences=...)` runs for the reference's image example (image_embeddings_infinity.py:76-77, 298-306).
+# Blob order (fp32): token [V, H] | pos [max_pos, H] | per layer: ln1.g ln1.b qkv.w [3H,H] qkv.b ao.w ao.b ln2.g ln2.b
+# ff1.w [I,H] ff1.b ff2.w [H,I] ff2.b | final.g final.b | proj.w [P, H] (text_projection, no bias).
+# eos_id: 2 in the original openai configs, which selects HF's legacy pooling (the first position of the largest id).
+
+CLIP_TEXT_B16_GEOMETRY = dict(vocab=49408, hidden=512, layers=12, heads=8, inter=2048, max_pos=77, proj=512, eos_id=2, eps=1e-5)
+
+
+def clip_text_blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
+    h, i = g["hidden"], g["inter"]
+    lay = [("token", (g["vocab"], h)), ("pos", (g["max_pos"], h))]
+    for l in range(g["layers"]):
+        p = f"l{l}."
+        lay += [(p + "ln1.g", (h,)), (p + "ln1.b", (h,)), (p + "qkv.w", (3 * h, h)), (p + "qkv.b", (3 * h,)),
+                (p + "ao.w", (h, h)), (p + "ao.b", (h,)), (p + "ln2.g", (h,)), (p + "ln2.b", (h,)),
+                (p + "ff1.w", (i, h)), (p + "ff1.b", (i,)), (p + "ff2.w", (h, i)), (p + "ff2.b", (h,))]
+    lay += [("final.g", (h,)), ("final.b", (h,)), ("proj.w", (g["proj"], h))]
+    return lay
+
+
+def clip_text_blob_numel(g: dict) -> int:
+    return sum(int(np.prod(s)) for _, s in clip_text_blob_layout(g))
+
+
+def random_clip_text_blob(g: dict = CLIP_TEXT_B16_GEOMETRY, seed: int = 0) -> np.ndarray:
+    """Seeded weights of the geometry: normal sigma 0.02 matrices / embeddings, zero biases, unit LayerNorm."""
+    rng = np.random.default_rng(seed)
+    out = np.empty(clip_text_blob_numel(g), np.float32)
+    o = 0
+    for name, shape in clip_text_blob_layout(g):
+        n = int(np.prod(shape))
+        if name.endswith(".g"):
+            out[o:o + n] = 1.0
+        elif name.endswith(".b"):
+            out[o:o + n] = 0.0
+        else:
+            out[o:o + n] = (rng.standard_normal(shape, dtype=np.float32) * np.float32(0.02)).reshape(-1)
+        o += n
+    return out
+
+
+def load_clip_text_state_dict(sd: dict, eps: float = 1e-5, heads: int | None = None, eos_id: int = 2) -> tuple[dict, np.ndarray]:
+    """HF ``CLIPModel`` / ``CLIPTextModelWithProjection`` state dict -> (geometry, fp32 blob).  Parameter names as in HF
+    ``modeling_clip.py`` (``text_model.embeddings.*``, ``text_model.encoder.layers.N.*``, ``text_model.final_layer_norm``,
+    ``text_projection.weight``).  A state dict without ``text_projection.weight`` (a bare ``CLIPTextModel``) is refused: its
+    pooled output is not the embedding infinity serves."""
+
+    def arr(v):
+        if hasattr(v, "detach"):
+            v = v.detach().to("cpu").float().numpy()
+        return np.ascontiguousarray(v, dtype=np.float32)
+
+    if "text_projection.weight" not in sd:
+        raise KeyError("no text_projection.weight: a CLIPModel or CLIPTextModelWithProjection checkpoint is needed")
+    s0 = "text_model."
+    vocab, h = sd[s0 + "embeddings.token_embedding.weight"].shape
+    layers = 0
+    while f"{s0}encoder.layers.{layers}.self_attn.q_proj.weight" in sd:
+        layers += 1
+    g = dict(vocab=int(vocab), hidden=int(h), layers=layers, heads=int(heads or h // 64),
+             inter=int(sd[s0 + "encoder.layers.0.mlp.fc1.weight"].shape[0]),
+             max_pos=int(sd[s0 + "embeddings.position_embedding.weight"].shape[0]), proj=int(sd["text_projection.weight"].shape[0]),
+             eos_id=int(eos_id), eps=float(eps))
+    out = np.empty(clip_text_blob_numel(g), np.float32)
+    o = 0
+
+    def put(a, shape):
+        nonlocal o
+        a = arr(a)
+        if a.shape != tuple(shape):
+            raise ValueError(f"checkpoint tensor has shape {a.shape}, geometry needs {tuple(shape)}")
+        out[o:o + a.size] = a.reshape(-1)
+        o += a.size
+
+    i = g["inter"]
+    put(sd[s0 + "embeddings.token_embedding.weight"], (g["vocab"], h))
+    put(sd[s0 + "embeddings.position_embedding.weight"], (g["max_pos"], h))
+    for l in range(layers):
+        s = f"{s0}encoder.layers.{l}."
+        put(sd[s + "layer_norm1.weight"], (h,))
+        put(sd[s + "layer_norm1.bias"], (h,))
+        put(np.concatenate([arr(sd[s + f"self_attn.{n}.weight"]) for n in ("q_proj", "k_proj", "v_proj")], 0), (3 * h, h))
+        put(np.concatenate([arr(sd[s + f"self_attn.{n}.bias"]) for n in ("q_proj", "k_proj", "v_proj")], 0), (3 * h,))
+        put(sd[s + "self_attn.out_proj.weight"], (h, h))
+        put(sd[s + "self_attn.out_proj.bias"], (h,))
+        put(sd[s + "layer_norm2.weight"], (h,))
+        put(sd[s + "layer_norm2.bias"], (h,))
+        put(sd[s + "mlp.fc1.weight"], (i, h))
+        put(sd[s + "mlp.fc1.bias"], (i,))
+        put(sd[s + "mlp.fc2.weight"], (h, i))
+        put(sd[s + "mlp.fc2.bias"], (h,))
+    put(sd[s0 + "final_layer_norm.weight"], (h,))
+    put(sd[s0 + "final_layer_norm.bias"], (h,))
+    put(sd["text_projection.weight"], (g["proj"], h))
+    assert o == out.size
+    return g, out
+
+
+def clip_text_config_from_dir(path: str) -> dict:
+    """(eps, heads, eos_id) of a CLIP snapshot's ``config.json`` ``text_config`` (a CLIPModel) or top level (a
+    CLIPTextModelWithProjection); eos_id is 2 -- the original openai configs' value -- when the config does not give it."""
+    out = dict(eps=1e-5, heads=None, eos_id=2)
+    p = os.path.join(path, "config.json")
+    if os.path.exists(p):
+        with open(p) as f:
+            cfg = json.load(f)
+        tc = cfg.get("text_config") or cfg
+        out.update(eps=tc.get("layer_norm_eps", 1e-5), heads=tc.get("num_attention_heads"), eos_id=tc.get("eos_token_id", 2))
+    return out

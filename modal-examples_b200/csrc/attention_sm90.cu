@@ -1,6 +1,7 @@
-// Multi-head self-attention for S <= 512, NH heads of d: 12 of 64 (bge-base), 12 of 32 (bge-small) or 16 of 64 (bge-large),
-// on wgmma (sm_90a): persistent CTAs.  The kernel is a template on (d, NH); the comments below give the d = 64 figures, d = 32
-// differences follow.  NH only sets the unit decode and the column offsets of K and V.
+// Multi-head self-attention for S <= 512, NH heads of d: 12 of 64 (bge-base), 12 of 32 (bge-small), 16 of 64 (bge-large) or,
+// causal, 8 of 64 (CLIP's text tower), on wgmma (sm_90a): persistent CTAs.  The kernel is a template on (d, NH, CAUSAL); the
+// comments below give the d = 64 figures, d = 32 differences follow.  NH only sets the unit decode and the column offsets of K
+// and V.
 //
 // A work unit is one (item, head) -- or, for batches with fewer units than SMs, one (item, head, query tile).  Each CTA walks
 // the units u = blockIdx.x, blockIdx.x + gridDim.x, ...  For the unit in hand one thread TMA-loads the head's K and V
@@ -20,7 +21,15 @@
 // is two k-steps of m64n64k16 and O += P . V four m64n32k16 (16 fp32 O registers per thread); the softmax scale is 1/sqrt(32).
 //
 // Keys >= len are masked to -inf before the max (exactly P = 0, matching HF's additive -inf mask); sub-blocks wholly past
-// len are skipped.  Every query tile is computed the same way whether the item travels as one unit or split by query tile,
+// len are skipped.
+//
+// CAUSAL (CLIPTextTransformer's causal mask): key k is also masked for query row q when k > q, at the same place as the len
+// mask.  The rows of warpgroup wg in query tile t are (t0 + t) 128 + 64 wg ... + 63, so its sub-block 2 (t0 + t) + wg is the
+// diagonal one (masked per row) and every later sub-block is wholly masked: the warpgroup stops there.  Running a wholly
+// masked sub-block would change nothing bitwise -- the row max stays, alpha = exp2(0) = 1, p = exp2(-inf) = 0, O and l get
+// exact zeros added -- so skipping it keeps the output independent of batch, bucket, CTA and query-tile split.  A unit loads
+// only the K / V tiles its last query tile reaches (warpgroup 1 of that tile waits on every one of them).  Sub-block 0 holds
+// key 0 for every row, so no row is ever fully masked and padding rows stay finite.  Every query tile is computed the same way whether the item travels as one unit or split by query tile,
 // alone or in any batch, on any CTA, so an item's embedding is bit-identical in any batch (tests: scheduler / size-independent
 // properties).
 //
@@ -67,7 +76,7 @@ struct Unit {
     int len, nsb, nkb; // valid keys, 64-key sub-blocks, 128-key K/V tiles
 };
 
-template <int NH>
+template <int NH, bool CAUSAL>
 __device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const int32_t* __restrict__ lens, int S) {
     Unit U;
     int unit = u;
@@ -83,11 +92,12 @@ __device__ __forceinline__ Unit decode_unit(int u, int nq_all, int split, const 
     U.len = len;
     U.nq = split ? 1 : nq_all;
     U.nsb = (len + SB - 1) / SB;
+    if constexpr (CAUSAL) U.nsb = min(U.nsb, 2 * (U.t0 + U.nq));  // keys past the unit's last query row are never needed
     U.nkb = (U.nsb + 1) / 2;
     return U;
 }
 
-template <int D, int NH>
+template <int D, int NH, bool CAUSAL = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tctx,
                  const int32_t* __restrict__ lens, int S, int split, int n_units) {
@@ -126,7 +136,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
     uint32_t kv_par = 0;                 // bit j: parity of the number of loads of K/V tile j so far
     uint32_t gt = 0;                     // the CTA's running query-tile index
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        const Unit U = decode_unit<NH>(u, nq_all, split, lens, S);
+        const Unit U = decode_unit<NH, CAUSAL>(u, nq_all, split, lens, S);
         auto load_q = [&](uint32_t g, int t) {
             mbar_arrive_expect_tx(&q_full[g & 1], TILE_BYTES);
             tma_load_3d(smem + OFF_Q + (g & 1) * TILE_BYTES, &tq, &q_full[g & 1], U.h * D, (U.t0 + t) * QT, U.b);
@@ -149,8 +159,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
             for (int i = 0; i < NO; ++i) o[i] = 0.f;
             float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
             const uint32_t q_addr = q_buf + wg * (64 * RB);
+            int nsb = U.nsb;
+            if constexpr (CAUSAL) nsb = min(nsb, 2 * (U.t0 + t) + wg + 1);  // up to this warpgroup's diagonal sub-block
 #pragma unroll 1
-            for (int sb = 0; sb < U.nsb; ++sb) {
+            for (int sb = 0; sb < nsb; ++sb) {
                 if ((sb & 1) == 0) mbar_wait(&kv_full[sb >> 1], (kv_par >> (sb >> 1)) & 1);
                 const uint32_t k_addr = smem_u32(smem + OFF_K) + sb * (SB * RB);
                 float s[32];
@@ -167,6 +179,13 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
 #pragma unroll
                     for (int i = 0; i < 32; ++i)
                         if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) s[i] = -INFINITY;
+                }
+                if constexpr (CAUSAL) {
+                    if (sb == 2 * (U.t0 + t) + wg) {  // diagonal: key column c > row r of the warpgroup's 64 is in the future
+#pragma unroll
+                        for (int i = 0; i < 32; ++i)
+                            if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) > w4 * 16 + (lane >> 2) + 8 * ((i >> 1) & 1)) s[i] = -INFINITY;
+                    }
                 }
                 uint32_t pa[4][4];  // P as the A fragments of the four 16-key steps
 #pragma unroll
@@ -241,12 +260,12 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
 
 }  // namespace attn
 
-template <int D, int NH>
+template <int D, int NH, bool CAUSAL = false>
 static cudaError_t setup() {
-    return cudaFuncSetAttribute(attn::attention_kernel<D, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<D>::SMEM_BYTES);
+    return cudaFuncSetAttribute(attn::attention_kernel<D, NH, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<D>::SMEM_BYTES);
 }
 
-template <int D, int NH>
+template <int D, int NH, bool CAUSAL = false>
 static cudaError_t launch_one(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
                               cudaStream_t stream) {
     // fewer (item, head) units than SMs: split them by query tile (K and V are then loaded once per tile, but a single item
@@ -255,7 +274,7 @@ static cudaError_t launch_one(const CUtensorMap& tq, const CUtensorMap& tctx, co
     const int split = (B * NH < sm_count && nq > 1) ? 1 : 0;
     const int n_units = B * NH * (split ? nq : 1);
     const int grid = n_units < sm_count ? n_units : sm_count;
-    return launch_pdl(attn::attention_kernel<D, NH>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<D>::SMEM_BYTES, stream, tq, tctx, lens,
+    return launch_pdl(attn::attention_kernel<D, NH, CAUSAL>, dim3(grid), dim3(attn::NUM_THREADS), attn::Layout<D>::SMEM_BYTES, stream, tq, tctx, lens,
                       S, split, n_units);
 }
 
@@ -263,12 +282,14 @@ cudaError_t attention_init_device() {
     cudaError_t e;
     if ((e = setup<64, 12>()) != cudaSuccess) return e;
     if ((e = setup<32, 12>()) != cudaSuccess) return e;
-    return setup<64, 16>();
+    if ((e = setup<64, 16>()) != cudaSuccess) return e;
+    return setup<64, 8, true>();
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                             cudaStream_t stream, int head_dim, int heads) {
+                             cudaStream_t stream, int head_dim, int heads, bool causal) {
     if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1) return cudaErrorInvalidValue;
+    if (causal) return head_dim == 64 && heads == 8 ? launch_one<64, 8, true>(tq, tctx, lens, B, S, sm_count, stream) : cudaErrorInvalidValue;
     if (head_dim == 64 && heads == 12) return launch_one<64, 12>(tq, tctx, lens, B, S, sm_count, stream);
     if (head_dim == 32 && heads == 12) return launch_one<32, 12>(tq, tctx, lens, B, S, sm_count, stream);
     if (head_dim == 64 && heads == 16) return launch_one<64, 16>(tq, tctx, lens, B, S, sm_count, stream);

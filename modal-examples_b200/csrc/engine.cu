@@ -121,13 +121,15 @@ constexpr int MIN_ITEMS_PER_REPLICA = 8;  // a wave uses fewer replicas rather t
 constexpr int MAX_SEQ = 512;
 constexpr int VIT_WAVE_ITEMS = 64;  // images one replica takes per wave (64 x 197 tokens; 38.5 MB of pixels per wave slot)
 
-// The text geometries the kernels cover (hidden, heads, inter): bge-base, bge-small and bge-large.  The ViT tower is
-// bge-base-wide.
+// The text geometries the kernels cover (hidden, heads, inter, causal): bge-base, bge-small and bge-large (kind "bert") and the
+// CLIP text tower (kind "clip_text", causal attention).  The ViT tower is bge-base-wide.
 struct TextGeometry {
     int hidden, heads, inter;
+    bool causal;
 };
-constexpr int N_TEXT_GEOMETRIES = 3;
-constexpr TextGeometry TEXT_GEOMETRIES[N_TEXT_GEOMETRIES] = {{768, 12, 3072}, {384, 12, 1536}, {1024, 16, 4096}};
+constexpr int N_TEXT_GEOMETRIES = 4;
+constexpr TextGeometry TEXT_GEOMETRIES[N_TEXT_GEOMETRIES] = {
+    {768, 12, 3072, false}, {384, 12, 1536, false}, {1024, 16, 4096, false}, {512, 8, 2048, true}};
 // index into TEXT_GEOMETRIES of the geometry `hidden` wide (-1: none); the hidden widths are distinct
 inline int text_geometry(int hidden) {
     for (int g = 0; g < N_TEXT_GEOMETRIES; ++g)
@@ -136,8 +138,8 @@ inline int text_geometry(int hidden) {
 }
 // Rows of a `hidden`-wide model that the workspace holds: the buffers are sized for bge-base (HIDDEN, QKV_DIM, 3072,
 // STAT_PARTS) at the runtime's cap_rows, so a wider model gets cap_rows * 768 / hidden rows, rounded down to a multiple of
-// 128 (bge-large: 3/4).  Every width of bge-large is 4/3 of bge-base's, so each of its buffers is then full; bge-base and
-// bge-small keep cap_rows.
+// 128 (bge-large: 3/4).  Every width of bge-large is 4/3 of bge-base's, so each of its buffers is then full; bge-base,
+// bge-small and the CLIP text tower keep cap_rows.
 inline int model_cap_rows(int rt_cap_rows, int hidden) {
     const int64_t r = static_cast<int64_t>(rt_cap_rows) * HIDDEN / hidden;
     return r >= rt_cap_rows ? rt_cap_rows : static_cast<int>(r / 128 * 128);
@@ -163,15 +165,19 @@ struct DevWeights {
     __half* patch_w = nullptr;
     CUtensorMap m_patch;
     float *cls = nullptr, *pre_g = nullptr, *pre_b = nullptr, *post_g = nullptr, *post_b = nullptr, *proj_w = nullptr, *zero_bias = nullptr;
+    // CLIP text (kind "clip_text"): word = token_embedding, pos = position_embedding padded to 128 zero rows, type = a zero row,
+    // post_g / post_b = final_layer_norm, proj_w = text_projection [proj, hidden]; layers as for ViT (pre-LN).
 };
 
-enum ModelKind { KIND_BERT = 0, KIND_VIT = 1 };
+enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2 };
 
 struct Model {
     ModelKind kind = KIND_BERT;
     bool pool_mean = false;  // text: mean of the valid tokens' final hidden states (B200RT_LOAD_POOL_MEAN) instead of the CLS row
     b200rt_bert_config cfg{};
     b200rt_vit_config vcfg{};
+    b200rt_clip_text_config tcfg{};
+    int vocab = 0, max_pos = 0;  // token-id models (bert, clip_text): the bounds submit checks ids and lengths against
     int hidden = 0, inter = 0, heads = 0, layers = 0;  // encoder geometry, from whichever config the kind has
     int cap_rows = 0;        // rows of this model one replica's workspace holds (model_cap_rows): bounds every wave of it
     float eps = 0.f;
@@ -368,12 +374,13 @@ int get_qkv_map(Dev& d, const Model& model, int S, const CUtensorMap** out, cons
 // Enqueue the forward of one padded batch on `stream` and add the launches it enqueued to `launches`.  out: fp32 [B, out_dim],
 // may be peer memory.  Widths, statistic partials and the attention head size follow the model's geometry.
 // BERT is post-LN: a residual epilogue re-applies the LayerNorm of the rows it adds to (the embedding LN or LN2 of the layer
-// before, then LN1).  CLIPVisionTransformer is pre-LN: LayerNorm1 / LayerNorm2 are folded into QKV / FFN1, the residual
-// epilogues add the raw stream and emit the statistics the next fold needs.
+// before, then LN1).  CLIPVisionTransformer and CLIPTextTransformer are pre-LN: LayerNorm1 / LayerNorm2 are folded into QKV /
+// FFN1, the residual epilogues add the raw stream and emit the statistics the next fold needs.  The text tower's attention is
+// causal and its pooled row is chosen per item from its ids (launch_clip_text_pool).
 int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
                     LaunchHook* hook) {
     const DevWeights& w = m.per_dev[dev_index];
-    const bool vit = m.kind == KIND_VIT;
+    const bool vit = m.kind == KIND_VIT, clip_text = m.kind == KIND_CLIP_TEXT, pre_ln = m.kind != KIND_BERT;
     const int B = in.B, S = in.S, M = B * S;
     if (M > m.cap_rows || (vit && B > VIT_WAVE_ITEMS))
         return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the model's wave capacity (%d rows)", B, S, m.cap_rows);
@@ -384,7 +391,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
     const int32_t* lens = vit ? d.lens_const : in.lens;
     // residual epilogue: y <- acc + bias + LN(y), LN given by (stats, gamma, beta) -- or + y (pre-LN); new statistics to stats_out
     auto residual = [&](const float* bias, const float2* stats, const float* gamma, const float* beta, float2* stats_out) {
-        return vit ? GemmEpi{bias, nullptr, P, nullptr, nullptr, stats_out, m.eps} : GemmEpi{bias, stats, P, gamma, beta, stats_out, m.eps};
+        return pre_ln ? GemmEpi{bias, nullptr, P, nullptr, nullptr, stats_out, m.eps} : GemmEpi{bias, stats, P, gamma, beta, stats_out, m.eps};
     };
     uint64_t nl = 0;
     // counts the launch just enqueued; true once the hook wants no more
@@ -406,7 +413,8 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, S, m.eps, stream));
             if (step("vit_embed")) return 0;
         } else {
-            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, m.cfg.vocab, H, stream));
+            // clip_text: token + position, its zero type row leaves (word + 0) + pos bit-exact; no embedding LayerNorm
+            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, m.vocab, H, stream));
             if (step("embed")) return 0;
         }
         const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // BERT: the LayerNorm that applies to the current residual rows
@@ -416,15 +424,15 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
             CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
             if (step("gemm_qkv")) return 0;
-            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads));
+            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, clip_text));
             if (step("attention")) return 0;
             // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
             const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
             CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
             if (step("gemm_attn_out")) return 0;
             GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(vit ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
-            if (step(vit ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
+            CUDA_TRY(launch_gemm(pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+            if (step(pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
             // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
             const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
             CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
@@ -433,9 +441,12 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             prev_b = lw.ln2_b;
         }
         if (vit) CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
+        else if (clip_text)
+            CUDA_TRY(launch_clip_text_pool(d.yhi, d.ylo, in.ids, in.lens, w.post_g, w.post_b, w.proj_w, out, B, S, m.tcfg.proj, m.eps,
+                                           m.tcfg.eos_id, stream));
         else if (m.pool_mean) CUDA_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
         else CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
-        step(vit ? "vit_pool" : (m.pool_mean ? "mean_pool_normalize" : "pool_normalize"));
+        step(vit ? "vit_pool" : clip_text ? "clip_text_pool" : (m.pool_mean ? "mean_pool_normalize" : "pool_normalize"));
         return 0;
     };
     if (int rc = enqueue()) return rc;
@@ -1071,10 +1082,70 @@ struct BlobCursor {
     size_t f32 = 0, f16 = 0;
 };
 
+// ---- load steps every model kind shares (the caller holds the root replica's mu)
+
+// the fp32 blob onto the root, an fp32 and an fp16 arena (m.f32_elems, m.f16_elems) on every replica; leaves the root current
+int upload_blob(Runtime& rt, Model& m, const float* blob, size_t nbytes, float** d_blob) {
+    Dev& root = *rt.devs[0];
+    CUDA_TRY(cudaSetDevice(root.id));
+    CUDA_TRY(cudaMalloc(d_blob, nbytes));
+    CUDA_TRY(cudaMemcpy(*d_blob, blob, nbytes, cudaMemcpyHostToDevice));
+    for (size_t g = 0; g < rt.devs.size(); ++g) {
+        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
+        CUDA_TRY(cudaMalloc(&m.per_dev[g].f32_arena, m.f32_elems * 4));
+        CUDA_TRY(cudaMalloc(&m.per_dev[g].f16_arena, m.f16_elems * 2));
+    }
+    CUDA_TRY(cudaSetDevice(root.id));
+    return 0;
+}
+
+// once the root's carve (enqueued on its compute stream) is done: free the blob, then the one-time broadcast of the root's
+// arenas to the other replicas over NVLink
+int broadcast_arenas(Runtime& rt, Model& m, float* d_blob) {
+    Dev& root = *rt.devs[0];
+    CUDA_TRY(cudaStreamSynchronize(root.compute));
+    CUDA_TRY(cudaFree(d_blob));
+    for (size_t g = 1; g < rt.devs.size(); ++g) {
+        CUDA_TRY(cudaMemcpyPeerAsync(m.per_dev[g].f32_arena, rt.devs[g]->id, m.per_dev[0].f32_arena, root.id, m.f32_elems * 4, root.compute));
+        CUDA_TRY(cudaMemcpyPeerAsync(m.per_dev[g].f16_arena, rt.devs[g]->id, m.per_dev[0].f16_arena, root.id, m.f16_elems * 2, root.compute));
+    }
+    CUDA_TRY(cudaStreamSynchronize(root.compute));
+    return 0;
+}
+
+// the GEMM B-operand maps of one layer's weights (box {64,128})
+int make_layer_maps(LayerW& lw, size_t H, size_t I) {
+    if (int rc = make_map_2d(&lw.m_qkv, lw.qkv_w, 3 * H, H, 128)) return rc;
+    if (int rc = make_map_2d(&lw.m_ao, lw.ao_w, H, H, 128)) return rc;
+    if (int rc = make_map_2d(&lw.m_ff1, lw.ff1_w, I, H, 128)) return rc;
+    return make_map_2d(&lw.m_ff2, lw.ff2_w, H, I, 128);
+}
+
+// one pre-LN layer's pointers (ViT and CLIP text arenas): fp32 ln1.g ln1.b qkv.b ao.b ln2.g ln2.b ff1.b ff2.b qkv_c ff1_c, fp16
+// qkv.w ao.w ff1.w ff2.w
+void carve_pre_ln_layer(LayerW& lw, float*& p, __half*& q, size_t H, size_t I) {
+    lw.ln1_g = p; p += H;  lw.ln1_b = p; p += H;
+    lw.qkv_w = q; q += 3 * H * H;  lw.qkv_b = p; p += 3 * H;
+    lw.ao_w = q;  q += H * H;      lw.ao_b = p;  p += H;
+    lw.ln2_g = p; p += H;  lw.ln2_b = p; p += H;
+    lw.ff1_w = q; q += I * H;      lw.ff1_b = p; p += I;
+    lw.ff2_w = q; q += H * I;      lw.ff2_b = p; p += H;
+    lw.qkv_c = p; p += 3 * H;
+    lw.ff1_c = p; p += I;
+}
+
+int register_model(Runtime& rt, std::unique_ptr<Model> m, int* model_out) {
+    CUDA_TRY(cudaSetDevice(rt.devs[0]->id));
+    std::lock_guard<std::mutex> lk(rt.mu);
+    rt.models.push_back(std::move(m));
+    *model_out = static_cast<int>(rt.models.size()) - 1;
+    return 0;
+}
+
 int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out) {
     Runtime& rt = *g_rt;
     bool known = false;
-    for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
+    for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= !tg.causal && c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
     if (!known || c.max_pos > MAX_SEQ || c.max_pos < 1 || c.layers < 1 || c.vocab < 1 || c.type_vocab < 1)
         return fail(B200RT_E_UNSUPPORTED,
                     "kernels cover three geometries, bge-base (hidden=768 heads=12 inter=3072), bge-small (hidden=384 heads=12 "
@@ -1094,6 +1165,7 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
 
     auto m = std::make_unique<Model>();
     m->cfg = c;
+    m->vocab = c.vocab, m->max_pos = c.max_pos;
     m->pool_mean = pool_mean;
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->cap_rows = cap_rows;
@@ -1109,16 +1181,8 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
     // l = 0), FFN1 takes the layer's own LN1.
     Dev& root = *rt.devs[0];
     std::lock_guard<std::mutex> dl(root.mu);
-    CUDA_TRY(cudaSetDevice(root.id));
     float* d_blob = nullptr;
-    CUDA_TRY(cudaMalloc(&d_blob, nbytes));
-    CUDA_TRY(cudaMemcpy(d_blob, blob, nbytes, cudaMemcpyHostToDevice));
-    for (size_t g = 0; g < rt.devs.size(); ++g) {
-        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
-        CUDA_TRY(cudaMalloc(&m->per_dev[g].f32_arena, m->f32_elems * 4));
-        CUDA_TRY(cudaMalloc(&m->per_dev[g].f16_arena, m->f16_elems * 2));
-    }
-    CUDA_TRY(cudaSetDevice(root.id));
+    if (int rc = upload_blob(rt, *m, blob, nbytes, &d_blob)) return rc;
     DevWeights& rw = m->per_dev[0];
     {
         size_t src = 0, o32 = 0, o16 = 0, ox = blob_f32;
@@ -1154,14 +1218,7 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
             CUDA_TRY(take32(H + 2 * H));                                                  // ff2.b, ln2.g, ln2.b
         }
     }
-    CUDA_TRY(cudaStreamSynchronize(root.compute));
-    CUDA_TRY(cudaFree(d_blob));
-    // one-time broadcast of the device-resident weights to the other replicas over NVLink
-    for (size_t g = 1; g < rt.devs.size(); ++g) {
-        CUDA_TRY(cudaMemcpyPeerAsync(m->per_dev[g].f32_arena, rt.devs[g]->id, rw.f32_arena, root.id, m->f32_elems * 4, root.compute));
-        CUDA_TRY(cudaMemcpyPeerAsync(m->per_dev[g].f16_arena, rt.devs[g]->id, rw.f16_arena, root.id, m->f16_elems * 2, root.compute));
-    }
-    CUDA_TRY(cudaStreamSynchronize(root.compute));
+    if (int rc = broadcast_arenas(rt, *m, d_blob)) return rc;
     // carve pointers + weight tensor maps per replica
     for (size_t g = 0; g < rt.devs.size(); ++g) {
         DevWeights& w = m->per_dev[g];
@@ -1182,19 +1239,10 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
             lw.ff2_w = q; q += H * I;      lw.ff2_b = p; p += H;  lw.ln2_g = p; p += H;  lw.ln2_b = p; p += H;
             float* x = w.f32_arena + blob_f32 + static_cast<size_t>(l) * per_layer_x;
             lw.qkv_c = x; lw.ff1_c = x + 3 * H;
-            if (int rc = make_map_2d(&lw.m_qkv, lw.qkv_w, 3 * H, H, 128)) return rc;
-            if (int rc = make_map_2d(&lw.m_ao, lw.ao_w, H, H, 128)) return rc;
-            if (int rc = make_map_2d(&lw.m_ff1, lw.ff1_w, I, H, 128)) return rc;
-            if (int rc = make_map_2d(&lw.m_ff2, lw.ff2_w, H, I, 128)) return rc;
+            if (int rc = make_layer_maps(lw, H, I)) return rc;
         }
     }
-    CUDA_TRY(cudaSetDevice(root.id));
-    {
-        std::lock_guard<std::mutex> lk(rt.mu);
-        rt.models.push_back(std::move(m));
-        *model_out = static_cast<int>(rt.models.size()) - 1;
-    }
-    return 0;
+    return register_model(rt, std::move(m), model_out);
 }
 
 int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes, int* model_out) {
@@ -1227,15 +1275,11 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
 
     Dev& root = *rt.devs[0];
     std::lock_guard<std::mutex> dl(root.mu);
-    CUDA_TRY(cudaSetDevice(root.id));
     float* d_blob = nullptr;
-    CUDA_TRY(cudaMalloc(&d_blob, nbytes));
-    CUDA_TRY(cudaMemcpy(d_blob, blob, nbytes, cudaMemcpyHostToDevice));
+    if (int rc = upload_blob(rt, *m, blob, nbytes, &d_blob)) return rc;
     for (size_t g = 0; g < rt.devs.size(); ++g) {
         Dev& d = *rt.devs[g];
         CUDA_TRY(cudaSetDevice(d.id));
-        CUDA_TRY(cudaMalloc(&m->per_dev[g].f32_arena, m->f32_elems * 4));
-        CUDA_TRY(cudaMalloc(&m->per_dev[g].f16_arena, m->f16_elems * 2));
         // per-replica image input slots and constants, once
         if (!d.lens_const) {
             std::vector<int32_t> lens(VIT_WAVE_ITEMS, T);
@@ -1295,13 +1339,7 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
         o32 += H;
         if (o32 != m->f32_elems || o16 != m->f16_elems || src != total) return fail(B200RT_E_STATE, "internal: vit blob carve mismatch");
     }
-    CUDA_TRY(cudaStreamSynchronize(root.compute));
-    CUDA_TRY(cudaFree(d_blob));
-    for (size_t g = 1; g < rt.devs.size(); ++g) {
-        CUDA_TRY(cudaMemcpyPeerAsync(m->per_dev[g].f32_arena, rt.devs[g]->id, rw.f32_arena, root.id, m->f32_elems * 4, root.compute));
-        CUDA_TRY(cudaMemcpyPeerAsync(m->per_dev[g].f16_arena, rt.devs[g]->id, rw.f16_arena, root.id, m->f16_elems * 2, root.compute));
-    }
-    CUDA_TRY(cudaStreamSynchronize(root.compute));
+    if (int rc = broadcast_arenas(rt, *m, d_blob)) return rc;
     for (size_t g = 0; g < rt.devs.size(); ++g) {
         DevWeights& w = m->per_dev[g];
         CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
@@ -1316,31 +1354,116 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
         w.layers.resize(c.layers);
         for (int l = 0; l < c.layers; ++l) {
             LayerW& lw = w.layers[l];
-            lw.ln1_g = p; p += H;  lw.ln1_b = p; p += H;
-            lw.qkv_w = q; q += 3 * H * H;  lw.qkv_b = p; p += 3 * H;
-            lw.ao_w = q;  q += H * H;      lw.ao_b = p;  p += H;
-            lw.ln2_g = p; p += H;  lw.ln2_b = p; p += H;
-            lw.ff1_w = q; q += I * H;      lw.ff1_b = p; p += I;
-            lw.ff2_w = q; q += H * I;      lw.ff2_b = p; p += H;
-            lw.qkv_c = p; p += 3 * H;
-            lw.ff1_c = p; p += I;
-            if (int rc = make_map_2d(&lw.m_qkv, lw.qkv_w, 3 * H, H, 128)) return rc;
-            if (int rc = make_map_2d(&lw.m_ao, lw.ao_w, H, H, 128)) return rc;
-            if (int rc = make_map_2d(&lw.m_ff1, lw.ff1_w, I, H, 128)) return rc;
-            if (int rc = make_map_2d(&lw.m_ff2, lw.ff2_w, H, I, 128)) return rc;
+            carve_pre_ln_layer(lw, p, q, H, I);
+            if (int rc = make_layer_maps(lw, H, I)) return rc;
         }
         w.post_g = p; p += H;
         w.post_b = p; p += H;
         w.proj_w = p; p += P * H;
         w.zero_bias = p; p += H;
     }
-    CUDA_TRY(cudaSetDevice(root.id));
+    return register_model(rt, std::move(m), model_out);
+}
+
+// CLIP text tower (kind "clip_text").  Blob order (fp32, b200rt.weights.clip_text_blob_layout): token [V, H] | pos [max_pos, H] |
+// per layer ln1.g ln1.b qkv.w [3H,H] qkv.b ao.w ao.b ln2.g ln2.b ff1.w [I,H] ff1.b ff2.w [H,I] ff2.b | final.g final.b |
+// proj.w [P, H].  fp32 arena: token | pos padded to TEXT_POS_ROWS zero rows | a zero type row | per layer ln1.g ln1.b qkv.b ao.b
+// ln2.g ln2.b ff1.b ff2.b qkv_c ff1_c | final.g final.b | proj.w.
+constexpr int TEXT_POS_ROWS = 128;  // embed_kernel reads pos[t % S] for every row of a wave padded to its bucket (<= 128)
+int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, size_t nbytes, int* model_out) {
+    Runtime& rt = *g_rt;
+    const TextGeometry* tgp = TEXT_GEOMETRIES;
+    while (!tgp->causal) ++tgp;  // the one causal geometry of the table
+    const TextGeometry& tg = *tgp;
+    if (c.hidden != tg.hidden || c.heads != tg.heads || c.inter != tg.inter || c.layers < 1 || c.vocab < 1 || c.proj < 1 || c.proj > 1024)
+        return fail(B200RT_E_UNSUPPORTED, "kernels cover the CLIP text tower of clip-vit-base-patch16 / -patch32: hidden=512 heads=8 inter=2048, "
+                                          "proj <= 1024 (got hidden %d heads %d inter %d proj %d)", c.hidden, c.heads, c.inter, c.proj);
+    if (c.max_pos < 1 || c.max_pos > TEXT_POS_ROWS)
+        return fail(B200RT_E_UNSUPPORTED, "max_pos %d outside [1, %d]", c.max_pos, TEXT_POS_ROWS);
+    if (c.eos_id < 0 || c.eos_id >= c.vocab) return fail(B200RT_E_INVALID, "eos_id %d outside the vocabulary [0, %d)", c.eos_id, c.vocab);
+    const size_t H = c.hidden, I = c.inter, P = c.proj, V = c.vocab;
+    const size_t per_layer_w = 3 * H * H + H * H + I * H + H * I;
+    const size_t per_layer_p = 2 * H + 3 * H + H + 2 * H + I + H;  // ln1, qkv.b, ao.b, ln2, ff1.b, ff2.b
+    const size_t per_layer_x = 3 * H + I;                          // qkv_c, ff1_c
+    const size_t total = V * H + static_cast<size_t>(c.max_pos) * H + static_cast<size_t>(c.layers) * (per_layer_w + per_layer_p) + 2 * H + P * H;
+    if (nbytes != total * 4) return fail(B200RT_E_INVALID, "weight blob is %zu bytes, geometry needs %zu", nbytes, total * 4);
+
+    auto m = std::make_unique<Model>();
+    m->kind = KIND_CLIP_TEXT;
+    m->tcfg = c;
+    m->vocab = c.vocab, m->max_pos = c.max_pos;
+    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
+    m->cap_rows = model_cap_rows(rt.cap_rows, c.hidden);
+    m->out_dim = c.proj;
+    m->f32_elems = V * H + TEXT_POS_ROWS * H + H + static_cast<size_t>(c.layers) * (per_layer_p + per_layer_x) + 2 * H + P * H;
+    m->f16_elems = static_cast<size_t>(c.layers) * per_layer_w;
+    m->per_dev.resize(rt.devs.size());
+
+    Dev& root = *rt.devs[0];
+    std::lock_guard<std::mutex> dl(root.mu);
+    float* d_blob = nullptr;
+    if (int rc = upload_blob(rt, *m, blob, nbytes, &d_blob)) return rc;
+    DevWeights& rw = m->per_dev[0];
     {
-        std::lock_guard<std::mutex> lk(rt.mu);
-        rt.models.push_back(std::move(m));
-        *model_out = static_cast<int>(rt.models.size()) - 1;
+        size_t src = 0, o32 = 0, o16 = 0;
+        auto take32 = [&](size_t n) -> cudaError_t {
+            cudaError_t e = cudaMemcpyAsync(rw.f32_arena + o32, d_blob + src, n * 4, cudaMemcpyDeviceToDevice, root.compute);
+            src += n; o32 += n;
+            return e;
+        };
+        auto zero32 = [&](size_t n) -> cudaError_t {  // arena-only zeros (position padding, type row)
+            cudaError_t e = cudaMemsetAsync(rw.f32_arena + o32, 0, n * 4, root.compute);
+            o32 += n;
+            return e;
+        };
+        auto take16 = [&](size_t N_, size_t K_, const float* gamma, const float* beta, const float* bias, float* cv) -> cudaError_t {
+            cudaError_t e = launch_fold_ln(d_blob + src, gamma, beta, bias, rw.f16_arena + o16, cv, static_cast<int>(N_), static_cast<int>(K_), root.compute);
+            src += N_ * K_; o16 += N_ * K_;
+            return e;
+        };
+        CUDA_TRY(take32(V * H + static_cast<size_t>(c.max_pos) * H));  // token, pos
+        CUDA_TRY(zero32((TEXT_POS_ROWS - static_cast<size_t>(c.max_pos)) * H + H));  // pos padding, type row
+        for (int l = 0; l < c.layers; ++l) {
+            float* lb = rw.f32_arena + o32;  // this layer's f32 region: its derived vectors follow its per_layer_p params
+            const float* ln1_g = d_blob + src;
+            const float* ln1_b = d_blob + src + H;
+            CUDA_TRY(take32(2 * H));                                        // ln1.g, ln1.b
+            CUDA_TRY(take16(3 * H, H, ln1_g, ln1_b, d_blob + src + 3 * H * H, lb + per_layer_p));  // qkv.w folded with ln1
+            CUDA_TRY(take32(3 * H));                                        // qkv.b
+            CUDA_TRY(take16(H, H, nullptr, nullptr, nullptr, nullptr));     // ao.w
+            CUDA_TRY(take32(H));                                            // ao.b
+            const float* ln2_g = d_blob + src;
+            const float* ln2_b = d_blob + src + H;
+            CUDA_TRY(take32(2 * H));                                        // ln2.g, ln2.b
+            CUDA_TRY(take16(I, H, ln2_g, ln2_b, d_blob + src + I * H, lb + per_layer_p + 3 * H));  // ff1.w folded with ln2
+            CUDA_TRY(take32(I));                                            // ff1.b
+            CUDA_TRY(take16(H, I, nullptr, nullptr, nullptr, nullptr));     // ff2.w
+            CUDA_TRY(take32(H));                                            // ff2.b
+            o32 += per_layer_x;                                             // qkv_c, ff1_c (written by the folds)
+        }
+        CUDA_TRY(take32(2 * H + P * H));                                    // final.g, final.b, proj.w
+        if (o32 != m->f32_elems || o16 != m->f16_elems || src != total) return fail(B200RT_E_STATE, "internal: clip_text blob carve mismatch");
     }
-    return 0;
+    if (int rc = broadcast_arenas(rt, *m, d_blob)) return rc;
+    for (size_t g = 0; g < rt.devs.size(); ++g) {
+        DevWeights& w = m->per_dev[g];
+        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
+        float* p = w.f32_arena;
+        __half* q = w.f16_arena;
+        w.word = p; p += V * H;
+        w.pos = p;  p += TEXT_POS_ROWS * H;
+        w.type = p; p += H;
+        w.layers.resize(c.layers);
+        for (int l = 0; l < c.layers; ++l) {
+            LayerW& lw = w.layers[l];
+            carve_pre_ln_layer(lw, p, q, H, I);
+            if (int rc = make_layer_maps(lw, H, I)) return rc;
+        }
+        w.post_g = p; p += H;
+        w.post_b = p; p += H;
+        w.proj_w = p; p += P * H;
+    }
+    return register_model(rt, std::move(m), model_out);
 }
 
 Runtime* live_rt() {
@@ -1365,16 +1488,23 @@ const Model* get_model(Runtime& rt, int model) {
     return rt.models[model].get();
 }
 
-int check_ids(const b200rt_bert_config& c, const int32_t* ids, const int32_t* lens, int n_items, int max_len) {
+// The longest padded length a forward of this model runs at: the CLIP text tower's waves go up to the 128-token bucket (its
+// position table is padded to TEXT_POS_ROWS zero rows for that), a BERT model's up to max_pos.
+inline int max_wave_len(const Model& m) { return m.kind == KIND_CLIP_TEXT ? TEXT_POS_ROWS : m.max_pos; }
+
+// ids [n_items, max_len] with max_len <= S_cap (submit: max_pos; device-resident / debug forwards: max_wave_len) and every
+// item's length in [1, min(max_len, max_pos)], its ids inside the vocabulary.
+int check_ids(const Model& m, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int S_cap) {
     if (!ids || n_items < 1) return fail(B200RT_E_INVALID, "empty input (n_items=%d)", n_items);
-    if (max_len < 1 || max_len > c.max_pos) return fail(B200RT_E_INVALID, "max_len %d outside [1, %d]", max_len, c.max_pos);
+    if (max_len < 1 || max_len > S_cap) return fail(B200RT_E_INVALID, "max_len %d outside [1, %d]", max_len, S_cap);
+    const int len_cap = std::min(max_len, m.max_pos);
     for (int i = 0; i < n_items; ++i) {
         const int L = lens ? lens[i] : max_len;
-        if (L < 1 || L > max_len) return fail(B200RT_E_INVALID, "lens[%d] = %d outside [1, %d]", i, L, max_len);
+        if (L < 1 || L > len_cap) return fail(B200RT_E_INVALID, "lens[%d] = %d outside [1, %d]", i, L, len_cap);
         const int32_t* row = ids + static_cast<size_t>(i) * max_len;
         for (int j = 0; j < L; ++j)
-            if (row[j] < 0 || row[j] >= c.vocab)
-                return fail(B200RT_E_INVALID, "ids[%d][%d] = %d outside the vocabulary [0, %d)", i, j, row[j], c.vocab);
+            if (row[j] < 0 || row[j] >= m.vocab)
+                return fail(B200RT_E_INVALID, "ids[%d][%d] = %d outside the vocabulary [0, %d)", i, j, row[j], m.vocab);
     }
     return 0;
 }
@@ -1497,14 +1627,18 @@ int b200rt_model_load(const char* kind, const void* cfg, const void* weights, si
 int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0))
-        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\" or \"vit\")", kind ? kind : "(null)");
+    if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0 && strcmp(kind, "clip_text") != 0))
+        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"vit\" or \"clip_text\")", kind ? kind : "(null)");
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
     if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
     const bool pool_mean = (flags & B200RT_LOAD_POOL_MEAN) != 0;
     if (strcmp(kind, "vit") == 0) {
         if (pool_mean) return fail(B200RT_E_INVALID, "B200RT_LOAD_POOL_MEAN applies to text encoders (kind \"bert\"), not \"vit\"");
         return model_load_vit(*static_cast<const b200rt_vit_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
+    }
+    if (strcmp(kind, "clip_text") == 0) {
+        if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"clip_text\"", flags);
+        return model_load_clip_text(*static_cast<const b200rt_clip_text_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
     }
     return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean, model_out);
 }
@@ -1516,9 +1650,9 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
     if (!out || !ticket_out) return fail(B200RT_E_INVALID, "null out / ticket_out");
-    if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d takes pixels (b200rt_submit_pixels), not token ids", model);
+    if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d takes pixels (b200rt_submit_pixels), not token ids", model);
     if (flags & ~static_cast<uint32_t>(B200RT_SUBMIT_BORROW_IDS)) return fail(B200RT_E_INVALID, "unknown submit flags 0x%x", flags);
-    if (int rc = check_ids(m->cfg, ids, lens, n_items, max_len)) return rc;
+    if (int rc = check_ids(*m, ids, lens, n_items, max_len, m->max_pos)) return rc;
     auto t = std::make_shared<Ticket>();
     t->model = model;
     t->mp = m;
@@ -1693,8 +1827,8 @@ int b200rt_embed_device(int model, int gpu, const int32_t* d_ids, const int32_t*
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
     if (gpu < 0 || gpu >= static_cast<int>(rt->devs.size())) return fail(B200RT_E_INVALID, "gpu index %d outside the pool", gpu);
-    if (m->kind != KIND_BERT) return fail(B200RT_E_UNSUPPORTED, "b200rt_embed_device takes token ids: model %d is not a text encoder", model);
-    if (!d_ids || !d_lens || !d_out || n_items < 1 || max_len < 1 || max_len > m->cfg.max_pos) return fail(B200RT_E_INVALID, "bad argument");
+    if (m->kind == KIND_VIT) return fail(B200RT_E_UNSUPPORTED, "b200rt_embed_device takes token ids: model %d is not a text encoder", model);
+    if (!d_ids || !d_lens || !d_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
     Dev& d = *rt->devs[gpu];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
@@ -1817,15 +1951,26 @@ void b200rt_shutdown(void) {
 int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid, void* out,
                       int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
                       const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out) {
+    return b200rt_debug_gemm_ex(epi, a, w, bias, resid, out, M, N, K, iters, ms_out, ln_stats, ln_gamma, ln_beta, eps, stats_out, sms,
+                                ctas_out, 0);
+}
+
+int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid, void* out,
+                         int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
+                         const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out, uint32_t flags) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (flags & ~B200RT_DEBUG_GEMM_LN512) return fail(B200RT_E_INVALID, "unknown gemm flags 0x%x", flags);
     if (!a || !w || !bias || !out || M < 1 || N % 128 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
     if (epi == 2 && !resid) return fail(B200RT_E_INVALID, "epi 2 needs resid");
     const int ln_w = epi == 2 ? N : K;
-    if (ln_stats && ln_w != 768 && ln_w != 384 && ln_w != 1024)
-        return fail(B200RT_E_INVALID, "the LayerNorm'd width must be 768, 384 or 1024");
+    const bool ln512 = (flags & B200RT_DEBUG_GEMM_LN512) != 0;
+    if (ln_stats && ln_w != 768 && ln_w != 384 && ln_w != 1024 && !(ln512 && ln_w == 512))
+        return fail(B200RT_E_INVALID, ln512 ? "the LayerNorm'd width must be 768, 384, 1024 or 512" : "the LayerNorm'd width must be 768, 384 or 1024");
     if (ln_stats && ln_w == 1024 && (epi == 3 || N % 256 != 0))
         return fail(B200RT_E_INVALID, "a 1024-wide LayerNorm needs epi 0, 1 or 2 and N %% 256 == 0");
+    if (ln_stats && ln_w == 512 && ((epi != 0 && epi != 3) || N % 256 != 0))
+        return fail(B200RT_E_INVALID, "a 512-wide LayerNorm needs epi 0 or 3 and N %% 256 == 0");
     if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
     Dev& d = *rt->devs[0];
     if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
@@ -1905,12 +2050,21 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
 
 int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms,
                            int head_dim, int heads) {
+    return b200rt_debug_attention_ex(qkv, lens, ctx, B, S, iters, ms_out, sms, head_dim, heads, 0);
+}
+
+int b200rt_debug_attention_ex(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms,
+                              int head_dim, int heads, uint32_t flags) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!qkv || !lens || !ctx || B < 1 || S < 1 || S > MAX_SEQ) return fail(B200RT_E_INVALID, "bad attention arguments");
+    if (flags & ~B200RT_DEBUG_ATTN_CAUSAL) return fail(B200RT_E_INVALID, "unknown attention flags 0x%x", flags);
+    const bool causal = (flags & B200RT_DEBUG_ATTN_CAUSAL) != 0;
     if (head_dim == 0) head_dim = 64;
     if (heads == 0) heads = HEADS;
-    if (!((head_dim == 64 && heads == 12) || (head_dim == 32 && heads == 12) || (head_dim == 64 && heads == 16)))
+    if (causal && !(head_dim == 64 && heads == 8))
+        return fail(B200RT_E_INVALID, "causal attention exists for (head_dim, heads) = (64, 8), got (%d, %d)", head_dim, heads);
+    if (!causal && !((head_dim == 64 && heads == 12) || (head_dim == 32 && heads == 12) || (head_dim == 64 && heads == 16)))
         return fail(B200RT_E_INVALID, "(head_dim, heads) must be (64, 12), (32, 12) or (64, 16) (0 = 64, 12), got (%d, %d)", head_dim, heads);
     const size_t H = static_cast<size_t>(heads) * head_dim;
     Dev& d = *rt->devs[0];
@@ -1933,9 +2087,9 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
     CUDA_TRY(b.event(&e0));
     CUDA_TRY(b.event(&e1));
     if (iters < 1) iters = 1;
-    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads));
+    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads, causal));
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads));
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads, causal));
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
@@ -1952,8 +2106,8 @@ int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, 
     if (!ids || !word || !pos || !type0 || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1)
         return fail(B200RT_E_INVALID, "bad embed arguments");
     if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384 && hidden != 1024)
-        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024 (0 = 768), got %d", hidden);
+    if (hidden != 768 && hidden != 384 && hidden != 1024 && hidden != 512)
+        return fail(B200RT_E_INVALID, "row width must be 768, 384, 1024 or 512 (0 = 768), got %d", hidden);
     const size_t H = hidden, P = H / 128;
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
@@ -2086,6 +2240,35 @@ int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* g
     return 0;
 }
 
+int b200rt_debug_clip_text_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* ids, const int32_t* lens, const float* gamma,
+                                const float* beta, const float* proj, int n_items, int S, int P, float eps, int eos_id, float* out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!hi || !lo || !ids || !lens || !gamma || !beta || !proj || !out || n_items < 1 || S < 1)
+        return fail(B200RT_E_INVALID, "bad clip_text_pool arguments");
+    if (P < 1 || P > 1024) return fail(B200RT_E_INVALID, "projection width %d outside [1, 1024]", P);
+    constexpr size_t H = 512;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_items) * S;
+    DebugBuffers b(d.compute);
+    __half *dhi, *dlo;
+    int32_t *dids, *dlens;
+    float *dg, *dbt, *dproj, *dout;
+    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+    CUDA_TRY(b.upload(&dids, ids, rows * 4));
+    CUDA_TRY(b.upload(&dlens, lens, static_cast<size_t>(n_items) * 4));  // passed through unchecked: the kernel clamps to [1, S]
+    CUDA_TRY(b.upload(&dg, gamma, H * 4));
+    CUDA_TRY(b.upload(&dbt, beta, H * 4));
+    CUDA_TRY(b.upload(&dproj, proj, static_cast<size_t>(P) * H * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * P * 4));
+    CUDA_TRY(launch_clip_text_pool(dhi, dlo, dids, dlens, dg, dbt, dproj, dout, n_items, S, P, eps, eos_id, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * P * 4));
+    return 0;
+}
+
 int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,
                          float* cvec_out) {
     Runtime* rt = live_rt();
@@ -2120,8 +2303,8 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
-    if (int rc = check_ids(m->cfg, ids, lens, n_items, max_len)) return rc;
+    if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+    if (int rc = check_ids(*m, ids, lens, n_items, max_len, max_wave_len(*m))) return rc;
     const int total = 5 * m->layers + 2;
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
@@ -2177,16 +2360,16 @@ int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters,
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    if (m->kind != KIND_BERT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
-    if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > m->cfg.max_pos) return fail(B200RT_E_INVALID, "bad argument");
+    if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+    if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
     const size_t M = static_cast<size_t>(n_items) * max_len;
     if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
     Dev& d = *rt->devs[0];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
-    std::vector<int32_t> ids(M), l(n_items, max_len);
+    std::vector<int32_t> ids(M), l(n_items, std::min(max_len, m->max_pos));  // a clip_text wave may be longer than its items
     uint32_t x = 12345;
-    for (auto& v : ids) { x = x * 1664525u + 1013904223u; v = 1000 + static_cast<int32_t>((x >> 8) % (m->cfg.vocab - 1000)); }
+    for (auto& v : ids) { x = x * 1664525u + 1013904223u; v = 1000 + static_cast<int32_t>((x >> 8) % (m->vocab - 1000)); }
     DebugBuffers b(d.compute);
     int32_t *dids = nullptr, *dlens = nullptr;
     float* dout = nullptr;

@@ -2,8 +2,8 @@
 //
 // Persistent clusters of CM = 2 CTAs walk pairs of 128 x BN output tiles that share their columns, BN = 256, or 128 where
 // N % 256 != 0 (bge-small's 384 / 1152-wide projections; the figures below are BN = 256's, BN = 128 halves the W box, the
-// stage and the accumulators).  The LayerNorm statistics a tile reads come as PARTS partials per row: 6 (768 wide), 3 (384)
-// or 8 (bge-large's 1024).  Pair p = (m-pair p / num_n, n-block p % num_n), n fastest; CTA rank r of the cluster takes
+// stage and the accumulators).  The LayerNorm statistics a tile reads come as PARTS partials per row: 6 (768 wide), 3 (384),
+// 8 (bge-large's 1024) or 4 (the CLIP text tower's 512).  Pair p = (m-pair p / num_n, n-block p % num_n), n fastest; CTA rank r of the cluster takes
 // m-tile CM (p / num_n) + r; cluster c walks p = c, c + clusters, ..., its two CTAs in step.  Three warpgroups per CTA:
 //   warpgroup 0  : one thread TMA-loads its own A [128 x 64] per 64-wide k-block into a STAGES-deep ring (48 KB per stage,
 //                  128B-swizzled), plus its share of the pair's W [256 x 64] -- 128-row box b is loaded by rank b % CM and
@@ -80,10 +80,10 @@ __device__ __forceinline__ float gelu_quick(float x) {
 }
 
 // LayerNorm statistics of a row from its PARTS (sum, M2) partials (Chan et al.): 8 for a 1024-wide row, 6 for a 768-wide one,
-// 3 for a 384-wide one
+// 4 for a 512-wide one, 3 for a 384-wide one
 template <int PARTS>
 __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float eps, float& mean, float& rstd) {
-    static_assert(PARTS == 8 || PARTS == 6 || PARTS == 3, "LayerNorm width 1024, 768 or 384");
+    static_assert(PARTS == 8 || PARTS == 6 || PARTS == 4 || PARTS == 3, "LayerNorm width 1024, 768, 512 or 384");
     constexpr float inv_n = 1.0f / (128.0f * PARTS);
     if constexpr (PARTS == 8) {
         const float4* __restrict__ pp = reinterpret_cast<const float4*>(st);
@@ -111,6 +111,19 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float e
             m2[i] = fmaf(128.0f * d, d, p[i].y);
         }
         rstd = rsqrtf((((m2[0] + m2[1]) + (m2[2] + m2[3])) + (m2[4] + m2[5])) * inv_n + eps);
+    } else if constexpr (PARTS == 4) {
+        // a pairwise tree, as for 8
+        const float4* __restrict__ pp = reinterpret_cast<const float4*>(st);
+        const float4 a = __ldg(pp), b = __ldg(pp + 1);
+        const float2 p[PARTS] = {make_float2(a.x, a.y), make_float2(a.z, a.w), make_float2(b.x, b.y), make_float2(b.z, b.w)};
+        mean = ((p[0].x + p[1].x) + (p[2].x + p[3].x)) * inv_n;
+        float m2[PARTS];
+#pragma unroll
+        for (int i = 0; i < PARTS; ++i) {
+            const float d = p[i].x * (1.0f / 128.0f) - mean;
+            m2[i] = fmaf(128.0f * d, d, p[i].y);
+        }
+        rstd = rsqrtf(((m2[0] + m2[1]) + (m2[2] + m2[3])) * inv_n + eps);
     } else {
         // a row's three partials are 24 bytes: 8-byte loads
         const float2 p[PARTS] = {__ldg(st), __ldg(st + 1), __ldg(st + 2)};
@@ -334,9 +347,10 @@ static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __ha
                       stream, ta, tb, e, out, out_lo, M, N, K);
 }
 
-// the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT launch), else
-// 128.  Eight partials (bge-large's 1024-wide LayerNorm) exist for BN = 256 and the text epilogues only: every bge-large N is a
-// multiple of 256.
+// the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT / CLIP text
+// launch), else 128.  Eight partials (bge-large's 1024-wide LayerNorm) exist for BN = 256 and the text epilogues only: every
+// bge-large N is a multiple of 256.  Four partials (the CLIP text tower's 512-wide LayerNorm, folded into QKV and the quick-GELU
+// FFN1) exist for BN = 256 and EPI 0 / 3 only; its residual epilogues take no statistics (pre-LN, stats_in NULL).
 template <int EPI>
 static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                               int K, int sm_count, cudaStream_t stream, int* ctas) {
@@ -344,6 +358,12 @@ static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __ha
     if (e.stats_in != nullptr && e.parts_in == 8) {
         if constexpr (EPI != EPI_BIAS_QGELU_F16) {
             if (wide) return launch_one<EPI, 256, 8>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+        }
+        return cudaErrorInvalidValue;
+    }
+    if (e.stats_in != nullptr && e.parts_in == 4) {
+        if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16) {
+            if (wide) return launch_one<EPI, 256, 4>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
         }
         return cudaErrorInvalidValue;
     }
@@ -377,6 +397,8 @@ static cudaError_t setup_epi() {
     if ((e = setup<EPI, 256, 3>()) != cudaSuccess) return e;
     if ((e = setup<EPI, 128, 6>()) != cudaSuccess) return e;
     if ((e = setup<EPI, 128, 3>()) != cudaSuccess) return e;
+    if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16)
+        if ((e = setup<EPI, 256, 4>()) != cudaSuccess) return e;
     if constexpr (EPI != EPI_BIAS_QGELU_F16) return setup<EPI, 256, 8>();
     return cudaSuccess;
 }
@@ -392,10 +414,10 @@ cudaError_t gemm_init_device() {
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                         int K, int sm_count, cudaStream_t stream, int* ctas) {
     if (N % 128 != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
-    // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 1024, 768
-    // or 384
+    // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 1024, 768,
+    // 512 or 384
     const int ln_width = epi == EPI_BIAS_RES_SPLIT ? N : K;
-    if (e.stats_in != nullptr && ((e.parts_in != 8 && e.parts_in != 6 && e.parts_in != 3) || e.parts_in * 128 != ln_width))
+    if (e.stats_in != nullptr && ((e.parts_in != 8 && e.parts_in != 6 && e.parts_in != 4 && e.parts_in != 3) || e.parts_in * 128 != ln_width))
         return cudaErrorInvalidValue;
     switch (epi) {
         case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);

@@ -14,14 +14,15 @@ enum GemmEpilogue : int {
     EPI_BIAS_QGELU_F16 = 3, // out fp16 = quick_gelu(LNfold(acc) + bias), x * sigmoid(1.702 x)   (CLIP MLP up-projection)
 };
 
-// Three text geometries: bge-base (hidden 768, 12 heads of 64, inter 3072), bge-small (hidden 384, 12 heads of 32, inter 1536)
-// and bge-large (hidden 1024, 16 heads of 64, inter 4096); the ViT tower is 768 wide.  The constants below are bge-base's:
+// Four text geometries: bge-base (hidden 768, 12 heads of 64, inter 3072), bge-small (hidden 384, 12 heads of 32, inter 1536),
+// bge-large (hidden 1024, 16 heads of 64, inter 4096) and the CLIP text tower (hidden 512, 8 heads of 64, inter 2048); the ViT
+// tower is 768 wide.  The constants below are bge-base's:
 // workspaces are sized by them for the runtime's row capacity.  bge-small uses the same buffers densely at its own widths;
 // bge-large, 4/3 of bge-base in every width, uses them densely for 3/4 of the rows (the engine's per-model row capacity).
 constexpr int HIDDEN = 768;
 constexpr int HEADS = 12;  // bge-base, bge-small and the ViT tower
 constexpr int QKV_DIM = 3 * HIDDEN;
-constexpr int STAT_PARTS = HIDDEN / 128;  // row statistics travel as one (sum, M2) partial per 128 columns: 6 (768), 3 (384) or 8 (1024)
+constexpr int STAT_PARTS = HIDDEN / 128;  // row statistics travel as one (sum, M2) partial per 128 columns: 6 (768), 3 (384), 8 (1024) or 4 (512)
 
 // One-time per-device setup (dynamic shared memory opt-in for every kernel). Call with the device current.
 cudaError_t kernels_init_device();
@@ -43,7 +44,7 @@ cudaError_t kernels_init_device();
 //              receives the partials of the new rows (N / 128 per row; must not alias stats_in: other tiles still read those).
 //   N % 128 == 0, K % 64 == 0; rows past M are neither read from out nor written.  Tiles are 128 x 256 when N % 256 == 0,
 //   else 128 x 128.  e.parts_in (with stats_in) must be the LayerNorm'd width / 128, that width being 768 or 384 (K for
-//   EPI 0/1/3, N for EPI 2), or 1024 for EPI 0/1/2 with N % 256 == 0.  ta's map may end at M rows or run past them: a tile's A rows past M only feed rows no store
+//   EPI 0/1/3, N for EPI 2), 1024 for EPI 0/1/2 with N % 256 == 0, or 512 for EPI 0/3 with N % 256 == 0.  ta's map may end at M rows or run past them: a tile's A rows past M only feed rows no store
 //   reaches.
 //   The kernel runs as 2-CTA clusters (two m-tiles sharing one W tile):  min(tile pairs, sm_count / 2, the clusters that
 //   fit at once) clusters, at least one -- sm_count bounds the CTAs from above, rounded down to whole clusters, except that
@@ -67,13 +68,13 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
                            int N, int K, cudaStream_t stream);
 
 // Multi-head self-attention over a padded batch of `heads` heads of head_dim, H = heads head_dim: (head_dim, heads) is
-// (64, 12), (32, 12) or (64, 16).  qkv fp16 [B, S, 3H] (Q | K | V, head-major within each), lens[B] valid keys per item, ctx
+// (64, 12), (32, 12) or (64, 16); causal (key k masked for query row q when k > q, CLIP's text tower): (64, 8) only.  qkv fp16 [B, S, 3H] (Q | K | V, head-major within each), lens[B] valid keys per item, ctx
 // fp16 [B*S, H].  tq: 3D map over qkv {3H, S, B}, tctx: 3D map over ctx {H, S, B}; both box {head_dim, 128, 1}, 128B (d = 64)
 // or 64B (d = 32) swizzle.  Persistent: min(units, sm_count) CTAs walk the (item, head[, query tile]) units.
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                             cudaStream_t stream, int head_dim, int heads);
+                             cudaStream_t stream, int head_dim, int heads, bool causal);
 
-// Text row kernels on rows of `width` (768, 384 or 1024) columns.
+// Text row kernels on rows of `width` (768, 384 or 1024; embed also 512) columns.
 // word + position + token_type(0) embedding gather -> y = hi + lo (pre-LN residual stream) + the row's statistic partials.
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,
                          float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream);
@@ -97,6 +98,15 @@ cudaError_t launch_vit_embed(const __half* patch_out, const float* cls, const fl
                              __half* yhi, __half* ylo, float2* stats, int n_rows, int T, float eps, cudaStream_t stream);
 cudaError_t launch_vit_pool(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const float* proj, float* out,
                             int n_items, int T, int P, float eps, cudaStream_t stream);
+
+// CLIP text tower's pooled head, one block per item: the pooled row p_i of item i is chosen from its ids[i * S .. + len_i)
+// (len_i = lens[i] clamped to [1, S]; ids past it are never read): eos_id == 2 (HF's legacy branch, the original openai
+// configs): the first position of the largest id; otherwise the first position equal to eos_id, 0 when there is none.  Then
+// final_layer_norm(hi + lo of row i * S + p_i) -> projection [P, 512] -> L2 normalise, stored at out + i * P (possibly peer
+// memory).  1 <= P <= 1024.
+cudaError_t launch_clip_text_pool(const __half* yhi, const __half* ylo, const int32_t* ids, const int32_t* lens, const float* gamma,
+                                  const float* beta, const float* proj, float* out, int n_items, int S, int P, float eps, int eos_id,
+                                  cudaStream_t stream);
 
 // Root-side scatter of a wave's token ids / lengths into each shard's (possibly peer) input slot.
 struct ScatterPlan {

@@ -2,7 +2,8 @@
 // L2 normalise with the store aimed at the root GPU's gather buffer, the root-side scatter of token ids into (peer) shard
 // inputs, and the load-time weight preparation (fp32 -> fp16, LayerNorm gamma folded into weight columns).
 //
-// Row kernels: one warp per row (768 wide, or 384 / 1024 for bge-small's / bge-large's embed / pool / LayerNorm), 128-bit accesses, statistics
+// Row kernels: one warp per row (768 wide, or 384 / 1024 for bge-small's / bge-large's embed / pool / LayerNorm, 512 for the CLIP
+// text tower's embed and pool), 128-bit accesses, statistics
 // by warp shuffle in fp32, two-pass variance on register-resident data (no E[x^2]-E[x]^2 cancellation).
 //
 // The residual stream is stored PRE-LayerNorm as y = hi + lo (fp16 + fp16) together with one (sum, M2) partial per 128
@@ -11,6 +12,8 @@
 // Restates BertEmbeddings.forward (HF modeling_bert.py:72-111), the LayerNorm halves of
 // BertSelfOutput :287-298 / BertOutput :345-356, and sentence-transformers' CLS pooling + Normalize
 // (reference 06_gpu_and_ml/gpu_snapshot.py:58, `normalize_embeddings=True`).
+#include <climits>
+
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -22,8 +25,8 @@ namespace rw {
 constexpr int H = HIDDEN;  // 768
 template <int W>
 struct Row {
-    static_assert(W == 768 || W == 384 || W == 1024, "row width");
-    static constexpr int V4 = W / 128;  // float4 per lane: 6, 3 or 8
+    static_assert(W == 768 || W == 384 || W == 1024 || W == 512, "row width");
+    static constexpr int V4 = W / 128;  // float4 per lane: 6, 3, 8 or 4
 };
 constexpr int V4 = Row<H>::V4;
 constexpr int WARPS_PER_BLOCK = 8;
@@ -332,6 +335,76 @@ vit_pool_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, 
     for (int n = threadIdx.x; n < P; n += WARPS_PER_BLOCK * 32) o[n] = s_out[n] * inv;
 }
 
+// ------------------------------------------------------------------------------------------ CLIP text tower (W = 512)
+// Restates the pooled head of CLIPTextTransformer.forward + CLIPTextModelWithProjection.text_projection (HF modeling_clip.py)
+// for infinity's `embed(sentences=...)` on the reference's CLIP model (image_embeddings_infinity.py:76-77, 298-306).
+// One block per item.  The pooled position (see kernels.h) is reduced over the item's valid ids as (key, position) with the
+// smallest position winning ties, so it does not depend on how the ids are strided over the threads.  Every warp then
+// LayerNorms its own copy of the row and takes projection rows n = warp, warp + 8, ..., as vit_pool does.
+constexpr int CLIP_TEXT_POOL_MAX_P = 1024;
+template <int W>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
+clip_text_pool_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, const int32_t* __restrict__ ids,
+                      const int32_t* __restrict__ lens, const float* __restrict__ gamma, const float* __restrict__ beta,
+                      const float* __restrict__ proj, float* __restrict__ out, int S, int P, float eps, int eos_id) {
+    constexpr int V4 = Row<W>::V4;
+    __shared__ float s_out[CLIP_TEXT_POOL_MAX_P];
+    __shared__ float s_red[WARPS_PER_BLOCK];
+    __shared__ int s_key[WARPS_PER_BLOCK], s_pos[WARPS_PER_BLOCK];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int item = blockIdx.x;
+    int L = lens[item];
+    L = L < 1 ? 1 : (L > S ? S : L);
+    const int32_t* row_ids = ids + static_cast<size_t>(item) * S;
+    // key of position p: its id (argmax branch) or 1 where id == eos_id (first-match branch); best = largest key, then the
+    // smallest position.  First-match with no eos in the item: every key is 0 and position 0 wins.  A thread without positions
+    // starts at (INT_MIN, 0), which no valid position loses to except at position 0 itself, so the winner is always in [0, L)
+    // whatever the ids (a device-resident caller's ids are not validated).
+    const bool argmax = eos_id == 2;
+    int key = INT_MIN, pos = 0;
+    for (int p = threadIdx.x; p < L; p += WARPS_PER_BLOCK * 32) {
+        const int id = row_ids[p];
+        const int k = argmax ? id : (id == eos_id ? 1 : 0);
+        if (k > key) { key = k; pos = p; }  // p increases: a tie keeps the earlier position
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const int k2 = __shfl_xor_sync(0xffffffff, key, o), p2 = __shfl_xor_sync(0xffffffff, pos, o);
+        if (k2 > key || (k2 == key && p2 < pos)) { key = k2; pos = p2; }
+    }
+    if (lane == 0) { s_key[warp] = key; s_pos[warp] = pos; }
+    __syncthreads();
+    key = s_key[0];
+    pos = s_pos[0];
+#pragma unroll
+    for (int w = 1; w < WARPS_PER_BLOCK; ++w)
+        if (s_key[w] > key || (s_key[w] == key && s_pos[w] < pos)) { key = s_key[w]; pos = s_pos[w]; }
+    float4 x[V4];
+    load_split_row<W>(yhi, ylo, static_cast<size_t>(item) * S + pos, lane, x);
+    ln_inplace<W>(x, gamma, beta, eps, lane);  // final_layer_norm
+    float sq = 0.f;
+    for (int n = warp; n < P; n += WARPS_PER_BLOCK) {
+        const float4* w4 = reinterpret_cast<const float4*>(proj + static_cast<size_t>(n) * W);
+        float acc = 0.f;
+#pragma unroll
+        for (int i = 0; i < V4; ++i) {
+            const float4 w = __ldg(w4 + i * 32 + lane);
+            acc = fmaf(x[i].x, w.x, fmaf(x[i].y, w.y, fmaf(x[i].z, w.z, fmaf(x[i].w, w.w, acc))));
+        }
+        acc = warp_sum(acc);
+        if (lane == 0) s_out[n] = acc;
+        sq = fmaf(acc, acc, sq);  // identical on every lane after warp_sum
+    }
+    if (lane == 0) s_red[warp] = sq;
+    __syncthreads();
+    float tot = 0.f;
+#pragma unroll
+    for (int w = 0; w < WARPS_PER_BLOCK; ++w) tot += s_red[w];
+    const float inv = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
+    float* o = out + static_cast<size_t>(item) * P;  // may be peer memory
+    for (int n = threadIdx.x; n < P; n += WARPS_PER_BLOCK * 32) o[n] = s_out[n] * inv;
+}
+
 // Load-time weight preparation, one warp per output row n of W[N,K] (see kernels.h, "LNfold"):
 //   gamma given: w_out[n,k] = fp16(w[n,k] gamma[k] - m_n),  m_n = mean_k(w[n,k] gamma[k])   (rows centred: the LayerNorm's mean
 //                subtraction then happens inside the GEMM),  cvec[n] = sum_k w[n,k] beta[k] + bias[n]
@@ -394,6 +467,7 @@ cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos
     if (width == 768) rw::embed_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
     else if (width == 384) rw::embed_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
     else if (width == 1024) rw::embed_kernel<1024><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
+    else if (width == 512) rw::embed_kernel<512><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
@@ -438,6 +512,15 @@ cudaError_t launch_vit_pool(const __half* yhi, const __half* ylo, const float* g
                             int n_items, int T, int P, float eps, cudaStream_t stream) {
     if (P < 1 || P > rw::VIT_POOL_MAX_P) return cudaErrorInvalidValue;
     rw::vit_pool_kernel<<<n_items, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, gamma, beta, proj, out, T, P, eps);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_clip_text_pool(const __half* yhi, const __half* ylo, const int32_t* ids, const int32_t* lens, const float* gamma,
+                                  const float* beta, const float* proj, float* out, int n_items, int S, int P, float eps, int eos_id,
+                                  cudaStream_t stream) {
+    if (n_items < 1 || S < 1 || P < 1 || P > rw::CLIP_TEXT_POOL_MAX_P) return cudaErrorInvalidValue;
+    rw::clip_text_pool_kernel<512><<<n_items, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(yhi, ylo, ids, lens, gamma, beta, proj, out, S, P, eps,
+                                                                                     eos_id);
     return cudaGetLastError();
 }
 

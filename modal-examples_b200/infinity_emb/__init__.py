@@ -1,11 +1,14 @@
 """In-box stand-in for the ``infinity_emb`` engine API that the reference's image-embedding example drives
 (06_gpu_and_ml/embeddings/image_embeddings_infinity.py:126-127, 296-306, 340-356): ``AsyncEmbeddingEngine.from_args(
 EngineArgs(model_name_or_path="openai/clip-vit-base-patch16", engine=torch, dtype=float16, device="cuda"))``,
-``await engine.astart()``, ``embeddings, usage = await engine.image_embed(images=[PIL images])``, ``await engine.astop()``.
+``await engine.astart()``, ``embeddings, usage = await engine.image_embed(images=[PIL images])``, ``await engine.astop()``
+-- and, for searching those images with text, ``embeddings, usage = await engine.embed(sentences=[...])``.
 
 Like ``text-embeddings-router`` (tei_router/), it is the boundary the reference script already talks to, re-implemented
-over the b200rt C ABI: the CLIP ViT-B/16 image tower runs on the hand-written sm_90a kernels (kind "vit"), preprocessing
-is preprocess.clip_preprocess.  The reference starts one engine per concurrent input to pack a GPU with model copies
+over the b200rt C ABI: both towers of the CLIP model run on the hand-written sm_90a kernels -- the ViT-B/16 image tower
+(kind "vit", preprocessing by preprocess.clip_preprocess) and the text tower (kind "clip_text", tokenisation by
+clip_tokenizer, CLIP's byte-level BPE) -- loaded from the same checkpoint, so ``100 cos(image, text)`` is CLIP's
+``logits_per_image``.  The reference starts one engine per concurrent input to pack a GPU with model copies
 (``n_engines``, :283-306); here every engine object of a process shares ONE loaded model and the scheduler's replica pool --
 concurrency comes from tickets in flight, not from model copies.  There is no CPU path: without the CUDA library (or a
 GPU) ``astart`` raises.
@@ -48,46 +51,64 @@ class EngineArgs:
 
 
 _lock = threading.Lock()
-_models: dict[str, dict] = {}  # model name -> {"model": ImageEmbedModel, "refs": n}
+_models: dict[str, dict] = {}  # model name -> {"model": ImageEmbedModel, "text": ClipTextModel, "tok": ClipTokenizer, "refs": n}
 _runtime_refs = 0
 _owns_runtime = False  # whether the first engine brought the runtime up (then the last one shuts it down)
 
 
-def _load_clip(args: EngineArgs):
-    """(geometry, blob, source) for ``args.model_name_or_path``: an explicit weights file / HF directory, else the hub
-    snapshot under $HF_HOME/hub (the reference points HF_HOME at its volume, :112-117), else seeded random init."""
+def _towers(sd: dict, cfg_dir: str):
+    """(vision (geometry, blob), text (geometry, blob) or None) of one CLIPModel state dict; the text tower's eps, heads and
+    eos_token_id come from the snapshot's config.json (``text_config``) when there is one."""
+    from b200rt import weights as W
+
+    text = None
+    if "text_projection.weight" in sd and "text_model.embeddings.token_embedding.weight" in sd:
+        text = W.load_clip_text_state_dict(sd, **W.clip_text_config_from_dir(cfg_dir))
+    return W.load_clip_vision_state_dict(sd), text
+
+
+def _load_clip(args: EngineArgs) -> dict:
+    """Both towers of ``args.model_name_or_path`` from one source: an explicit weights file / HF directory, else the hub
+    snapshot under $HF_HOME/hub (the reference points HF_HOME at its volume, :112-117), else seeded random init.  Returns
+    dict(vision=(geometry, blob), text=(geometry, blob) or None when the source holds no text tower, source=path or None,
+    tok_dir=the directory holding vocab.json / merges.txt, if any)."""
     import numpy as np
     from b200rt import weights as W
+
+    def from_file(p):
+        if p.endswith(".safetensors"):
+            sd = W.read_safetensors(p)
+        else:
+            import torch
+
+            sd = {k: v.float().numpy() for k, v in torch.load(p, map_location="cpu", weights_only=True).items()}
+        d = os.path.dirname(os.path.abspath(p))
+        vision, text = _towers(sd, d)
+        return dict(vision=vision, text=text, source=p, tok_dir=d)
 
     def from_dir(d):
         for name in ("model.safetensors", "pytorch_model.bin"):
             p = os.path.join(d, name)
             if os.path.exists(p):
-                if name.endswith(".safetensors"):
-                    sd = W.read_safetensors(p)
-                else:
-                    import torch
-
-                    sd = {k: v.float().numpy() for k, v in torch.load(p, map_location="cpu", weights_only=True).items()}
-                return W.load_clip_vision_state_dict(sd) + (p,)
+                return from_file(p)
         return None
 
     cand = args.weights or args.model_name_or_path
     if cand.endswith(".safetensors") and os.path.exists(cand):
-        return W.load_clip_vision_state_dict(W.read_safetensors(cand)) + (cand,)
+        return from_file(cand)
     if os.path.isdir(cand):
         got = from_dir(cand)
         if got:
             return got
     if args.weights and os.path.isfile(args.weights):
-        return dict(W.CLIP_VIT_B16_GEOMETRY), np.fromfile(args.weights, np.float32), args.weights
+        return dict(vision=(dict(W.CLIP_VIT_B16_GEOMETRY), np.fromfile(args.weights, np.float32)), text=None, source=args.weights, tok_dir=None)
     for root in (os.environ.get("HF_HUB_CACHE"), os.path.join(os.environ.get("HF_HOME", ""), "hub") if os.environ.get("HF_HOME") else None):
         if root and os.path.isdir(root):
             snap = W.resolve_hub_snapshot(root, args.model_name_or_path)
             got = from_dir(snap) if snap else None
             if got:
                 return got
-    return dict(W.CLIP_VIT_B16_GEOMETRY), W.random_vit_blob(W.CLIP_VIT_B16_GEOMETRY), None
+    return dict(vision=(dict(W.CLIP_VIT_B16_GEOMETRY), W.random_vit_blob(W.CLIP_VIT_B16_GEOMETRY)), text=None, source=None, tok_dir=None)
 
 
 class AsyncEmbeddingEngine:
@@ -106,7 +127,7 @@ class AsyncEmbeddingEngine:
 
     @property
     def capabilities(self) -> set:
-        return {"image_embed"}
+        return {"embed", "image_embed"}
 
     def _start(self):
         global _runtime_refs, _owns_runtime
@@ -130,12 +151,28 @@ class AsyncEmbeddingEngine:
             try:
                 e = _models.get(a.model_name_or_path)
                 if e is None:
-                    geometry, blob, source = _load_clip(a)
-                    if source is None:
+                    from b200rt import weights as W
+
+                    from .clip_tokenizer import ClipTokenizer
+
+                    got = _load_clip(a)
+                    if got["source"] is None:
                         print(f"[infinity_emb/b200] no weights for {a.model_name_or_path!r} offline: seeded random init", file=sys.stderr)
                     else:
-                        print(f"[infinity_emb/b200] weights: {source}", file=sys.stderr)
-                    e = _models[a.model_name_or_path] = {"model": b200rt.ImageEmbedModel(geometry, blob), "refs": 0, "image": geometry["image"]}
+                        print(f"[infinity_emb/b200] weights: {got['source']}", file=sys.stderr)
+                    vg, vblob = got["vision"]
+                    tg, tblob = got["text"] or (dict(W.CLIP_TEXT_B16_GEOMETRY), W.random_clip_text_blob(W.CLIP_TEXT_B16_GEOMETRY))
+                    if got["text"] is None and got["source"] is not None:
+                        print(f"[infinity_emb/b200] {got['source']} holds no text tower: the text tower is seeded random init", file=sys.stderr)
+                    tok = ClipTokenizer.from_dir(got["tok_dir"])
+                    if tok.synthetic:
+                        print("[infinity_emb/b200] ********************************************************************\n"
+                              "[infinity_emb/b200] NO CLIP vocab.json / merges.txt next to the weights: sentences are tokenised with\n"
+                              "[infinity_emb/b200] CLIP's merge-free base vocabulary (one token per byte).  Text embeddings are NOT\n"
+                              "[infinity_emb/b200] the real model's; token-id inputs are unaffected.\n"
+                              "[infinity_emb/b200] ********************************************************************", file=sys.stderr)
+                    e = _models[a.model_name_or_path] = {"model": b200rt.ImageEmbedModel(vg, vblob), "text": b200rt.ClipTextModel(tg, tblob),
+                                                         "tok": tok, "refs": 0, "image": vg["image"]}
             except BaseException:  # a failed load must not leave the runtime referenced by an engine that never ran
                 _runtime_refs -= 1
                 if _runtime_refs == 0 and _owns_runtime:
@@ -190,8 +227,20 @@ class AsyncEmbeddingEngine:
             return [], 0
         return await asyncio.get_running_loop().run_in_executor(None, self._image_embed, list(images))
 
+    def _embed(self, sentences):
+        if not self.running:
+            raise RuntimeError("engine is not running: call `await engine.astart()` first")
+        e = self._entry
+        ids, lens = e["tok"].batch(sentences)
+        out = e["text"].embed(ids, lens)  # [n, proj] float32, unit norm, in the image tower's space
+        return list(out), int(lens.sum())
+
     async def embed(self, *, sentences):
-        raise NotImplementedError("infinity_emb/b200rt serves the image tower only; text goes through text-embeddings-router (tei_router)")
+        """``(embeddings, usage)``: one unit-norm float32 vector per sentence, in the image embeddings' space (CLIP's text
+        tower); usage is the number of tokens, start and end tokens included."""
+        if len(sentences) == 0:
+            return [], 0
+        return await asyncio.get_running_loop().run_in_executor(None, self._embed, list(sentences))
 
 
 class AsyncEngineArray:
