@@ -79,18 +79,44 @@ def random_blob(g: dict = BGE_BASE_GEOMETRY, seed: int = 0) -> np.ndarray:
     """HF default init (normal sigma 0.02, zero biases, unit LayerNorm) drawn tensor by tensor, in blob order, from
     ``numpy.random.default_rng(seed)`` -- the workload weights of BASELINE.md section 3 (bit-identical to the oracle's
     ``pack_blob(make_weights(g, seed, "hf"))``, which tests/test_weights.py checks)."""
+    return _random_blob(blob_layout(g), seed)
+
+
+def _random_blob(layout: list, seed: int) -> np.ndarray:
+    """Seeded weights of a layout, drawn tensor by tensor in blob order: unit LayerNorm gains (``.g``), zero biases and
+    LayerNorm offsets (``.b``), normal sigma 0.02 matrices and embeddings (everything else)."""
     rng = np.random.default_rng(seed)
-    out = np.empty(blob_numel(g), np.float32)
+    out = np.empty(sum(int(np.prod(s)) for _, s in layout), np.float32)
     o = 0
-    for name, shape in blob_layout(g):
+    for name, shape in layout:
         n = int(np.prod(shape))
-        if name.endswith(".w") or (name.startswith("emb.") and not name.startswith("emb.ln")):
-            out[o:o + n] = (rng.standard_normal(shape, dtype=np.float32) * np.float32(0.02)).reshape(-1)
-        elif name.endswith(".g"):
+        if name.endswith(".g"):
             out[o:o + n] = 1.0
-        else:
+        elif name.endswith(".b"):
             out[o:o + n] = 0.0
+        else:
+            out[o:o + n] = (rng.standard_normal(shape, dtype=np.float32) * np.float32(0.02)).reshape(-1)
         o += n
+    return out
+
+
+def _arr(v) -> np.ndarray:
+    """A numpy array or torch tensor of any float dtype as a contiguous fp32 numpy array."""
+    if hasattr(v, "detach"):  # torch tensor
+        v = v.detach().to("cpu").float().numpy()
+    return np.ascontiguousarray(v, dtype=np.float32)
+
+
+def _pack(layout: list, tensors: dict) -> np.ndarray:
+    """The fp32 blob of ``layout`` from ``{layout name: tensor}``; each tensor must have its entry's shape."""
+    out = np.empty(sum(int(np.prod(s)) for _, s in layout), np.float32)
+    o = 0
+    for name, shape in layout:
+        a = _arr(tensors[name])
+        if a.shape != tuple(shape):
+            raise ValueError(f"checkpoint tensor has shape {a.shape}, geometry needs {tuple(shape)}")
+        out[o:o + a.size] = a.reshape(-1)
+        o += a.size
     return out
 
 
@@ -125,47 +151,25 @@ def load_hf_state_dict(sd: dict, g: dict | None = None) -> tuple[dict, np.ndarra
     """HF ``BertModel`` state dict (values: numpy arrays or torch tensors, any float dtype) -> (geometry, fp32 blob).
     Restates the parameter naming of HF ``modeling_bert.py`` (BertEmbeddings :72-111, BertSelfAttention :143-207,
     BertSelfOutput :287-298, BertIntermediate :330-342, BertOutput :345-356)."""
-
-    def arr(v):
-        if hasattr(v, "detach"):  # torch tensor
-            v = v.detach().to("cpu").float().numpy()
-        return np.ascontiguousarray(v, dtype=np.float32)
-
     sd = _strip_prefix(sd)
     g = dict(g) if g is not None else geometry_from_state_dict(sd)
-    out = np.empty(blob_numel(g), np.float32)
-    o = 0
-
-    def put(a, shape):
-        nonlocal o
-        a = arr(a)
-        if a.shape != tuple(shape):
-            raise ValueError(f"checkpoint tensor has shape {a.shape}, geometry needs {tuple(shape)}")
-        out[o:o + a.size] = a.reshape(-1)
-        o += a.size
-
-    h, i = g["hidden"], g["inter"]
-    put(sd["embeddings.word_embeddings.weight"], (g["vocab"], h))
-    put(sd["embeddings.position_embeddings.weight"], (g["max_pos"], h))
-    put(sd["embeddings.token_type_embeddings.weight"], (g["type_vocab"], h))
-    put(sd["embeddings.LayerNorm.weight"], (h,))
-    put(sd["embeddings.LayerNorm.bias"], (h,))
+    t = {"emb.word": sd["embeddings.word_embeddings.weight"], "emb.pos": sd["embeddings.position_embeddings.weight"],
+         "emb.type": sd["embeddings.token_type_embeddings.weight"], "emb.ln.g": sd["embeddings.LayerNorm.weight"],
+         "emb.ln.b": sd["embeddings.LayerNorm.bias"]}
     for l in range(g["layers"]):
-        s = f"encoder.layer.{l}."
-        put(np.concatenate([arr(sd[s + f"attention.self.{n}.weight"]) for n in ("query", "key", "value")], 0), (3 * h, h))
-        put(np.concatenate([arr(sd[s + f"attention.self.{n}.bias"]) for n in ("query", "key", "value")], 0), (3 * h,))
-        put(sd[s + "attention.output.dense.weight"], (h, h))
-        put(sd[s + "attention.output.dense.bias"], (h,))
-        put(sd[s + "attention.output.LayerNorm.weight"], (h,))
-        put(sd[s + "attention.output.LayerNorm.bias"], (h,))
-        put(sd[s + "intermediate.dense.weight"], (i, h))
-        put(sd[s + "intermediate.dense.bias"], (i,))
-        put(sd[s + "output.dense.weight"], (h, i))
-        put(sd[s + "output.dense.bias"], (h,))
-        put(sd[s + "output.LayerNorm.weight"], (h,))
-        put(sd[s + "output.LayerNorm.bias"], (h,))
-    assert o == out.size
-    return g, out
+        s, p = f"encoder.layer.{l}.", f"l{l}."
+        t[p + "qkv.w"] = np.concatenate([_arr(sd[s + f"attention.self.{n}.weight"]) for n in ("query", "key", "value")], 0)
+        t[p + "qkv.b"] = np.concatenate([_arr(sd[s + f"attention.self.{n}.bias"]) for n in ("query", "key", "value")], 0)
+        t.update({p + name: sd[s + hf] for name, hf in _BERT_LAYER.items()})
+    return g, _pack(blob_layout(g), t)
+
+
+# a BERT layer's tensors other than Q, K, V: layout name -> HF name under encoder.layer.N.
+_BERT_LAYER = {"ao.w": "attention.output.dense.weight", "ao.b": "attention.output.dense.bias",
+               "ln1.g": "attention.output.LayerNorm.weight", "ln1.b": "attention.output.LayerNorm.bias",
+               "ff1.w": "intermediate.dense.weight", "ff1.b": "intermediate.dense.bias",
+               "ff2.w": "output.dense.weight", "ff2.b": "output.dense.bias",
+               "ln2.g": "output.LayerNorm.weight", "ln2.b": "output.LayerNorm.bias"}
 
 
 _ST_DTYPES = {"F32": np.float32, "F16": np.float16, "F64": np.float64, "I64": np.int64, "I32": np.int32, "U8": np.uint8}
@@ -264,15 +268,38 @@ def resolve_hub_snapshot(cache_dir: str, model_id: str) -> str | None:
 CLIP_VIT_B16_GEOMETRY = dict(image=224, patch=16, hidden=768, layers=12, heads=12, inter=3072, proj=512, eps=1e-5)
 
 
+def _pre_ln_layer(l: int, h: int, i: int) -> list[tuple[str, tuple[int, ...]]]:
+    """One CLIP encoder layer (both towers) in blob order."""
+    p = f"l{l}."
+    return [(p + "ln1.g", (h,)), (p + "ln1.b", (h,)), (p + "qkv.w", (3 * h, h)), (p + "qkv.b", (3 * h,)),
+            (p + "ao.w", (h, h)), (p + "ao.b", (h,)), (p + "ln2.g", (h,)), (p + "ln2.b", (h,)),
+            (p + "ff1.w", (i, h)), (p + "ff1.b", (i,)), (p + "ff2.w", (h, i)), (p + "ff2.b", (h,))]
+
+
+# a CLIP encoder layer's tensors other than Q, K, V: layout name -> HF name under {vision,text}_model.encoder.layers.N.
+_CLIP_LAYER = {"ln1.g": "layer_norm1.weight", "ln1.b": "layer_norm1.bias",
+               "ao.w": "self_attn.out_proj.weight", "ao.b": "self_attn.out_proj.bias",
+               "ln2.g": "layer_norm2.weight", "ln2.b": "layer_norm2.bias",
+               "ff1.w": "mlp.fc1.weight", "ff1.b": "mlp.fc1.bias", "ff2.w": "mlp.fc2.weight", "ff2.b": "mlp.fc2.bias"}
+
+
+def _clip_layers(sd: dict, prefix: str, layers: int) -> dict:
+    """``{layout name: tensor}`` of the encoder layers under ``prefix`` (``vision_model.`` / ``text_model.``)."""
+    t = {}
+    for l in range(layers):
+        s, p = f"{prefix}encoder.layers.{l}.", f"l{l}."
+        t[p + "qkv.w"] = np.concatenate([_arr(sd[s + f"self_attn.{n}.weight"]) for n in ("q_proj", "k_proj", "v_proj")], 0)
+        t[p + "qkv.b"] = np.concatenate([_arr(sd[s + f"self_attn.{n}.bias"]) for n in ("q_proj", "k_proj", "v_proj")], 0)
+        t.update({p + name: sd[s + hf] for name, hf in _CLIP_LAYER.items()})
+    return t
+
+
 def vit_blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
     h, i = g["hidden"], g["inter"]
     tokens = (g["image"] // g["patch"]) ** 2 + 1
     lay = [("patch.w", (h, 3 * g["patch"] * g["patch"])), ("cls", (h,)), ("pos", (tokens, h)), ("pre.g", (h,)), ("pre.b", (h,))]
     for l in range(g["layers"]):
-        p = f"l{l}."
-        lay += [(p + "ln1.g", (h,)), (p + "ln1.b", (h,)), (p + "qkv.w", (3 * h, h)), (p + "qkv.b", (3 * h,)),
-                (p + "ao.w", (h, h)), (p + "ao.b", (h,)), (p + "ln2.g", (h,)), (p + "ln2.b", (h,)),
-                (p + "ff1.w", (i, h)), (p + "ff1.b", (i,)), (p + "ff2.w", (h, i)), (p + "ff2.b", (h,))]
+        lay += _pre_ln_layer(l, h, i)
     lay += [("post.g", (h,)), ("post.b", (h,)), ("proj.w", (g["proj"], h))]
     return lay
 
@@ -283,31 +310,13 @@ def vit_blob_numel(g: dict) -> int:
 
 def random_vit_blob(g: dict = CLIP_VIT_B16_GEOMETRY, seed: int = 0) -> np.ndarray:
     """Seeded weights of the geometry: normal sigma 0.02 matrices / embeddings, zero biases, unit LayerNorm."""
-    rng = np.random.default_rng(seed)
-    out = np.empty(vit_blob_numel(g), np.float32)
-    o = 0
-    for name, shape in vit_blob_layout(g):
-        n = int(np.prod(shape))
-        if name.endswith(".g"):
-            out[o:o + n] = 1.0
-        elif name.endswith(".b"):
-            out[o:o + n] = 0.0
-        else:
-            out[o:o + n] = (rng.standard_normal(shape, dtype=np.float32) * np.float32(0.02)).reshape(-1)
-        o += n
-    return out
+    return _random_blob(vit_blob_layout(g), seed)
 
 
 def load_clip_vision_state_dict(sd: dict, eps: float = 1e-5, heads: int | None = None) -> tuple[dict, np.ndarray]:
     """HF ``CLIPModel`` / ``CLIPVisionModelWithProjection`` state dict -> (geometry, fp32 blob).  Parameter names as in HF
     ``modeling_clip.py`` (``vision_model.embeddings.*``, ``vision_model.encoder.layers.N.*``, ``visual_projection.weight``)."""
-
-    def arr(v):
-        if hasattr(v, "detach"):
-            v = v.detach().to("cpu").float().numpy()
-        return np.ascontiguousarray(v, dtype=np.float32)
-
-    pw = arr(sd["vision_model.embeddings.patch_embedding.weight"])
+    pw = _arr(sd["vision_model.embeddings.patch_embedding.weight"])
     h, _, p, _ = pw.shape
     tokens = sd["vision_model.embeddings.position_embedding.weight"].shape[0]
     layers = 0
@@ -316,42 +325,12 @@ def load_clip_vision_state_dict(sd: dict, eps: float = 1e-5, heads: int | None =
     grid = int(round((tokens - 1) ** 0.5))
     g = dict(image=grid * p, patch=int(p), hidden=int(h), layers=layers, heads=int(heads or h // 64),
              inter=int(sd["vision_model.encoder.layers.0.mlp.fc1.weight"].shape[0]), proj=int(sd["visual_projection.weight"].shape[0]), eps=float(eps))
-    out = np.empty(vit_blob_numel(g), np.float32)
-    o = 0
-
-    def put(a, shape):
-        nonlocal o
-        a = arr(a)
-        if a.shape != tuple(shape):
-            raise ValueError(f"checkpoint tensor has shape {a.shape}, geometry needs {tuple(shape)}")
-        out[o:o + a.size] = a.reshape(-1)
-        o += a.size
-
-    i = g["inter"]
-    put(pw.reshape(h, 3 * p * p), (h, 3 * p * p))
-    put(sd["vision_model.embeddings.class_embedding"], (h,))
-    put(sd["vision_model.embeddings.position_embedding.weight"], (tokens, h))
-    put(sd["vision_model.pre_layrnorm.weight"], (h,))
-    put(sd["vision_model.pre_layrnorm.bias"], (h,))
-    for l in range(layers):
-        s = f"vision_model.encoder.layers.{l}."
-        put(sd[s + "layer_norm1.weight"], (h,))
-        put(sd[s + "layer_norm1.bias"], (h,))
-        put(np.concatenate([arr(sd[s + f"self_attn.{n}.weight"]) for n in ("q_proj", "k_proj", "v_proj")], 0), (3 * h, h))
-        put(np.concatenate([arr(sd[s + f"self_attn.{n}.bias"]) for n in ("q_proj", "k_proj", "v_proj")], 0), (3 * h,))
-        put(sd[s + "self_attn.out_proj.weight"], (h, h))
-        put(sd[s + "self_attn.out_proj.bias"], (h,))
-        put(sd[s + "layer_norm2.weight"], (h,))
-        put(sd[s + "layer_norm2.bias"], (h,))
-        put(sd[s + "mlp.fc1.weight"], (i, h))
-        put(sd[s + "mlp.fc1.bias"], (i,))
-        put(sd[s + "mlp.fc2.weight"], (h, i))
-        put(sd[s + "mlp.fc2.bias"], (h,))
-    put(sd["vision_model.post_layernorm.weight"], (h,))
-    put(sd["vision_model.post_layernorm.bias"], (h,))
-    put(sd["visual_projection.weight"], (g["proj"], h))
-    assert o == out.size
-    return g, out
+    t = {"patch.w": pw.reshape(h, 3 * p * p), "cls": sd["vision_model.embeddings.class_embedding"],
+         "pos": sd["vision_model.embeddings.position_embedding.weight"], "pre.g": sd["vision_model.pre_layrnorm.weight"],
+         "pre.b": sd["vision_model.pre_layrnorm.bias"], **_clip_layers(sd, "vision_model.", layers),
+         "post.g": sd["vision_model.post_layernorm.weight"], "post.b": sd["vision_model.post_layernorm.bias"],
+         "proj.w": sd["visual_projection.weight"]}
+    return g, _pack(vit_blob_layout(g), t)
 
 
 # ----------------------------------------------------------------------------------------------- CLIP text tower
@@ -368,10 +347,7 @@ def clip_text_blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
     h, i = g["hidden"], g["inter"]
     lay = [("token", (g["vocab"], h)), ("pos", (g["max_pos"], h))]
     for l in range(g["layers"]):
-        p = f"l{l}."
-        lay += [(p + "ln1.g", (h,)), (p + "ln1.b", (h,)), (p + "qkv.w", (3 * h, h)), (p + "qkv.b", (3 * h,)),
-                (p + "ao.w", (h, h)), (p + "ao.b", (h,)), (p + "ln2.g", (h,)), (p + "ln2.b", (h,)),
-                (p + "ff1.w", (i, h)), (p + "ff1.b", (i,)), (p + "ff2.w", (h, i)), (p + "ff2.b", (h,))]
+        lay += _pre_ln_layer(l, h, i)
     lay += [("final.g", (h,)), ("final.b", (h,)), ("proj.w", (g["proj"], h))]
     return lay
 
@@ -382,19 +358,7 @@ def clip_text_blob_numel(g: dict) -> int:
 
 def random_clip_text_blob(g: dict = CLIP_TEXT_B16_GEOMETRY, seed: int = 0) -> np.ndarray:
     """Seeded weights of the geometry: normal sigma 0.02 matrices / embeddings, zero biases, unit LayerNorm."""
-    rng = np.random.default_rng(seed)
-    out = np.empty(clip_text_blob_numel(g), np.float32)
-    o = 0
-    for name, shape in clip_text_blob_layout(g):
-        n = int(np.prod(shape))
-        if name.endswith(".g"):
-            out[o:o + n] = 1.0
-        elif name.endswith(".b"):
-            out[o:o + n] = 0.0
-        else:
-            out[o:o + n] = (rng.standard_normal(shape, dtype=np.float32) * np.float32(0.02)).reshape(-1)
-        o += n
-    return out
+    return _random_blob(clip_text_blob_layout(g), seed)
 
 
 def load_clip_text_state_dict(sd: dict, eps: float = 1e-5, heads: int | None = None, eos_id: int = 2) -> tuple[dict, np.ndarray]:
@@ -402,12 +366,6 @@ def load_clip_text_state_dict(sd: dict, eps: float = 1e-5, heads: int | None = N
     ``modeling_clip.py`` (``text_model.embeddings.*``, ``text_model.encoder.layers.N.*``, ``text_model.final_layer_norm``,
     ``text_projection.weight``).  A state dict without ``text_projection.weight`` (a bare ``CLIPTextModel``) is refused: its
     pooled output is not the embedding infinity serves."""
-
-    def arr(v):
-        if hasattr(v, "detach"):
-            v = v.detach().to("cpu").float().numpy()
-        return np.ascontiguousarray(v, dtype=np.float32)
-
     if "text_projection.weight" not in sd:
         raise KeyError("no text_projection.weight: a CLIPModel or CLIPTextModelWithProjection checkpoint is needed")
     s0 = "text_model."
@@ -419,39 +377,10 @@ def load_clip_text_state_dict(sd: dict, eps: float = 1e-5, heads: int | None = N
              inter=int(sd[s0 + "encoder.layers.0.mlp.fc1.weight"].shape[0]),
              max_pos=int(sd[s0 + "embeddings.position_embedding.weight"].shape[0]), proj=int(sd["text_projection.weight"].shape[0]),
              eos_id=int(eos_id), eps=float(eps))
-    out = np.empty(clip_text_blob_numel(g), np.float32)
-    o = 0
-
-    def put(a, shape):
-        nonlocal o
-        a = arr(a)
-        if a.shape != tuple(shape):
-            raise ValueError(f"checkpoint tensor has shape {a.shape}, geometry needs {tuple(shape)}")
-        out[o:o + a.size] = a.reshape(-1)
-        o += a.size
-
-    i = g["inter"]
-    put(sd[s0 + "embeddings.token_embedding.weight"], (g["vocab"], h))
-    put(sd[s0 + "embeddings.position_embedding.weight"], (g["max_pos"], h))
-    for l in range(layers):
-        s = f"{s0}encoder.layers.{l}."
-        put(sd[s + "layer_norm1.weight"], (h,))
-        put(sd[s + "layer_norm1.bias"], (h,))
-        put(np.concatenate([arr(sd[s + f"self_attn.{n}.weight"]) for n in ("q_proj", "k_proj", "v_proj")], 0), (3 * h, h))
-        put(np.concatenate([arr(sd[s + f"self_attn.{n}.bias"]) for n in ("q_proj", "k_proj", "v_proj")], 0), (3 * h,))
-        put(sd[s + "self_attn.out_proj.weight"], (h, h))
-        put(sd[s + "self_attn.out_proj.bias"], (h,))
-        put(sd[s + "layer_norm2.weight"], (h,))
-        put(sd[s + "layer_norm2.bias"], (h,))
-        put(sd[s + "mlp.fc1.weight"], (i, h))
-        put(sd[s + "mlp.fc1.bias"], (i,))
-        put(sd[s + "mlp.fc2.weight"], (h, i))
-        put(sd[s + "mlp.fc2.bias"], (h,))
-    put(sd[s0 + "final_layer_norm.weight"], (h,))
-    put(sd[s0 + "final_layer_norm.bias"], (h,))
-    put(sd["text_projection.weight"], (g["proj"], h))
-    assert o == out.size
-    return g, out
+    t = {"token": sd[s0 + "embeddings.token_embedding.weight"], "pos": sd[s0 + "embeddings.position_embedding.weight"],
+         **_clip_layers(sd, s0, layers), "final.g": sd[s0 + "final_layer_norm.weight"], "final.b": sd[s0 + "final_layer_norm.bias"],
+         "proj.w": sd["text_projection.weight"]}
+    return g, _pack(clip_text_blob_layout(g), t)
 
 
 def clip_text_config_from_dir(path: str) -> dict:

@@ -1078,11 +1078,75 @@ int rt_init(const int* devices, int n, uint32_t flags) {
     return 0;
 }
 
-struct BlobCursor {
-    size_t f32 = 0, f16 = 0;
+// ---- weight layouts
+//
+// A model kind describes its weights as one list: the blob's tensors in blob order, plus arena-only vectors that have no blob
+// bytes.  Each entry gives the tensor's size, where it lands in a replica's DevWeights and what the root does with it.
+// load_weights walks the list once for every blob offset and arena offset; the root's copies and every replica's pointers
+// are both taken from those offsets.
+
+// a DevWeights member (layer < 0) or a member of its layers[layer]
+template <class T>
+struct Slot {
+    using Top = T DevWeights::*;
+    using PerLayer = T LayerW::*;
+    Top top = nullptr;
+    PerLayer per_layer = nullptr;
+    T* in(DevWeights& w, int layer) const { return layer >= 0 ? &(w.layers[layer].*per_layer) : top ? &(w.*top) : nullptr; }
 };
 
-// ---- load steps every model kind shares (the caller holds the root replica's mu)
+struct LayoutEntry {
+    enum Op {
+        COPY,     // fp32 blob tensor, copied
+        HALF,     // fp32 blob GEMM weight [n, k] -> fp16, with a LayerNorm folded in when gamma >= 0 (kernels.h)
+        ZERO,     // arena only: zero fp32
+        DERIVED,  // arena only: the fp32 c = W beta + b that the folding HALF entry naming it writes
+    } op;
+    size_t n, k;  // n * k elements (fp32 entries: k = 1)
+    int layer;
+    Slot<float*> f32;
+    Slot<__half*> f16;      // HALF: the weight and its GEMM B-operand map (box {64,128})
+    Slot<CUtensorMap> map;
+    int gamma = -1, beta = -1, bias = -1, cvec = -1;  // a folding HALF: the entries it reads and the DERIVED one it writes
+    size_t src = 0, off = 0;  // blob offset, arena offset (set by load_weights)
+};
+
+struct Layout {
+    std::vector<LayoutEntry> e;
+    int add(const LayoutEntry& x) {
+        e.push_back(x);
+        return static_cast<int>(e.size()) - 1;
+    }
+    int copy(size_t n, float* DevWeights::*dst) { return add({LayoutEntry::COPY, n, 1, -1, {dst}}); }
+    int copy(int l, size_t n, float* LayerW::*dst) { return add({LayoutEntry::COPY, n, 1, l, {nullptr, dst}}); }
+    void zero(size_t n, float* DevWeights::*dst = nullptr) { add({LayoutEntry::ZERO, n, 1, -1, {dst}}); }
+    void half(size_t n, size_t k, __half* DevWeights::*dst, CUtensorMap DevWeights::*map) {
+        add({LayoutEntry::HALF, n, k, -1, {}, {dst}, {map}});
+    }
+    int half(int l, size_t n, size_t k, __half* LayerW::*dst, CUtensorMap LayerW::*map) {
+        return add({LayoutEntry::HALF, n, k, l, {}, {nullptr, dst}, {nullptr, map}});
+    }
+    // fold the LayerNorm (entries gamma, beta) into HALF entry w; c = W beta + (entry bias) lands in w's layer's member `c`
+    void fold(int w, int gamma, int beta, int bias, float* LayerW::*c) {
+        const int cv = add({LayoutEntry::DERIVED, e[w].n, 1, e[w].layer, {nullptr, c}});
+        LayoutEntry& x = e[w];
+        x.gamma = gamma, x.beta = beta, x.bias = bias, x.cvec = cv;
+    }
+};
+
+// a pre-LN layer (ViT, CLIP text): ln1.g ln1.b qkv.w qkv.b ao.w ao.b ln2.g ln2.b ff1.w ff1.b ff2.w ff2.b; QKV folds ln1, FFN1 ln2
+void pre_ln_layer(Layout& L, int l, size_t H, size_t I) {
+    const int ln1_g = L.copy(l, H, &LayerW::ln1_g), ln1_b = L.copy(l, H, &LayerW::ln1_b);
+    const int qkv = L.half(l, 3 * H, H, &LayerW::qkv_w, &LayerW::m_qkv);
+    L.fold(qkv, ln1_g, ln1_b, L.copy(l, 3 * H, &LayerW::qkv_b), &LayerW::qkv_c);
+    L.half(l, H, H, &LayerW::ao_w, &LayerW::m_ao);
+    L.copy(l, H, &LayerW::ao_b);
+    const int ln2_g = L.copy(l, H, &LayerW::ln2_g), ln2_b = L.copy(l, H, &LayerW::ln2_b);
+    const int ff1 = L.half(l, I, H, &LayerW::ff1_w, &LayerW::m_ff1);
+    L.fold(ff1, ln2_g, ln2_b, L.copy(l, I, &LayerW::ff1_b), &LayerW::ff1_c);
+    L.half(l, H, I, &LayerW::ff2_w, &LayerW::m_ff2);
+    L.copy(l, H, &LayerW::ff2_b);
+}
 
 // the fp32 blob onto the root, an fp32 and an fp16 arena (m.f32_elems, m.f16_elems) on every replica; leaves the root current
 int upload_blob(Runtime& rt, Model& m, const float* blob, size_t nbytes, float** d_blob) {
@@ -1113,25 +1177,53 @@ int broadcast_arenas(Runtime& rt, Model& m, float* d_blob) {
     return 0;
 }
 
-// the GEMM B-operand maps of one layer's weights (box {64,128})
-int make_layer_maps(LayerW& lw, size_t H, size_t I) {
-    if (int rc = make_map_2d(&lw.m_qkv, lw.qkv_w, 3 * H, H, 128)) return rc;
-    if (int rc = make_map_2d(&lw.m_ao, lw.ao_w, H, H, 128)) return rc;
-    if (int rc = make_map_2d(&lw.m_ff1, lw.ff1_w, I, H, 128)) return rc;
-    return make_map_2d(&lw.m_ff2, lw.ff2_w, H, I, 128);
-}
+// m's weights as L lists them, on every replica: checks the blob's size, has the root carve its arenas out of the blob on the
+// GPU (copies, fp16 conversions, LayerNorm folds, zero fills), broadcasts them, and sets every replica's pointers and weight
+// tensor maps.  The caller holds the root replica's mu.
+int load_weights(Runtime& rt, Model& m, Layout& L, const float* blob, size_t nbytes) {
+    size_t blob_elems = 0;
+    for (LayoutEntry& e : L.e) {
+        // Tensors lie back to back, so each size keeps the next tensor 16-byte aligned: the row kernels read fp32 vectors as
+        // float4, the GEMM epilogues as float2, and TMA needs 16-byte fp16 bases.
+        if (e.n * e.k % 8 != 0) return fail(B200RT_E_STATE, "internal: a %zu-element weight tensor misaligns the arena", e.n * e.k);
+        size_t& arena = e.op == LayoutEntry::HALF ? m.f16_elems : m.f32_elems;
+        e.src = blob_elems, e.off = arena;
+        arena += e.n * e.k;
+        if (e.op == LayoutEntry::COPY || e.op == LayoutEntry::HALF) blob_elems += e.n * e.k;
+    }
+    if (nbytes != blob_elems * 4) return fail(B200RT_E_INVALID, "weight blob is %zu bytes, geometry needs %zu", nbytes, blob_elems * 4);
 
-// one pre-LN layer's pointers (ViT and CLIP text arenas): fp32 ln1.g ln1.b qkv.b ao.b ln2.g ln2.b ff1.b ff2.b qkv_c ff1_c, fp16
-// qkv.w ao.w ff1.w ff2.w
-void carve_pre_ln_layer(LayerW& lw, float*& p, __half*& q, size_t H, size_t I) {
-    lw.ln1_g = p; p += H;  lw.ln1_b = p; p += H;
-    lw.qkv_w = q; q += 3 * H * H;  lw.qkv_b = p; p += 3 * H;
-    lw.ao_w = q;  q += H * H;      lw.ao_b = p;  p += H;
-    lw.ln2_g = p; p += H;  lw.ln2_b = p; p += H;
-    lw.ff1_w = q; q += I * H;      lw.ff1_b = p; p += I;
-    lw.ff2_w = q; q += H * I;      lw.ff2_b = p; p += H;
-    lw.qkv_c = p; p += 3 * H;
-    lw.ff1_c = p; p += I;
+    m.per_dev.resize(rt.devs.size());
+    Dev& root = *rt.devs[0];
+    float* d_blob = nullptr;
+    if (int rc = upload_blob(rt, m, blob, nbytes, &d_blob)) return rc;
+    const DevWeights& rw = m.per_dev[0];
+    auto blob_at = [&](int i) -> const float* { return i < 0 ? nullptr : d_blob + L.e[i].src; };
+    for (const LayoutEntry& e : L.e) {
+        if (e.op == LayoutEntry::COPY)
+            CUDA_TRY(cudaMemcpyAsync(rw.f32_arena + e.off, d_blob + e.src, e.n * 4, cudaMemcpyDeviceToDevice, root.compute));
+        else if (e.op == LayoutEntry::ZERO)
+            CUDA_TRY(cudaMemsetAsync(rw.f32_arena + e.off, 0, e.n * 4, root.compute));
+        else if (e.op == LayoutEntry::HALF)
+            CUDA_TRY(launch_fold_ln(d_blob + e.src, blob_at(e.gamma), blob_at(e.beta), blob_at(e.bias), rw.f16_arena + e.off,
+                                    e.cvec < 0 ? nullptr : rw.f32_arena + L.e[e.cvec].off, static_cast<int>(e.n), static_cast<int>(e.k),
+                                    root.compute));
+    }
+    if (int rc = broadcast_arenas(rt, m, d_blob)) return rc;
+    for (size_t g = 0; g < rt.devs.size(); ++g) {
+        DevWeights& w = m.per_dev[g];
+        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
+        w.layers.resize(m.layers);
+        for (const LayoutEntry& e : L.e) {
+            if (e.op != LayoutEntry::HALF) {
+                if (float** p = e.f32.in(w, e.layer)) *p = w.f32_arena + e.off;
+                continue;
+            }
+            __half* q = *e.f16.in(w, e.layer) = w.f16_arena + e.off;
+            if (int rc = make_map_2d(e.map.in(w, e.layer), q, e.n, e.k, 128)) return rc;
+        }
+    }
+    return 0;
 }
 
 int register_model(Runtime& rt, std::unique_ptr<Model> m, int* model_out) {
@@ -1141,6 +1233,8 @@ int register_model(Runtime& rt, std::unique_ptr<Model> m, int* model_out) {
     *model_out = static_cast<int>(rt.models.size()) - 1;
     return 0;
 }
+
+// model_load* run under the root replica's mu (b200rt_model_load_ex)
 
 int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out) {
     Runtime& rt = *g_rt;
@@ -1156,12 +1250,6 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
         return fail(B200RT_E_INVALID,
                     "a hidden=%d model needs room for one %d-token item, and the workspace holds %d of its rows: initialise with a "
                     "larger B200RT_INIT_WAVE_ITEMS (now %d)", c.hidden, MAX_SEQ, cap_rows, rt.cap_items);
-    const size_t H = c.hidden, I = c.inter;
-    const size_t emb = (static_cast<size_t>(c.vocab) + c.max_pos + c.type_vocab) * H + 2 * H;
-    const size_t per_layer_w = 3 * H * H + H * H + I * H + H * I;
-    const size_t per_layer_p = 3 * H + H + 2 * H + I + H + 2 * H;
-    const size_t total = emb + static_cast<size_t>(c.layers) * (per_layer_w + per_layer_p);
-    if (nbytes != total * 4) return fail(B200RT_E_INVALID, "weight blob is %zu bytes, geometry needs %zu", nbytes, total * 4);
 
     auto m = std::make_unique<Model>();
     m->cfg = c;
@@ -1170,78 +1258,30 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->cap_rows = cap_rows;
     m->out_dim = c.hidden;
-    const size_t per_layer_x = 3 * H + I;  // derived vectors: qkv_c, ff1_c
-    const size_t blob_f32 = emb + static_cast<size_t>(c.layers) * per_layer_p;
-    m->f32_elems = blob_f32 + static_cast<size_t>(c.layers) * per_layer_x;
-    m->f16_elems = static_cast<size_t>(c.layers) * per_layer_w;
-    m->per_dev.resize(rt.devs.size());
 
-    // root: upload the fp32 blob once, carve fp32 params / convert GEMM weights to fp16 on the GPU.  The LayerNorm in front of
-    // a projection is folded into it here (kernels.h): QKV of layer l takes the previous layer's LN2 (the embedding LN for
-    // l = 0), FFN1 takes the layer's own LN1.
-    Dev& root = *rt.devs[0];
-    std::lock_guard<std::mutex> dl(root.mu);
-    float* d_blob = nullptr;
-    if (int rc = upload_blob(rt, *m, blob, nbytes, &d_blob)) return rc;
-    DevWeights& rw = m->per_dev[0];
-    {
-        size_t src = 0, o32 = 0, o16 = 0, ox = blob_f32;
-        auto take32 = [&](size_t n) -> cudaError_t {
-            cudaError_t e = cudaMemcpyAsync(rw.f32_arena + o32, d_blob + src, n * 4, cudaMemcpyDeviceToDevice, root.compute);
-            src += n; o32 += n;
-            return e;
-        };
-        // W [N,K] at the cursor -> fp16 (gamma folded in and rows centred when given; W beta + b into the derived region)
-        auto take16 = [&](size_t N_, size_t K_, const float* gamma, const float* beta, const float* bias) -> cudaError_t {
-            float* cv = gamma ? rw.f32_arena + ox : nullptr;
-            cudaError_t e = launch_fold_ln(d_blob + src, gamma, beta, bias, rw.f16_arena + o16, cv, static_cast<int>(N_),
-                                           static_cast<int>(K_), root.compute);
-            src += N_ * K_; o16 += N_ * K_;
-            if (gamma) ox += N_;
-            return e;
-        };
-        const float* ln_g = d_blob + emb - 2 * H;  // the LayerNorm in front of the next QKV: embedding LN first
-        const float* ln_b = d_blob + emb - H;
-        CUDA_TRY(take32(emb));
-        for (int l = 0; l < c.layers; ++l) {
-            const float* qkv_b = d_blob + src + 3 * H * H;
-            CUDA_TRY(take16(3 * H, H, ln_g, ln_b, qkv_b)); CUDA_TRY(take32(3 * H));      // qkv.w (folded), qkv.b
-            CUDA_TRY(take16(H, H, nullptr, nullptr, nullptr));                            // ao.w
-            const float* ln1_g = d_blob + src + H;
-            const float* ln1_b = d_blob + src + 2 * H;
-            CUDA_TRY(take32(H + 2 * H));                                                  // ao.b, ln1.g, ln1.b
-            const float* ff1_b = d_blob + src + I * H;
-            CUDA_TRY(take16(I, H, ln1_g, ln1_b, ff1_b)); CUDA_TRY(take32(I));            // ff1.w (folded), ff1.b
-            CUDA_TRY(take16(H, I, nullptr, nullptr, nullptr));                            // ff2.w
-            ln_g = d_blob + src + H;                                                      // ln2 of this layer feeds the next QKV
-            ln_b = d_blob + src + 2 * H;
-            CUDA_TRY(take32(H + 2 * H));                                                  // ff2.b, ln2.g, ln2.b
-        }
+    // b200rt.weights.blob_layout.  QKV of layer l folds the LayerNorm in front of it, the previous layer's ln2 (the embedding
+    // LN for l = 0); FFN1 folds the layer's own ln1.
+    const size_t H = c.hidden, I = c.inter;
+    Layout L;
+    L.copy(c.vocab * H, &DevWeights::word);
+    L.copy(c.max_pos * H, &DevWeights::pos);
+    L.copy(c.type_vocab * H, &DevWeights::type);
+    int ln_g = L.copy(H, &DevWeights::emb_g);
+    int ln_b = L.copy(H, &DevWeights::emb_b);
+    for (int l = 0; l < c.layers; ++l) {
+        const int qkv = L.half(l, 3 * H, H, &LayerW::qkv_w, &LayerW::m_qkv);
+        L.fold(qkv, ln_g, ln_b, L.copy(l, 3 * H, &LayerW::qkv_b), &LayerW::qkv_c);
+        L.half(l, H, H, &LayerW::ao_w, &LayerW::m_ao);
+        L.copy(l, H, &LayerW::ao_b);
+        const int ln1_g = L.copy(l, H, &LayerW::ln1_g), ln1_b = L.copy(l, H, &LayerW::ln1_b);
+        const int ff1 = L.half(l, I, H, &LayerW::ff1_w, &LayerW::m_ff1);
+        L.fold(ff1, ln1_g, ln1_b, L.copy(l, I, &LayerW::ff1_b), &LayerW::ff1_c);
+        L.half(l, H, I, &LayerW::ff2_w, &LayerW::m_ff2);
+        L.copy(l, H, &LayerW::ff2_b);
+        ln_g = L.copy(l, H, &LayerW::ln2_g);
+        ln_b = L.copy(l, H, &LayerW::ln2_b);
     }
-    if (int rc = broadcast_arenas(rt, *m, d_blob)) return rc;
-    // carve pointers + weight tensor maps per replica
-    for (size_t g = 0; g < rt.devs.size(); ++g) {
-        DevWeights& w = m->per_dev[g];
-        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
-        float* p = w.f32_arena;
-        __half* q = w.f16_arena;
-        w.word = p; p += static_cast<size_t>(c.vocab) * H;
-        w.pos = p;  p += static_cast<size_t>(c.max_pos) * H;
-        w.type = p; p += static_cast<size_t>(c.type_vocab) * H;
-        w.emb_g = p; p += H;
-        w.emb_b = p; p += H;
-        w.layers.resize(c.layers);
-        for (int l = 0; l < c.layers; ++l) {
-            LayerW& lw = w.layers[l];
-            lw.qkv_w = q; q += 3 * H * H;  lw.qkv_b = p; p += 3 * H;
-            lw.ao_w = q;  q += H * H;      lw.ao_b = p;  p += H;  lw.ln1_g = p; p += H;  lw.ln1_b = p; p += H;
-            lw.ff1_w = q; q += I * H;      lw.ff1_b = p; p += I;
-            lw.ff2_w = q; q += H * I;      lw.ff2_b = p; p += H;  lw.ln2_g = p; p += H;  lw.ln2_b = p; p += H;
-            float* x = w.f32_arena + blob_f32 + static_cast<size_t>(l) * per_layer_x;
-            lw.qkv_c = x; lw.ff1_c = x + 3 * H;
-            if (int rc = make_layer_maps(lw, H, I)) return rc;
-        }
-    }
+    if (int rc = load_weights(rt, *m, L, blob, nbytes)) return rc;
     return register_model(rt, std::move(m), model_out);
 }
 
@@ -1254,11 +1294,6 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
         PD != HIDDEN || c.patch % 2 != 0 || c.proj < 1 || c.proj > 1024)
         return fail(B200RT_E_UNSUPPORTED, "kernels are specialised for ViT-B: hidden=768 heads=12 inter=3072, <= 512 tokens, 3*patch^2 %% 64 == 0, proj <= 1024 "
                                           "(got hidden %d heads %d inter %d image %d patch %d proj %d)", c.hidden, c.heads, c.inter, c.image, c.patch, c.proj);
-    const size_t per_layer_w = 3 * H * H + H * H + I * H + H * I;
-    const size_t per_layer_p = 2 * H + 3 * H + H + 2 * H + I + H;  // ln1, qkv.b, ao.b, ln2, ff1.b, ff2.b
-    const size_t head = H * PD + H + static_cast<size_t>(T) * H + 2 * H, tail = 2 * H + P * H;
-    const size_t total = head + static_cast<size_t>(c.layers) * (per_layer_w + per_layer_p) + tail;
-    if (nbytes != total * 4) return fail(B200RT_E_INVALID, "weight blob is %zu bytes, geometry needs %zu", nbytes, total * 4);
 
     auto m = std::make_unique<Model>();
     m->kind = KIND_VIT;
@@ -1268,15 +1303,21 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
     m->tokens = T;
     m->out_dim = c.proj;
     m->item_bytes = static_cast<size_t>(3) * c.image * c.image * 4;
-    const size_t per_layer_x = 3 * H + I;  // qkv_c, ff1_c
-    m->f32_elems = (head - H * PD) + static_cast<size_t>(c.layers) * (per_layer_p + per_layer_x) + tail + H /* zero bias */;
-    m->f16_elems = H * PD + static_cast<size_t>(c.layers) * per_layer_w;
-    m->per_dev.resize(rt.devs.size());
 
-    Dev& root = *rt.devs[0];
-    std::lock_guard<std::mutex> dl(root.mu);
-    float* d_blob = nullptr;
-    if (int rc = upload_blob(rt, *m, blob, nbytes, &d_blob)) return rc;
+    // b200rt.weights.vit_blob_layout, plus the patch projection's zero bias
+    Layout L;
+    L.half(H, PD, &DevWeights::patch_w, &DevWeights::m_patch);
+    L.copy(H, &DevWeights::cls);
+    L.copy(T * H, &DevWeights::pos);
+    L.copy(H, &DevWeights::pre_g);
+    L.copy(H, &DevWeights::pre_b);
+    for (int l = 0; l < c.layers; ++l) pre_ln_layer(L, l, H, I);
+    L.copy(H, &DevWeights::post_g);
+    L.copy(H, &DevWeights::post_b);
+    L.copy(P * H, &DevWeights::proj_w);
+    L.zero(H, &DevWeights::zero_bias);
+    if (int rc = load_weights(rt, *m, L, blob, nbytes)) return rc;
+
     for (size_t g = 0; g < rt.devs.size(); ++g) {
         Dev& d = *rt.devs[g];
         CUDA_TRY(cudaSetDevice(d.id));
@@ -1296,79 +1337,9 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
     if (rt.vit_item_bytes != 0 && rt.vit_item_bytes != m->item_bytes)
         return fail(B200RT_E_UNSUPPORTED, "a second vit model with a different image size is not supported in one runtime");
     rt.vit_item_bytes = m->item_bytes;
-    CUDA_TRY(cudaSetDevice(root.id));
-    DevWeights& rw = m->per_dev[0];
-    {
-        size_t src = 0, o32 = 0, o16 = 0;
-        auto take32 = [&](size_t n) -> cudaError_t {
-            cudaError_t e = cudaMemcpyAsync(rw.f32_arena + o32, d_blob + src, n * 4, cudaMemcpyDeviceToDevice, root.compute);
-            src += n; o32 += n;
-            return e;
-        };
-        auto skip32 = [&](size_t n) { o32 += n; };  // derived vectors are written in place by the fold kernel
-        auto take16 = [&](size_t N_, size_t K_, const float* gamma, const float* beta, const float* bias, float* cv) -> cudaError_t {
-            cudaError_t e = launch_fold_ln(d_blob + src, gamma, beta, bias, rw.f16_arena + o16, cv, static_cast<int>(N_), static_cast<int>(K_), root.compute);
-            src += N_ * K_; o16 += N_ * K_;
-            return e;
-        };
-        CUDA_TRY(take16(H, PD, nullptr, nullptr, nullptr, nullptr));   // patch.w
-        CUDA_TRY(take32(H + static_cast<size_t>(T) * H + 2 * H));       // cls, pos, pre.g, pre.b
-        for (int l = 0; l < c.layers; ++l) {
-            const float* ln1_g = d_blob + src;
-            const float* ln1_b = d_blob + src + H;
-            CUDA_TRY(take32(2 * H));                                    // ln1.g, ln1.b
-            const float* qkv_b = d_blob + src + 3 * H * H;
-            float* qkv_c = rw.f32_arena + o32 + (3 * H) + H + 2 * H + I + H;  // after qkv.b ao.b ln2.g ln2.b ff1.b ff2.b
-            CUDA_TRY(take16(3 * H, H, ln1_g, ln1_b, qkv_b, qkv_c));     // qkv.w folded with ln1
-            CUDA_TRY(take32(3 * H));                                    // qkv.b
-            CUDA_TRY(take16(H, H, nullptr, nullptr, nullptr, nullptr)); // ao.w
-            CUDA_TRY(take32(H));                                        // ao.b
-            const float* ln2_g = d_blob + src;
-            const float* ln2_b = d_blob + src + H;
-            CUDA_TRY(take32(2 * H));                                    // ln2.g, ln2.b
-            const float* ff1_b = d_blob + src + I * H;
-            float* ff1_c = rw.f32_arena + o32 + I + H + 3 * H;          // after ff1.b ff2.b qkv_c
-            CUDA_TRY(take16(I, H, ln2_g, ln2_b, ff1_b, ff1_c));         // ff1.w folded with ln2
-            CUDA_TRY(take32(I));                                        // ff1.b
-            CUDA_TRY(take16(H, I, nullptr, nullptr, nullptr, nullptr)); // ff2.w
-            CUDA_TRY(take32(H));                                        // ff2.b
-            skip32(3 * H + I);                                          // qkv_c, ff1_c
-        }
-        CUDA_TRY(take32(2 * H + P * H));                                // post.g, post.b, proj.w
-        CUDA_TRY(cudaMemsetAsync(rw.f32_arena + o32, 0, H * 4, root.compute));  // zero bias for the patch projection
-        o32 += H;
-        if (o32 != m->f32_elems || o16 != m->f16_elems || src != total) return fail(B200RT_E_STATE, "internal: vit blob carve mismatch");
-    }
-    if (int rc = broadcast_arenas(rt, *m, d_blob)) return rc;
-    for (size_t g = 0; g < rt.devs.size(); ++g) {
-        DevWeights& w = m->per_dev[g];
-        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
-        float* p = w.f32_arena;
-        __half* q = w.f16_arena;
-        w.patch_w = q; q += H * PD;
-        if (int rc = make_map_2d(&w.m_patch, w.patch_w, H, PD, 128)) return rc;
-        w.cls = p; p += H;
-        w.pos = p; p += static_cast<size_t>(T) * H;
-        w.pre_g = p; p += H;
-        w.pre_b = p; p += H;
-        w.layers.resize(c.layers);
-        for (int l = 0; l < c.layers; ++l) {
-            LayerW& lw = w.layers[l];
-            carve_pre_ln_layer(lw, p, q, H, I);
-            if (int rc = make_layer_maps(lw, H, I)) return rc;
-        }
-        w.post_g = p; p += H;
-        w.post_b = p; p += H;
-        w.proj_w = p; p += P * H;
-        w.zero_bias = p; p += H;
-    }
     return register_model(rt, std::move(m), model_out);
 }
 
-// CLIP text tower (kind "clip_text").  Blob order (fp32, b200rt.weights.clip_text_blob_layout): token [V, H] | pos [max_pos, H] |
-// per layer ln1.g ln1.b qkv.w [3H,H] qkv.b ao.w ao.b ln2.g ln2.b ff1.w [I,H] ff1.b ff2.w [H,I] ff2.b | final.g final.b |
-// proj.w [P, H].  fp32 arena: token | pos padded to TEXT_POS_ROWS zero rows | a zero type row | per layer ln1.g ln1.b qkv.b ao.b
-// ln2.g ln2.b ff1.b ff2.b qkv_c ff1_c | final.g final.b | proj.w.
 constexpr int TEXT_POS_ROWS = 128;  // embed_kernel reads pos[t % S] for every row of a wave padded to its bucket (<= 128)
 int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, size_t nbytes, int* model_out) {
     Runtime& rt = *g_rt;
@@ -1381,12 +1352,6 @@ int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, si
     if (c.max_pos < 1 || c.max_pos > TEXT_POS_ROWS)
         return fail(B200RT_E_UNSUPPORTED, "max_pos %d outside [1, %d]", c.max_pos, TEXT_POS_ROWS);
     if (c.eos_id < 0 || c.eos_id >= c.vocab) return fail(B200RT_E_INVALID, "eos_id %d outside the vocabulary [0, %d)", c.eos_id, c.vocab);
-    const size_t H = c.hidden, I = c.inter, P = c.proj, V = c.vocab;
-    const size_t per_layer_w = 3 * H * H + H * H + I * H + H * I;
-    const size_t per_layer_p = 2 * H + 3 * H + H + 2 * H + I + H;  // ln1, qkv.b, ao.b, ln2, ff1.b, ff2.b
-    const size_t per_layer_x = 3 * H + I;                          // qkv_c, ff1_c
-    const size_t total = V * H + static_cast<size_t>(c.max_pos) * H + static_cast<size_t>(c.layers) * (per_layer_w + per_layer_p) + 2 * H + P * H;
-    if (nbytes != total * 4) return fail(B200RT_E_INVALID, "weight blob is %zu bytes, geometry needs %zu", nbytes, total * 4);
 
     auto m = std::make_unique<Model>();
     m->kind = KIND_CLIP_TEXT;
@@ -1395,74 +1360,19 @@ int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, si
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->cap_rows = model_cap_rows(rt.cap_rows, c.hidden);
     m->out_dim = c.proj;
-    m->f32_elems = V * H + TEXT_POS_ROWS * H + H + static_cast<size_t>(c.layers) * (per_layer_p + per_layer_x) + 2 * H + P * H;
-    m->f16_elems = static_cast<size_t>(c.layers) * per_layer_w;
-    m->per_dev.resize(rt.devs.size());
 
-    Dev& root = *rt.devs[0];
-    std::lock_guard<std::mutex> dl(root.mu);
-    float* d_blob = nullptr;
-    if (int rc = upload_blob(rt, *m, blob, nbytes, &d_blob)) return rc;
-    DevWeights& rw = m->per_dev[0];
-    {
-        size_t src = 0, o32 = 0, o16 = 0;
-        auto take32 = [&](size_t n) -> cudaError_t {
-            cudaError_t e = cudaMemcpyAsync(rw.f32_arena + o32, d_blob + src, n * 4, cudaMemcpyDeviceToDevice, root.compute);
-            src += n; o32 += n;
-            return e;
-        };
-        auto zero32 = [&](size_t n) -> cudaError_t {  // arena-only zeros (position padding, type row)
-            cudaError_t e = cudaMemsetAsync(rw.f32_arena + o32, 0, n * 4, root.compute);
-            o32 += n;
-            return e;
-        };
-        auto take16 = [&](size_t N_, size_t K_, const float* gamma, const float* beta, const float* bias, float* cv) -> cudaError_t {
-            cudaError_t e = launch_fold_ln(d_blob + src, gamma, beta, bias, rw.f16_arena + o16, cv, static_cast<int>(N_), static_cast<int>(K_), root.compute);
-            src += N_ * K_; o16 += N_ * K_;
-            return e;
-        };
-        CUDA_TRY(take32(V * H + static_cast<size_t>(c.max_pos) * H));  // token, pos
-        CUDA_TRY(zero32((TEXT_POS_ROWS - static_cast<size_t>(c.max_pos)) * H + H));  // pos padding, type row
-        for (int l = 0; l < c.layers; ++l) {
-            float* lb = rw.f32_arena + o32;  // this layer's f32 region: its derived vectors follow its per_layer_p params
-            const float* ln1_g = d_blob + src;
-            const float* ln1_b = d_blob + src + H;
-            CUDA_TRY(take32(2 * H));                                        // ln1.g, ln1.b
-            CUDA_TRY(take16(3 * H, H, ln1_g, ln1_b, d_blob + src + 3 * H * H, lb + per_layer_p));  // qkv.w folded with ln1
-            CUDA_TRY(take32(3 * H));                                        // qkv.b
-            CUDA_TRY(take16(H, H, nullptr, nullptr, nullptr, nullptr));     // ao.w
-            CUDA_TRY(take32(H));                                            // ao.b
-            const float* ln2_g = d_blob + src;
-            const float* ln2_b = d_blob + src + H;
-            CUDA_TRY(take32(2 * H));                                        // ln2.g, ln2.b
-            CUDA_TRY(take16(I, H, ln2_g, ln2_b, d_blob + src + I * H, lb + per_layer_p + 3 * H));  // ff1.w folded with ln2
-            CUDA_TRY(take32(I));                                            // ff1.b
-            CUDA_TRY(take16(H, I, nullptr, nullptr, nullptr, nullptr));     // ff2.w
-            CUDA_TRY(take32(H));                                            // ff2.b
-            o32 += per_layer_x;                                             // qkv_c, ff1_c (written by the folds)
-        }
-        CUDA_TRY(take32(2 * H + P * H));                                    // final.g, final.b, proj.w
-        if (o32 != m->f32_elems || o16 != m->f16_elems || src != total) return fail(B200RT_E_STATE, "internal: clip_text blob carve mismatch");
-    }
-    if (int rc = broadcast_arenas(rt, *m, d_blob)) return rc;
-    for (size_t g = 0; g < rt.devs.size(); ++g) {
-        DevWeights& w = m->per_dev[g];
-        CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
-        float* p = w.f32_arena;
-        __half* q = w.f16_arena;
-        w.word = p; p += V * H;
-        w.pos = p;  p += TEXT_POS_ROWS * H;
-        w.type = p; p += H;
-        w.layers.resize(c.layers);
-        for (int l = 0; l < c.layers; ++l) {
-            LayerW& lw = w.layers[l];
-            carve_pre_ln_layer(lw, p, q, H, I);
-            if (int rc = make_layer_maps(lw, H, I)) return rc;
-        }
-        w.post_g = p; p += H;
-        w.post_b = p; p += H;
-        w.proj_w = p; p += P * H;
-    }
+    // b200rt.weights.clip_text_blob_layout, with pos padded to TEXT_POS_ROWS zero rows and a zero type row
+    const size_t H = c.hidden, I = c.inter;
+    Layout L;
+    L.copy(c.vocab * H, &DevWeights::word);
+    L.copy(c.max_pos * H, &DevWeights::pos);
+    L.zero((TEXT_POS_ROWS - c.max_pos) * H);  // the rest of pos: the arena lays it right after pos's max_pos rows
+    L.zero(H, &DevWeights::type);
+    for (int l = 0; l < c.layers; ++l) pre_ln_layer(L, l, H, I);
+    L.copy(H, &DevWeights::post_g);
+    L.copy(H, &DevWeights::post_b);
+    L.copy(c.proj * H, &DevWeights::proj_w);
+    if (int rc = load_weights(rt, *m, L, blob, nbytes)) return rc;
     return register_model(rt, std::move(m), model_out);
 }
 
@@ -1632,6 +1542,7 @@ int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights,
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
     if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
     const bool pool_mean = (flags & B200RT_LOAD_POOL_MEAN) != 0;
+    std::lock_guard<std::mutex> dl(rt->devs[0]->mu);  // a load enqueues on the root's compute stream
     if (strcmp(kind, "vit") == 0) {
         if (pool_mean) return fail(B200RT_E_INVALID, "B200RT_LOAD_POOL_MEAN applies to text encoders (kind \"bert\"), not \"vit\"");
         return model_load_vit(*static_cast<const b200rt_vit_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);

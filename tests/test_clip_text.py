@@ -182,7 +182,9 @@ def test_blob_layout_sizes():
     g = W.CLIP_TEXT_B16_GEOMETRY
     n = W.clip_text_blob_numel(g)
     assert n == 49408 * 512 + 77 * 512 + 12 * (4 * 512 * 512 + 2 * 512 * 2048 + 9 * 512 + 2048) + 2 * 512 + 512 * 512
-    assert W.random_clip_text_blob(dict(g, vocab=1000, layers=1)).size == W.clip_text_blob_numel(dict(g, vocab=1000, layers=1))
+    small = dict(g, vocab=1000, layers=2)
+    for seed in (0, 7):
+        assert np.array_equal(W.random_clip_text_blob(small, seed), T.pack_blob(T.make_weights(small, seed, "hf"), small))
 
 
 def test_flops_per_item_at_bucket_128():
