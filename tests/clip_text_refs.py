@@ -178,21 +178,24 @@ def rel_l2(a, b):
 
 
 # ------------------------------------------------------------------------ kernel references at kernel precision
-def causal_attention_ref(qkv16, lens, B, S, heads=8, hd=64):
+def causal_attention_ref(qkv16, lens, B, S, heads=8, hd=64, rows=None):
     """What the causal attention kernel returns, in fp64 (keys >= len and keys after the query masked, len clamped to [1, S]),
-    and its elementwise tolerance: tests/attention_refs.py's terms, per query row over the keys that row sees."""
+    and its elementwise tolerance: tests/attention_refs.py's terms, per query row over the keys that row sees.  `rows`: for
+    each item, the query rows (within the item, ascending) to compute; the result then holds those rows, item after item."""
     from kernel_refs import SUB16, U16, U32, acc_ulps
 
-    qkv = np.asarray(qkv16, np.float16).astype(np.float64).reshape(B, S, 3, heads, hd)
+    qkv = np.asarray(qkv16, np.float16).reshape(B, S, 3, heads, hd)
     scale = 1.0 / np.sqrt(hd)
-    out, tol = np.empty((B, S, heads, hd)), np.empty((B, S, heads, hd))
+    out, tol = [], []
     for b in range(B):
         n = int(np.clip(lens[b], 1, S))
-        q = qkv[b, :, 0].transpose(1, 0, 2)
-        k, v = (qkv[b, :n, j].transpose(1, 0, 2) for j in (1, 2))
+        x = qkv[b].astype(np.float64)
+        qi = np.arange(S) if rows is None else np.asarray(rows[b], np.int64)
+        q = (x[:, 0] if rows is None else x[qi, 0]).transpose(1, 0, 2)
+        k, v = (x[:n, j].transpose(1, 0, 2) for j in (1, 2))
         s = q @ k.transpose(0, 2, 1)
         s_tol = acc_ulps(hd) * U32 * (np.abs(q) @ np.abs(k).transpose(0, 2, 1)) + 2.0 * U32 * np.abs(s)
-        s = np.where(np.arange(n)[None, None, :] > np.arange(S)[None, :, None], -np.inf, s)
+        s = np.where(np.arange(n)[None, None, :] > qi[None, :, None], -np.inf, s)
         e = np.exp((s - s.max(-1, keepdims=True)) * scale)
         p = e / e.sum(-1, keepdims=True)
         ctx = p @ v
@@ -200,14 +203,16 @@ def causal_attention_ref(qkv16, lens, B, S, heads=8, hd=64):
         spread = pv + np.abs(ctx)
         t = (U16 * np.abs(ctx) + U16 * pv + SUB16 * p.max(-1, keepdims=True) * np.abs(v).sum(-2, keepdims=True)
              + scale * np.where(p > 0, s_tol, 0).max(-1, keepdims=True) * spread + (acc_ulps(n) + 16.0) * U32 * spread + SUB16)
-        out[b], tol[b] = ctx.transpose(1, 0, 2), t.transpose(1, 0, 2)
-    return out.reshape(B * S, -1), tol.reshape(B * S, -1)
+        out.append(ctx.transpose(1, 0, 2).reshape(len(qi), -1))
+        tol.append(t.transpose(1, 0, 2).reshape(len(qi), -1))
+    return np.concatenate(out), np.concatenate(tol)
 
 
-def check_causal_attention(what, ctx, qkv16, lens, B, S):
+def check_causal_attention(what, ctx, qkv16, lens, B, S, rows=None):
+    """`rows` as causal_attention_ref's: ctx then holds those query rows only, item after item."""
     import kernel_refs as KR
 
-    ref, tol = causal_attention_ref(qkv16, lens, B, S)
+    ref, tol = causal_attention_ref(qkv16, lens, B, S, rows=rows)
     got = np.asarray(ctx, np.float16).astype(np.float64)
     assert np.isfinite(got).all(), f"{what}: non-finite output (padded query rows must stay finite too)"
     return KR.check(what, got, ref, tol)

@@ -190,15 +190,17 @@ def check_gemm_stats(what, stats_out, epi_args, **kw):
 
 # ------------------------------------------------------------------------------------------------ attention
 
-def attention_ref(qkv16, lens, B, S):
-    """ctx [B*S, 768] in fp64 (keys >= len masked, len clamped to [1, S] as the kernel does) and its tolerance."""
-    qkv = np.asarray(qkv16, np.float16).astype(np.float64).reshape(B, S, 3, 12, 64)
+def attention_ref(qkv16, lens, B, S, rows=None):
+    """ctx [B*S, 768] in fp64 (keys >= len masked, len clamped to [1, S] as the kernel does) and its tolerance.  `rows`: for
+    each item, the query rows (within the item, ascending) to compute; the result then holds those rows, item after item."""
+    qkv = np.asarray(qkv16, np.float16).reshape(B, S, 3, 12, 64)
     L = np.clip(np.asarray(lens, np.int64), 1, S)
-    ctx_all, tol_all = np.empty((B, S, 12, 64)), np.empty((B, S, 12, 64))
+    ctx_all, tol_all = [], []
     for b in range(B):  # one item at a time: [12, S, S] fp64 score arrays
         n = int(L[b])
-        qq = qkv[b, :, 0].transpose(1, 0, 2)        # [12, S, 64]
-        kk, vv = (qkv[b, :n, j].transpose(1, 0, 2) for j in (1, 2))  # valid keys only: [12, n, 64]
+        x = qkv[b].astype(np.float64)
+        qq = (x[:, 0] if rows is None else x[np.asarray(rows[b], np.int64), 0]).transpose(1, 0, 2)  # [12, S, 64]
+        kk, vv = (x[:n, j].transpose(1, 0, 2) for j in (1, 2))  # valid keys only: [12, n, 64]
         s = qq @ kk.transpose(0, 2, 1)
         s_tol = acc_ulps(64) * U32 * (np.abs(qq) @ np.abs(kk).transpose(0, 2, 1)) + 2.0 * U32 * np.abs(s)  # + the fma into ex2
         e = np.exp((s - s.max(-1, keepdims=True)) * 0.125)
@@ -212,12 +214,14 @@ def attention_ref(qkv16, lens, B, S):
                + 0.125 * s_tol.max(-1, keepdims=True) * spread  # score errors move P
                + (acc_ulps(n) + 16.0) * U32 * spread            # P.V and the row sum in fp32, ex2.approx, the rescales
                + SUB16)
-        ctx_all[b], tol_all[b] = ctx.transpose(1, 0, 2), tol.transpose(1, 0, 2)
-    return ctx_all.reshape(B * S, H), tol_all.reshape(B * S, H)
+        ctx_all.append(ctx.transpose(1, 0, 2).reshape(-1, H))
+        tol_all.append(tol.transpose(1, 0, 2).reshape(-1, H))
+    return np.concatenate(ctx_all), np.concatenate(tol_all)
 
 
-def check_attention(what, ctx, qkv16, lens, B, S):
-    ref, tol = attention_ref(qkv16, lens, B, S)
+def check_attention(what, ctx, qkv16, lens, B, S, rows=None):
+    """`rows` as attention_ref's: ctx then holds those query rows only, item after item."""
+    ref, tol = attention_ref(qkv16, lens, B, S, rows)
     got = np.asarray(ctx, np.float16).astype(np.float64)
     assert np.isfinite(got).all(), f"{what}: non-finite output (padded query rows must stay finite too)"
     return check(what, got, ref, tol)
@@ -267,10 +271,13 @@ def check_bits(what, got, want):
     assert not bad.any(), f"{what}: first differing at {np.argwhere(bad)[:4].tolist()}: got {g[bad][:4]}, want {w[bad][:4]}"
 
 
-def check_embed(what, hi, lo, stats, ids, word, pos, type0, S):
+def check_embed(what, hi, lo, stats, ids, word, pos, type0, S, rows=None):
+    """hi and lo bit for bit over every row; the partials over `rows` (stats then holds those rows), by default all."""
     hi_r, lo_r, x = embed_exact(ids, word, pos, type0, S)
     check_bits(f"{what} hi", hi, hi_r)
     check_bits(f"{what} lo", lo, lo_r)
+    if rows is not None:
+        x = x[rows]
     fin = np.isfinite(x).all(-1)  # rows that overflow fp32 have no meaningful statistics
     return check_partials(f"{what} partials", np.asarray(stats)[fin], x[fin].astype(np.float64))
 

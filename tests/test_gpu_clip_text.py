@@ -144,13 +144,14 @@ class ClipTextChain:
     """The text tower's weights as the engine holds them (pre-LN as tests/test_gpu_forward_chain.py's VitChain: LN1 folded
     into QKV, LN2 into FFN1, no LayerNorm re-applied to the residual), the batch, and the check of each launch at its kernel
     reference's precision on the operands the launch consumed.  The embedding reads the position table as the engine pads it
-    (128 rows, zero past max_pos)."""
+    (128 rows, zero past max_pos).  `rows` as tests/test_gpu_forward_chain.py's TextChain."""
 
-    def __init__(self, flat, g, ids, lens, fold):
+    def __init__(self, flat, g, ids, lens, fold, rows=None):
         self.flat, self.g = flat, g
         self.ids, self.lens = np.asarray(ids, np.int32), np.asarray(lens, np.int32)
         self.B, self.S = self.ids.shape
         self.M = self.B * self.S
+        FC.set_rows(self, rows)
         f, L, H = flat, g["layers"], g["hidden"]
         self.pos = np.zeros((128, H), np.float32)
         self.pos[:g["max_pos"]] = f["pos"]
@@ -162,40 +163,39 @@ class ClipTextChain:
     def check(self, tag, name, l, prev, cur):
         M, g, f, p, S = self.M, self.g, self.flat, f"l{l}.", self.S
         eps = g["eps"]
-        P = lambda t, b: t[b][:M]  # noqa: E731
+        P = lambda t, b: t[b][self.rows]  # noqa: E731
+        A = lambda t, b: t[b][:M]  # noqa: E731
         what = f"{tag} layer {l} {name}"
         if name == "embed":
-            return KR.check_embed(what, P(cur, "yhi"), P(cur, "ylo"), P(cur, "pstats0"), self.ids.reshape(-1), f["token"], self.pos[:S],
-                                  np.zeros(g["hidden"], np.float32), S)
+            return KR.check_embed(what, A(cur, "yhi"), A(cur, "ylo"), P(cur, "pstats0"), self.ids.reshape(-1), f["token"], self.pos[:S],
+                                  np.zeros(g["hidden"], np.float32), S, rows=self.rows)
         if name == "gemm_qkv":
             w16, c = self.qkv[l]
             return KR.check_gemm(what, P(cur, "qkv"), 0, P(prev, "yhi"), w16, c, ln_stats=P(prev, "pstats0"), eps=eps)
         if name == "attention":
-            return T.check_causal_attention(what, P(cur, "ctx"), P(prev, "qkv"), self.lens, self.B, S)
+            return T.check_causal_attention(what, P(cur, "ctx"), A(prev, "qkv"), self.lens, self.B, S, rows=self.q_rows)
         if name == "gemm_attn_out":
-            return FC._check_residual(what, cur, "pstats1", M, (P(prev, "ctx"), self.ao16[l], f[p + "ao.b"]),
+            return FC._check_residual(what, cur, "pstats1", self.rows, (P(prev, "ctx"), self.ao16[l], f[p + "ao.b"]),
                                       dict(resid_hilo=(P(prev, "yhi"), P(prev, "ylo"))))
         if name == "gemm_ffn1_qgelu":
             w16, c = self.ff1[l]
             return KR.check_gemm(what, P(cur, "ffn"), 3, P(prev, "yhi"), w16, c, ln_stats=P(prev, "pstats1"), eps=eps)
         if name == "gemm_ffn2":
-            return FC._check_residual(what, cur, "pstats0", M, (P(prev, "ffn"), self.ff216[l], f[p + "ff2.b"]),
+            return FC._check_residual(what, cur, "pstats0", self.rows, (P(prev, "ffn"), self.ff216[l], f[p + "ff2.b"]),
                                       dict(resid_hilo=(P(prev, "yhi"), P(prev, "ylo"))))
         if name == "clip_text_pool":
-            return T.check_clip_text_pool(what, cur["out"], P(prev, "yhi"), P(prev, "ylo"), self.ids, self.lens, f["final.g"], f["final.b"],
+            return T.check_clip_text_pool(what, cur["out"], A(prev, "yhi"), A(prev, "ylo"), self.ids, self.lens, f["final.g"], f["final.b"],
                                           f["proj.w"], S, eps, g["eos_id"])
         raise AssertionError(f"{tag}: unexpected launch {name!r}")
 
 
 @pytest.mark.parametrize("eos_id", [2, 49407])
-def test_clip_text_chain(rt, monkeypatch, eos_id):
+def test_clip_text_chain(rt, eos_id):
     """Every launch of a 2-layer tower through tests/test_gpu_forward_chain.py's run_chain (its buffer invariants: nothing
     written past M, guard rows still poison, every row < M finite, padding included) on a ragged batch in the 128-token
     bucket -- items of 65-77 tokens travel there, so the embedding reads position rows 77-127 of the padded table for the
     padding rows.  Then the product path: embed() of the same items, through the scheduler's 64- and 128-token buckets and
     graph replay, is bitwise the traced pooled output, and one forward is 5 L + 2 launches (+ the wave's scatter)."""
-    monkeypatch.setitem(FC.WRITES, "clip_text_pool", ())  # the pool launch writes only `out`, as the other pools
-    monkeypatch.setattr(FC, "POOLS", FC.POOLS + ("clip_text_pool",))
     g, flat, model = get_model(rt, 2, "trained", 1, eos_id)
     lens = np.array([77, 1, 64, 65, 30, 2], np.int32)
     ids = T.synth_ids(lens, 128, seed=5)  # <|endoftext|> padding past len, as the tokenizer pads

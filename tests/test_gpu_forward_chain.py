@@ -25,20 +25,22 @@ import pytest
 import attention_refs as AR
 import kernel_emul as KE
 import kernel_refs as KR
+import mean_pool_refs as MP
 from oracle import bge_ref as R
 from oracle import clip_ref as C
 
 gpu = pytest.mark.gpu
 
 BUFFERS = ("yhi", "ylo", "pstats0", "pstats1", "qkv", "ctx", "ffn")
-GUARD = 256  # rows past M a trace returns
+GUARD = 256  # rows past M a trace returns, as far as the model's capacity allows
 # the workspace buffers each launch writes (the pool launches write only `out`)
 WRITES = {
     "embed": ("yhi", "ylo", "pstats0"), "gemm_qkv": ("qkv",), "attention": ("ctx",), "gemm_attn_out": ("yhi", "ylo", "pstats1"),
     "gemm_ffn1_gelu": ("ffn",), "gemm_ffn2": ("yhi", "ylo", "pstats0"), "pool_normalize": (),
     "im2col": ("ffn",), "gemm_patch": ("ctx",), "vit_embed": ("yhi", "ylo", "pstats0"), "gemm_ffn1_qgelu": ("ffn",), "vit_pool": (),
+    "mean_pool_normalize": (), "clip_text_pool": (),
 }
-POOLS = ("pool_normalize", "vit_pool")
+POOLS = ("pool_normalize", "vit_pool", "mean_pool_normalize", "clip_text_pool")
 
 
 def _bits(a):
@@ -72,15 +74,30 @@ def check_invariants(tag, name, prev, cur, ch):
         assert np.isfinite(cur["out"]).all(), f"{tag}: {name}: non-finite pooled output"
 
 
+def set_rows(ch, rows):
+    """The rows the row-wise checks of `ch` read: all M (rows None) or an ascending sample.  Sets ch.rows (an index into the
+    first M rows) and ch.q_rows (None, or each item's sampled rows within the item, for the attention references)."""
+    if rows is None:
+        ch.rows, ch.q_rows = slice(0, ch.M), None
+        return
+    rows = np.asarray(rows, np.int64)
+    assert (np.diff(rows) > 0).all() and rows[0] >= 0 and rows[-1] < ch.M, "rows must be ascending and below M"
+    ch.rows = rows
+    cut = np.searchsorted(rows, np.arange(ch.B + 1) * ch.S)
+    ch.q_rows = [rows[cut[b]:cut[b + 1]] - b * ch.S for b in range(ch.B)]
+
+
 class TextChain:
     """A text encoder's weights as the engine holds them, the batch, and the check of each launch.  `fold(w, gamma, beta, bias)`
-    gives the fp16 folded weight and cvec (gamma None: fp16(w), None)."""
+    gives the fp16 folded weight and cvec (gamma None: fp16(w), None).  `rows` (ascending, < M): check the GEMM, attention and
+    statistics outputs on those rows only, every column of each; the embedding's bits and the pools are checked in full."""
 
-    def __init__(self, flat, g, ids, lens, fold):
+    def __init__(self, flat, g, ids, lens, fold, rows=None):
         self.flat, self.g, self.ids, self.lens = flat, g, np.asarray(ids, np.int32), np.asarray(lens, np.int32)
         self.B, self.S = self.ids.shape
         self.M = self.B * self.S
         self.hd = g.hidden // g.heads
+        set_rows(self, rows)
         f = flat
         self.qkv, self.ff1, self.ao16, self.ff216 = [], [], [], []
         for l in range(g.layers):
@@ -99,41 +116,47 @@ class TextChain:
     def check(self, tag, name, l, prev, cur):
         M, g, f, p = self.M, self.g, self.flat, f"l{l}."
         eps = g.eps
-        P = lambda t, b: t[b][:M]  # noqa: E731
+        P = lambda t, b: t[b][self.rows]  # noqa: E731
+        A = lambda t, b: t[b][:M]  # noqa: E731
         what = f"{tag} layer {l} {name}"
         if name == "embed":
-            return KR.check_embed(what, P(cur, "yhi"), P(cur, "ylo"), P(cur, "pstats0"), self.ids.reshape(-1), f["emb.word"],
-                                  f["emb.pos"], f["emb.type"][0], self.S)
+            return KR.check_embed(what, A(cur, "yhi"), A(cur, "ylo"), P(cur, "pstats0"), self.ids.reshape(-1), f["emb.word"],
+                                  f["emb.pos"], f["emb.type"][0], self.S, rows=self.rows)
         if name == "gemm_qkv":
             w16, c = self.qkv[l]
             return KR.check_gemm(what, P(cur, "qkv"), 0, P(prev, "yhi"), w16, c, ln_stats=P(prev, "pstats0"), eps=eps)
         if name == "attention":
-            if self.hd == 64:
-                return KR.check_attention(what, P(cur, "ctx"), P(prev, "qkv"), self.lens, self.B, self.S)
-            return AR.check_attention(what, P(cur, "ctx"), P(prev, "qkv"), self.lens, self.B, self.S, heads=g.heads, head_dim=self.hd)
+            if self.hd == 64 and g.heads == 12:
+                return KR.check_attention(what, P(cur, "ctx"), A(prev, "qkv"), self.lens, self.B, self.S, rows=self.q_rows)
+            return AR.check_attention(what, P(cur, "ctx"), A(prev, "qkv"), self.lens, self.B, self.S, heads=g.heads, head_dim=self.hd,
+                                      rows=self.q_rows)
         if name in ("gemm_attn_out", "gemm_ffn2"):
             if name == "gemm_attn_out":
                 a, w16, bias, (lg, lb), st_in, st_out = P(prev, "ctx"), self.ao16[l], f[p + "ao.b"], self.prev_ln(l), "pstats0", "pstats1"
             else:
                 a, w16, bias, (lg, lb), st_in, st_out = P(prev, "ffn"), self.ff216[l], f[p + "ff2.b"], (f[p + "ln1.g"], f[p + "ln1.b"]), "pstats1", "pstats0"
             kw = dict(resid_hilo=(P(prev, "yhi"), P(prev, "ylo")), ln_stats=P(prev, st_in), ln_gamma=lg, ln_beta=lb, eps=eps)
-            return _check_residual(what, cur, st_out, M, (a, w16, bias), kw)
+            return _check_residual(what, cur, st_out, self.rows, (a, w16, bias), kw)
         if name == "gemm_ffn1_gelu":
             w16, c = self.ff1[l]
             return KR.check_gemm(what, P(cur, "ffn"), 1, P(prev, "yhi"), w16, c, ln_stats=P(prev, "pstats1"), eps=eps)
         if name == "pool_normalize":
             last = f"l{g.layers - 1}.ln2."
-            return KR.check_pool_normalize(what, cur["out"], P(prev, "yhi"), P(prev, "ylo"), f[last + "g"], f[last + "b"], self.S, eps)
+            return KR.check_pool_normalize(what, cur["out"], A(prev, "yhi"), A(prev, "ylo"), f[last + "g"], f[last + "b"], self.S, eps)
+        if name == "mean_pool_normalize":
+            last = f"l{g.layers - 1}.ln2."
+            return MP.check_mean_pool_normalize(what, cur["out"], A(prev, "yhi"), A(prev, "ylo"), f[last + "g"], f[last + "b"], self.lens,
+                                                self.S, eps)
         raise AssertionError(f"{tag}: unexpected launch {name!r}")
 
 
-def _check_residual(what, cur, st_out, M, args, kw):
+def _check_residual(what, cur, st_out, rows, args, kw):
     """A residual epilogue: the new hi + lo in place against the fp64 reference, hi the nearest fp16, and the partials of the new
-    rows in `st_out`."""
-    hi, lo = cur["yhi"][:M], cur["ylo"][:M]
+    rows in `st_out` -- on `rows` (the operands in args / kw are those rows')."""
+    hi, lo = cur["yhi"][rows], cur["ylo"][rows]
     m = KR.check_gemm(what, KR.hilo64(hi, lo), 2, *args, **kw)
     KR.hi_is_nearest(what, hi, lo)
-    return max(m, KR.check_gemm_stats(f"{what} {st_out}", cur[st_out][:M], args, **kw))
+    return max(m, KR.check_gemm_stats(f"{what} {st_out}", cur[st_out][rows], args, **kw))
 
 
 def im2col_ref(pixels, g):
@@ -145,12 +168,13 @@ def im2col_ref(pixels, g):
 
 class VitChain:
     """The ViT tower's weights as the engine holds them (LN1 folded into QKV, LN2 into FFN1, no LayerNorm re-applied to the
-    residual), the batch, and the check of each launch."""
+    residual), the batch, and the check of each launch.  `rows` as TextChain's (im2col, vit_embed and the pool in full)."""
 
-    def __init__(self, flat, g, pixels, fold):
+    def __init__(self, flat, g, pixels, fold, rows=None):
         self.flat, self.g, self.pixels = flat, g, np.asarray(pixels, np.float32)
         self.B, self.S = self.pixels.shape[0], g.tokens
         self.M = self.B * self.S
+        set_rows(self, rows)
         f = flat
         self.patch16 = fold(f["patch.w"])[0]
         self.qkv = [fold(f[f"l{l}.qkv.w"], f[f"l{l}.ln1.g"], f[f"l{l}.ln1.b"], f[f"l{l}.qkv.b"]) for l in range(g.layers)]
@@ -161,43 +185,45 @@ class VitChain:
     def check(self, tag, name, l, prev, cur):
         M, g, f, p = self.M, self.g, self.flat, f"l{l}."
         eps, T = g.eps, self.S
-        P = lambda t, b: t[b][:M]  # noqa: E731
+        P = lambda t, b: t[b][self.rows]  # noqa: E731
+        A = lambda t, b: t[b][:M]  # noqa: E731
         what = f"{tag} layer {l} {name}"
         im2col = lambda t: t["ffn"].reshape(-1)[:M * 3 * g.patch ** 2].reshape(M, -1)  # noqa: E731
         if name == "im2col":
             KR.check_bits(what, im2col(cur), im2col_ref(self.pixels, g))
             return 0.0
         if name == "gemm_patch":
-            return KR.check_gemm(what, P(cur, "ctx"), 0, im2col(prev), self.patch16, np.zeros(g.hidden, np.float32))
+            return KR.check_gemm(what, P(cur, "ctx"), 0, im2col(prev)[self.rows], self.patch16, np.zeros(g.hidden, np.float32))
         if name == "vit_embed":
-            return KR.check_vit_embed(what, P(cur, "yhi"), P(cur, "ylo"), P(cur, "pstats0"), P(prev, "ctx"), f["cls"], f["pos"],
+            return KR.check_vit_embed(what, A(cur, "yhi"), A(cur, "ylo"), A(cur, "pstats0"), A(prev, "ctx"), f["cls"], f["pos"],
                                       f["pre.g"], f["pre.b"], T, eps)
         if name == "gemm_qkv":
             w16, c = self.qkv[l]
             return KR.check_gemm(what, P(cur, "qkv"), 0, P(prev, "yhi"), w16, c, ln_stats=P(prev, "pstats0"), eps=eps)
         if name == "attention":
-            return KR.check_attention(what, P(cur, "ctx"), P(prev, "qkv"), [T] * self.B, self.B, T)
+            return KR.check_attention(what, P(cur, "ctx"), A(prev, "qkv"), [T] * self.B, self.B, T, rows=self.q_rows)
         if name == "gemm_attn_out":
-            return _check_residual(what, cur, "pstats1", M, (P(prev, "ctx"), self.ao16[l], f[p + "ao.b"]),
+            return _check_residual(what, cur, "pstats1", self.rows, (P(prev, "ctx"), self.ao16[l], f[p + "ao.b"]),
                                    dict(resid_hilo=(P(prev, "yhi"), P(prev, "ylo"))))
         if name == "gemm_ffn1_qgelu":
             w16, c = self.ff1[l]
             return KR.check_gemm(what, P(cur, "ffn"), 3, P(prev, "yhi"), w16, c, ln_stats=P(prev, "pstats1"), eps=eps)
         if name == "gemm_ffn2":
-            return _check_residual(what, cur, "pstats0", M, (P(prev, "ffn"), self.ff216[l], f[p + "ff2.b"]),
+            return _check_residual(what, cur, "pstats0", self.rows, (P(prev, "ffn"), self.ff216[l], f[p + "ff2.b"]),
                                    dict(resid_hilo=(P(prev, "yhi"), P(prev, "ylo"))))
         if name == "vit_pool":
-            return KR.check_vit_pool(what, cur["out"], P(prev, "yhi"), P(prev, "ylo"), f["post.g"], f["post.b"], f["proj.w"], T, eps)
+            return KR.check_vit_pool(what, cur["out"], A(prev, "yhi"), A(prev, "ylo"), f["post.g"], f["post.b"], f["proj.w"], T, eps)
         raise AssertionError(f"{tag}: unexpected launch {name!r}")
 
 
-def run_chain(tag, ch, trace, margins=None):
+def run_chain(tag, ch, trace, margins=None, cap_rows=None):
     """Checks every launch of the forward: trace(k) is the workspace after k launches.  Holds two traces at a time; returns the
-    last one and fills `margins` with the worst err / tol per launch name."""
+    last one and fills `margins` with the worst err / tol per launch name.  `cap_rows`: the model's workspace rows, which bound
+    the rows a trace returns (at capacity there are no guard rows)."""
     margins = {} if margins is None else margins
     prev = trace(0)
     n_total = prev["n_total"]
-    assert prev["names"] == [] and prev["rows"] == ch.M + GUARD
+    assert prev["names"] == [] and prev["rows"] == min(ch.M + GUARD, cap_rows or ch.M + GUARD)
     for buf in BUFFERS:
         assert (_bits(prev[buf]) == _poison_bits(prev[buf])).all(), f"{tag}: {buf} not poisoned before the first launch"
     layer = -1
