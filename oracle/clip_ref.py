@@ -67,7 +67,21 @@ def blob_numel(g: VitGeometry) -> int:
 
 def make_weights(g: VitGeometry = CLIP_B16, seed: int = 0, style: str = "hf") -> dict:
     """Seeded weights.  "hf": normal sigma 0.02 matrices/embeddings, zero biases, unit LayerNorm; "trained": non-zero biases
-    and non-unit LayerNorm gains/offsets on top."""
+    and non-unit LayerNorm gains/offsets on top.
+
+    "hard": the statistics of a trained pre-LN tower that seeded-normal weights never produce (drawn after the "hf" draws,
+    so "hf" / "trained" keep their bits):
+      * massive activations: three residual channels (HARD_CHANNELS) hold about 200 on the class token and, with the
+        opposite signs, on two fixed patch tokens (HARD_PATCH_TOKENS), 60-125x the median |x| of the stream -- put there by the class
+        embedding / the position rows and pre_layrnorm's gain on those channels.  The pre-LN stream is never renormalised,
+        so they persist through every layer;
+      * LN1 / LN2 / post_layernorm gains of 0.05 on those channels, and the columns that consume them (Q, V, FFN1, the
+        projection) scaled down 25x;
+      * an attention sink on the class token: in 8 of the 12 heads one query / key dimension reads only the massive channels
+        (key) and a bias (query: 10 here, 6 in the text tower), so that 20-45 % of the (query, head) rows put more than half
+        their weight on key 0;
+      * peaked attention (Q and K 1.5x), LayerNorm gains around 2.5 (+-20 %), non-zero biases everywhere.
+    Every activation stays far inside fp16 (below 2 000).  tests/test_gpu_pre_ln_chain.py asserts these statistics."""
     rng = np.random.default_rng(seed)
     flat = {}
     for name, shape in blob_layout(g):
@@ -85,9 +99,57 @@ def make_weights(g: VitGeometry = CLIP_B16, seed: int = 0, style: str = "hf") ->
                 flat[name] = (0.05 * rng.standard_normal(shape, dtype=np.float32)).astype(np.float32)
         for l in range(g.layers):
             flat[f"l{l}.qkv.w"][: 2 * g.hidden] *= np.float32(2.0)
+    elif style == "hard":
+        h = g.hidden
+        pre_ln_hard(flat, blob_layout(g), h, g.heads, g.layers, "post.", rng, sink=10.0)
+        ch = HARD_CHANNELS
+        flat["pre.g"][ch] = np.float32(12.5)  # a row whose variance the three channels dominate: |z| ~ 16 there, x ~ 200
+        flat["cls"][ch] = np.float32(20.0) * HARD_SIGNS
+        for t in HARD_PATCH_TOKENS:
+            flat["pos"][t, ch] = np.float32(-20.0) * HARD_SIGNS
+        flat["patch.w"][ch] *= np.float32(0.05)  # ordinary patches stay ordinary on those channels
     elif style != "hf":
         raise ValueError(style)
     return flat
+
+
+HARD_CHANNELS = np.array([37, 301, 470])  # the massive residual channels of the "hard" style (both CLIP towers)
+HARD_SIGNS = np.array([1.0, -1.0, 1.0], np.float32)  # their signs on token 0
+HARD_PATCH_TOKENS = (19, 150)  # ViT: two patch tokens that carry them too, with the opposite signs (no sink there)
+
+
+def pre_ln_hard(flat: dict, layout, h: int, heads: int, layers: int, final: str, rng, sink: float) -> None:
+    """The "hard" statistics both pre-LN CLIP towers share (see make_weights), drawn from `rng` after the "hf" draws: gains,
+    biases, the scaled-down consumers of HARD_CHANNELS, peaked Q / K and the sink dimension of 2 heads in 3."""
+    ch, hd = HARD_CHANNELS, h // heads
+    for name, shape in layout:
+        if name.endswith(".g"):
+            gain = (2.5 * np.clip(1.0 + 0.2 * rng.standard_normal(shape, dtype=np.float32), 0.3, None)).astype(np.float32)
+            gain[ch] = 0.05
+            flat[name] = gain
+        elif name.endswith(".b"):
+            is_ln = name.endswith(("ln1.b", "ln2.b")) or name in ("pre.b", final + "b")
+            off = ((0.1 if is_ln else 0.05) * rng.standard_normal(shape, dtype=np.float32)).astype(np.float32)
+            if is_ln:
+                off[ch] = 0.0
+            flat[name] = off
+    for l in range(layers):
+        p = f"l{l}."
+        w, b = flat[p + "qkv.w"], flat[p + "qkv.b"]
+        w[: 2 * h] *= np.float32(1.5)
+        w[:h, ch] *= np.float32(1.0 / 25.0)
+        w[2 * h:, ch] *= np.float32(1.0 / 25.0)
+        flat[p + "ff1.w"][:, ch] *= np.float32(1.0 / 25.0)
+        for head in range(heads):
+            if head % 3 == 2:
+                continue
+            j = head * hd + hd - 1  # the sink dimension: the key reads the massive channels only, the query a constant
+            w[h + j] = 0.0
+            w[h + j, ch] = np.float32(4.0) * HARD_SIGNS
+            b[h + j] = 0.0
+            w[j] *= np.float32(0.25)
+            b[j] = np.float32(sink)
+    flat["proj.w"][:, ch] *= np.float32(1.0 / 25.0)
 
 
 def pack_blob(flat: dict, g: VitGeometry) -> np.ndarray:

@@ -26,7 +26,9 @@ def geometry(**kw) -> dict:
 
 def make_weights(g: dict, seed: int = 0, style: str = "hf") -> dict:
     """Seeded weights.  "hf": normal sigma 0.02 matrices/embeddings, zero biases, unit LayerNorm; "trained": non-zero biases,
-    non-unit LayerNorm gains/offsets and sharper attention (Q, K rows doubled)."""
+    non-unit LayerNorm gains/offsets and sharper attention (Q, K rows doubled); "hard": oracle/clip_ref.make_weights' "hard"
+    statistics for this tower -- the massive channels come from position row 0 (always <|startoftext|>, or the only token),
+    +-200, and every query of the causal tower sees the sink on key 0."""
     rng = np.random.default_rng(seed)
     flat = {}
     for name, shape in clip_text_blob_layout(g):
@@ -44,6 +46,11 @@ def make_weights(g: dict, seed: int = 0, style: str = "hf") -> dict:
                 flat[name] = (0.05 * rng.standard_normal(shape, dtype=np.float32)).astype(np.float32)
         for l in range(g["layers"]):
             flat[f"l{l}.qkv.w"][: 2 * g["hidden"]] *= np.float32(2.0)
+    elif style == "hard":
+        from oracle import clip_ref as C
+
+        C.pre_ln_hard(flat, clip_text_blob_layout(g), g["hidden"], g["heads"], g["layers"], "final.", rng, sink=6.0)
+        flat["pos"][0, C.HARD_CHANNELS] = np.float32(200.0) * C.HARD_SIGNS  # position 0 (<|startoftext|>) carries them
     elif style != "hf":
         raise ValueError(style)
     return flat

@@ -83,30 +83,35 @@ def emulate_gemm(epi, a16, w16, bias, resid=None, ln_stats=None, ln_gamma=None, 
     return out
 
 
-def emulate_attention(qkv16, lens, B, S, mutant=None, head_dim=64):
+def emulate_attention(qkv16, lens, B, S, mutant=None, head_dim=64, heads=12, causal=False):
     """attention_sm90.cu's rounding: fp32 scores, online softmax over 64-key sub-blocks with exp2, P rounded to fp16, fp32
-    P.V, ctx = fp16(O / l).  12 heads of head_dim."""
+    P.V, ctx = fp16(O / l).  `heads` heads of head_dim.  `causal`: a query row skips the sub-blocks that start after it and
+    masks the keys after it in the sub-block it sits in (the diagonal one)."""
     c = np.float32(1.4426950408889634 / np.sqrt(head_dim))
-    H = 12 * head_dim
-    q = qkv16.reshape(B, S, 3, 12, head_dim).astype(np.float32)
-    ctx = np.zeros((B, S, 12, head_dim), np.float16)
+    H = heads * head_dim
+    q = qkv16.reshape(B, S, 3, heads, head_dim).astype(np.float32)
+    ctx = np.zeros((B, S, heads, head_dim), np.float16)
     for b in range(B):
         n = int(min(max(lens[b], 1), S)) + {"mask_plus": 1, "mask_minus": -1}.get(mutant, 0)
         qq, kk, vv = (q[b, :, j].transpose(1, 0, 2) for j in range(3))
-        o = np.zeros((12, S, head_dim), np.float32)
-        m = np.full((12, S, 1), -np.inf, np.float32)
-        l = np.zeros((12, S, 1), np.float32)
+        o = np.zeros((heads, S, head_dim), np.float32)
+        m = np.full((heads, S, 1), -np.inf, np.float32)
+        l = np.zeros((heads, S, 1), np.float32)
         for k0 in range(0, n, 64):
-            s = qq @ kk[:, k0:k0 + 64].transpose(0, 2, 1)
+            r = slice(k0, S) if causal else slice(0, S)  # the query rows that read this sub-block
+            s = qq[:, r] @ kk[:, k0:k0 + 64].transpose(0, 2, 1)
             s[:, :, max(n - k0, 0):] = -np.inf
-            m_new = np.maximum(m, s.max(-1, keepdims=True))
-            alpha = np.exp2((m - m_new) * c).astype(np.float32)
+            if causal:
+                nr, nk = min(64, s.shape[1]), s.shape[2]
+                s[:, :nr][:, np.arange(nk)[None, :] > np.arange(nr)[:, None]] = -np.inf
+            m_new = np.maximum(m[:, r], s.max(-1, keepdims=True))
+            alpha = np.exp2((m[:, r] - m_new) * c).astype(np.float32)
             if mutant == "no_rescale":
-                alpha = np.where(np.isinf(m), 0.0, 1.0).astype(np.float32)
+                alpha = np.where(np.isinf(m[:, r]), 0.0, 1.0).astype(np.float32)
             p = np.exp2(s * c - m_new * c).astype(np.float32)
-            l = l * alpha + p.sum(-1, keepdims=True)
-            o = o * alpha + p.astype(np.float16).astype(np.float32) @ vv[:, k0:k0 + 64]
-            m = m_new
+            l[:, r] = l[:, r] * alpha + p.sum(-1, keepdims=True)
+            o[:, r] = o[:, r] * alpha + p.astype(np.float16).astype(np.float32) @ vv[:, k0:k0 + 64]
+            m[:, r] = m_new
         ctx[b] = (o / l).astype(np.float16).transpose(1, 0, 2)
     return ctx.reshape(B * S, H)
 
