@@ -36,6 +36,16 @@ typedef struct b200rt_bert_config {
     float eps;
 } b200rt_bert_config;
 
+/* A BERT cross-encoder / sequence classifier (HF BertForSequenceClassification): the encoder of `bert` -- one of the three
+ * geometries above, type_vocab == 2 -- then BertPooler (dense [hidden, hidden] + tanh on the final LayerNorm of the [CLS] row)
+ * and the classifier [num_labels, hidden], 1 <= num_labels <= 64.  Results are num_labels raw logits per item (no sigmoid or
+ * softmax: the caller applies them), e.g. cross-encoder/ms-marco-MiniLM-L-6-v2's relevance logit (num_labels = 1), which
+ * TEI serves through POST /rerank.                                                                                      */
+typedef struct b200rt_bert_classifier_config {
+    b200rt_bert_config bert;
+    int32_t num_labels;
+} b200rt_bert_classifier_config;
+
 /* Geometry of a CLIP-style ViT image tower (HF CLIPVisionConfig fields + projection_dim).  The kernels are specialised for
  * ViT-B/16: hidden 768, 12 heads of 64, inter 3072, (image/patch)^2 + 1 <= 512 tokens, 3*patch*patch a multiple of 64. */
 typedef struct b200rt_vit_config {
@@ -85,7 +95,9 @@ int b200rt_num_gpus(void);
  * "vit" (cfg: b200rt_vit_config; the CLIP ViT-B/16 image tower behind 06_gpu_and_ml/embeddings/image_embeddings_infinity.py:76-77;
  * blob order: b200rt.weights.vit_blob_layout) or "clip_text" (cfg: b200rt_clip_text_config; the same model's text tower, which
  * infinity's `embed(sentences=...)` runs -- image_embeddings_infinity.py:298-306; blob order:
- * b200rt.weights.clip_text_blob_layout).  A "clip_text" model takes token ids through b200rt_submit[_ex] (max_len <= max_pos,
+ * b200rt.weights.clip_text_blob_layout) or "bert_classifier" (cfg: b200rt_bert_classifier_config; blob order:
+ * b200rt.weights.classifier_blob_layout -- BERT's, then pool.w [H,H] | pool.b [H] | cls.w [L,H] | cls.b padded to 128 floats).
+ * A "clip_text" model takes token ids through b200rt_submit[_ex] (max_len <= max_pos,
  * ids < vocab; items travel in the 64- or 128-token bucket) and b200rt_embed_device (max_len <= 128, the longest wave the
  * scheduler forms for it: device-resident callers can run the bucket the scheduler would), and is refused by
  * b200rt_submit_pixels.                                                                                              */
@@ -118,6 +130,12 @@ int b200rt_submit_ex(int model, const int32_t* ids, const int32_t* lens, int n_i
  * the ticket completes; each replica pulls its share of the pixels over its own PCIe link (no scatter through the root:
  * an image is 600 KB, not 2 KB).  Pinned memory (b200rt_alloc_pinned) makes the copies asynchronous.  model: kind "vit". */
 int b200rt_submit_pixels(int model, const float* pixels, int n_items, float* out, uint64_t* ticket_out);
+/* Sentence pairs for a "bert_classifier" model (TEI's POST /rerank and /predict with [text, text] inputs): as b200rt_submit_ex,
+ * plus segs [n_items]: item i is [CLS] a [SEP] b [SEP] and its second segment (token type 1) starts at token segs[i],
+ * 0 <= segs[i] <= lens[i]; segs == NULL means one segment (all type 0).  out receives [n_items, num_labels] raw logits.  segs
+ * for a model of any other kind is B200RT_E_INVALID.  b200rt_submit[_ex] on a classifier model classifies single sequences.  */
+int b200rt_submit_pairs(int model, const int32_t* ids, const int32_t* lens, const int32_t* segs, int n_items, int max_len, float* out,
+                        uint32_t flags, uint64_t* ticket_out);
 /* Completion, ordered (`order_outputs=True`): a ticket being waited on is never handed to b200rt_poll_any ...  */
 int b200rt_wait(uint64_t ticket, int timeout_ms); /* timeout_ms < 0: forever */
 /* ... and unordered (`order_outputs=False`, text_embeddings_inference.py:167): next finished ticket
@@ -130,6 +148,10 @@ int b200rt_poll_any(uint64_t* ticket_out, int timeout_ms);
  * (512 b200rt_model_wave_capacity_items(model) tokens, or B200RT_E_INVALID).                           */
 int b200rt_embed_device(int model, int gpu, const int32_t* d_ids, const int32_t* d_lens, int n_items, int max_len,
                         float* d_out, void* stream);
+/* b200rt_embed_device with device-resident segment starts d_segs [n_items] (classifier models; NULL: one segment; each is
+ * clamped to [0, max_len] on the device, not validated).  b200rt_embed_device is this with d_segs = NULL.                */
+int b200rt_embed_device_pairs(int model, int gpu, const int32_t* d_ids, const int32_t* d_lens, const int32_t* d_segs, int n_items,
+                              int max_len, float* d_out, void* stream);
 int b200rt_device_sync(int gpu);
 int b200rt_wave_capacity_items(void); /* items of 512 tokens one replica takes per wave (bge-base, bge-small) */
 /* items of 512 tokens one replica takes per wave of this model: b200rt_wave_capacity_items() for bge-base and bge-small,

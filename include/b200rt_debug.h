@@ -68,6 +68,16 @@ int b200rt_debug_attention_ex(const uint16_t* qkv, const int32_t* lens, uint16_t
  *                   gamma NULL: w_out = fp16(w) and cvec_out is not written.  w fp32 [N, K], K % 64 == 0.    */
 int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, int n_tokens, int S, int vocab,
                        uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden);
+/*   embed_segs:     embed with token types: token t takes type row 1 when t % S >= segs[t / S] (clamped to [0, S] on the device),
+ *                   else row 0.  type [2, W], segs [n_tokens / S], n_tokens a multiple of S; W = hidden (768, 384 or 1024).
+ *   cls_head:       out[i] = cls_w . tanh(pool_w . LayerNorm(hi + lo of row i * S) + pool_b) + cls_b, raw logits, out fp32
+ *                   [n_items, L], 1 <= L <= 64; pool_w fp32 [W, W], cls_w [L, W], cls_b [L]; W = hidden (768, 384 or 1024).
+ *                   ctas: the most blocks launched (0 = one per item); the result must not depend on it.                  */
+int b200rt_debug_embed_segs(const int32_t* ids, const int32_t* segs, const float* word, const float* pos, const float* type, int n_tokens,
+                            int S, int vocab, uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden);
+int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* pool_w,
+                          const float* pool_b, const float* cls_w, const float* cls_b, int n_items, int S, int L, float eps, float* out,
+                          int hidden, int ctas);
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out);
 int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
@@ -98,6 +108,11 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
 int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_launches,
                                uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx,
                                uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total);
+/* b200rt_debug_forward_trace of a sentence-pair batch: segs [n_items] as for b200rt_submit_pairs (classifier models; NULL: one
+ * segment).  The last launch of a "bert_classifier" model is "cls_head", which writes out [n_items, num_labels].            */
+int b200rt_debug_forward_trace_segs(int model, const int32_t* ids, const int32_t* lens, const int32_t* segs, int n_items, int max_len,
+                                    int n_launches, uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv,
+                                    uint16_t* ctx, uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total);
 int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
                                    float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx, uint16_t* ffn, float* out,
                                    char* names_out, size_t names_cap, int* n_total);

@@ -25,13 +25,14 @@ E_INVALID, E_STATE, E_CUDA, E_NOMEM, E_UNSUPPORTED = -1, -2, -3, -4, -5
 # every symbol include/b200rt.h and include/b200rt_debug.h declare (tests check the export list)
 ABI_SYMBOLS = [
     "b200rt_init", "b200rt_init_devices", "b200rt_num_gpus", "b200rt_model_load", "b200rt_model_load_ex", "b200rt_submit", "b200rt_submit_ex", "b200rt_submit_pixels", "b200rt_wait",
-    "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_wave_capacity_items", "b200rt_model_wave_capacity_items",
+    "b200rt_poll_any", "b200rt_embed_device", "b200rt_device_sync", "b200rt_submit_pairs", "b200rt_embed_device_pairs", "b200rt_wave_capacity_items", "b200rt_model_wave_capacity_items",
     "b200rt_alloc_pinned", "b200rt_free_pinned", "b200rt_stats", "b200rt_last_error", "b200rt_shutdown",
 ]
 DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_gemm_ex", "b200rt_debug_attention", "b200rt_debug_attention_ex", "b200rt_debug_profile_forward",
                  "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_mean_pool_normalize",
                  "b200rt_debug_vit_pool", "b200rt_debug_clip_text_pool", "b200rt_debug_fold_ln",
-                 "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace", "b200rt_debug_model_cap_rows"]
+                 "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace", "b200rt_debug_model_cap_rows",
+                 "b200rt_debug_embed_segs", "b200rt_debug_cls_head", "b200rt_debug_forward_trace_segs"]
 
 
 def SPLIT_SMS(k: int) -> int:
@@ -49,6 +50,10 @@ class BertConfig(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("vocab", "hidden", "layers", "heads", "inter", "max_pos", "type_vocab")] + [
         ("eps", ctypes.c_float)
     ]
+
+
+class BertClassifierConfig(ctypes.Structure):
+    _fields_ = [("bert", BertConfig), ("num_labels", ctypes.c_int32)]
 
 
 class VitConfig(ctypes.Structure):
@@ -96,9 +101,13 @@ def load_library():
         lib.b200rt_submit_ex.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.c_uint32, u64p]
         lib.b200rt_submit_pixels.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, u64p]
+        lib.b200rt_submit_pairs.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                            ctypes.c_void_p, ctypes.c_uint32, u64p]
         lib.b200rt_wait.argtypes = [ctypes.c_uint64, ctypes.c_int]
         lib.b200rt_poll_any.argtypes = [u64p, ctypes.c_int]
         lib.b200rt_embed_device.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+        lib.b200rt_embed_device_pairs.argtypes = [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int,
+                                                                                                      ctypes.c_void_p, ctypes.c_void_p]
         lib.b200rt_device_sync.argtypes = [ctypes.c_int]
         lib.b200rt_model_wave_capacity_items.argtypes = [ctypes.c_int]
         lib.b200rt_debug_model_cap_rows.argtypes = [ctypes.c_int]
@@ -120,6 +129,8 @@ def load_library():
         vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
         lib.b200rt_debug_embed.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, vp, vp, ci]
         lib.b200rt_debug_vit_embed.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, vp, vp]
+        lib.b200rt_debug_embed_segs.argtypes = [vp] * 5 + [ci, ci, ci, vp, vp, vp, ci]
+        lib.b200rt_debug_cls_head.argtypes = [vp] * 8 + [ci, ci, ci, cf, vp, ci, ci]
         lib.b200rt_debug_pool_normalize.argtypes = [vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_mean_pool_normalize.argtypes = [vp, vp, vp, vp, vp, ci, ci, cf, vp, ci]
         lib.b200rt_debug_vit_pool.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
@@ -127,6 +138,7 @@ def load_library():
         lib.b200rt_debug_fold_ln.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp]
         lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_vit_forward_trace.argtypes = [ci, vp, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
+        lib.b200rt_debug_forward_trace_segs.argtypes = [ci, vp, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                      f32p, i32p, ctypes.c_int]
         _lib = lib
@@ -278,6 +290,10 @@ class EmbedModel:
     def submit(self, ids: np.ndarray, lens=None, out: np.ndarray | None = None, tag=None, borrow_ids: bool = False) -> Ticket:
         """``borrow_ids``: the caller promises not to touch ``ids`` until the ticket completes; the library then takes
         no private copy and, when ``ids``/``out`` live in :class:`PinnedBuffer` memory, DMAs from/to them directly."""
+        return self._submit(ids, lens, None, out, tag, borrow_ids)
+
+    def _submit(self, ids, lens, segs, out, tag, borrow_ids) -> Ticket:
+        """b200rt_submit_ex, or b200rt_submit_pairs when ``segs`` (int32 [n_items]) is given."""
         if borrow_ids and not (isinstance(ids, np.ndarray) and ids.dtype == np.int32 and ids.flags.c_contiguous):
             raise B200RTError(E_INVALID, "borrow_ids needs a C-contiguous int32 array (a converted copy would be freed too early)")
         ids = np.ascontiguousarray(ids, dtype=np.int32)
@@ -292,10 +308,18 @@ class EmbedModel:
             out = np.empty((n, self.out_dim), np.float32)
         elif out.dtype != np.float32 or not out.flags.c_contiguous or out.shape != (n, self.out_dim):
             raise B200RTError(E_INVALID, f"out must be a C-contiguous float32 [n_items, {self.out_dim}] array")
+        if segs is not None:
+            segs = np.ascontiguousarray(segs, dtype=np.int32)
+            if segs.shape != (n,):
+                raise B200RTError(E_INVALID, f"segs must have shape ({n},), got {segs.shape}")
         t = ctypes.c_uint64(0)
+        flags = SUBMIT_BORROW_IDS if borrow_ids else 0
+        lens_p = _ptr(lens) if lens is not None else None
         with _live_lock:
-            _check(self._lib.b200rt_submit_ex(self.handle, _ptr(ids), _ptr(lens) if lens is not None else None, n, S, _ptr(out),
-                                              SUBMIT_BORROW_IDS if borrow_ids else 0, ctypes.byref(t)))
+            if segs is None:
+                _check(self._lib.b200rt_submit_ex(self.handle, _ptr(ids), lens_p, n, S, _ptr(out), flags, ctypes.byref(t)))
+            else:
+                _check(self._lib.b200rt_submit_pairs(self.handle, _ptr(ids), lens_p, _ptr(segs), n, S, _ptr(out), flags, ctypes.byref(t)))
             tk = Ticket(t.value, out, tag, ids if borrow_ids else None)
             _live[tk.id] = tk
         return tk
@@ -337,12 +361,17 @@ class EmbedModel:
     # ---- debug helpers (tests only)
     def debug_trace(self, ids: np.ndarray, lens, n_launches: int) -> dict:
         """The workspace after the first ``n_launches`` launches of this batch's forward (see :func:`_debug_trace`)."""
+        return self._trace(ids, lens, None, n_launches)
+
+    def _trace(self, ids, lens, segs, n_launches: int) -> dict:
+        """b200rt_debug_forward_trace_segs (segs None: one segment per item, as b200rt_debug_forward_trace)."""
         ids = np.ascontiguousarray(ids, dtype=np.int32)
         n, S = ids.shape
-        lens_a = np.ascontiguousarray(lens, dtype=np.int32) if lens is not None else None
-        return _debug_trace(lambda *bufs: self._lib.b200rt_debug_forward_trace(
-            self.handle, _ptr(ids), _ptr(lens_a) if lens_a is not None else None, n, S, n_launches, *bufs),
-            n * S, n, self.hidden, self.inter, self.out_dim, n_launches, self.debug_cap_rows())
+        p = lambda v: _ptr(v) if v is not None else None  # noqa: E731
+        lens_a, segs_a = (np.ascontiguousarray(v, dtype=np.int32) if v is not None else None for v in (lens, segs))
+        return _debug_trace(lambda *bufs: self._lib.b200rt_debug_forward_trace_segs(self.handle, _ptr(ids), p(lens_a), p(segs_a), n, S,
+                                                                                    n_launches, *bufs),
+                            n * S, n, self.hidden, self.inter, self.out_dim, n_launches, self.debug_cap_rows())
 
     def debug_residual(self, ids: np.ndarray, lens, n_layers: int) -> np.ndarray:
         """The residual stream after ``n_layers`` encoder layers (0: the embedding sum), pre-LayerNorm as the forward carries
@@ -376,6 +405,47 @@ class ClipTextModel(EmbedModel):
         _check(lib.b200rt_model_load(b"clip_text", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
         self.handle = h.value
         self._lib = lib
+
+
+class ClassifierModel(EmbedModel):
+    """A loaded BERT sequence classifier / cross-encoder (kind "bert_classifier", HF ``BertForSequenceClassification``):
+    token ids in -- single sequences, or ``[CLS] a [SEP] b [SEP]`` pairs whose second segment starts at ``segs[i]`` --
+    ``[n, num_labels]`` raw logits out.  TEI serves such a model through ``/rerank`` (``num_labels == 1``: a relevance logit per
+    (query, text) pair) and ``/predict``; the sigmoid / softmax is the caller's.  ``submit``/``wait``/``poll_any`` are
+    :class:`EmbedModel`'s: same tickets, same scheduler, width ``num_labels``."""
+
+    def __init__(self, geometry: dict, blob: np.ndarray):
+        lib = load_library()
+        blob = np.ascontiguousarray(blob, dtype=np.float32)
+        g = geometry
+        self.cfg = BertClassifierConfig(BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"],
+                                                   g["eps"]), g["num_labels"])
+        self.hidden, self.inter, self.num_labels = g["hidden"], g["inter"], g["num_labels"]
+        self.out_dim = self.num_labels
+        self.pooling = "cls_head"
+        h = ctypes.c_int32(-1)
+        _check(lib.b200rt_model_load(b"bert_classifier", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
+        self.handle = h.value
+        self._lib = lib
+
+    def submit(self, ids: np.ndarray, lens=None, out: np.ndarray | None = None, tag=None, borrow_ids: bool = False, segs=None) -> Ticket:
+        """As :meth:`EmbedModel.submit`; ``segs`` [n_items]: where each item's second segment starts (0 <= segs[i] <= lens[i];
+        None: one segment)."""
+        return self._submit(ids, lens, segs, out, tag, borrow_ids)
+
+    def classify(self, ids: np.ndarray, lens=None, segs=None) -> np.ndarray:
+        """Synchronous: ``[n, num_labels]`` raw logits of one batch."""
+        lend = isinstance(ids, np.ndarray) and ids.dtype == np.int32 and ids.flags.c_contiguous
+        return self.wait(self.submit(ids, lens, borrow_ids=lend, segs=segs))
+
+    def embed_device(self, gpu: int, d_ids: int, d_lens: int, n_items: int, max_len: int, d_out: int, stream: int = 0, d_segs: int = 0):
+        """Device-resident forward (raw device addresses; ``d_segs`` 0: one segment); asynchronous on ``stream``."""
+        _check(self._lib.b200rt_embed_device_pairs(self.handle, gpu, d_ids, d_lens, d_segs or None, n_items, max_len, d_out, stream or None))
+
+    def debug_trace(self, ids: np.ndarray, lens, n_launches: int, segs=None) -> dict:
+        """The workspace after the first ``n_launches`` launches of this batch's forward (see :func:`_debug_trace`); the last
+        launch is ``cls_head``, whose logits come back as ``out``."""
+        return self._trace(ids, lens, segs, n_launches)
 
 
 class ImageEmbedModel:
@@ -536,6 +606,40 @@ def debug_embed(ids: np.ndarray, word: np.ndarray, pos: np.ndarray, type0: np.nd
     _check(load_library().b200rt_debug_embed(_ptr(ids), _ptr(word), _ptr(pos), _ptr(type0), n, S, word.shape[0], _ptr(hi), _ptr(lo), _ptr(st),
                                              hidden))
     return hi, lo, st
+
+
+def debug_embed_segs(ids: np.ndarray, segs, word: np.ndarray, pos: np.ndarray, type2: np.ndarray, S: int, hidden: int = 768):
+    """ids [n_items * S] (token t sits at position t % S of item t // S), segs [n_items] (passed as given; the kernel clamps each
+    to [0, S]), type2 [2, hidden]: token t takes type row 1 when t % S >= segs[t // S]; returns (hi, lo, stats)."""
+    ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+    segs = np.ascontiguousarray(segs, dtype=np.int32).reshape(-1)
+    word, pos, type2 = _f32(word), _f32(pos), _f32(type2)
+    if word.shape[1] != hidden or pos.shape[1] != hidden or type2.shape != (2, hidden):
+        raise B200RTError(E_INVALID, f"embedding tables must be {hidden} wide and type2 [2, {hidden}]")
+    n = ids.size
+    if n % S or segs.size != n // S:
+        raise B200RTError(E_INVALID, f"ids must hold whole items of {S} tokens and segs one entry per item")
+    hi, lo = np.empty((n, hidden), np.float16), np.empty((n, hidden), np.float16)
+    st = np.empty((n, hidden // 128, 2), np.float32)
+    _check(load_library().b200rt_debug_embed_segs(_ptr(ids), _ptr(segs), _ptr(word), _ptr(pos), _ptr(type2), n, S, word.shape[0], _ptr(hi),
+                                                  _ptr(lo), _ptr(st), hidden))
+    return hi, lo, st
+
+
+def debug_cls_head(hi: np.ndarray, lo: np.ndarray, gamma, beta, pool_w, pool_b, cls_w, cls_b, S: int, eps: float, hidden: int = 768,
+                   ctas: int = 0):
+    """hi, lo [n_items * S, hidden], pool_w [hidden, hidden], cls_w [L, hidden]: the raw logits
+    cls_w . tanh(pool_w . LayerNorm(row i * S) + pool_b) + cls_b, [n_items, L].  ``ctas``: the most blocks (0 = one per item)."""
+    hi, lo, gamma, beta = _f16(hi), _f16(lo), _f32(gamma), _f32(beta)
+    pool_w, pool_b, cls_w, cls_b = _f32(pool_w), _f32(pool_b), _f32(cls_w), _f32(cls_b)
+    L = cls_w.shape[0]
+    if hi.shape[1] != hidden or pool_w.shape != (hidden, hidden) or cls_w.shape[1] != hidden or cls_b.size < L:
+        raise B200RTError(E_INVALID, f"rows and head weights must be {hidden} wide")
+    n = hi.shape[0] // S
+    out = np.empty((n, max(L, 1)), np.float32)
+    _check(load_library().b200rt_debug_cls_head(_ptr(hi), _ptr(lo), _ptr(gamma), _ptr(beta), _ptr(pool_w), _ptr(pool_b), _ptr(cls_w),
+                                                _ptr(cls_b), n, S, L, eps, _ptr(out), hidden, ctas))
+    return out
 
 
 def debug_vit_embed(patch_out: np.ndarray, cls: np.ndarray, pos: np.ndarray, gamma: np.ndarray, beta: np.ndarray, T: int, eps: float):

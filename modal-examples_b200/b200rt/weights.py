@@ -25,6 +25,9 @@ BGE_SMALL_GEOMETRY = dict(vocab=30522, hidden=384, layers=12, heads=12, inter=15
 MINILM_L6_GEOMETRY = dict(vocab=30522, hidden=384, layers=6, heads=12, inter=1536, max_pos=512, type_vocab=2, eps=1e-12)
 # BAAI/bge-large-en-v1.5 (BERT-large): 16 heads of 64, 24 layers; also the shape of e5-large-v2, gte-large, mxbai-embed-large-v1
 BGE_LARGE_GEOMETRY = dict(vocab=30522, hidden=1024, layers=24, heads=16, inter=4096, max_pos=512, type_vocab=2, eps=1e-12)
+# cross-encoder/ms-marco-MiniLM-L-6-v2 (BertForSequenceClassification): MiniLM-L6's encoder, a pooler and one relevance logit;
+# -L-12-v2 is the same with 12 layers
+MS_MARCO_MINILM_L6_GEOMETRY = dict(MINILM_L6_GEOMETRY, num_labels=1)
 
 _ST_POOLING_MODULE = "sentence_transformers.models.Pooling"
 _ST_POOLING_MODES = ("pooling_mode_cls_token", "pooling_mode_mean_tokens", "pooling_mode_max_tokens",
@@ -231,22 +234,91 @@ def load_safetensors(path: str, eps: float | None = None) -> tuple[dict, np.ndar
     return load_hf_state_dict(sd, g)
 
 
+def hf_architectures(path: str) -> list:
+    """``architectures`` of a snapshot directory's ``config.json`` ([] without one)."""
+    p = os.path.join(path, "config.json")
+    if not os.path.exists(p):
+        return []
+    with open(p) as f:
+        return list(json.load(f).get("architectures") or [])
+
+
 def load_hf_dir(path: str) -> tuple[dict, np.ndarray]:
     """A local HF snapshot directory (what ``--huggingface-hub-cache`` + ``--model-id`` resolve to): picks
-    ``model.safetensors``, else ``pytorch_model.bin`` (needs torch)."""
+    ``model.safetensors``, else ``pytorch_model.bin`` (needs torch).  A snapshot whose ``config.json`` names
+    ``BertForSequenceClassification`` loads as a classifier: the geometry then carries ``num_labels`` and ``id2label``
+    (the config's, else ``LABEL_i``) and the blob is :func:`classifier_blob_layout`'s."""
+    cfg_path = os.path.join(path, "config.json")
+    cfg = json.load(open(cfg_path)) if os.path.exists(cfg_path) else {}
     st = os.path.join(path, "model.safetensors")
-    if os.path.exists(st):
-        return load_safetensors(st)
     pt = os.path.join(path, "pytorch_model.bin")
-    if os.path.exists(pt):
+    if os.path.exists(st):
+        sd = read_safetensors(st)
+    elif os.path.exists(pt):
         import torch
 
         sd = torch.load(pt, map_location="cpu", weights_only=True)
-        cfg_path = os.path.join(path, "config.json")
-        cfg = json.load(open(cfg_path)) if os.path.exists(cfg_path) else {}
-        g = geometry_from_state_dict(sd, cfg.get("layer_norm_eps", 1e-12), cfg.get("num_attention_heads"))
-        return load_hf_state_dict(sd, g)
-    raise FileNotFoundError(f"no model.safetensors / pytorch_model.bin under {path}")
+    else:
+        raise FileNotFoundError(f"no model.safetensors / pytorch_model.bin under {path}")
+    if CLASSIFIER_ARCHITECTURE in (cfg.get("architectures") or []):
+        return load_hf_classifier(sd, cfg)
+    return load_hf_state_dict(sd, geometry_from_state_dict(sd, cfg.get("layer_norm_eps", 1e-12), cfg.get("num_attention_heads")))
+
+
+# ----------------------------------------------------------------------------------------------- BERT sequence classifiers
+# Cross-encoders such as cross-encoder/ms-marco-MiniLM-L-6-v2 (HF BertForSequenceClassification), which TEI serves through
+# /rerank and /predict.  Blob order: blob_layout(g), then pool.w [H,H] | pool.b [H] | cls.w [L,H] | cls.b [128] -- the
+# classifier bias padded with zeros to 128 floats, as the engine's loader keeps every tensor a whole number of 128 floats.
+
+CLASSIFIER_ARCHITECTURE = "BertForSequenceClassification"
+CLS_B_PAD = 128
+
+
+def default_id2label(num_labels: int) -> dict:
+    return {i: f"LABEL_{i}" for i in range(num_labels)}
+
+
+def classifier_blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
+    h, L = g["hidden"], g["num_labels"]
+    if not 1 <= L <= 64:
+        raise ValueError(f"num_labels {L} outside [1, 64]")
+    return blob_layout(g) + [("pool.w", (h, h)), ("pool.b", (h,)), ("cls.w", (L, h)), ("cls.b", (CLS_B_PAD,))]
+
+
+def random_classifier_blob(g: dict = MS_MARCO_MINILM_L6_GEOMETRY, seed: int = 0) -> np.ndarray:
+    """Seeded weights of a classifier geometry: BERT's tensors drawn exactly as :func:`random_blob` draws them (the blob's
+    prefix is bit-identical), then the head the same way (sigma 0.02 matrices, zero biases)."""
+    return _random_blob(classifier_blob_layout(g), seed)
+
+
+def load_hf_classifier_state_dict(sd: dict, g: dict | None = None) -> tuple[dict, np.ndarray]:
+    """HF ``BertForSequenceClassification`` state dict (``bert.*``, ``bert.pooler.dense.*``, ``classifier.*``) -> (geometry
+    with ``num_labels`` from ``classifier.weight``, fp32 blob).  A checkpoint without the pooler (``add_pooling_layer=False``)
+    is refused: its logits are not computed from the tanh pooler this runtime applies."""
+    if "classifier.weight" not in sd or "classifier.bias" not in sd:
+        raise KeyError("no classifier.weight / classifier.bias: a BertForSequenceClassification checkpoint is needed")
+    enc = _strip_prefix(sd)
+    if "pooler.dense.weight" not in enc or "pooler.dense.bias" not in enc:
+        raise ValueError("the checkpoint has no bert.pooler.dense (a model built with add_pooling_layer=False); the classifier "
+                         "head here is classifier(tanh(pooler(CLS))) and cannot serve it")
+    g, blob = load_hf_state_dict(sd, g)
+    cw = _arr(sd["classifier.weight"])
+    g["num_labels"] = int(cw.shape[0])
+    cb = np.zeros(CLS_B_PAD, np.float32)
+    cb[: cw.shape[0]] = _arr(sd["classifier.bias"])
+    head = _pack(classifier_blob_layout(g)[len(blob_layout(g)):],
+                 {"pool.w": enc["pooler.dense.weight"], "pool.b": enc["pooler.dense.bias"], "cls.w": cw, "cls.b": cb})
+    return g, np.concatenate([blob, head])
+
+
+def load_hf_classifier(sd: dict, cfg: dict) -> tuple[dict, np.ndarray]:
+    """A classifier checkpoint's state dict and ``config.json`` (``{}`` without one) -> (geometry with ``num_labels`` and
+    ``id2label`` -- the config's, else ``LABEL_i`` --, blob)."""
+    g = geometry_from_state_dict(sd, cfg.get("layer_norm_eps", 1e-12), cfg.get("num_attention_heads"))
+    g, blob = load_hf_classifier_state_dict(sd, g)
+    labels = cfg.get("id2label") or {}
+    g["id2label"] = {int(k): str(v) for k, v in labels.items()} if len(labels) == g["num_labels"] else default_id2label(g["num_labels"])
+    return g, blob
 
 
 def resolve_hub_snapshot(cache_dir: str, model_id: str) -> str | None:

@@ -167,6 +167,8 @@ struct DevWeights {
     float *cls = nullptr, *pre_g = nullptr, *pre_b = nullptr, *post_g = nullptr, *post_b = nullptr, *proj_w = nullptr, *zero_bias = nullptr;
     // CLIP text (kind "clip_text"): word = token_embedding, pos = position_embedding padded to 128 zero rows, type = a zero row,
     // post_g / post_b = final_layer_norm, proj_w = text_projection [proj, hidden]; layers as for ViT (pre-LN).
+    // BERT classifier (kind "bert_classifier"): BertPooler dense [H, H] + bias, classifier [L, H] + bias (padded to 128).
+    float *pool_w = nullptr, *pool_b = nullptr, *cls_w = nullptr, *cls_b = nullptr;
 };
 
 enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2 };
@@ -174,6 +176,7 @@ enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2 };
 struct Model {
     ModelKind kind = KIND_BERT;
     bool pool_mean = false;  // text: mean of the valid tokens' final hidden states (B200RT_LOAD_POOL_MEAN) instead of the CLS row
+    int num_labels = 0;      // > 0: a BERT classifier (kind "bert_classifier"): the head's L logits per item instead of a pool
     b200rt_bert_config cfg{};
     b200rt_vit_config vcfg{};
     b200rt_clip_text_config tcfg{};
@@ -206,6 +209,7 @@ struct Dev {
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
     int32_t* ids_in[NSLOT] = {};
     int32_t* lens_in[NSLOT] = {};
+    int32_t* segs_in[NSLOT] = {};  // classifier waves' segment starts (allocated when the first classifier model loads)
     float* pix_in[NSLOT] = {};     // vit: this replica's share of a wave's pixels (allocated when the first vit model loads)
     cudaStream_t copy = nullptr;   // vit: H2D of wave k+1's pixels runs here, under the forward of wave k on `compute`
     cudaEvent_t ev_pix[NSLOT] = {};
@@ -240,6 +244,7 @@ struct Ticket {
     bool borrowed = false, ids_pinned = false, out_pinned = false;
     const int32_t* ids_ptr() const { return borrowed ? ids_ext : ids.data(); }
     std::vector<int32_t> lens;
+    std::vector<int32_t> segs;  // segment starts (b200rt_submit_pairs); empty: one segment per item
     int n_items, S;
     float* out;
     // Items travel in length buckets of 64 tokens (each bucket is padded to its own length, not to the input's max_len):
@@ -284,6 +289,7 @@ struct Runtime {
     int32_t *h_ids[NSLOT], *h_lens[NSLOT];
     float* h_out[NSLOT];
     int32_t *d_ids_stage[NSLOT], *d_lens_stage[NSLOT];
+    int32_t *h_segs[NSLOT] = {}, *d_segs_stage[NSLOT] = {};  // classifier waves only (allocated with the first classifier model)
     float* d_out_gather[NSLOT];
     cudaStream_t s_in = nullptr, s_out = nullptr;  // on root
     cudaEvent_t ev_scatter[NSLOT], ev_wave[NSLOT], ev_t0[NSLOT], ev_fwd_end[NSLOT];
@@ -320,6 +326,7 @@ struct Input {
     const int32_t* lens;
     const float* pixels;
     int B, S;
+    const int32_t* segs = nullptr;  // text: per-item segment starts (token types of sentence pairs); NULL: type 0 throughout
 };
 
 // A debug view of one forward; the product path passes none.  The forward calls at() ahead of its first launch (name NULL)
@@ -414,7 +421,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             if (step("vit_embed")) return 0;
         } else {
             // clip_text: token + position, its zero type row leaves (word + 0) + pos bit-exact; no embedding LayerNorm
-            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, m.vocab, H, stream));
+            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, m.vocab, H, stream, in.segs));
             if (step("embed")) return 0;
         }
         const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // BERT: the LayerNorm that applies to the current residual rows
@@ -444,9 +451,12 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
         else if (clip_text)
             CUDA_TRY(launch_clip_text_pool(d.yhi, d.ylo, in.ids, in.lens, w.post_g, w.post_b, w.proj_w, out, B, S, m.tcfg.proj, m.eps,
                                            m.tcfg.eos_id, stream));
+        else if (m.num_labels > 0)
+            CUDA_TRY(launch_cls_head(d.yhi, d.ylo, prev_g, prev_b, w.pool_w, w.pool_b, w.cls_w, w.cls_b, out, B, S, m.num_labels, m.eps, H,
+                                     stream));
         else if (m.pool_mean) CUDA_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
         else CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
-        step(vit ? "vit_pool" : clip_text ? "clip_text_pool" : (m.pool_mean ? "mean_pool_normalize" : "pool_normalize"));
+        step(vit ? "vit_pool" : clip_text ? "clip_text_pool" : m.num_labels > 0 ? "cls_head" : (m.pool_mean ? "mean_pool_normalize" : "pool_normalize"));
         return 0;
     };
     if (int rc = enqueue()) return rc;
@@ -466,8 +476,9 @@ struct GraphKey {
     const void *model, *ids, *lens, *out;
     cudaStream_t stream;
     int B, S;
+    const void* segs;
     bool operator<(const GraphKey& o) const {
-        return std::tie(model, ids, lens, out, stream, B, S) < std::tie(o.model, o.ids, o.lens, o.out, o.stream, o.B, o.S);
+        return std::tie(model, ids, lens, out, stream, B, S, segs) < std::tie(o.model, o.ids, o.lens, o.out, o.stream, o.B, o.S, o.segs);
     }
 };
 struct GraphEntry {
@@ -502,7 +513,7 @@ int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, 
         if (int rc = forward_enqueue(d, m, dev_index, in, out, stream, launches, hook)) return rc;
     } else {
         GraphCache& cache = graph_cache(d);
-        const GraphKey key{&m, in.ids, in.lens, out, stream, in.B, in.S};
+        const GraphKey key{&m, in.ids, in.lens, out, stream, in.B, in.S, in.segs};
         auto it = cache.entries.find(key);
         if (it == cache.entries.end()) {
             if (cache.entries.size() >= GRAPH_CACHE_MAX) {  // evict the least recently replayed graph
@@ -704,6 +715,14 @@ void dispatcher_main(Runtime* rtp) {
         if (!vit)
             for (const Segment& sg : wv.segs)
                 for (int i = 0; i < sg.count; ++i) rt.h_lens[slot][sg.wave_off + i] = sg.t->lens[sg.t->item_at(sg.ticket_off + i)];
+        // a classifier wave carries every item's segment start; an item submitted without one is a single segment (start = len)
+        const bool pairs = model.num_labels > 0;
+        if (pairs)
+            for (const Segment& sg : wv.segs)
+                for (int i = 0; i < sg.count; ++i) {
+                    const int it = sg.t->item_at(sg.ticket_off + i);
+                    rt.h_segs[slot][sg.wave_off + i] = sg.t->segs.empty() ? sg.t->lens[it] : sg.t->segs[it];
+                }
         auto t_host1 = std::chrono::steady_clock::now();
         if (staged) {
             if (!wv.direct_h2d) {
@@ -721,6 +740,9 @@ void dispatcher_main(Runtime* rtp) {
         if (!vit)
             SCHED_TRY(cudaMemcpyAsync(rt.d_lens_stage[slot], rt.h_lens[slot], static_cast<size_t>(n) * 4,
                                       cudaMemcpyHostToDevice, rt.s_in));
+        if (pairs)
+            SCHED_TRY(cudaMemcpyAsync(rt.d_segs_stage[slot], rt.h_segs[slot], static_cast<size_t>(n) * 4,
+                                      cudaMemcpyHostToDevice, rt.s_in));
         // Replicas used by this wave: everyone when there is enough work, otherwise as many as get at least
         // MIN_ITEMS_PER_REPLICA items each, starting from a rotating replica so that consecutive small waves land on
         // different GPUs.  Contiguous item ranges, as even as possible.
@@ -735,6 +757,7 @@ void dispatcher_main(Runtime* rtp) {
         for (int g = 0; g < G; ++g) {
             plan.dst_ids[g] = rt.devs[g]->ids_in[slot];
             plan.dst_lens[g] = rt.devs[g]->lens_in[slot];
+            plan.dst_segs[g] = rt.devs[g]->segs_in[slot];
             plan.item_begin[g] = 0;
             plan.item_count[g] = 0;
         }
@@ -743,9 +766,9 @@ void dispatcher_main(Runtime* rtp) {
             const int b0 = std::min(n, k * per), b1 = std::min(n, (k + 1) * per);
             plan.item_begin[g] = b0;
             plan.item_count[g] = b1 - b0;
-            if (g != 0) peer_bytes += static_cast<uint64_t>(b1 - b0) * (vit ? out_dim * 4 : S * 4 + 4 + out_dim * 4);
+            if (g != 0) peer_bytes += static_cast<uint64_t>(b1 - b0) * (vit ? out_dim * 4 : S * 4 + 4 + (pairs ? 4 : 0) + out_dim * 4);
         }
-        if (!vit) SCHED_TRY(launch_scatter(rt.d_ids_stage[slot], rt.d_lens_stage[slot], plan, rt.s_in));
+        if (!vit) SCHED_TRY(launch_scatter(rt.d_ids_stage[slot], rt.d_lens_stage[slot], plan, rt.s_in, pairs ? rt.d_segs_stage[slot] : nullptr));
         SCHED_TRY(cudaEventRecord(rt.ev_scatter[slot], rt.s_in));
         // every participating replica's launcher thread enqueues its own forward (~85 launches each, in parallel)
         std::atomic<uint64_t> launches{1};
@@ -793,8 +816,8 @@ void dispatcher_main(Runtime* rtp) {
                                 rc = forward(dd, model, g, Input{nullptr, nullptr, dd.pix_in[slot], plan.item_count[g], model.tokens}, dst,
                                              dd.compute, nl);
                         } else {
-                            rc = forward(dd, model, g, Input{dd.ids_in[slot], dd.lens_in[slot], nullptr, plan.item_count[g], S}, dst,
-                                         dd.compute, nl);
+                            rc = forward(dd, model, g, Input{dd.ids_in[slot], dd.lens_in[slot], nullptr, plan.item_count[g], S,
+                                                             pairs ? dd.segs_in[slot] : nullptr}, dst, dd.compute, nl);
                         }
                         if (rc) { e = t_last_error; code = rc; }
                         else {
@@ -845,7 +868,7 @@ void dispatcher_main(Runtime* rtp) {
         {
             std::lock_guard<std::mutex> sl(rt.stats_mu);
             rt.stats.kernel_launches += launches.load();
-            rt.stats.h2d_bytes += vit ? static_cast<uint64_t>(n) * model.item_bytes : static_cast<uint64_t>(n) * (S * 4 + 4);
+            rt.stats.h2d_bytes += vit ? static_cast<uint64_t>(n) * model.item_bytes : static_cast<uint64_t>(n) * (S * 4 + 4 + (pairs ? 4 : 0));
             rt.stats.d2h_bytes += static_cast<uint64_t>(n) * out_dim * 4;
             rt.stats.peer_bytes += peer_bytes;
             rt.stats.stage_us += std::chrono::duration<double, std::micro>(t_host1 - t_host0).count();
@@ -1236,7 +1259,29 @@ int register_model(Runtime& rt, std::unique_ptr<Model> m, int* model_out) {
 
 // model_load* run under the root replica's mu (b200rt_model_load_ex)
 
-int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out) {
+// Segment-start buffers of classifier waves: root staging per slot and every replica's input slots, allocated once, when the
+// first classifier model loads (an embedding-only runtime never has them).
+int alloc_seg_slots(Runtime& rt) {
+    if (rt.h_segs[0]) return 0;
+    const size_t wave_rows = static_cast<size_t>(rt.cap_rows) * rt.devs.size();
+    for (auto& d : rt.devs) {
+        CUDA_TRY(cudaSetDevice(d->id));
+        for (int s = 0; s < NSLOT; ++s) CUDA_TRY(cudaMalloc(&d->segs_in[s], rt.cap_rows * 4));
+    }
+    CUDA_TRY(cudaSetDevice(rt.devs[0]->id));
+    for (int s = 0; s < NSLOT; ++s) {
+        CUDA_TRY(cudaMalloc(&rt.d_segs_stage[s], wave_rows * 4));
+        CUDA_TRY(cudaMallocHost(&rt.h_segs[s], wave_rows * 4));
+    }
+    return 0;
+}
+
+constexpr int MAX_LABELS = 64;   // the classifier head's logits per item (launch_cls_head)
+constexpr int CLS_B_FLOATS = 128;  // the classifier bias is padded to 128 floats in the blob (tensor sizes keep the arena aligned)
+
+// num_labels > 0: kind "bert_classifier" -- the BERT layout followed by the pooler and the classifier, and the head as the last
+// launch instead of a pool.
+int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out, int num_labels = 0) {
     Runtime& rt = *g_rt;
     bool known = false;
     for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= !tg.causal && c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
@@ -1245,6 +1290,9 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
                     "kernels cover three geometries, bge-base (hidden=768 heads=12 inter=3072), bge-small (hidden=384 heads=12 "
                     "inter=1536) and bge-large (hidden=1024 heads=16 inter=4096), with max_pos<=512 (got hidden %d heads %d inter %d "
                     "max_pos %d)", c.hidden, c.heads, c.inter, c.max_pos);
+    if (num_labels > 0 && c.type_vocab != 2)
+        return fail(B200RT_E_UNSUPPORTED, "a classifier takes sentence pairs through two token types: type_vocab must be 2, got %d",
+                    c.type_vocab);
     const int cap_rows = model_cap_rows(rt.cap_rows, c.hidden);
     if (cap_rows < MAX_SEQ)
         return fail(B200RT_E_INVALID,
@@ -1258,6 +1306,8 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
     m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
     m->cap_rows = cap_rows;
     m->out_dim = c.hidden;
+    m->num_labels = num_labels;
+    if (num_labels > 0) m->out_dim = num_labels;
 
     // b200rt.weights.blob_layout.  QKV of layer l folds the LayerNorm in front of it, the previous layer's ln2 (the embedding
     // LN for l = 0); FFN1 folds the layer's own ln1.
@@ -1280,6 +1330,13 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
         L.copy(l, H, &LayerW::ff2_b);
         ln_g = L.copy(l, H, &LayerW::ln2_g);
         ln_b = L.copy(l, H, &LayerW::ln2_b);
+    }
+    if (num_labels > 0) {  // b200rt.weights.classifier_blob_layout: pool.w [H,H] | pool.b [H] | cls.w [L,H] | cls.b [128]
+        L.copy(H * H, &DevWeights::pool_w);
+        L.copy(H, &DevWeights::pool_b);
+        L.copy(static_cast<size_t>(num_labels) * H, &DevWeights::cls_w);
+        L.copy(CLS_B_FLOATS, &DevWeights::cls_b);
+        if (int rc = alloc_seg_slots(rt)) return rc;
     }
     if (int rc = load_weights(rt, *m, L, blob, nbytes)) return rc;
     return register_model(rt, std::move(m), model_out);
@@ -1537,8 +1594,10 @@ int b200rt_model_load(const char* kind, const void* cfg, const void* weights, si
 int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0 && strcmp(kind, "clip_text") != 0))
-        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"vit\" or \"clip_text\")", kind ? kind : "(null)");
+    if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0 && strcmp(kind, "clip_text") != 0 &&
+                  strcmp(kind, "bert_classifier") != 0))
+        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"bert_classifier\", \"vit\" or \"clip_text\")",
+                    kind ? kind : "(null)");
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
     if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
     const bool pool_mean = (flags & B200RT_LOAD_POOL_MEAN) != 0;
@@ -1551,11 +1610,30 @@ int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights,
         if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"clip_text\"", flags);
         return model_load_clip_text(*static_cast<const b200rt_clip_text_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
     }
+    if (strcmp(kind, "bert_classifier") == 0) {
+        if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"bert_classifier\"", flags);
+        const b200rt_bert_classifier_config& cc = *static_cast<const b200rt_bert_classifier_config*>(cfg);
+        if (cc.num_labels < 1 || cc.num_labels > MAX_LABELS)
+            return fail(B200RT_E_UNSUPPORTED, "num_labels %d outside [1, %d]", cc.num_labels, MAX_LABELS);
+        return model_load(cc.bert, static_cast<const float*>(weights), nbytes, false, model_out, cc.num_labels);
+    }
     return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean, model_out);
 }
 
+// segs [n_items] (b200rt_submit_pairs, classifier models only): item i's second segment starts at token segs[i], 0 <= segs[i] <=
+// lens[i]; NULL: one segment.
+int check_segs(const Model& m, const int32_t* lens, const int32_t* segs, int n_items, int max_len) {
+    if (!segs) return 0;
+    if (m.num_labels == 0) return fail(B200RT_E_INVALID, "token segments (segs) apply to classifier models (kind \"bert_classifier\")");
+    for (int i = 0; i < n_items; ++i) {
+        const int L = lens ? lens[i] : max_len;
+        if (segs[i] < 0 || segs[i] > L) return fail(B200RT_E_INVALID, "segs[%d] = %d outside [0, lens[%d] = %d]", i, segs[i], i, L);
+    }
+    return 0;
+}
+
 static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, float* out,
-                       uint32_t flags, uint64_t* ticket_out) {
+                       uint32_t flags, uint64_t* ticket_out, const int32_t* segs = nullptr) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
@@ -1564,6 +1642,7 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d takes pixels (b200rt_submit_pixels), not token ids", model);
     if (flags & ~static_cast<uint32_t>(B200RT_SUBMIT_BORROW_IDS)) return fail(B200RT_E_INVALID, "unknown submit flags 0x%x", flags);
     if (int rc = check_ids(*m, ids, lens, n_items, max_len, m->max_pos)) return rc;
+    if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
     auto t = std::make_shared<Ticket>();
     t->model = model;
     t->mp = m;
@@ -1582,6 +1661,7 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     t->out_pinned = is_pinned(out, static_cast<size_t>(n_items) * m->out_dim * 4);
     if (lens) t->lens.assign(lens, lens + n_items);
     else t->lens.assign(n_items, max_len);
+    if (segs) t->segs.assign(segs, segs + n_items);
     // runs of items per 64-token length bucket (TEI batches by token budget, un-padded; here every bucket is padded to its
     // own length, so a ragged input wastes at most 63 tokens per item instead of max_len - len)
     std::vector<Run> runs;
@@ -1625,6 +1705,11 @@ int b200rt_submit(int model, const int32_t* ids, const int32_t* lens, int n_item
 int b200rt_submit_ex(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, float* out,
                      uint32_t flags, uint64_t* ticket_out) {
     return submit_impl(model, ids, lens, n_items, max_len, out, flags, ticket_out);
+}
+
+int b200rt_submit_pairs(int model, const int32_t* ids, const int32_t* lens, const int32_t* segs, int n_items, int max_len, float* out,
+                        uint32_t flags, uint64_t* ticket_out) {
+    return submit_impl(model, ids, lens, n_items, max_len, out, flags, ticket_out, segs);
 }
 
 int b200rt_submit_pixels(int model, const float* pixels, int n_items, float* out, uint64_t* ticket_out) {
@@ -1733,6 +1818,11 @@ int b200rt_poll_any(uint64_t* ticket_out, int timeout_ms) {
 
 int b200rt_embed_device(int model, int gpu, const int32_t* d_ids, const int32_t* d_lens, int n_items, int max_len,
                         float* d_out, void* stream) {
+    return b200rt_embed_device_pairs(model, gpu, d_ids, d_lens, nullptr, n_items, max_len, d_out, stream);
+}
+
+int b200rt_embed_device_pairs(int model, int gpu, const int32_t* d_ids, const int32_t* d_lens, const int32_t* d_segs, int n_items,
+                              int max_len, float* d_out, void* stream) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
@@ -1740,11 +1830,13 @@ int b200rt_embed_device(int model, int gpu, const int32_t* d_ids, const int32_t*
     if (gpu < 0 || gpu >= static_cast<int>(rt->devs.size())) return fail(B200RT_E_INVALID, "gpu index %d outside the pool", gpu);
     if (m->kind == KIND_VIT) return fail(B200RT_E_UNSUPPORTED, "b200rt_embed_device takes token ids: model %d is not a text encoder", model);
     if (!d_ids || !d_lens || !d_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
+    if (d_segs && m->num_labels == 0)
+        return fail(B200RT_E_INVALID, "token segments (d_segs) apply to classifier models (kind \"bert_classifier\")");
     Dev& d = *rt->devs[gpu];
     std::lock_guard<std::mutex> dl(d.mu);
     CUDA_TRY(cudaSetDevice(d.id));
     uint64_t launches = 0;
-    int rc = forward(d, *m, gpu, Input{d_ids, d_lens, nullptr, n_items, max_len}, d_out,
+    int rc = forward(d, *m, gpu, Input{d_ids, d_lens, nullptr, n_items, max_len, d_segs}, d_out,
                      stream ? static_cast<cudaStream_t>(stream) : d.compute, launches);
     std::lock_guard<std::mutex> sl(rt->stats_mu);
     rt->stats.kernel_launches += launches;
@@ -1841,7 +1933,7 @@ void b200rt_shutdown(void) {
         cudaFree(d->lens_const);
         if (d->copy) cudaStreamDestroy(d->copy);
         for (int s = 0; s < NSLOT; ++s) if (d->ev_pix[s]) cudaEventDestroy(d->ev_pix[s]);
-        for (int s = 0; s < NSLOT; ++s) { cudaFree(d->pix_in[s]); cudaFree(d->ids_in[s]); cudaFree(d->lens_in[s]); cudaEventDestroy(d->ev_done[s]); cudaEventDestroy(d->ev_begin[s]); cudaEventDestroy(d->ev_end[s]); }
+        for (int s = 0; s < NSLOT; ++s) { cudaFree(d->pix_in[s]); cudaFree(d->ids_in[s]); cudaFree(d->lens_in[s]); cudaFree(d->segs_in[s]); cudaEventDestroy(d->ev_done[s]); cudaEventDestroy(d->ev_begin[s]); cudaEventDestroy(d->ev_end[s]); }
         cudaEventDestroy(d->ev_ws);
         cudaStreamDestroy(d->compute);
     }
@@ -1849,6 +1941,8 @@ void b200rt_shutdown(void) {
     for (int s = 0; s < NSLOT; ++s) {
         cudaFreeHost(rt->h_ids[s]); cudaFreeHost(rt->h_lens[s]); cudaFreeHost(rt->h_out[s]);
         cudaFree(rt->d_ids_stage[s]); cudaFree(rt->d_lens_stage[s]); cudaFree(rt->d_out_gather[s]);
+        if (rt->h_segs[s]) cudaFreeHost(rt->h_segs[s]);
+        cudaFree(rt->d_segs_stage[s]);
         cudaEventDestroy(rt->ev_scatter[s]); cudaEventDestroy(rt->ev_wave[s]); cudaEventDestroy(rt->ev_t0[s]); cudaEventDestroy(rt->ev_fwd_end[s]);
     }
     cudaStreamDestroy(rt->s_in);
@@ -2043,6 +2137,72 @@ int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, 
     return 0;
 }
 
+int b200rt_debug_embed_segs(const int32_t* ids, const int32_t* segs, const float* word, const float* pos, const float* type, int n_tokens,
+                            int S, int vocab, uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!ids || !segs || !word || !pos || !type || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1 || n_tokens % S)
+        return fail(B200RT_E_INVALID, "bad embed_segs arguments (n_tokens must be a multiple of S)");
+    if (hidden != 768 && hidden != 384 && hidden != 1024)
+        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024, got %d", hidden);
+    const size_t H = hidden, P = H / 128;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_tokens);
+    DebugBuffers b(d.compute);
+    int32_t *dids, *dsegs;
+    float *dw, *dp, *dt;
+    __half *dhi, *dlo;
+    float2* dst;
+    CUDA_TRY(b.upload(&dids, ids, rows * 4));
+    CUDA_TRY(b.upload(&dsegs, segs, rows / S * 4));  // passed through unchecked: the kernel clamps to [0, S]
+    CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * H * 4));
+    CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * H * 4));
+    CUDA_TRY(b.upload(&dt, type, 2 * H * 4));
+    CUDA_TRY(b.upload(&dhi, nullptr, rows * H * 2));
+    CUDA_TRY(b.upload(&dlo, nullptr, rows * H * 2));
+    CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
+    CUDA_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, hidden, d.compute, dsegs));
+    CUDA_TRY(b.download(hi_out, dhi, rows * H * 2));
+    CUDA_TRY(b.download(lo_out, dlo, rows * H * 2));
+    CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
+    return 0;
+}
+
+int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* pool_w,
+                          const float* pool_b, const float* cls_w, const float* cls_b, int n_items, int S, int L, float eps, float* out,
+                          int hidden, int ctas) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!hi || !lo || !gamma || !beta || !pool_w || !pool_b || !cls_w || !cls_b || !out || n_items < 1 || S < 1 || ctas < 0)
+        return fail(B200RT_E_INVALID, "bad cls_head arguments");
+    if (L < 1 || L > MAX_LABELS) return fail(B200RT_E_INVALID, "num_labels %d outside [1, %d]", L, MAX_LABELS);
+    if (hidden != 768 && hidden != 384 && hidden != 1024)
+        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024, got %d", hidden);
+    const size_t H = hidden;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t rows = static_cast<size_t>(n_items) * S;
+    DebugBuffers b(d.compute);
+    __half *dhi, *dlo;
+    float *dg, *dbt, *dpw, *dpb, *dcw, *dcb, *dout;
+    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+    CUDA_TRY(b.upload(&dg, gamma, H * 4));
+    CUDA_TRY(b.upload(&dbt, beta, H * 4));
+    CUDA_TRY(b.upload(&dpw, pool_w, H * H * 4));
+    CUDA_TRY(b.upload(&dpb, pool_b, H * 4));
+    CUDA_TRY(b.upload(&dcw, cls_w, static_cast<size_t>(L) * H * 4));
+    CUDA_TRY(b.upload(&dcb, cls_b, static_cast<size_t>(L) * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * L * 4));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, static_cast<size_t>(n_items) * L * 4, d.compute));
+    CUDA_TRY(launch_cls_head(dhi, dlo, dg, dbt, dpw, dpb, dcw, dcb, dout, n_items, S, L, eps, hidden, d.compute, ctas));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * L * 4));
+    return 0;
+}
+
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out) {
     Runtime* rt = live_rt();
@@ -2210,12 +2370,20 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
 int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_launches,
                                uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx,
                                uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total) {
+    return b200rt_debug_forward_trace_segs(model, ids, lens, nullptr, n_items, max_len, n_launches, yhi, ylo, pstats0, pstats1, qkv, ctx,
+                                           ffn, out, names_out, names_cap, n_total);
+}
+
+int b200rt_debug_forward_trace_segs(int model, const int32_t* ids, const int32_t* lens, const int32_t* segs, int n_items, int max_len,
+                                    int n_launches, uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv,
+                                    uint16_t* ctx, uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
     if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (int rc = check_ids(*m, ids, lens, n_items, max_len, max_wave_len(*m))) return rc;
+    if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
     const int total = 5 * m->layers + 2;
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
@@ -2231,8 +2399,10 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
     int32_t *dids = nullptr, *dlens = nullptr;
     CUDA_TRY(b.upload(&dids, ids, M * 4));
     CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
+    int32_t* dsegs = nullptr;
+    if (segs) CUDA_TRY(b.upload(&dsegs, segs, static_cast<size_t>(n_items) * 4));
     const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(b, d, *m, Input{dids, dlens, nullptr, n_items, max_len}, n_launches, o);
+    return trace_forward(b, d, *m, Input{dids, dlens, nullptr, n_items, max_len, dsegs}, n_launches, o);
 }
 
 int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,

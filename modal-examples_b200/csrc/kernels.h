@@ -75,9 +75,19 @@ cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, con
                              cudaStream_t stream, int head_dim, int heads, bool causal);
 
 // Text row kernels on rows of `width` (768, 384 or 1024; embed also 512) columns.
-// word + position + token_type(0) embedding gather -> y = hi + lo (pre-LN residual stream) + the row's statistic partials.
+// word + position + token_type embedding gather -> y = hi + lo (pre-LN residual stream) + the row's statistic partials.
+// segs NULL: every token takes type row 0.  segs [n_tokens / S] (768, 384, 1024 only): token p of item i takes type row 1
+// (type0 + width) when p >= segs[i], clamped to [0, S] on the device, else row 0 -- the second segment of a sentence pair.
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,
-                         float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream);
+                         float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream, const int32_t* segs = nullptr);
+
+// BertForSequenceClassification's head: out + i * L = W_c tanh(W_p LN(hi + lo of row i * S) + b_p) + b_c, L raw logits per
+// item (1 <= L <= 64), pool_w fp32 [width, width], cls_w fp32 [L, width].  Reductions run in a fixed order per item, so the
+// logits do not depend on the batch, the grid or the replica.  ctas: the most blocks launched (0 = one per item; blocks walk
+// the items).  `out` may be peer memory.
+cudaError_t launch_cls_head(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const float* pool_w,
+                            const float* pool_b, const float* cls_w, const float* cls_b, float* out, int n_items, int S, int L, float eps,
+                            int width, cudaStream_t stream, int ctas = 0);
 
 // final LayerNorm of the CLS row of every item + L2 normalise; row i is stored at out + i * width,
 // where `out` may be a peer-mapped pointer into the root GPU's gather buffer (the fused gather).
@@ -108,7 +118,8 @@ cudaError_t launch_clip_text_pool(const __half* yhi, const __half* ylo, const in
                                   const float* beta, const float* proj, float* out, int n_items, int S, int P, float eps, int eos_id,
                                   cudaStream_t stream);
 
-// Root-side scatter of a wave's token ids / lengths into each shard's (possibly peer) input slot.
+// Root-side scatter of a wave's token ids / lengths (and, src_segs given, segment starts into dst_segs) into each shard's
+// (possibly peer) input slot.
 struct ScatterPlan {
     static constexpr int MAX_SHARDS = 16;
     int n_shards;
@@ -117,9 +128,10 @@ struct ScatterPlan {
     int32_t* dst_lens[MAX_SHARDS];
     int item_begin[MAX_SHARDS];
     int item_count[MAX_SHARDS];
+    int32_t* dst_segs[MAX_SHARDS];  // read only when launch_scatter is given src_segs
 };
 cudaError_t launch_scatter(const int32_t* src_ids, const int32_t* src_lens, const ScatterPlan& plan,
-                           cudaStream_t stream);
+                           cudaStream_t stream, const int32_t* src_segs = nullptr);
 
 }  // namespace b200
 

@@ -86,11 +86,14 @@ __device__ __forceinline__ void load_split_row(const __half* __restrict__ yhi, c
     }
 }
 
-template <int W>
+// SEGS: `type` holds two rows and token p of item i takes row 1 when p >= segs[i] (the second segment of a
+// [CLS] a [SEP] b [SEP] pair), row 0 otherwise; segs[i] is clamped to [0, S] (a device-resident caller's segs are not
+// validated).  Without SEGS every token takes row 0 and `segs` is not read.
+template <int W, bool SEGS>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ word, const float* __restrict__ pos,
              const float* __restrict__ type0, __half* __restrict__ yhi, __half* __restrict__ ylo, float2* __restrict__ stats,
-             int n_tokens, int S, int vocab) {
+             int n_tokens, int S, int vocab, const int32_t* __restrict__ segs) {
     constexpr int V4 = Row<W>::V4;
     const int lane = threadIdx.x & 31;
     const int tok = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
@@ -100,7 +103,13 @@ embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ word, co
     const int p = tok % S;
     const float4* w4 = reinterpret_cast<const float4*>(word + static_cast<size_t>(id) * W);
     const float4* p4 = reinterpret_cast<const float4*>(pos + static_cast<size_t>(p) * W);
-    const float4* t4 = reinterpret_cast<const float4*>(type0);
+    const float* type_row = type0;
+    if constexpr (SEGS) {
+        int sg = segs[tok / S];
+        sg = sg < 0 ? 0 : (sg > S ? S : sg);
+        if (p >= sg) type_row += W;
+    }
+    const float4* t4 = reinterpret_cast<const float4*>(type_row);
     uint2* oh = reinterpret_cast<uint2*>(yhi + static_cast<size_t>(tok) * W);
     uint2* ol = reinterpret_cast<uint2*>(ylo + static_cast<size_t>(tok) * W);
     float ps = 0.f, pq = 0.f;  // lane i < V4 keeps partial i
@@ -222,6 +231,57 @@ mean_pool_normalize_kernel(const __half* __restrict__ yhi, const __half* __restr
     for (int k = 0; k < PER_THREAD; ++k) {
         const int c = threadIdx.x + k * WARPS_PER_BLOCK * 32;
         if (c < W) o[c] = v[k] * inv;
+    }
+}
+
+// BertForSequenceClassification's head (HF modeling_bert.py BertPooler + the classifier Linear): out[i] = W_c tanh(W_p x + b_p)
+// + b_c, x = the last LayerNorm of the CLS row of item i, L raw logits per item (no sigmoid / softmax: the caller applies
+// them).  Blocks walk items i = blockIdx.x, + gridDim.x, ...  Every warp LayerNorms its own copy of the CLS row (the
+// load_split_row / ln_inplace of pool_normalize) and takes pooler rows n = warp, warp + 8, ...: a per-lane fma chain over the
+// lane's columns then a warp_sum, so each h[n] is reduced in one fixed order.  The classifier rows j = warp, warp + 8, ... < L
+// read h from shared memory in the same column layout.  Nothing depends on the grid, the batch or the replica, so an item's
+// logits are bit-identical wherever it runs.  W_p fp32 [W, W] and W_c fp32 [L, W] are read by every item and stay L2-resident.
+constexpr int CLS_HEAD_MAX_L = 64;
+template <int W>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
+cls_head_kernel(const __half* __restrict__ yhi, const __half* __restrict__ ylo, const float* __restrict__ gamma,
+                const float* __restrict__ beta, const float* __restrict__ pool_w, const float* __restrict__ pool_b,
+                const float* __restrict__ cls_w, const float* __restrict__ cls_b, float* __restrict__ out, int n_items, int S, int L,
+                float eps) {
+    constexpr int V4 = Row<W>::V4;
+    __shared__ __align__(16) float s_h[W];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        float4 x[V4];
+        load_split_row<W>(yhi, ylo, static_cast<size_t>(item) * S, lane, x);  // CLS row
+        ln_inplace<W>(x, gamma, beta, eps, lane);
+        for (int n = warp; n < W; n += WARPS_PER_BLOCK) {
+            const float4* w4 = reinterpret_cast<const float4*>(pool_w + static_cast<size_t>(n) * W);
+            float acc = 0.f;
+#pragma unroll
+            for (int i = 0; i < V4; ++i) {
+                const float4 w = __ldg(w4 + i * 32 + lane);
+                acc = fmaf(x[i].x, w.x, fmaf(x[i].y, w.y, fmaf(x[i].z, w.z, fmaf(x[i].w, w.w, acc))));
+            }
+            acc = warp_sum(acc);
+            if (lane == 0) s_h[n] = tanhf(acc + __ldg(pool_b + n));
+        }
+        __syncthreads();
+        float4 h[V4];
+#pragma unroll
+        for (int i = 0; i < V4; ++i) h[i] = *reinterpret_cast<const float4*>(&s_h[i * 128 + 4 * lane]);
+        for (int j = warp; j < L; j += WARPS_PER_BLOCK) {
+            const float4* w4 = reinterpret_cast<const float4*>(cls_w + static_cast<size_t>(j) * W);
+            float acc = 0.f;
+#pragma unroll
+            for (int i = 0; i < V4; ++i) {
+                const float4 w = __ldg(w4 + i * 32 + lane);
+                acc = fmaf(h[i].x, w.x, fmaf(h[i].y, w.y, fmaf(h[i].z, w.z, fmaf(h[i].w, w.w, acc))));
+            }
+            acc = warp_sum(acc);
+            if (lane == 0) out[static_cast<size_t>(item) * L + j] = acc + __ldg(cls_b + j);  // may be peer memory
+        }
+        __syncthreads();  // s_h is rewritten by the next item
     }
 }
 
@@ -436,10 +496,12 @@ fold_ln_kernel(const float* __restrict__ w, const float* __restrict__ gamma, con
     }
 }
 
-// blockIdx.y = shard.  Copies ids[item_begin*S .. (item_begin+item_count)*S) and the matching lens to the
-// shard's input slot; dst pointers of remote shards are peer-mapped, so the stores cross NVLink directly.
+// blockIdx.y = shard.  Copies ids[item_begin*S .. (item_begin+item_count)*S) and the matching lens (and, SEGS, segment
+// starts) to the shard's input slot; dst pointers of remote shards are peer-mapped, so the stores cross NVLink directly.
+template <bool SEGS>
 __global__ void __launch_bounds__(256)
-scatter_kernel(const int32_t* __restrict__ src_ids, const int32_t* __restrict__ src_lens, const ScatterPlan plan) {
+scatter_kernel(const int32_t* __restrict__ src_ids, const int32_t* __restrict__ src_lens, const ScatterPlan plan,
+               const int32_t* __restrict__ src_segs) {
     const int sh = blockIdx.y;
     const int cnt = plan.item_count[sh];
     if (cnt <= 0) return;
@@ -457,17 +519,40 @@ scatter_kernel(const int32_t* __restrict__ src_ids, const int32_t* __restrict__ 
         for (size_t i = tid; i < n; i += stride) d[i] = s[i];
     }
     for (size_t i = tid; i < static_cast<size_t>(cnt); i += stride) plan.dst_lens[sh][i] = src_lens[plan.item_begin[sh] + i];
+    if constexpr (SEGS)
+        for (size_t i = tid; i < static_cast<size_t>(cnt); i += stride) plan.dst_segs[sh][i] = src_segs[plan.item_begin[sh] + i];
 }
 
 }  // namespace rw
 
 cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, __half* yhi, __half* ylo,
-                         float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream) {
+                         float2* stats, int n_tokens, int S, int vocab, int width, cudaStream_t stream, const int32_t* segs) {
     const int grid = (n_tokens + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
-    if (width == 768) rw::embed_kernel<768><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
-    else if (width == 384) rw::embed_kernel<384><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
-    else if (width == 1024) rw::embed_kernel<1024><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
-    else if (width == 512) rw::embed_kernel<512><<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab);
+    const int block = rw::WARPS_PER_BLOCK * 32;
+    if (segs) {  // token pairs: BERT classifiers only (768, 384, 1024)
+        if (width == 768) rw::embed_kernel<768, true><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, segs);
+        else if (width == 384) rw::embed_kernel<384, true><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, segs);
+        else if (width == 1024) rw::embed_kernel<1024, true><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, segs);
+        else return cudaErrorInvalidValue;
+        return cudaGetLastError();
+    }
+    if (width == 768) rw::embed_kernel<768, false><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, nullptr);
+    else if (width == 384) rw::embed_kernel<384, false><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, nullptr);
+    else if (width == 1024) rw::embed_kernel<1024, false><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, nullptr);
+    else if (width == 512) rw::embed_kernel<512, false><<<grid, block, 0, stream>>>(ids, word, pos, type0, yhi, ylo, stats, n_tokens, S, vocab, nullptr);
+    else return cudaErrorInvalidValue;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_cls_head(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const float* pool_w,
+                            const float* pool_b, const float* cls_w, const float* cls_b, float* out, int n_items, int S, int L, float eps,
+                            int width, cudaStream_t stream, int ctas) {
+    if (n_items < 1 || S < 1 || L < 1 || L > rw::CLS_HEAD_MAX_L || ctas < 0) return cudaErrorInvalidValue;
+    const int grid = ctas == 0 || ctas > n_items ? n_items : ctas;
+    const int block = rw::WARPS_PER_BLOCK * 32;
+    if (width == 768) rw::cls_head_kernel<768><<<grid, block, 0, stream>>>(yhi, ylo, gamma, beta, pool_w, pool_b, cls_w, cls_b, out, n_items, S, L, eps);
+    else if (width == 384) rw::cls_head_kernel<384><<<grid, block, 0, stream>>>(yhi, ylo, gamma, beta, pool_w, pool_b, cls_w, cls_b, out, n_items, S, L, eps);
+    else if (width == 1024) rw::cls_head_kernel<1024><<<grid, block, 0, stream>>>(yhi, ylo, gamma, beta, pool_w, pool_b, cls_w, cls_b, out, n_items, S, L, eps);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
@@ -533,7 +618,7 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
 }
 
 cudaError_t launch_scatter(const int32_t* src_ids, const int32_t* src_lens, const ScatterPlan& plan,
-                           cudaStream_t stream) {
+                           cudaStream_t stream, const int32_t* src_segs) {
     if (plan.n_shards < 1 || plan.n_shards > ScatterPlan::MAX_SHARDS) return cudaErrorInvalidValue;
     int max_cnt = 0;
     for (int i = 0; i < plan.n_shards; ++i) max_cnt = plan.item_count[i] > max_cnt ? plan.item_count[i] : max_cnt;
@@ -541,7 +626,8 @@ cudaError_t launch_scatter(const int32_t* src_ids, const int32_t* src_lens, cons
     const size_t n4 = (static_cast<size_t>(max_cnt) * plan.S + 3) / 4;
     int gx = static_cast<int>((n4 + 255) / 256);
     gx = gx < 1 ? 1 : (gx > 132 * 4 ? 132 * 4 : gx);
-    rw::scatter_kernel<<<dim3(gx, plan.n_shards), 256, 0, stream>>>(src_ids, src_lens, plan);
+    if (src_segs) rw::scatter_kernel<true><<<dim3(gx, plan.n_shards), 256, 0, stream>>>(src_ids, src_lens, plan, src_segs);
+    else rw::scatter_kernel<false><<<dim3(gx, plan.n_shards), 256, 0, stream>>>(src_ids, src_lens, plan, nullptr);
     return cudaGetLastError();
 }
 

@@ -20,6 +20,8 @@ BGE_LARGE_ID = "BAAI/bge-large-en-v1.5"
 MINILM_L6_ID = "sentence-transformers/all-MiniLM-L6-v2"
 POOLING_BY_MODEL_ID = {MINILM_L6_ID: "mean"}  # models whose sentence-transformers config pools other than by [CLS]
 POOLINGS = ("cls", "mean")  # TEI also knows splade and last-token; this runtime does not
+MS_MARCO_L6_ID = "cross-encoder/ms-marco-MiniLM-L-6-v2"
+MS_MARCO_L12_ID = "cross-encoder/ms-marco-MiniLM-L-12-v2"
 
 
 def geometry_for_model_id(model_id: str) -> dict:
@@ -27,11 +29,74 @@ def geometry_for_model_id(model_id: str) -> dict:
     BAAI/bge-small-en-v1.5, bge-large's for BAAI/bge-large-en-v1.5, MiniLM-L6's (bge-small's with 6 layers) for
     sentence-transformers/all-MiniLM-L6-v2, bge-base's for BAAI/bge-base-en-v1.5 and for any id this table does not know.
     A hub snapshot takes its geometry from its own config.json instead."""
-    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_LARGE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY
+    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_LARGE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY, MS_MARCO_MINILM_L6_GEOMETRY
 
     known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY, BGE_LARGE_ID: BGE_LARGE_GEOMETRY,
-             MINILM_L6_ID: MINILM_L6_GEOMETRY}
+             MINILM_L6_ID: MINILM_L6_GEOMETRY, MS_MARCO_L6_ID: MS_MARCO_MINILM_L6_GEOMETRY,
+             MS_MARCO_L12_ID: dict(MS_MARCO_MINILM_L6_GEOMETRY, layers=12)}
     return dict(known.get(model_id, BGE_BASE_GEOMETRY))
+
+
+# --------------------------------------------------------------------------- classifier scoring (host side, as TEI does it)
+
+def _sigmoid(x):
+    import numpy as np
+
+    x = np.asarray(x, np.float64)
+    return np.where(x >= 0, 1.0 / (1.0 + np.exp(-np.abs(x))), np.exp(-np.abs(x)) / (1.0 + np.exp(-np.abs(x))))
+
+
+def label_scores(logits, raw_scores: bool):
+    """Per-item label scores from ``[n, L]`` raw logits: the logits themselves (raw_scores), else a sigmoid when L == 1 and a
+    softmax over the labels otherwise."""
+    import numpy as np
+
+    z = np.asarray(logits, np.float64)
+    if raw_scores:
+        return z
+    if z.shape[1] == 1:
+        return _sigmoid(z)
+    e = np.exp(z - z.max(1, keepdims=True))
+    return e / e.sum(1, keepdims=True)
+
+
+def rerank_response(logits, texts, raw_scores: bool, return_text: bool) -> list:
+    """``[{"index", "score"[, "text"]}]`` sorted by score, highest first (ties keep the input order), from ``[n, 1]`` logits."""
+    scores = label_scores(logits, raw_scores)[:, 0]
+    order = sorted(range(len(scores)), key=lambda i: -scores[i])
+    out = []
+    for i in order:
+        r = {"index": i, "score": float(scores[i])}
+        if return_text:
+            r["text"] = texts[i]
+        out.append(r)
+    return out
+
+
+def predict_response(logits_row, id2label: dict, raw_scores: bool) -> list:
+    """``[{"label", "score"}]`` of one input, sorted by score, highest first."""
+    scores = label_scores(logits_row[None, :], raw_scores)[0]
+    order = sorted(range(len(scores)), key=lambda j: -scores[j])
+    return [{"label": id2label.get(j, f"LABEL_{j}"), "score": float(scores[j])} for j in order]
+
+
+def parse_predict_inputs(inputs):
+    """TEI's /predict ``inputs``: a string, a ``[text, text]`` pair, or a list of those.  Returns (list of str or (str, str),
+    whether it was a batch)."""
+    def seq(x):
+        if isinstance(x, str):
+            return x
+        if isinstance(x, list) and len(x) == 2 and all(isinstance(t, str) for t in x):
+            return (x[0], x[1])
+        raise TypeError("each input must be a string or a [string, string] pair")
+
+    if isinstance(inputs, str):
+        return [inputs], False
+    if isinstance(inputs, list) and len(inputs) == 2 and all(isinstance(t, str) for t in inputs):
+        return [(inputs[0], inputs[1])], False
+    if isinstance(inputs, list) and inputs:
+        return [seq(x) for x in inputs], True
+    raise TypeError("`inputs` must be a string, a [string, string] pair or a non-empty list of those")
 
 
 def resolve_pooling(flag: str | None, snapshot_dir: str | None, model_id: str) -> str:
@@ -102,6 +167,11 @@ def load_weights(args):
 
     if args.weights:
         if args.weights.endswith(".safetensors"):
+            sd = W.read_safetensors(args.weights)
+            if "classifier.weight" in sd:  # a BertForSequenceClassification checkpoint
+                cfg_path = os.path.join(os.path.dirname(os.path.abspath(args.weights)), "config.json")
+                cfg = json.load(open(cfg_path)) if os.path.exists(cfg_path) else {}
+                return W.load_hf_classifier(sd, cfg) + (f"safetensors {args.weights}",)
             return W.load_safetensors(args.weights) + (f"safetensors {args.weights}",)
         if os.path.isdir(args.weights):
             return W.load_hf_dir(args.weights) + (f"HF directory {args.weights}",)
@@ -112,6 +182,8 @@ def load_weights(args):
         if snap:
             return W.load_hf_dir(snap) + (f"hub snapshot {snap}",)
     g = geometry_for_model_id(args.model_id)
+    if "num_labels" in g:
+        return g, W.random_classifier_blob(g, 0), None
     return g, random_blob(geometry=g), None
 
 
@@ -142,7 +214,17 @@ class Engine:
             print(f"[text-embeddings-router/b200] weights: {source}", file=sys.stderr)
         print(f"[text-embeddings-router/b200] pooling: {self.pooling}", file=sys.stderr)
         self.geometry = geometry
-        self.model = b200rt.EmbedModel(geometry, blob, pooling=self.pooling)
+        self.classifier = "num_labels" in geometry
+        if self.classifier:
+            from b200rt.weights import default_id2label
+
+            self.id2label = geometry.get("id2label") or default_id2label(geometry["num_labels"])
+            kind = "reranker" if geometry["num_labels"] == 1 else "classifier"
+            print(f"[text-embeddings-router/b200] {kind}: BertForSequenceClassification, {geometry['num_labels']} label(s)"
+                  + (" -- SEEDED weights, scores are not the real model's" if source is None else ""), file=sys.stderr)
+            self.model = b200rt.ClassifierModel(geometry, blob)
+        else:
+            self.model = b200rt.EmbedModel(geometry, blob, pooling=self.pooling)
         self.n_gpus = n_gpus
 
     def embed(self, inputs):
@@ -153,6 +235,38 @@ class Engine:
         for i, r in enumerate(rows):
             ids[i, : len(r)] = r
         return self.model.embed(ids, lens)
+
+    def classify(self, inputs, truncate: bool):
+        """``[n, num_labels]`` raw logits of strings and (text, text) pairs; ValueError when one is too long (TEI: 413)."""
+        np = self.np
+        n = self.geometry["max_pos"]
+        rows, segs = [], []
+        for x in inputs:
+            if isinstance(x, tuple):
+                r, sg = self.tok.encode_pair(x[0], x[1], n, truncate)
+            else:
+                r = self.tok.encode(x, n, truncate)
+                sg = len(r)
+            rows.append(r)
+            segs.append(sg)
+        lens = np.array([len(r) for r in rows], np.int32)
+        ids = np.zeros((len(rows), int(lens.max())), np.int32)
+        for i, r in enumerate(rows):
+            ids[i, : len(r)] = r
+        return self.model.classify(ids, lens, np.array(segs, np.int32))
+
+    def info(self) -> dict:
+        """TEI's /info.  An embedding model's is what it always was; a classifier's reports model_type as TEI does."""
+        args = self.args
+        d = {"model_id": args.model_id, "model_dtype": "float16", "max_client_batch_size": args.max_client_batch_size,
+             "max_input_length": GEOMETRY["max_pos"], "backend": f"b200rt x{self.n_gpus}"}
+        if not self.classifier:
+            d["pooling"] = self.pooling
+            return d
+        labels = {str(k): v for k, v in sorted(self.id2label.items())}
+        kind = "reranker" if self.geometry["num_labels"] == 1 else "classifier"
+        d["model_type"] = {kind: {"id2label": labels, "label2id": {v: int(k) for k, v in labels.items()}}}
+        return d
 
 
 def make_handler(engine: Engine):
@@ -174,14 +288,23 @@ def make_handler(engine: Engine):
             if self.path == "/health":
                 self._send(200, {})
             elif self.path == "/info":
-                self._send(200, {"model_id": engine.args.model_id, "model_dtype": "float16", "max_client_batch_size": engine.args.max_client_batch_size,
-                                 "max_input_length": GEOMETRY["max_pos"], "backend": f"b200rt x{engine.n_gpus}", "pooling": engine.pooling})
+                self._send(200, engine.info())
             else:
                 self._send(404, {"error": "not found", "error_type": "NotFound"})
 
+        def _rerank(self, req):
+            query, texts = req.get("query"), req.get("texts")
+            if not isinstance(query, str) or not isinstance(texts, list) or not texts or not all(isinstance(t, str) for t in texts):
+                raise TypeError("`query` must be a string and `texts` a non-empty list of strings")
+            return query, texts
+
         def do_POST(self):
+            if self.path in ("/rerank", "/predict"):
+                return self._classify()
             if self.path not in ("/embed", "/"):
                 return self._send(404, {"error": "not found", "error_type": "NotFound"})
+            if engine.classifier:
+                return self._send(400, {"error": f"{engine.args.model_id} is a classifier: use /rerank or /predict", "error_type": "Backend"})
             try:
                 req = json.loads(self.rfile.read(int(self.headers.get("Content-Length", "0"))))
                 inputs = req["inputs"]
@@ -201,6 +324,37 @@ def make_handler(engine: Engine):
             except Exception as e:  # noqa: BLE001
                 return self._send(500, {"error": str(e), "error_type": "Backend"})
             self._send(200, vecs.tolist())
+
+        def _classify(self):
+            if not engine.classifier:
+                return self._send(400, {"error": f"{engine.args.model_id} is an embedding model: use /embed", "error_type": "Backend"})
+            rerank = self.path == "/rerank"
+            try:
+                req = json.loads(self.rfile.read(int(self.headers.get("Content-Length", "0"))))
+                if rerank:
+                    query, texts = self._rerank(req)
+                    inputs, batch = [(query, t) for t in texts], True
+                else:
+                    inputs, batch = parse_predict_inputs(req.get("inputs"))
+            except Exception as e:  # noqa: BLE001
+                return self._send(422, {"error": f"Failed to deserialize the JSON body: {e}", "error_type": "Validation"})
+            if rerank and engine.geometry["num_labels"] != 1:
+                return self._send(400, {"error": "/rerank needs a model with one label (a reranker); use /predict", "error_type": "Backend"})
+            if len(inputs) > engine.args.max_client_batch_size:
+                return self._send(413, {"error": f"batch size {len(inputs)} > maximum allowed batch size {engine.args.max_client_batch_size}",
+                                        "error_type": "Validation"})
+            truncate = bool(req.get("truncate", False)) or engine.args.auto_truncate
+            raw = bool(req.get("raw_scores", False))
+            try:
+                logits = engine.classify(inputs, truncate)
+            except ValueError as e:
+                return self._send(413, {"error": str(e), "error_type": "Validation"})
+            except Exception as e:  # noqa: BLE001
+                return self._send(500, {"error": str(e), "error_type": "Backend"})
+            if rerank:
+                return self._send(200, rerank_response(logits, texts, raw, bool(req.get("return_text", False))))
+            res = [predict_response(row, engine.id2label, raw) for row in logits]
+            self._send(200, res if batch else res[0])
 
     return Handler
 

@@ -160,3 +160,41 @@ class WordPiece:
                 raise ValueError(f"`inputs` must have less than {max_len} tokens. Given: {len(ids)}")
             ids = ids[: max_len - 1] + [self.sep]
         return ids
+
+    def pieces(self, text: str) -> list:
+        """The WordPiece ids of ``text``, no special tokens."""
+        ids = []
+        for w in basic_tokenize(text):
+            ids.extend(self.word_ids(w))
+        return ids
+
+    def encode_pair(self, a: str, b: str, max_len: int = 512, truncate: bool = False) -> tuple[list, int]:
+        """``[CLS] a [SEP] b [SEP]`` and where b's segment (token type 1) starts: ``(ids, seg)``.  Longer than max_len: raises
+        ValueError unless truncating (TEI: 413), else trims the pair as the Rust tokenizers' ``longest_first`` strategy does
+        (what TEI runs, and ``BertTokenizerFast(a, b, truncation="longest_first")``): with m = max_len - 3 tokens for the two
+        texts, a shorter text that fits in half of m is kept whole and the other gets the rest; otherwise each gets m // 2 and
+        the longer one (b on a tie) the odd token."""
+        pa, pb = self.pieces(a), self.pieces(b)
+        total = len(pa) + len(pb) + 3
+        if total > max_len:
+            if not truncate:
+                raise ValueError(f"`inputs` must have less than {max_len} tokens. Given: {total}")
+            na, nb = _longest_first(len(pa), len(pb), max(max_len - 3, 0))
+            pa, pb = pa[:na], pb[:nb]
+        ids = [self.cls] + pa + [self.sep] + pb + [self.sep]
+        return ids, len(pa) + 2
+
+
+def _longest_first(n_a: int, n_b: int, m: int) -> tuple[int, int]:
+    """Lengths two texts of n_a and n_b tokens keep under the tokenizers crate's LongestFirst truncation to m tokens together."""
+    swap = n_a > n_b
+    n1, n2 = (n_b, n_a) if swap else (n_a, n_b)  # n1 <= n2
+    if n1 > m:
+        n2 = n1
+    else:
+        n2 = max(n1, m - n1)
+    if n1 + n2 > m:
+        n1 = m // 2
+        n2 = n1 + m % 2
+    ka, kb = (n2, n1) if swap else (n1, n2)
+    return min(ka, n_a), min(kb, n_b)
