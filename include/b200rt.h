@@ -97,6 +97,11 @@ int b200rt_num_gpus(void);
  * infinity's `embed(sentences=...)` runs -- image_embeddings_infinity.py:298-306; blob order:
  * b200rt.weights.clip_text_blob_layout) or "bert_classifier" (cfg: b200rt_bert_classifier_config; blob order:
  * b200rt.weights.classifier_blob_layout -- BERT's, then pool.w [H,H] | pool.b [H] | cls.w [L,H] | cls.b padded to 128 floats).
+ * kind "bert_splade" (cfg: b200rt_bert_config, one of the three geometries, vocab <= 49152 else B200RT_E_UNSUPPORTED) is a
+ * SPLADE sparse encoder (HF BertForMaskedLM + SpladePooling(max, relu), e.g. naver/splade-v3): results are vocab floats per item,
+ * out[i, v] = log(1 + max over the item's tokens of relu(MLM logit v)); blob order b200rt.weights.splade_blob_layout -- BERT's,
+ * then mlm.t.w [H,H] | mlm.t.b [H] | mlm.ln.g [H] | mlm.ln.b [H] | mlm.dec.w [vocab,H] | mlm.dec.b padded to a multiple of 128
+ * floats.  It takes b200rt_submit[_ex] and b200rt_embed_device (max_len a multiple of 64); segs are B200RT_E_INVALID.
  * A "clip_text" model takes token ids through b200rt_submit[_ex] (max_len <= max_pos,
  * ids < vocab; items travel in the 64- or 128-token bucket) and b200rt_embed_device (max_len <= 128, the longest wave the
  * scheduler forms for it: device-resident callers can run the bucket the scheduler would), and is refused by

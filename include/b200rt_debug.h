@@ -78,6 +78,19 @@ int b200rt_debug_embed_segs(const int32_t* ids, const int32_t* segs, const float
 int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* pool_w,
                           const float* pool_b, const float* cls_w, const float* cls_b, int n_items, int S, int L, float eps, float* out,
                           int hidden, int ctas);
+/*   gemm_splade:    the SPLADE decoder GEMM (EPI_SPLADE_MAX): vmax_out[i, n] = fp32 bits of max(0, max over rows r = i S + t,
+ *                   t < lens[i] (clamped to [0, S]), of rstd_r (a_r . w_n) + c[n]) for n < vocab, 0 for n >= vocab.  a fp16
+ *                   [B S, K], w fp16 [vocab, K] (rows past vocab read as zeros), c fp32 [N], stats (sum, M2) [B S, K / 128],
+ *                   vmax_out uint32 [B, N]; K = 768, 384 or 1024, N % 256 == 0, S % 64 == 0.  iters launches are timed into ms_out
+ *                   (optional); the maxima come from one more launch on a zeroed buffer.  sms as for b200rt_debug_gemm: the result
+ *                   must not depend on it.
+ *   mlm_ln_stats:   stats_out [n_rows, hidden / 128] (sum, M2) partials of the fp16 rows u [n_rows, hidden]; vmax_out [n_max]
+ *                   is poisoned (0xFF) and comes back as the kernel leaves it (zeroed).
+ *   splade_finalize: out[i, v] = log1p(fp32 bits vmax[i, v]) for v < vocab, vmax uint32 [n_items, vpad], out [n_items, vocab]. */
+int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const int32_t* lens, int B, int S,
+                             int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out);
+int b200rt_debug_mlm_ln_stats(const uint16_t* u, int n_rows, int hidden, size_t n_max, uint32_t* vmax_out, float* stats_out);
+int b200rt_debug_splade_finalize(const uint32_t* vmax, int n_items, int vpad, int vocab, float* out);
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out);
 int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
@@ -95,7 +108,10 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
  * n_launches launches of the forward of this batch run exactly as the product enqueues them (same kernels, buffers and stream,
  * no sync or copy between them), and the workspace is copied out once they finish.  n_launches is in [0, n_total], n_total =
  * 5 layers + 2 (text: embed, 5 per layer, pool_normalize -- mean_pool_normalize for a B200RT_LOAD_POOL_MEAN model,
- * clip_text_pool for kind "clip_text") or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer, vit_pool).
+ * clip_text_pool for kind "clip_text") or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer, vit_pool), or 5 layers + 5
+ * for kind "bert_splade" (embed, 5 per layer, gemm_mlm_transform writing u [M, H] into ctx, mlm_ln_stats writing u's partials
+ * into pstats1 and zeroing the uint32 [n_items, vpad] maxima at the start of ffn, gemm_splade raising them, splade_finalize
+ * writing out [n_items, vocab]; vpad = vocab rounded up to 256).
  * max_len may be up to the longest wave the model runs (kind "clip_text": 128, its bucket for items of 65-77 tokens; the
  * lengths stay <= max_pos), as for b200rt_debug_profile_forward.  Every buffer comes back for rows = min(M + 256, R) rows, R = b200rt_debug_model_cap_rows(model) (512
  * b200rt_wave_capacity_items(), or 3/4 of that rounded down to 128 for bge-large), M = n_items * max_len

@@ -32,7 +32,8 @@ DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_gemm_ex", "b200rt_debug_atte
                  "b200rt_debug_embed", "b200rt_debug_vit_embed", "b200rt_debug_pool_normalize", "b200rt_debug_mean_pool_normalize",
                  "b200rt_debug_vit_pool", "b200rt_debug_clip_text_pool", "b200rt_debug_fold_ln",
                  "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace", "b200rt_debug_model_cap_rows",
-                 "b200rt_debug_embed_segs", "b200rt_debug_cls_head", "b200rt_debug_forward_trace_segs"]
+                 "b200rt_debug_embed_segs", "b200rt_debug_cls_head", "b200rt_debug_forward_trace_segs",
+                 "b200rt_debug_gemm_splade", "b200rt_debug_mlm_ln_stats", "b200rt_debug_splade_finalize"]
 
 
 def SPLIT_SMS(k: int) -> int:
@@ -139,6 +140,9 @@ def load_library():
         lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_vit_forward_trace.argtypes = [ci, vp, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_forward_trace_segs.argtypes = [ci, vp, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
+        lib.b200rt_debug_gemm_splade.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, ci, f32p, vp]
+        lib.b200rt_debug_mlm_ln_stats.argtypes = [vp, ci, ci, ctypes.c_size_t, vp, vp]
+        lib.b200rt_debug_splade_finalize.argtypes = [vp, ci, ci, ci, vp]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                      f32p, i32p, ctypes.c_int]
         _lib = lib
@@ -448,6 +452,27 @@ class ClassifierModel(EmbedModel):
         return self._trace(ids, lens, segs, n_launches)
 
 
+class SparseEmbedModel(EmbedModel):
+    """A loaded SPLADE sparse encoder (kind "bert_splade": HF ``BertForMaskedLM`` + sentence-transformers'
+    ``SpladePooling(max, relu)``, e.g. naver/splade-v3): token ids in, ``[n, vocab]`` float32 out, ``log(1 + max over the item's
+    tokens of relu(MLM logit))`` -- mostly zeros, unnormalised.  TEI serves such a model through ``/embed_sparse``.
+    ``submit``/``wait``/``poll_any``/``embed_device`` are :class:`EmbedModel`'s: same tickets, same scheduler, width ``vocab``;
+    ``embed_device`` takes ``max_len`` a multiple of 64."""
+
+    def __init__(self, geometry: dict, blob: np.ndarray):
+        lib = load_library()
+        blob = np.ascontiguousarray(blob, dtype=np.float32)
+        g = geometry
+        self.cfg = BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"], g["eps"])
+        self.hidden, self.inter, self.vocab = g["hidden"], g["inter"], g["vocab"]
+        self.out_dim = self.vocab
+        self.pooling = "splade"
+        h = ctypes.c_int32(-1)
+        _check(lib.b200rt_model_load(b"bert_splade", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
+        self.handle = h.value
+        self._lib = lib
+
+
 class ImageEmbedModel:
     """A loaded CLIP-style ViT image tower (kind "vit"): ``submit``/``wait`` take preprocessed pixels
     ``[n, 3, image, image]`` float32 and give ``[n, proj]`` unit-norm embeddings -- the in-box stand-in for
@@ -716,3 +741,37 @@ def debug_fold_ln(w: np.ndarray, gamma=None, beta=None, bias=None):
     cvec = np.empty(N, np.float32) if gamma is not None else None
     _check(load_library().b200rt_debug_fold_ln(_ptr(w), p(g), p(b), p(bs), N, K, _ptr(w_out), p(cvec)))
     return w_out, cvec
+
+
+def debug_gemm_splade(a16: np.ndarray, w16: np.ndarray, c, stats, lens, S: int, N: int, eps: float, sms: int = 0, iters: int = 1):
+    """The SPLADE decoder GEMM (b200rt_debug_gemm_splade): a16 [B S, K], w16 [vocab, K] float16, c [N], stats [B S, K / 128, 2],
+    lens [B]; returns (uint32 maxima [B, N] -- the fp32 bits of max(0, max over item i's valid rows) --, ms per launch)."""
+    a16 = np.ascontiguousarray(a16, dtype=np.float16)
+    w16 = np.ascontiguousarray(w16, dtype=np.float16)
+    lens = np.ascontiguousarray(lens, dtype=np.int32)
+    c, stats = _f32(c), _f32(stats)
+    B, K, vocab = len(lens), a16.shape[1], w16.shape[0]
+    out = np.empty((B, N), np.uint32)
+    ms = ctypes.c_float(0)
+    _check(load_library().b200rt_debug_gemm_splade(_ptr(a16), _ptr(w16), _ptr(c), _ptr(stats), _ptr(lens), B, S, N, K, vocab,
+                                                   eps, sms, iters, ctypes.byref(ms), _ptr(out)))
+    return out, ms.value
+
+
+def debug_mlm_ln_stats(u16: np.ndarray, n_max: int = 0):
+    """(stats [rows, W / 128, 2] of the fp16 rows u16 [rows, W], the n_max-word max buffer as the launch leaves it)."""
+    u16 = np.ascontiguousarray(u16, dtype=np.float16)
+    rows, W = u16.shape
+    st = np.empty((rows, W // 128, 2), np.float32)
+    vmax = np.empty(max(n_max, 1), np.uint32)
+    _check(load_library().b200rt_debug_mlm_ln_stats(_ptr(u16), rows, W, n_max, _ptr(vmax), _ptr(st)))
+    return st, vmax[:n_max]
+
+
+def debug_splade_finalize(vmax: np.ndarray, vocab: int) -> np.ndarray:
+    """log1p of the fp32 bits of uint32 vmax [n, vpad], first ``vocab`` columns: float32 [n, vocab]."""
+    vmax = np.ascontiguousarray(vmax, dtype=np.uint32)
+    n, vpad = vmax.shape
+    out = np.empty((n, vocab), np.float32)
+    _check(load_library().b200rt_debug_splade_finalize(_ptr(vmax), n, vpad, vocab, _ptr(out)))
+    return out

@@ -321,6 +321,91 @@ def load_hf_classifier(sd: dict, cfg: dict) -> tuple[dict, np.ndarray]:
     return g, blob
 
 
+# ----------------------------------------------------------------------------------------------- SPLADE sparse encoders
+# HF BertForMaskedLM checkpoints (naver/splade-v3, naver/splade-cocondenser-ensembledistil, prithivida/Splade_PP_en_v1) that TEI
+# serves with --pooling splade through /embed_sparse.  Blob order: blob_layout(g), then mlm.t.w [H,H] | mlm.t.b [H] | mlm.ln.g [H]
+# | mlm.ln.b [H] | mlm.dec.w [V,H] | mlm.dec.b [V rounded up to 128] -- the decoder bias padded with zeros, as cls.b is.
+
+MASKED_LM_ARCHITECTURE = "BertForMaskedLM"
+_MLM = "cls.predictions."
+
+
+def splade_blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
+    h, v = g["hidden"], g["vocab"]
+    return blob_layout(g) + [("mlm.t.w", (h, h)), ("mlm.t.b", (h,)), ("mlm.ln.g", (h,)), ("mlm.ln.b", (h,)), ("mlm.dec.w", (v, h)),
+                             ("mlm.dec.b", ((v + 127) // 128 * 128,))]
+
+
+def random_splade_blob(g: dict = BGE_BASE_GEOMETRY, seed: int = 0) -> np.ndarray:
+    """Seeded weights of a SPLADE geometry: BERT's tensors drawn exactly as :func:`random_blob` draws them (the blob's prefix is
+    bit-identical), then the masked-LM head the same way (sigma 0.02 matrices, zero biases, unit LayerNorm; the decoder is not
+    tied to the word embeddings)."""
+    return _random_blob(splade_blob_layout(g), seed)
+
+
+def has_masked_lm_head(sd: dict) -> bool:
+    return _MLM + "transform.dense.weight" in sd
+
+
+def load_hf_masked_lm_state_dict(sd: dict, g: dict | None = None) -> tuple[dict, np.ndarray]:
+    """HF ``BertForMaskedLM`` state dict (``bert.*`` + ``cls.predictions.*``) -> (geometry, fp32 blob of
+    :func:`splade_blob_layout`).  The decoder is ``cls.predictions.decoder.weight``, or the word embeddings when a tied checkpoint
+    (safetensors drops the tied copy) leaves it out; its bias is ``cls.predictions.bias`` or ``cls.predictions.decoder.bias``.
+    A checkpoint without ``cls.predictions.transform`` is refused: SPLADE's logits come from that head."""
+    if not has_masked_lm_head(sd):
+        raise ValueError("no cls.predictions.transform.dense.weight: a BertForMaskedLM checkpoint (the masked-LM head SPLADE "
+                         "pools) is needed")
+    g, blob = load_hf_state_dict(sd, g)
+    enc = _strip_prefix(sd)
+    dec = sd.get(_MLM + "decoder.weight")
+    if dec is None:
+        dec = enc["embeddings.word_embeddings.weight"]
+    bias = sd.get(_MLM + "bias")
+    if bias is None:
+        bias = sd.get(_MLM + "decoder.bias")
+    if bias is None:
+        raise KeyError("no cls.predictions.bias / cls.predictions.decoder.bias")
+    head_layout = splade_blob_layout(g)[len(blob_layout(g)):]
+    db = np.zeros(head_layout[-1][1], np.float32)
+    db[: g["vocab"]] = _arr(bias)
+    t = _MLM + "transform."
+    head = _pack(head_layout, {"mlm.t.w": sd[t + "dense.weight"], "mlm.t.b": sd[t + "dense.bias"], "mlm.ln.g": sd[t + "LayerNorm.weight"],
+                               "mlm.ln.b": sd[t + "LayerNorm.bias"], "mlm.dec.w": dec, "mlm.dec.b": db})
+    return g, np.concatenate([blob, head])
+
+
+def _read_state_dict(path: str) -> dict:
+    st = os.path.join(path, "model.safetensors")
+    pt = os.path.join(path, "pytorch_model.bin")
+    if os.path.exists(st):
+        return read_safetensors(st)
+    if os.path.exists(pt):
+        import torch
+
+        return torch.load(pt, map_location="cpu", weights_only=True)
+    raise FileNotFoundError(f"no model.safetensors / pytorch_model.bin under {path}")
+
+
+def is_masked_lm_dir(path: str) -> bool:
+    """Whether a snapshot directory holds a masked-LM checkpoint SPLADE can pool: ``config.json`` names ``BertForMaskedLM``, or
+    its weights carry ``cls.predictions.transform``."""
+    if MASKED_LM_ARCHITECTURE in hf_architectures(path):
+        return True
+    try:
+        return has_masked_lm_head(_read_state_dict(path))
+    except FileNotFoundError:
+        return False
+
+
+def load_hf_masked_lm_dir(path: str) -> tuple[dict, np.ndarray]:
+    """A local ``BertForMaskedLM`` snapshot directory -> (geometry, :func:`splade_blob_layout` blob); ``eps`` and the head count
+    from its ``config.json``."""
+    cfg_path = os.path.join(path, "config.json")
+    cfg = json.load(open(cfg_path)) if os.path.exists(cfg_path) else {}
+    sd = _read_state_dict(path)
+    return load_hf_masked_lm_state_dict(sd, geometry_from_state_dict(sd, cfg.get("layer_norm_eps", 1e-12), cfg.get("num_attention_heads")))
+
+
 def resolve_hub_snapshot(cache_dir: str, model_id: str) -> str | None:
     """``<cache>/models--ORG--NAME/snapshots/<rev>/`` as ``huggingface_hub.snapshot_download`` lays it out (the reference
     mounts that cache as a Volume: text_embeddings_inference.py:20-24, 29-34)."""

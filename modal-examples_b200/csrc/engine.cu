@@ -169,6 +169,11 @@ struct DevWeights {
     // post_g / post_b = final_layer_norm, proj_w = text_projection [proj, hidden]; layers as for ViT (pre-LN).
     // BERT classifier (kind "bert_classifier"): BertPooler dense [H, H] + bias, classifier [L, H] + bias (padded to 128).
     float *pool_w = nullptr, *pool_b = nullptr, *cls_w = nullptr, *cls_b = nullptr;
+    // SPLADE (kind "bert_splade"): the MLM head's transform dense (fp16, the last layer's LN2 folded in; mlm_t_c = W beta + b) and
+    // decoder (fp16 [vocab, H], its transform LayerNorm folded in, read past vocab as zero rows by TMA; mlm_dec_c [vpad])
+    __half *mlm_t_w = nullptr, *mlm_dec_w = nullptr;
+    CUtensorMap m_mlm_t, m_mlm_dec;
+    float *mlm_t_c = nullptr, *mlm_dec_c = nullptr;
 };
 
 enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2 };
@@ -177,6 +182,7 @@ struct Model {
     ModelKind kind = KIND_BERT;
     bool pool_mean = false;  // text: mean of the valid tokens' final hidden states (B200RT_LOAD_POOL_MEAN) instead of the CLS row
     int num_labels = 0;      // > 0: a BERT classifier (kind "bert_classifier"): the head's L logits per item instead of a pool
+    int splade_vpad = 0;     // > 0: a SPLADE encoder (kind "bert_splade"): vocab-wide sparse vectors, the vocabulary tiled to this
     b200rt_bert_config cfg{};
     b200rt_vit_config vcfg{};
     b200rt_clip_text_config tcfg{};
@@ -391,6 +397,8 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
     const int B = in.B, S = in.S, M = B * S;
     if (M > m.cap_rows || (vit && B > VIT_WAVE_ITEMS))
         return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the model's wave capacity (%d rows)", B, S, m.cap_rows);
+    if (m.splade_vpad > 0 && S % 64 != 0)
+        return fail(B200RT_E_INVALID, "a bert_splade forward runs at padded lengths that are multiples of 64 (got %d)", S);
     const int H = m.hidden, I = m.inter, P = H / 128;
     const Dev::ActMaps& am = d.act[text_geometry(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
@@ -446,6 +454,25 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             if (step("gemm_ffn2")) return 0;
             prev_g = lw.ln2_g;
             prev_b = lw.ln2_b;
+        }
+        if (m.splade_vpad > 0) {
+            // SPLADE (BertForMaskedLM + max pooling): u = gelu(LN2(y) W_t^T + b_t) into the idle ctx buffer; the partials of u's
+            // LayerNorm into the idle pstats[1] and the wave's max buffer (uint32 [B, vpad] in the idle ffn buffer) zeroed; the
+            // decoder GEMM max-reduces relu(LN_t(u) W_dec^T + b) over each item's valid tokens into it, and never stores the
+            // [M, vocab] logits; log1p once per (item, word) into out
+            GemmEpi e_t{w.mlm_t_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
+            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, w.m_mlm_t, d.ctx, nullptr, e_t, M, H, H, d.sm_gemm, stream));
+            if (step("gemm_mlm_transform")) return 0;
+            uint32_t* vmax = reinterpret_cast<uint32_t*>(d.ffn);
+            CUDA_TRY(launch_mlm_ln_stats(d.ctx, d.pstats[1], vmax, M, static_cast<size_t>(B) * m.splade_vpad, H, stream));
+            if (step("mlm_ln_stats")) return 0;
+            GemmEpi e_dec{w.mlm_dec_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
+            CUDA_TRY(launch_gemm_splade(am.ctx, w.m_mlm_dec, e_dec, SpladeEpi{in.lens, S, vmax, m.vocab}, M, m.splade_vpad, H, d.sm_gemm,
+                                        stream));
+            if (step("gemm_splade")) return 0;
+            CUDA_TRY(launch_splade_finalize(vmax, out, B, m.splade_vpad, m.vocab, stream));
+            step("splade_finalize");
+            return 0;
         }
         if (vit) CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
         else if (clip_text)
@@ -1143,8 +1170,8 @@ struct Layout {
     int copy(size_t n, float* DevWeights::*dst) { return add({LayoutEntry::COPY, n, 1, -1, {dst}}); }
     int copy(int l, size_t n, float* LayerW::*dst) { return add({LayoutEntry::COPY, n, 1, l, {nullptr, dst}}); }
     void zero(size_t n, float* DevWeights::*dst = nullptr) { add({LayoutEntry::ZERO, n, 1, -1, {dst}}); }
-    void half(size_t n, size_t k, __half* DevWeights::*dst, CUtensorMap DevWeights::*map) {
-        add({LayoutEntry::HALF, n, k, -1, {}, {dst}, {map}});
+    int half(size_t n, size_t k, __half* DevWeights::*dst, CUtensorMap DevWeights::*map) {
+        return add({LayoutEntry::HALF, n, k, -1, {}, {dst}, {map}});
     }
     int half(int l, size_t n, size_t k, __half* LayerW::*dst, CUtensorMap LayerW::*map) {
         return add({LayoutEntry::HALF, n, k, l, {}, {nullptr, dst}, {nullptr, map}});
@@ -1152,6 +1179,12 @@ struct Layout {
     // fold the LayerNorm (entries gamma, beta) into HALF entry w; c = W beta + (entry bias) lands in w's layer's member `c`
     void fold(int w, int gamma, int beta, int bias, float* LayerW::*c) {
         const int cv = add({LayoutEntry::DERIVED, e[w].n, 1, e[w].layer, {nullptr, c}});
+        LayoutEntry& x = e[w];
+        x.gamma = gamma, x.beta = beta, x.bias = bias, x.cvec = cv;
+    }
+    // a DevWeights-level HALF entry w: c has c_n >= e[w].n floats, the ones past e[w].n zero
+    void fold(int w, int gamma, int beta, int bias, float* DevWeights::*c, size_t c_n) {
+        const int cv = add({LayoutEntry::DERIVED, c_n, 1, -1, {c}});
         LayoutEntry& x = e[w];
         x.gamma = gamma, x.beta = beta, x.bias = bias, x.cvec = cv;
     }
@@ -1222,6 +1255,8 @@ int load_weights(Runtime& rt, Model& m, Layout& L, const float* blob, size_t nby
     if (int rc = upload_blob(rt, m, blob, nbytes, &d_blob)) return rc;
     const DevWeights& rw = m.per_dev[0];
     auto blob_at = [&](int i) -> const float* { return i < 0 ? nullptr : d_blob + L.e[i].src; };
+    // a DERIVED entry may be longer than the fold that writes it (the SPLADE decoder's c, padded to its tiles): zeros past it
+    CUDA_TRY(cudaMemsetAsync(rw.f32_arena, 0, m.f32_elems * 4, root.compute));
     for (const LayoutEntry& e : L.e) {
         if (e.op == LayoutEntry::COPY)
             CUDA_TRY(cudaMemcpyAsync(rw.f32_arena + e.off, d_blob + e.src, e.n * 4, cudaMemcpyDeviceToDevice, root.compute));
@@ -1278,10 +1313,17 @@ int alloc_seg_slots(Runtime& rt) {
 
 constexpr int MAX_LABELS = 64;   // the classifier head's logits per item (launch_cls_head)
 constexpr int CLS_B_FLOATS = 128;  // the classifier bias is padded to 128 floats in the blob (tensor sizes keep the arena aligned)
+// A SPLADE result is vocab floats per item and an item has at least 64 rows, so vocab <= 64 HIDDEN keeps every wave's results
+// inside the gather and pinned staging buffers (HIDDEN floats per row of the wave), and its uint32 [B, vpad] maxima inside the
+// ffn buffer (3072 fp16 per row), with no new allocation.
+constexpr int SPLADE_MAX_VOCAB = 64 * HIDDEN;
+static_assert(static_cast<size_t>((SPLADE_MAX_VOCAB + 255) / 256 * 256) * 4 <= static_cast<size_t>(64) * 3072 * 2, "SPLADE maxima in ffn");
 
 // num_labels > 0: kind "bert_classifier" -- the BERT layout followed by the pooler and the classifier, and the head as the last
-// launch instead of a pool.
-int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out, int num_labels = 0) {
+// launch instead of a pool.  splade: kind "bert_splade" -- the BERT layout followed by BertForMaskedLM's head, and the four
+// SPLADE launches instead of a pool.
+int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out, int num_labels = 0,
+               bool splade = false) {
     Runtime& rt = *g_rt;
     bool known = false;
     for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= !tg.causal && c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
@@ -1290,6 +1332,9 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
                     "kernels cover three geometries, bge-base (hidden=768 heads=12 inter=3072), bge-small (hidden=384 heads=12 "
                     "inter=1536) and bge-large (hidden=1024 heads=16 inter=4096), with max_pos<=512 (got hidden %d heads %d inter %d "
                     "max_pos %d)", c.hidden, c.heads, c.inter, c.max_pos);
+    if (splade && c.vocab > SPLADE_MAX_VOCAB)
+        return fail(B200RT_E_UNSUPPORTED, "a SPLADE vocabulary of %d words exceeds %d (one vocab-wide result per 64 tokens must fit the "
+                    "wave's result buffers)", c.vocab, SPLADE_MAX_VOCAB);
     if (num_labels > 0 && c.type_vocab != 2)
         return fail(B200RT_E_UNSUPPORTED, "a classifier takes sentence pairs through two token types: type_vocab must be 2, got %d",
                     c.type_vocab);
@@ -1308,6 +1353,10 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
     m->out_dim = c.hidden;
     m->num_labels = num_labels;
     if (num_labels > 0) m->out_dim = num_labels;
+    if (splade) {
+        m->splade_vpad = (c.vocab + 255) / 256 * 256;
+        m->out_dim = c.vocab;
+    }
 
     // b200rt.weights.blob_layout.  QKV of layer l folds the LayerNorm in front of it, the previous layer's ln2 (the embedding
     // LN for l = 0); FFN1 folds the layer's own ln1.
@@ -1337,6 +1386,14 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
         L.copy(static_cast<size_t>(num_labels) * H, &DevWeights::cls_w);
         L.copy(CLS_B_FLOATS, &DevWeights::cls_b);
         if (int rc = alloc_seg_slots(rt)) return rc;
+    }
+    if (splade) {  // b200rt.weights.splade_blob_layout: mlm.t.w [H,H] | mlm.t.b [H] | mlm.ln.g [H] | mlm.ln.b [H] | mlm.dec.w [V,H] | mlm.dec.b
+        // [V rounded up to 128]; the transform folds the last layer's LN2, the decoder the transform's LayerNorm
+        const int tw = L.half(H, H, &DevWeights::mlm_t_w, &DevWeights::m_mlm_t);
+        L.fold(tw, ln_g, ln_b, L.copy(H, nullptr), &DevWeights::mlm_t_c, H);
+        const int tg = L.copy(H, nullptr), tb = L.copy(H, nullptr);
+        const int dw = L.half(c.vocab, H, &DevWeights::mlm_dec_w, &DevWeights::m_mlm_dec);
+        L.fold(dw, tg, tb, L.copy((c.vocab + 127) / 128 * 128, nullptr), &DevWeights::mlm_dec_c, m->splade_vpad);
     }
     if (int rc = load_weights(rt, *m, L, blob, nbytes)) return rc;
     return register_model(rt, std::move(m), model_out);
@@ -1595,8 +1652,8 @@ int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights,
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0 && strcmp(kind, "clip_text") != 0 &&
-                  strcmp(kind, "bert_classifier") != 0))
-        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"bert_classifier\", \"vit\" or \"clip_text\")",
+                  strcmp(kind, "bert_classifier") != 0 && strcmp(kind, "bert_splade") != 0))
+        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"bert_classifier\", \"bert_splade\", \"vit\" or \"clip_text\")",
                     kind ? kind : "(null)");
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
     if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
@@ -1616,6 +1673,10 @@ int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights,
         if (cc.num_labels < 1 || cc.num_labels > MAX_LABELS)
             return fail(B200RT_E_UNSUPPORTED, "num_labels %d outside [1, %d]", cc.num_labels, MAX_LABELS);
         return model_load(cc.bert, static_cast<const float*>(weights), nbytes, false, model_out, cc.num_labels);
+    }
+    if (strcmp(kind, "bert_splade") == 0) {
+        if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"bert_splade\"", flags);
+        return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, false, model_out, 0, true);
     }
     return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean, model_out);
 }
@@ -2203,6 +2264,98 @@ int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* g
     return 0;
 }
 
+int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const int32_t* lens, int B, int S,
+                             int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!a || !w || !c || !stats || !lens || !vmax_out || B < 1 || S < 64 || S % 64 || N % 256 || vocab < 1 || vocab > N)
+        return fail(B200RT_E_INVALID, "bad gemm_splade arguments (S a multiple of 64, N of 256, 1 <= vocab <= N)");
+    if (K != 768 && K != 384 && K != 1024) return fail(B200RT_E_INVALID, "K (the LayerNorm'd width) must be 768, 384 or 1024, got %d", K);
+    Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t M = static_cast<size_t>(B) * S, Mp = (M + 255) / 256 * 256, P = K / 128, nmax = static_cast<size_t>(B) * N;
+    DebugBuffers b(d.compute);
+    __half *da, *dw;
+    float *dc;
+    float2* dst;
+    int32_t* dl_;
+    uint32_t* dmax;
+    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));
+    CUDA_TRY(cudaMemcpyAsync(da, a, M * K * 2, cudaMemcpyHostToDevice, d.compute));
+    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(vocab) * K * 2));  // [vocab, K]: the map reads rows past vocab as zeros, as a model's
+    CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
+    CUDA_TRY(b.upload(&dst, stats, M * P * sizeof(float2)));
+    CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));
+    CUDA_TRY(b.upload(&dmax, nullptr, nmax * 4));
+    CUtensorMap ta, tb;
+    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
+    if (int rc = make_map_2d(&tb, dw, vocab, K, 128)) return rc;
+    const GemmEpi e{dc, dst, static_cast<int>(P), nullptr, nullptr, nullptr, eps};
+    const SpladeEpi sp{dl_, S, dmax, vocab};
+    const int grid_sms = sms ? sms : d.sm_count;
+    cudaEvent_t e0, e1;
+    CUDA_TRY(b.event(&e0));
+    CUDA_TRY(b.event(&e1));
+    if (iters < 1) iters = 1;
+    CUDA_TRY(cudaEventRecord(e0, d.compute));
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute));
+    CUDA_TRY(cudaEventRecord(e1, d.compute));
+    CUDA_TRY(cudaMemsetAsync(dmax, 0, nmax * 4, d.compute));  // the returned maxima come from one launch on a zeroed buffer
+    CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute));
+    CUDA_TRY(cudaStreamSynchronize(d.compute));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    if (ms_out) *ms_out = ms / iters;
+    CUDA_TRY(b.download(vmax_out, dmax, nmax * 4));
+    return 0;
+}
+
+int b200rt_debug_mlm_ln_stats(const uint16_t* u, int n_rows, int hidden, size_t n_max, uint32_t* vmax_out, float* stats_out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!u || !stats_out || n_rows < 1 || (n_max > 0 && !vmax_out)) return fail(B200RT_E_INVALID, "bad mlm_ln_stats arguments");
+    if (hidden != 768 && hidden != 384 && hidden != 1024) return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024, got %d", hidden);
+    const size_t rows = static_cast<size_t>(n_rows), H = hidden, P = H / 128;
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    DebugBuffers b(d.compute);
+    __half* du;
+    float2* dst;
+    uint32_t* dmax = nullptr;
+    CUDA_TRY(b.upload(&du, u, rows * H * 2));
+    CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
+    if (n_max > 0) {
+        CUDA_TRY(b.upload(&dmax, nullptr, n_max * 4));
+        CUDA_TRY(cudaMemsetAsync(dmax, 0xFF, n_max * 4, d.compute));
+    }
+    CUDA_TRY(launch_mlm_ln_stats(du, dst, dmax, n_rows, n_max, hidden, d.compute));
+    CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
+    if (n_max > 0) CUDA_TRY(b.download(vmax_out, dmax, n_max * 4));
+    return 0;
+}
+
+int b200rt_debug_splade_finalize(const uint32_t* vmax, int n_items, int vpad, int vocab, float* out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!vmax || !out || n_items < 1 || vocab < 1 || vpad < vocab) return fail(B200RT_E_INVALID, "bad splade_finalize arguments");
+    Dev& d = *rt->devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t n_out = static_cast<size_t>(n_items) * vocab;
+    DebugBuffers b(d.compute);
+    uint32_t* dmax;
+    float* dout;
+    CUDA_TRY(b.upload(&dmax, vmax, static_cast<size_t>(n_items) * vpad * 4));
+    CUDA_TRY(b.upload(&dout, nullptr, n_out * 4));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, n_out * 4, d.compute));
+    CUDA_TRY(launch_splade_finalize(dmax, dout, n_items, vpad, vocab, d.compute));
+    CUDA_TRY(b.download(out, dout, n_out * 4));
+    return 0;
+}
+
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out) {
     Runtime* rt = live_rt();
@@ -2384,7 +2537,7 @@ int b200rt_debug_forward_trace_segs(int model, const int32_t* ids, const int32_t
     if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (int rc = check_ids(*m, ids, lens, n_items, max_len, max_wave_len(*m))) return rc;
     if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
-    const int total = 5 * m->layers + 2;
+    const int total = 5 * m->layers + (m->splade_vpad > 0 ? 5 : 2);
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
     const size_t M = static_cast<size_t>(n_items) * max_len;

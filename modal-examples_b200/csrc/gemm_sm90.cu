@@ -25,7 +25,10 @@
 // Epilogues (see kernels.h for the residual-stream format):
 //   EPI_BIAS(_GELU / _QGELU)_F16 : folded LayerNorm  rstd * acc + c  (c = W beta + b), optional GELU, fp16 out;
 //   EPI_BIAS_RES_SPLIT           : y' = acc + bias + LN(y) with the LayerNorm re-applied from the row's statistics, y' split
-//                                  into fp16 hi + lo in place, and the (sum, M2) partial of each new 128-column row slice.
+//                                  into fp16 hi + lo in place, and the (sum, M2) partial of each new 128-column row slice;
+//   EPI_SPLADE_MAX               : v = max(rstd * acc + c, 0) on the item's valid rows, max-reduced over the consumer's 64 rows
+//                                  (one item: S % 64 == 0) by shuffles and a 4 KB shared-memory pass, then one
+//                                  red.global.max.u32 per non-zero column < vocab into the item's row of the max buffer.
 //
 // The accumulator fragment of thread (warp w of the consumer warpgroup, lane l) holds rows 16w + l/4 and 16w + l/4 + 8,
 // columns 8j + 2(l%4) + {0, 1} for j = 0..31: acc[4j + {0, 1}] on the first row, acc[4j + {2, 3}] on the second.
@@ -56,7 +59,13 @@ struct Tiles {
     static constexpr int OFF_BAR = STAGES * STAGE_BYTES;
     static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
     static_assert(SMEM_BYTES <= 232448, "shared memory");
+    // EPI_SPLADE_MAX: behind the barriers, each consumer warpgroup's [4 warps][BN] column maxima
+    static constexpr int OFF_RED = OFF_BAR + 256;
+    static constexpr int SPLADE_SMEM_BYTES = SMEM_BYTES + 2 * 4 * BN * 4;
+    static_assert(SPLADE_SMEM_BYTES <= 232448, "shared memory");
 };
+template <int EPI, int BN>
+constexpr int smem_bytes() { return EPI == EPI_SPLADE_MAX ? Tiles<BN>::SPLADE_SMEM_BYTES : Tiles<BN>::SMEM_BYTES; }
 
 // erf-GELU x * Phi(x), erf by Abramowitz-Stegun 7.1.26 (abs err <= 1.5e-7): 2 MUFU (rcp, ex2) per value
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -138,11 +147,12 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float e
     }
 }
 
-// BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128)
+// BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128).  sp is read by
+// EPI_SPLADE_MAX only; as the last parameter it leaves every other instantiation's parameter offsets as they were.
 template <int EPI, int BN, int PARTS>
 __global__ void __cluster_dims__(CM, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
-            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K) {
+            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K, const SpladeEpi sp) {
     static_assert(BN == 256 || BN == 128, "tile width");
     constexpr int STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
     constexpr int NACC = BN / 2;     // fp32 accumulators per consumer thread
@@ -249,7 +259,45 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             for (int h = 0; h < 2; ++h)
                 if (r0 + 8 * h < M) row_stats<PARTS>(ep.stats_in + static_cast<size_t>(r0 + 8 * h) * PARTS, ep.eps, mean[h], rstd[h]);
         }
-        if constexpr (EPI != EPI_BIAS_RES_SPLIT) {
+        if constexpr (EPI == EPI_SPLADE_MAX) {
+            // the consumer's 64 rows hrow0 .. hrow0 + 63 lie in item hrow0 / S (S % 64 == 0, M = B S); `valid` of them, from
+            // hrow0 on, are inside the item's length -- the same for every thread of the warpgroup
+            const int hrow0 = m0 + cw * 64;
+            const int item = hrow0 / sp.S;
+            const int valid = hrow0 < M ? min(max(__ldg(sp.lens + item), 0), sp.S) - (hrow0 - item * sp.S) : 0;
+            if (valid > 0) {
+                float* red = reinterpret_cast<float*>(smem + Tiles<BN>::OFF_RED) + cw * (4 * BN);  // [warp][column]
+                const int lr = w4 * 16 + (lane >> 2);  // this thread's rows within the half: lr and lr + 8
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
+                    float v0 = 0.f, v1 = 0.f;  // relu: the max starts at 0
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        if (lr + 8 * h < valid) {
+                            v0 = fmaxf(v0, fmaf(rstd[h], acc[4 * j + 2 * h], bv.x));
+                            v1 = fmaxf(v1, fmaf(rstd[h], acc[4 * j + 2 * h + 1], bv.y));
+                        }
+                    // the 8 lanes of a warp that hold these two columns differ in lane bits 2..4
+#pragma unroll
+                    for (int o = 4; o < 32; o <<= 1) {
+                        v0 = fmaxf(v0, __shfl_xor_sync(0xffffffff, v0, o));
+                        v1 = fmaxf(v1, __shfl_xor_sync(0xffffffff, v1, o));
+                    }
+                    if (lane < 4) *reinterpret_cast<float2*>(red + w4 * BN + 8 * j + 2 * lane) = make_float2(v0, v1);
+                }
+                named_bar_sync(1 + cw, 128);
+                const int t = threadIdx.x - 128 * (cw + 1);
+                uint32_t* vrow = sp.vmax + static_cast<size_t>(item) * N;
+#pragma unroll
+                for (int cl = t; cl < BN; cl += 128) {
+                    const float v = fmaxf(fmaxf(red[cl], red[BN + cl]), fmaxf(red[2 * BN + cl], red[3 * BN + cl]));
+                    // values are >= 0, so the integer max of the fp32 bits is the float max, in any order
+                    if (v > 0.f && n0 + cl < sp.vocab) atomicMax(vrow + n0 + cl, __float_as_uint(v));
+                }
+                named_bar_sync(1 + cw, 128);  // the next tile rewrites red
+            }
+        } else if constexpr (EPI != EPI_BIAS_RES_SPLIT) {
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
@@ -338,13 +386,13 @@ static int& max_clusters() {
 
 template <int EPI, int BN, int PARTS>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                              int K, int sm_count, cudaStream_t stream, int* ctas) {
+                              int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{}) {
     const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
     int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
     if (clusters < 1) clusters = 1;
     if (ctas) *ctas = clusters * gemm::CM;
-    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::Tiles<BN>::SMEM_BYTES,
-                      stream, ta, tb, e, out, out_lo, M, N, K);
+    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::smem_bytes<EPI, BN>(),
+                      stream, ta, tb, e, out, out_lo, M, N, K, sp);
 }
 
 // the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT / CLIP text
@@ -377,12 +425,12 @@ static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __ha
 template <int EPI, int BN, int PARTS>
 static cudaError_t setup() {
     auto kernel = gemm::gemm_kernel<EPI, BN, PARTS>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::Tiles<BN>::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::smem_bytes<EPI, BN>());
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};  // the cluster shape comes from the kernel's __cluster_dims__
     cfg.gridDim = dim3(gemm::CM);
     cfg.blockDim = dim3(gemm::NUM_THREADS);
-    cfg.dynamicSmemBytes = gemm::Tiles<BN>::SMEM_BYTES;
+    cfg.dynamicSmemBytes = gemm::smem_bytes<EPI, BN>();
     int n = 0;
     if ((e = cudaOccupancyMaxActiveClusters(&n, kernel, &cfg)) != cudaSuccess) return e;
     if (n < 1) return cudaErrorInvalidConfiguration;
@@ -408,7 +456,10 @@ cudaError_t gemm_init_device() {
     if ((e = setup_epi<EPI_BIAS_F16>()) != cudaSuccess) return e;
     if ((e = setup_epi<EPI_BIAS_GELU_F16>()) != cudaSuccess) return e;
     if ((e = setup_epi<EPI_BIAS_QGELU_F16>()) != cudaSuccess) return e;
-    return setup_epi<EPI_BIAS_RES_SPLIT>();
+    if ((e = setup_epi<EPI_BIAS_RES_SPLIT>()) != cudaSuccess) return e;
+    if ((e = setup<EPI_SPLADE_MAX, 256, 6>()) != cudaSuccess) return e;
+    if ((e = setup<EPI_SPLADE_MAX, 256, 3>()) != cudaSuccess) return e;
+    return setup<EPI_SPLADE_MAX, 256, 8>();
 }
 
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
@@ -427,6 +478,20 @@ cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, _
             if (out_lo == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr))) return cudaErrorInvalidValue;
             if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
             return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+    }
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi& e, const SpladeEpi& sp, int M, int N, int K,
+                               int sm_count, cudaStream_t stream, int* ctas) {
+    if (N % 256 != 0 || K % gemm::BK != 0 || M <= 0 || sm_count < 1 || e.bias == nullptr || e.stats_in == nullptr || e.parts_in * 128 != K)
+        return cudaErrorInvalidValue;
+    if (sp.lens == nullptr || sp.vmax == nullptr || sp.S < 64 || sp.S % 64 != 0 || M % sp.S != 0 || sp.vocab < 1 || sp.vocab > N)
+        return cudaErrorInvalidValue;
+    switch (e.parts_in) {
+        case 6: return launch_one<EPI_SPLADE_MAX, 256, 6>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
+        case 3: return launch_one<EPI_SPLADE_MAX, 256, 3>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
+        case 8: return launch_one<EPI_SPLADE_MAX, 256, 8>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
     }
     return cudaErrorInvalidValue;
 }

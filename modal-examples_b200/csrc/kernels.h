@@ -12,6 +12,7 @@ enum GemmEpilogue : int {
     EPI_BIAS_GELU_F16 = 1,  // out fp16 = gelu_erf(LNfold(acc) + bias)           (FFN up-projection)
     EPI_BIAS_RES_SPLIT = 2, // y (fp16 hi + fp16 lo, in place) = acc + bias + LN(y)  (attention-out / FFN down) + row statistics
     EPI_BIAS_QGELU_F16 = 3, // out fp16 = quick_gelu(LNfold(acc) + bias), x * sigmoid(1.702 x)   (CLIP MLP up-projection)
+    EPI_SPLADE_MAX = 4,     // per item and column: max over the item's valid rows of relu(LNfold(acc) + bias)   (SPLADE decoder)
 };
 
 // Four text geometries: bge-base (hidden 768, 12 heads of 64, inter 3072), bge-small (hidden 384, 12 heads of 32, inter 1536),
@@ -62,6 +63,21 @@ struct GemmEpi {
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                         int K, int sm_count, cudaStream_t stream, int* ctas = nullptr);
 
+// SPLADE's vocabulary max (EPI_SPLADE_MAX): the decoder GEMM C = LNfold(A . W^T) + bias over rows of items padded to S tokens
+// (S % 64 == 0, M = B S), never stored.  Instead, for item i and column n < vocab,
+//   vmax[i * N + n] = max(vmax[i * N + n], bits(max over rows r of item i with r % S < lens[i] of max(C[r, n], 0)))
+// by red.global.max.u32 on the fp32 bits (exact and order-independent for values >= 0), one per 64-row consumer half and
+// column, none for a zero.  vmax must hold zeros (or earlier maxima) for the B items; columns >= vocab are never written.
+// e.stats_in is required (the LayerNorm of A, K wide: 768, 384 or 1024); N % 256 == 0.  lens[i] is clamped to [0, S].
+struct SpladeEpi {
+    const int32_t* lens;  // [B]
+    int S;
+    uint32_t* vmax;       // [B, N]
+    int vocab;
+};
+cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi& e, const SpladeEpi& sp, int M, int N, int K,
+                               int sm_count, cudaStream_t stream, int* ctas = nullptr);
+
 // gamma != NULL: w_out[n,k] = fp16(w[n,k] gamma[k] - mean_k(w[n,:] gamma)), cvec[n] = sum_k w[n,k] beta[k] + bias[n]
 // gamma == NULL: w_out = fp16(w) (cvec untouched)
 cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, __half* w_out, float* cvec,
@@ -88,6 +104,15 @@ cudaError_t launch_embed(const int32_t* ids, const float* word, const float* pos
 cudaError_t launch_cls_head(const __half* yhi, const __half* ylo, const float* gamma, const float* beta, const float* pool_w,
                             const float* pool_b, const float* cls_w, const float* cls_b, float* out, int n_items, int S, int L, float eps,
                             int width, cudaStream_t stream, int ctas = 0);
+
+// SPLADE head, between the transform GEMM and the decoder GEMM: the (sum, M2) partial of every 128-column slice of the fp16 rows
+// u [n_rows, width] (the values the decoder GEMM reads) into stats [n_rows][width / 128], and vmax [n_max] zeroed (the
+// decoder's max buffer of the wave's items).  width 768, 384 or 1024.
+cudaError_t launch_mlm_ln_stats(const __half* u, float2* stats, uint32_t* vmax, int n_rows, size_t n_max, int width, cudaStream_t stream);
+
+// out[i * vocab + v] = log1pf(fp32 bits vmax[i * vpad + v]) for v < vocab: SPLADE's log(1 + relu) applied once per (item, word)
+// after the max (both are monotone).  `out` may be peer memory.
+cudaError_t launch_splade_finalize(const uint32_t* vmax, float* out, int n_items, int vpad, int vocab, cudaStream_t stream);
 
 // final LayerNorm of the CLS row of every item + L2 normalise; row i is stored at out + i * width,
 // where `out` may be a peer-mapped pointer into the root GPU's gather buffer (the fused gather).

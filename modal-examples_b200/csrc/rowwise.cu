@@ -496,6 +496,44 @@ fold_ln_kernel(const float* __restrict__ w, const float* __restrict__ gamma, con
     }
 }
 
+// SPLADE head, one warp per row of u (fp16, W wide): the (sum, M2 about its own mean) partial of each 128-column slice, from
+// the fp16 values the decoder GEMM reads, as embed_kernel computes them; and every thread zeroes its grid-stride share of
+// the decoder's max buffer vmax [n_max].
+template <int W>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
+mlm_ln_stats_kernel(const __half* __restrict__ u, float2* __restrict__ stats, uint32_t* __restrict__ vmax, int n_rows, size_t n_max) {
+    constexpr int V4 = Row<W>::V4;
+    const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x, nth = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t i = tid; i < n_max / 4; i += nth) reinterpret_cast<uint4*>(vmax)[i] = make_uint4(0, 0, 0, 0);
+    for (size_t i = n_max / 4 * 4 + tid; i < n_max; i += nth) vmax[i] = 0;
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
+    if (row >= n_rows) return;
+    const uint2* u2 = reinterpret_cast<const uint2*>(u + static_cast<size_t>(row) * W);
+    float ps = 0.f, pq = 0.f;  // lane i < V4 keeps partial i
+#pragma unroll
+    for (int i = 0; i < V4; ++i) {
+        const uint2 hv = u2[i * 32 + lane];
+        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&hv.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&hv.y));
+        const float s = warp_sum((a.x + a.y) + (b.x + b.y));
+        const float m = s * (1.0f / 128.0f);
+        const float dx = a.x - m, dy = a.y - m, dz = b.x - m, dw = b.y - m;
+        const float q = warp_sum((dx * dx + dy * dy) + (dz * dz + dw * dw));
+        if (lane == i) { ps = s; pq = q; }
+    }
+    if (lane < V4) stats[static_cast<size_t>(row) * V4 + lane] = make_float2(ps, pq);
+}
+
+// blockIdx.y = item: out[item * vocab + v] = log1p(max) for v < vocab; log1pf (not __logf(1 + x)): the small values decide
+// which words are non-zero.
+__global__ void __launch_bounds__(256)
+splade_finalize_kernel(const uint32_t* __restrict__ vmax, float* __restrict__ out, int vpad, int vocab) {
+    const int v = blockIdx.x * 256 + threadIdx.x;
+    if (v >= vocab) return;
+    const size_t item = blockIdx.y;
+    out[item * vocab + v] = log1pf(__uint_as_float(vmax[item * vpad + v]));
+}
+
 // blockIdx.y = shard.  Copies ids[item_begin*S .. (item_begin+item_count)*S) and the matching lens (and, SEGS, segment
 // starts) to the shard's input slot; dst pointers of remote shards are peer-mapped, so the stores cross NVLink directly.
 template <bool SEGS>
@@ -614,6 +652,23 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
     if (K % 64 != 0 || N < 1) return cudaErrorInvalidValue;
     const int grid = (N + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
     rw::fold_ln_kernel<<<grid, rw::WARPS_PER_BLOCK * 32, 0, stream>>>(w, gamma, beta, bias, w_out, cvec, N, K);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mlm_ln_stats(const __half* u, float2* stats, uint32_t* vmax, int n_rows, size_t n_max, int width, cudaStream_t stream) {
+    if (n_rows < 1 || (n_max > 0 && vmax == nullptr)) return cudaErrorInvalidValue;
+    const int grid = (n_rows + rw::WARPS_PER_BLOCK - 1) / rw::WARPS_PER_BLOCK;
+    const int block = rw::WARPS_PER_BLOCK * 32;
+    if (width == 768) rw::mlm_ln_stats_kernel<768><<<grid, block, 0, stream>>>(u, stats, vmax, n_rows, n_max);
+    else if (width == 384) rw::mlm_ln_stats_kernel<384><<<grid, block, 0, stream>>>(u, stats, vmax, n_rows, n_max);
+    else if (width == 1024) rw::mlm_ln_stats_kernel<1024><<<grid, block, 0, stream>>>(u, stats, vmax, n_rows, n_max);
+    else return cudaErrorInvalidValue;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_splade_finalize(const uint32_t* vmax, float* out, int n_items, int vpad, int vocab, cudaStream_t stream) {
+    if (n_items < 1 || n_items > 65535 || vocab < 1 || vocab > vpad) return cudaErrorInvalidValue;
+    rw::splade_finalize_kernel<<<dim3((vocab + 255) / 256, n_items), 256, 0, stream>>>(vmax, out, vpad, vocab);
     return cudaGetLastError();
 }
 

@@ -20,6 +20,9 @@ BGE_LARGE_ID = "BAAI/bge-large-en-v1.5"
 MINILM_L6_ID = "sentence-transformers/all-MiniLM-L6-v2"
 POOLING_BY_MODEL_ID = {MINILM_L6_ID: "mean"}  # models whose sentence-transformers config pools other than by [CLS]
 POOLINGS = ("cls", "mean")  # TEI also knows splade and last-token; this runtime does not
+# SPLADE encoders served offline on seeded weights (bge-base's geometry) when no masked-LM snapshot is at hand; a snapshot
+# whose config names BertForMaskedLM, or whose weights carry cls.predictions.transform, serves --pooling splade under any id
+SPLADE_MODEL_IDS = ("naver/splade-cocondenser-ensembledistil", "naver/splade-v3")
 MS_MARCO_L6_ID = "cross-encoder/ms-marco-MiniLM-L-6-v2"
 MS_MARCO_L12_ID = "cross-encoder/ms-marco-MiniLM-L-12-v2"
 
@@ -99,12 +102,27 @@ def parse_predict_inputs(inputs):
     raise TypeError("`inputs` must be a string, a [string, string] pair or a non-empty list of those")
 
 
+def splade_response(vecs) -> list:
+    """TEI's /embed_sparse body: per input, ``[{"index", "value"}]`` of its non-zero words in index order."""
+    import numpy as np
+
+    out = []
+    for v in vecs:
+        nz = np.flatnonzero(v > 0)
+        out.append([{"index": int(i), "value": float(v[i])} for i in nz])
+    return out
+
+
 def resolve_pooling(flag: str | None, snapshot_dir: str | None, model_id: str) -> str:
     """The pooling to serve, resolved as TEI resolves it: --pooling when given; else the Pooling module of the snapshot's
     sentence-transformers config (modules.json -> 1_Pooling/config.json); else the model-id table; else cls.  Raises
-    ValueError for a --pooling other than cls / mean and for a snapshot that declares a pooling other than those two."""
-    from b200rt.weights import pooling_from_dir
+    ValueError for a --pooling other than cls / mean and for a snapshot that declares a pooling other than those two.
+    --pooling splade is served for a masked-LM snapshot and for the SPLADE ids of SPLADE_MODEL_IDS (as TEI, which refuses it
+    on a model without an MLM head); anywhere else it is refused like any other pooling."""
+    from b200rt.weights import is_masked_lm_dir, pooling_from_dir
 
+    if flag == "splade" and (model_id in SPLADE_MODEL_IDS or (snapshot_dir and is_masked_lm_dir(snapshot_dir))):
+        return flag
     if flag is not None:
         if flag not in POOLINGS:
             raise ValueError(f"--pooling {flag!r} is not supported (supported: {', '.join(POOLINGS)})")
@@ -127,7 +145,8 @@ def parse_args(argv):
     ap.add_argument("--huggingface-hub-cache", default=None)
     ap.add_argument("--revision", default=None)
     ap.add_argument("--dtype", default="float16")
-    ap.add_argument("--pooling", default=None, help="cls or mean; default: the snapshot's sentence-transformers Pooling config, else cls")
+    ap.add_argument("--pooling", default=None, help="cls, mean or splade (a masked-LM model); default: the snapshot's sentence-transformers "
+                    "Pooling config, else cls")
     ap.add_argument("--auto-truncate", action="store_true")
     ap.add_argument("--tokenizer-vocab", default=os.environ.get("B200RT_VOCAB"))
     ap.add_argument("--weights", default=os.environ.get("B200RT_WEIGHTS"), help="flat fp32 blob (DESIGN.md §3), a .safetensors checkpoint or an HF snapshot directory; default: the hub cache, else seeded random init")
@@ -187,6 +206,20 @@ def load_weights(args):
     return g, random_blob(geometry=g), None
 
 
+def load_splade_weights(args):
+    """Weights of a SPLADE model: the masked-LM checkpoint the weights directory holds, else (an id of SPLADE_MODEL_IDS with no
+    snapshot) seeded random init of bge-base's geometry with a loud notice.  A snapshot without an MLM head is refused."""
+    from b200rt import weights as W
+
+    d = weights_dir(args)
+    if d:
+        if not W.is_masked_lm_dir(d):
+            raise ValueError(f"--pooling splade needs a masked-LM checkpoint (BertForMaskedLM); {d} has no cls.predictions head")
+        return W.load_hf_masked_lm_dir(d) + (f"masked-LM snapshot {d}",)
+    g = geometry_for_model_id(args.model_id)
+    return g, W.random_splade_blob(g, 0), None
+
+
 class Engine:
     def __init__(self, args):
         import numpy as np
@@ -207,7 +240,8 @@ class Engine:
 
             n_gpus = max(1, torch.cuda.device_count())
         b200rt.init(n_gpus)
-        geometry, blob, source = load_weights(args)
+        self.splade = self.pooling == "splade"
+        geometry, blob, source = load_splade_weights(args) if self.splade else load_weights(args)
         if source is None:
             print(f"[text-embeddings-router/b200] no weights for {args.model_id!r} offline: seeded random init", file=sys.stderr)
         else:
@@ -223,13 +257,17 @@ class Engine:
             print(f"[text-embeddings-router/b200] {kind}: BertForSequenceClassification, {geometry['num_labels']} label(s)"
                   + (" -- SEEDED weights, scores are not the real model's" if source is None else ""), file=sys.stderr)
             self.model = b200rt.ClassifierModel(geometry, blob)
+        elif self.splade:
+            print("[text-embeddings-router/b200] SPLADE: BertForMaskedLM, sparse vectors over the vocabulary through /embed_sparse"
+                  + (" -- SEEDED weights, vectors are not the real model's" if source is None else ""), file=sys.stderr)
+            self.model = b200rt.SparseEmbedModel(geometry, blob)
         else:
             self.model = b200rt.EmbedModel(geometry, blob, pooling=self.pooling)
         self.n_gpus = n_gpus
 
-    def embed(self, inputs):
+    def embed(self, inputs, truncate: bool = False):
         np = self.np
-        rows = [self.tok.encode(t, self.geometry["max_pos"], self.args.auto_truncate) for t in inputs]
+        rows = [self.tok.encode(t, self.geometry["max_pos"], truncate or self.args.auto_truncate) for t in inputs]
         lens = np.array([len(r) for r in rows], np.int32)
         ids = np.zeros((len(rows), int(lens.max())), np.int32)
         for i, r in enumerate(rows):
@@ -301,10 +339,19 @@ def make_handler(engine: Engine):
         def do_POST(self):
             if self.path in ("/rerank", "/predict"):
                 return self._classify()
+            if self.path == "/embed_sparse":
+                return self._embed(sparse=True)
             if self.path not in ("/embed", "/"):
                 return self._send(404, {"error": "not found", "error_type": "NotFound"})
+            return self._embed(sparse=False)
+
+        def _embed(self, sparse: bool):
             if engine.classifier:
                 return self._send(400, {"error": f"{engine.args.model_id} is a classifier: use /rerank or /predict", "error_type": "Backend"})
+            if engine.splade and not sparse:
+                return self._send(400, {"error": f"{engine.args.model_id} is a SPLADE model: use /embed_sparse", "error_type": "Backend"})
+            if sparse and not engine.splade:
+                return self._send(400, {"error": f"{engine.args.model_id} is not a SPLADE model: use /embed", "error_type": "Backend"})
             try:
                 req = json.loads(self.rfile.read(int(self.headers.get("Content-Length", "0"))))
                 inputs = req["inputs"]
@@ -312,18 +359,19 @@ def make_handler(engine: Engine):
                     inputs = [inputs]
                 if not isinstance(inputs, list) or not inputs or not all(isinstance(t, str) for t in inputs):
                     raise TypeError("`inputs` must be a string or a non-empty list of strings")
+                truncate = bool(req.get("truncate", False)) if sparse else False
             except Exception as e:  # noqa: BLE001
                 return self._send(422, {"error": f"Failed to deserialize the JSON body: {e}", "error_type": "Validation"})
             if len(inputs) > engine.args.max_client_batch_size:
                 return self._send(413, {"error": f"batch size {len(inputs)} > maximum allowed batch size {engine.args.max_client_batch_size}",
                                         "error_type": "Validation"})
             try:
-                vecs = engine.embed(inputs)
+                vecs = engine.embed(inputs, truncate)
             except ValueError as e:
                 return self._send(413, {"error": str(e), "error_type": "Validation"})
             except Exception as e:  # noqa: BLE001
                 return self._send(500, {"error": str(e), "error_type": "Backend"})
-            self._send(200, vecs.tolist())
+            self._send(200, splade_response(vecs) if sparse else vecs.tolist())
 
         def _classify(self):
             if not engine.classifier:
