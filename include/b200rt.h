@@ -46,6 +46,16 @@ typedef struct b200rt_bert_classifier_config {
     int32_t num_labels;
 } b200rt_bert_classifier_config;
 
+/* A nomic-bert encoder (HF NomicBertModel, e.g. nomic-ai/nomic-embed-text-v1 / -v1.5): bge-base's geometry and post-LN
+ * layers (bert.hidden 768, 12 heads of 64, inter 3072), with rotary position embeddings on Q and K (rotate_half pairs
+ * (d, d + 32) of each head, inv_freq_i = 1 / rope_theta^(i / 32)) instead of a position table, a SwiGLU MLP
+ * down(silu(gate(x)) * up(x)), and no biases.  Inputs up to bert.max_pos <= 8192 tokens; layers, vocab and type_vocab >= 1
+ * are free (every token takes type row 0).  Results are 768 floats per item.                                             */
+typedef struct b200rt_nomic_bert_config {
+    b200rt_bert_config bert;
+    float rope_theta;
+} b200rt_nomic_bert_config;
+
 /* Geometry of a CLIP-style ViT image tower (HF CLIPVisionConfig fields + projection_dim).  The kernels are specialised for
  * ViT-B/16: hidden 768, 12 heads of 64, inter 3072, (image/patch)^2 + 1 <= 512 tokens, 3*patch*patch a multiple of 64. */
 typedef struct b200rt_vit_config {
@@ -102,16 +112,22 @@ int b200rt_num_gpus(void);
  * out[i, v] = log(1 + max over the item's tokens of relu(MLM logit v)); blob order b200rt.weights.splade_blob_layout -- BERT's,
  * then mlm.t.w [H,H] | mlm.t.b [H] | mlm.ln.g [H] | mlm.ln.b [H] | mlm.dec.w [vocab,H] | mlm.dec.b padded to a multiple of 128
  * floats.  It takes b200rt_submit[_ex] and b200rt_embed_device (max_len a multiple of 64); segs are B200RT_E_INVALID.
+ * kind "nomic_bert" (cfg: b200rt_nomic_bert_config) is a long-context text encoder: blob order b200rt.weights.nomic_blob_layout
+ * -- word [V,H] | type [T,H] | emb.ln.g | emb.ln.b, then per layer qkv.w [3H,H] | ao.w [H,H] | ln1.g | ln1.b | gate.w [I,H] |
+ * up.w [I,H] | down.w [H,I] | ln2.g | ln2.b, no biases.  It takes b200rt_submit[_ex] with max_len <= max_pos (items travel in
+ * 64-token buckets up to max_pos rounded up to 64: a wave holds 8 items of 8192 tokens on an H100 SXM) and b200rt_embed_device
+ * (max_len a multiple of 64, up to max_pos rounded up to 64); segs are B200RT_E_INVALID.
  * A "clip_text" model takes token ids through b200rt_submit[_ex] (max_len <= max_pos,
  * ids < vocab; items travel in the 64- or 128-token bucket) and b200rt_embed_device (max_len <= 128, the longest wave the
  * scheduler forms for it: device-resident callers can run the bucket the scheduler would), and is refused by
  * b200rt_submit_pixels.                                                                                              */
 int b200rt_model_load(const char* kind, const void* cfg, const void* weights, size_t nbytes, int* model_out);
-/* b200rt_model_load with load flags (b200rt_model_load is this with flags = 0).  B200RT_LOAD_POOL_MEAN (kind "bert" only):
+/* b200rt_model_load with load flags (b200rt_model_load is this with flags = 0).  B200RT_LOAD_POOL_MEAN (kinds "bert" and
+ * "nomic_bert"):
  * pool each item as sentence-transformers' Pooling(mean) + Normalize does -- the mean over the item's lens[i] valid tokens
  * ([CLS] and [SEP] included) of the final hidden states, then L2 normalise -- instead of taking the [CLS] row; the pooling of
- * all-MiniLM-L6-v2, e5 and gte.  The forward before the pool, and its launch count, are the same either way.  With kind
- * "vit" or "clip_text", or with any other flag bit set, returns B200RT_E_INVALID.                                                       */
+ * all-MiniLM-L6-v2, e5, gte and nomic-embed-text.  The forward before the pool, and its launch count, are the same either way.
+ * With any other kind, or with any other flag bit set, returns B200RT_E_INVALID.                                                      */
 #define B200RT_LOAD_POOL_MEAN 1u
 int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out);
 

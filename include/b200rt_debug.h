@@ -89,6 +89,17 @@ int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* g
  *   splade_finalize: out[i, v] = log1p(fp32 bits vmax[i, v]) for v < vocab, vmax uint32 [n_items, vpad], out [n_items, vocab]. */
 int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const int32_t* lens, int B, int S,
                              int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out);
+/* nomic-bert kernels (kernels.h: launch_gemm_rope, launch_gemm_swiglu, launch_attention_stream), one launch each behind host
+ * buffers.  gemm_rope: a [M,768] fp16, w [N,768] fp16, c [N], stats [M][6] (NULL: plain acc + c), table float (cos, sin) pairs
+ * [n_pos][32] with n_pos >= S, S % 64 == 0, rot_cols a multiple of 256 <= N; out fp16 [M, N].  gemm_swiglu: w [N,768] with
+ * gate / up rows interleaved in groups of 8, out fp16 [M, N / 2].  attention_stream: qkv fp16 [B*S, 2304], 64 <= S <= 8192,
+ * S % 64 == 0, ctx fp16 [B*S, 768]; ms_out (may be NULL) the mean time of `iters` further launches.  sms: the most CTAs of
+ * the persistent launch (0 = every SM).                                                                                   */
+int b200rt_debug_gemm_rope(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const float* table, int n_pos, int M,
+                           int N, int S, int rot_cols, float eps, int sms, uint16_t* out);
+int b200rt_debug_gemm_swiglu(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, int M, int N, float eps, int sms,
+                             uint16_t* out);
+int b200rt_debug_attention_stream(const uint16_t* qkv, const int32_t* lens, int B, int S, uint16_t* ctx, int sms, int iters, float* ms_out);
 int b200rt_debug_mlm_ln_stats(const uint16_t* u, int n_rows, int hidden, size_t n_max, uint32_t* vmax_out, float* stats_out);
 int b200rt_debug_splade_finalize(const uint32_t* vmax, int n_items, int vpad, int vocab, float* out);
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
@@ -111,9 +122,10 @@ int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, 
  * clip_text_pool for kind "clip_text") or 5 layers + 4 (vit: im2col, gemm_patch, vit_embed, 5 per layer, vit_pool), or 5 layers + 5
  * for kind "bert_splade" (embed, 5 per layer, gemm_mlm_transform writing u [M, H] into ctx, mlm_ln_stats writing u's partials
  * into pstats1 and zeroing the uint32 [n_items, vpad] maxima at the start of ffn, gemm_splade raising them, splade_finalize
- * writing out [n_items, vocab]; vpad = vocab rounded up to 256).
+ * writing out [n_items, vocab]; vpad = vocab rounded up to 256).  Kind "nomic_bert" runs embed, then per layer gemm_qkv_rope,
+ * attention_stream, gemm_attn_out, gemm_ffn1_swiglu (silu(g) u [M, I] into ffn), gemm_ffn2, then the pool: 5 layers + 2.
  * max_len may be up to the longest wave the model runs (kind "clip_text": 128, its bucket for items of 65-77 tokens; the
- * lengths stay <= max_pos), as for b200rt_debug_profile_forward.  Every buffer comes back for rows = min(M + 256, R) rows, R = b200rt_debug_model_cap_rows(model) (512
+ * lengths stay <= max_pos; kind "nomic_bert": max_pos rounded up to 64, a multiple of 64), as for b200rt_debug_profile_forward.  Every buffer comes back for rows = min(M + 256, R) rows, R = b200rt_debug_model_cap_rows(model) (512
  * b200rt_wave_capacity_items(), or 3/4 of that rounded down to 128 for bge-large), M = n_items * max_len
  * (text) or n_items * tokens (vit), at the model's widths (H = hidden, I = inter, P = H / 128):
  *   yhi, ylo, ctx: fp16 bits [rows, H]; qkv: fp16 bits [rows, 3H]; ffn: fp16 bits [rows, I] (vit: the im2col matrix

@@ -33,7 +33,8 @@ DEBUG_SYMBOLS = ["b200rt_debug_gemm", "b200rt_debug_gemm_ex", "b200rt_debug_atte
                  "b200rt_debug_vit_pool", "b200rt_debug_clip_text_pool", "b200rt_debug_fold_ln",
                  "b200rt_debug_forward_trace", "b200rt_debug_vit_forward_trace", "b200rt_debug_model_cap_rows",
                  "b200rt_debug_embed_segs", "b200rt_debug_cls_head", "b200rt_debug_forward_trace_segs",
-                 "b200rt_debug_gemm_splade", "b200rt_debug_mlm_ln_stats", "b200rt_debug_splade_finalize"]
+                 "b200rt_debug_gemm_splade", "b200rt_debug_mlm_ln_stats", "b200rt_debug_splade_finalize",
+                 "b200rt_debug_gemm_rope", "b200rt_debug_gemm_swiglu", "b200rt_debug_attention_stream"]
 
 
 def SPLIT_SMS(k: int) -> int:
@@ -55,6 +56,10 @@ class BertConfig(ctypes.Structure):
 
 class BertClassifierConfig(ctypes.Structure):
     _fields_ = [("bert", BertConfig), ("num_labels", ctypes.c_int32)]
+
+
+class NomicBertConfig(ctypes.Structure):
+    _fields_ = [("bert", BertConfig), ("rope_theta", ctypes.c_float)]
 
 
 class VitConfig(ctypes.Structure):
@@ -143,6 +148,9 @@ def load_library():
         lib.b200rt_debug_gemm_splade.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, ci, f32p, vp]
         lib.b200rt_debug_mlm_ln_stats.argtypes = [vp, ci, ci, ctypes.c_size_t, vp, vp]
         lib.b200rt_debug_splade_finalize.argtypes = [vp, ci, ci, ci, vp]
+        lib.b200rt_debug_gemm_rope.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, vp]
+        lib.b200rt_debug_gemm_swiglu.argtypes = [vp] * 4 + [ci, ci, cf, ci, vp]
+        lib.b200rt_debug_attention_stream.argtypes = [vp, vp, ci, ci, vp, ci, ci, f32p]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                      f32p, i32p, ctypes.c_int]
         _lib = lib
@@ -473,6 +481,32 @@ class SparseEmbedModel(EmbedModel):
         self._lib = lib
 
 
+class NomicEmbedModel(EmbedModel):
+    """A loaded nomic-bert encoder (kind "nomic_bert", HF ``NomicBertModel``: nomic-ai/nomic-embed-text-v1 / -v1.5): rotary
+    positions, SwiGLU MLPs, inputs up to ``max_pos`` (at most 8192) tokens.  ``geometry`` is bge-base's plus ``rope_theta``
+    (b200rt.weights.NOMIC_EMBED_TEXT_GEOMETRY), the blob b200rt.weights.nomic_blob_layout's.  ``pooling``: "mean" (the
+    sentence-transformers pooling nomic-embed-text ships) or "cls"; either way L2-normalised 768-vectors.  ``submit``/``wait``/
+    ``embed``/``debug_trace`` are :class:`EmbedModel`'s; items travel in 64-token buckets up to max_pos, and ``embed_device``
+    takes ``max_len`` a multiple of 64."""
+
+    def __init__(self, geometry: dict, blob: np.ndarray, pooling: str = "mean"):
+        if pooling not in POOLINGS:
+            raise B200RTError(E_INVALID, f"pooling must be one of {POOLINGS}, got {pooling!r}")
+        lib = load_library()
+        blob = np.ascontiguousarray(blob, dtype=np.float32)
+        g = geometry
+        self.cfg = NomicBertConfig(BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"],
+                                              g["eps"]), g["rope_theta"])
+        self.hidden, self.inter, self.max_pos = g["hidden"], g["inter"], g["max_pos"]
+        self.out_dim = self.hidden
+        self.pooling = pooling
+        h = ctypes.c_int32(-1)
+        _check(lib.b200rt_model_load_ex(b"nomic_bert", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, LOAD_POOL_MEAN if pooling == "mean" else 0,
+                                        ctypes.byref(h)))
+        self.handle = h.value
+        self._lib = lib
+
+
 class ImageEmbedModel:
     """A loaded CLIP-style ViT image tower (kind "vit"): ``submit``/``wait`` take preprocessed pixels
     ``[n, 3, image, image]`` float32 and give ``[n, proj]`` unit-norm embeddings -- the in-box stand-in for
@@ -775,3 +809,42 @@ def debug_splade_finalize(vmax: np.ndarray, vocab: int) -> np.ndarray:
     out = np.empty((n, vocab), np.float32)
     _check(load_library().b200rt_debug_splade_finalize(_ptr(vmax), n, vpad, vocab, _ptr(out)))
     return out
+
+
+def debug_gemm_rope(a16: np.ndarray, w16: np.ndarray, c, stats, table: np.ndarray, S: int, rot_cols: int, eps: float, sms: int = 0):
+    """nomic-bert's QKV epilogue (b200rt_debug_gemm_rope): a16 [M, 768], w16 [N, 768] float16, c [N], stats [M, 6, 2] or None,
+    table float32 [n_pos, 32, 2] (cos, sin); returns out float16 [M, N]."""
+    a16 = np.ascontiguousarray(a16, dtype=np.float16)
+    w16 = np.ascontiguousarray(w16, dtype=np.float16)
+    M, N = a16.shape[0], w16.shape[0]
+    c, table = _f32(c), _f32(table)
+    st = _f32(stats) if stats is not None else None
+    out = np.empty((M, N), np.float16)
+    _check(load_library().b200rt_debug_gemm_rope(_ptr(a16), _ptr(w16), _ptr(c), _ptr(st) if st is not None else None, _ptr(table),
+                                                 table.shape[0], M, N, S, rot_cols, eps, sms, _ptr(out)))
+    return out
+
+
+def debug_gemm_swiglu(a16: np.ndarray, w16: np.ndarray, c, stats, eps: float, sms: int = 0):
+    """nomic-bert's FFN1 epilogue (b200rt_debug_gemm_swiglu): w16 [N, 768] with gate / up rows interleaved in groups of 8, c [N];
+    returns out float16 [M, N / 2] = silu(g) u."""
+    a16 = np.ascontiguousarray(a16, dtype=np.float16)
+    w16 = np.ascontiguousarray(w16, dtype=np.float16)
+    M, N = a16.shape[0], w16.shape[0]
+    c = _f32(c)
+    st = _f32(stats) if stats is not None else None
+    out = np.empty((M, N // 2), np.float16)
+    _check(load_library().b200rt_debug_gemm_swiglu(_ptr(a16), _ptr(w16), _ptr(c), _ptr(st) if st is not None else None, M, N, eps, sms,
+                                                   _ptr(out)))
+    return out
+
+
+def debug_attention_stream(qkv16: np.ndarray, lens, B: int, S: int, sms: int = 0, iters: int = 0):
+    """The streaming K/V attention (b200rt_debug_attention_stream): qkv16 [B*S, 2304] float16; returns (ctx [B*S, 768] float16,
+    mean ms of ``iters`` further launches, 0 when iters == 0)."""
+    qkv16 = np.ascontiguousarray(qkv16, dtype=np.float16)
+    lens = np.ascontiguousarray(lens, dtype=np.int32)
+    ctx = np.empty((B * S, 768), np.float16)
+    ms = ctypes.c_float(0)
+    _check(load_library().b200rt_debug_attention_stream(_ptr(qkv16), _ptr(lens), B, S, _ptr(ctx), sms, iters, ctypes.byref(ms)))
+    return ctx, ms.value

@@ -551,3 +551,144 @@ def clip_text_config_from_dir(path: str) -> dict:
         tc = cfg.get("text_config") or cfg
         out.update(eps=tc.get("layer_norm_eps", 1e-5), heads=tc.get("num_attention_heads"), eos_id=tc.get("eos_token_id", 2))
     return out
+
+
+# ---- nomic-bert (HF NomicBertModel: nomic-ai/nomic-embed-text-v1 / -v1.5)
+
+NOMIC_ARCHITECTURES = ("NomicBertModel", "NomicBertForPreTraining", "NomicBertForMaskedLM")
+NOMIC_MAX_POS = 8192  # the longest input the engine's rotary table and streaming attention take
+# nomic-embed-text-v1.5 at its full 8192-token context (rope_theta 1000, mean pooling)
+NOMIC_EMBED_TEXT_GEOMETRY = dict(vocab=30528, hidden=768, layers=12, heads=12, inter=3072, max_pos=8192, type_vocab=2, eps=1e-12,
+                                 rope_theta=1000.0)
+
+
+def nomic_blob_layout(g: dict) -> list[tuple[str, tuple[int, ...]]]:
+    """HF shapes and order, no biases: word | type | emb.ln, then per layer qkv.w [3H,H] | ao.w | ln1 | gate.w [I,H] | up.w [I,H] |
+    down.w [H,I] | ln2."""
+    h, i = g["hidden"], g["inter"]
+    lay = [("emb.word", (g["vocab"], h)), ("emb.type", (g["type_vocab"], h)), ("emb.ln.g", (h,)), ("emb.ln.b", (h,))]
+    for l in range(g["layers"]):
+        p = f"l{l}."
+        lay += [(p + "qkv.w", (3 * h, h)), (p + "ao.w", (h, h)), (p + "ln1.g", (h,)), (p + "ln1.b", (h,)), (p + "gate.w", (i, h)),
+                (p + "up.w", (i, h)), (p + "down.w", (h, i)), (p + "ln2.g", (h,)), (p + "ln2.b", (h,))]
+    return lay
+
+
+def random_nomic_blob(g: dict = NOMIC_EMBED_TEXT_GEOMETRY, seed: int = 0) -> np.ndarray:
+    """Seeded weights of a nomic-bert geometry, drawn as :func:`random_blob` draws BERT's (sigma 0.02 matrices and embeddings,
+    unit LayerNorm gains, zero offsets), tensor by tensor in :func:`nomic_blob_layout` order."""
+    return _random_blob(nomic_blob_layout(g), seed)
+
+
+def _nomic_names(sd: dict) -> tuple[dict, bool]:
+    """Strip a model prefix; True when the keys are the hub checkpoint's (remote-code) names."""
+    for pref in ("", "model.", "nomic_bert.", "bert.", "0.auto_model.", "auto_model."):
+        if pref + "embeddings.word_embeddings.weight" in sd:
+            sd = {k[len(pref):]: v for k, v in sd.items() if k.startswith(pref)}
+            return sd, "emb_ln.weight" in sd
+    raise KeyError("no nomic-bert weights found (looked for [model.]embeddings.word_embeddings.weight)")
+
+
+def load_hf_nomic_state_dict(sd: dict, g: dict | None = None) -> tuple[dict, np.ndarray]:
+    """A nomic-bert state dict -> (geometry, fp32 blob of :func:`nomic_blob_layout`).  Takes the transformers names
+    (``layers.N.self_attn.{q,k,v,o}_proj``, ``layers.N.mlp.{gate,up,down}_proj``, ``layers.N.{post_attention,post_mlp}_layernorm``,
+    ``embeddings.LayerNorm``) and the hub checkpoint's (``encoder.layers.N.attn.Wqkv`` = q | k | v on dim 0, ``attn.out_proj``,
+    ``mlp.fc12`` = gate, ``mlp.fc11`` = up, ``mlp.fc2`` = down, ``norm1``, ``norm2``, ``emb_ln``); both give the same blob.  ``g``
+    (e.g. from :func:`nomic_config_from_dir`) supplies eps, max_pos and rope_theta; the rest is read from the tensors."""
+    sd, hub = _nomic_names(sd)
+    if hub:
+        lp = lambda l: f"encoder.layers.{l}."  # noqa: E731
+        names = {"ao.w": "attn.out_proj.weight", "ln1.g": "norm1.weight", "ln1.b": "norm1.bias", "gate.w": "mlp.fc12.weight",
+                 "up.w": "mlp.fc11.weight", "down.w": "mlp.fc2.weight", "ln2.g": "norm2.weight", "ln2.b": "norm2.bias"}
+        emb_ln = "emb_ln."
+    else:
+        lp = lambda l: f"layers.{l}."  # noqa: E731
+        names = {"ao.w": "self_attn.o_proj.weight", "ln1.g": "post_attention_layernorm.weight", "ln1.b": "post_attention_layernorm.bias",
+                 "gate.w": "mlp.gate_proj.weight", "up.w": "mlp.up_proj.weight", "down.w": "mlp.down_proj.weight",
+                 "ln2.g": "post_mlp_layernorm.weight", "ln2.b": "post_mlp_layernorm.bias"}
+        emb_ln = "embeddings.LayerNorm."
+    biases = [k for k in sd if k.endswith(".bias") and "norm" not in k.lower() and not k.startswith("emb_ln")]
+    if biases:
+        raise ValueError(f"nomic-bert projections carry no bias, but the checkpoint has {biases[0]}")
+    layers = 0
+    while lp(layers) + names["ao.w"] in sd:
+        layers += 1
+    vocab, hidden = _arr(sd["embeddings.word_embeddings.weight"]).shape
+    base = dict(NOMIC_EMBED_TEXT_GEOMETRY)
+    base.update(g or {})
+    base.update(vocab=int(vocab), hidden=int(hidden), layers=layers, inter=int(_arr(sd[lp(0) + names["up.w"]]).shape[0]),
+                type_vocab=int(_arr(sd["embeddings.token_type_embeddings.weight"]).shape[0]))
+    g = base
+    t = {"emb.word": sd["embeddings.word_embeddings.weight"], "emb.type": sd["embeddings.token_type_embeddings.weight"],
+         "emb.ln.g": sd[emb_ln + "weight"], "emb.ln.b": sd[emb_ln + "bias"]}
+    for l in range(layers):
+        s, p = lp(l), f"l{l}."
+        if hub:
+            t[p + "qkv.w"] = sd[s + "attn.Wqkv.weight"]
+        else:
+            t[p + "qkv.w"] = np.concatenate([_arr(sd[s + f"self_attn.{n}_proj.weight"]) for n in "qkv"], 0)
+        t.update({p + name: sd[s + hf] for name, hf in names.items()})
+    return g, _pack(nomic_blob_layout(g), t)
+
+
+def is_nomic_dir(path: str) -> bool:
+    """A snapshot whose config.json names NomicBert in ``architectures`` or ``model_type``."""
+    p = os.path.join(path, "config.json")
+    if not os.path.exists(p):
+        return False
+    with open(p) as f:
+        cfg = json.load(f)
+    archs = cfg.get("architectures") or []
+    return cfg.get("model_type") == "nomic_bert" or any(a in NOMIC_ARCHITECTURES for a in archs)
+
+
+def nomic_config_from_dir(path: str) -> dict:
+    """The geometry of a nomic-bert snapshot's config.json.  Reads the transformers field names (``hidden_size``,
+    ``num_attention_heads``, ``intermediate_size``, ``num_hidden_layers``, ``max_position_embeddings``, ``layer_norm_eps``,
+    ``rope_parameters.rope_theta`` / ``rope_type``) or the remote-code ones (``n_embd``, ``n_head``, ``n_inner``, ``n_layer``,
+    ``layer_norm_epsilon``, ``rotary_emb_base``, ``max_trained_positions``).  Refuses, with a message, what the engine does not
+    compute: another rope_type, ``rotary_scaling_factor`` (dynamic NTK), interleaved or partial rotary, pre-norm, biases, and any
+    activation but SwiGLU.  max_pos is ``max_position_embeddings``, else ``max_trained_positions``, else 2048, at most 8192."""
+    with open(os.path.join(path, "config.json")) as f:
+        cfg = json.load(f)
+    return nomic_config(cfg)
+
+
+def nomic_config(cfg: dict) -> dict:
+    """:func:`nomic_config_from_dir` on a parsed config.json."""
+    def pick(*names, default=None):
+        for n in names:
+            if cfg.get(n) is not None:
+                return cfg[n]
+        return default
+
+    rope = cfg.get("rope_parameters") or {}
+    rope_type = rope.get("rope_type", cfg.get("rope_type", "default"))
+    if rope_type != "default":
+        raise ValueError(f"rope_type {rope_type!r} is not supported (only 'default' rotary embeddings)")
+    if cfg.get("rotary_scaling_factor") is not None:
+        raise ValueError("rotary_scaling_factor (dynamic-NTK context extension) is not supported")
+    if cfg.get("rotary_emb_interleaved"):
+        raise ValueError("rotary_emb_interleaved: true is not supported (rotate_half pairs (d, d + 32) only)")
+    if float(cfg.get("rotary_emb_fraction", 1.0)) != 1.0:
+        raise ValueError(f"rotary_emb_fraction {cfg['rotary_emb_fraction']} is not supported (every head dimension rotates)")
+    if cfg.get("prenorm"):
+        raise ValueError("prenorm: true is not supported (nomic-bert layers are post-LayerNorm)")
+    on = [k for k, v in cfg.items() if k.endswith("_bias") and v is True]
+    if on:
+        raise ValueError(f"{on[0]}: true is not supported (nomic-bert projections carry no bias)")
+    act = pick("activation_function", "hidden_act", default="swiglu")
+    if act not in ("swiglu", "silu"):
+        raise ValueError(f"activation {act!r} is not supported (SwiGLU only)")
+    max_pos = pick("max_position_embeddings", "max_trained_positions", default=2048)
+    theta = rope.get("rope_theta", pick("rotary_emb_base", "rope_theta", default=1000.0))
+    return dict(vocab=int(pick("vocab_size", default=30528)), hidden=int(pick("hidden_size", "n_embd", default=768)),
+                layers=int(pick("num_hidden_layers", "n_layer", default=12)), heads=int(pick("num_attention_heads", "n_head", default=12)),
+                inter=int(pick("intermediate_size", "n_inner", default=3072)), max_pos=min(int(max_pos), NOMIC_MAX_POS),
+                type_vocab=int(pick("type_vocab_size", default=2)), eps=float(pick("layer_norm_eps", "layer_norm_epsilon", default=1e-12)),
+                rope_theta=float(theta))
+
+
+def load_hf_nomic_dir(path: str) -> tuple[dict, np.ndarray]:
+    """A nomic-bert snapshot directory -> (geometry, blob)."""
+    return load_hf_nomic_state_dict(_read_state_dict(path), nomic_config_from_dir(path))

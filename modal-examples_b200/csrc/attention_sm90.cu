@@ -258,6 +258,200 @@ attention_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__
     if (loader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
 }
 
+
+// ------------------------------------------------------------------------------------------------------------------------
+// Streaming K/V attention, any S up to 8192 (a multiple of 64), 12 heads of 64 (nomic-bert): the K and V of a head no longer
+// fit in shared memory, so they stream through a ring of NSTAGE 128-key stages (K and V 16 KB each, one `full` mbarrier with
+// the stage's tx-count and one `empty` mbarrier taking an arrival from each of the 8 consumer warps).
+//
+// A unit is one (item b, head h, 128-row query tile t), numbered ((b NH + h) nq + t): the query tiles of a head are adjacent,
+// so the CTAs that run together read that head's K / V from L2 rather than HBM.  Persistent CTAs walk u = blockIdx.x,
+// blockIdx.x + gridDim.x, ...  Three warpgroups:
+//   warpgroup 0 (setmaxnreg 40): one thread TMA-loads the unit's Q tile (double buffered: q_full / q_empty) and its
+//       ceil(len / 128) K / V tiles into the ring -- never the padding past the item's length -- and runs ahead across units;
+//   warpgroups 1-2 (setmaxnreg 232): consumer c takes query rows 64c .. 64c + 63 of the tile and walks the keys in 64-key
+//       sub-blocks exactly as attention_kernel<64, NH> does: the same wgmma sequence, -inf mask past len, online softmax with
+//       ex2.approx, rescale and P . V from registers, in the same key order.  At S <= 512 its ctx is therefore bit-identical
+//       to attention_kernel's on the same qkv, and an item's ctx does not depend on the batch, the bucket, the grid or the CTA.
+//       A consumer frees a stage after its second sub-block (or the unit's last), the Q buffer after the unit's last
+//       sub-block, and stores ctx = O / l straight from its registers (rows past S are not stored).
+// Shared memory: Q 2 x 16 KB + NSTAGE x 32 KB + barriers = 165 120 bytes with NSTAGE = 4.
+namespace stream {
+constexpr int NSTAGE = 4;
+constexpr int NUM_THREADS = 384;
+constexpr int TILE_BYTES = 128 * 128;               // 128 rows of 64 fp16, 128B-swizzled
+constexpr int OFF_Q = 0;                            // 2 tiles
+constexpr int OFF_KV = 2 * TILE_BYTES;              // stage s: K at OFF_KV + 2 s TILE_BYTES, V one tile later
+constexpr int OFF_BAR = OFF_KV + NSTAGE * 2 * TILE_BYTES;
+constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+static_assert(SMEM_BYTES <= 232448, "shared memory");
+constexpr int MAX_S = 8192;
+}  // namespace stream
+
+template <int D, int NH>
+__global__ void __launch_bounds__(stream::NUM_THREADS, 1)
+attention_stream_kernel(const __grid_constant__ CUtensorMap tq, __half* __restrict__ ctx, const int32_t* __restrict__ lens, int S,
+                        int n_units) {
+    static_assert(D == 64, "128-byte rows");
+    using namespace stream;
+    constexpr int RB = 2 * D;
+    constexpr int HID = NH * D;
+    constexpr int NO = D / 2;
+    constexpr float kScaleLog2e = scale_log2e<D>();
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
+    uint64_t* kv_full = bars;                 // [NSTAGE]
+    uint64_t* kv_empty = bars + NSTAGE;       // [NSTAGE]
+    uint64_t* q_full = bars + 2 * NSTAGE;     // [2]
+    uint64_t* q_empty = bars + 2 * NSTAGE + 2;  // [2]
+
+    griddep_launch_dependents();
+    const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
+    const int lane = lane_id();
+    const int nq = (S + QT - 1) / QT;
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tq);
+        for (int s = 0; s < NSTAGE; ++s) {
+            mbar_init(&kv_full[s], 1);
+            mbar_init(&kv_empty[s], 8);  // the 8 consumer warps
+        }
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(&q_full[i], 1);
+            mbar_init(&q_empty[i], 8);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    griddep_wait();  // the prologue above overlapped the previous kernel's tail; nothing it wrote (qkv, lens) has been read yet
+
+    // unit u -> item, head, query tile and the item's valid keys (clamped to [1, S]), its 64-key sub-blocks
+    auto decode = [&](int u, int& b, int& h, int& t, int& len, int& nsb) {
+        t = u % nq;
+        const int bh = u / nq;
+        h = bh % NH;
+        b = bh / NH;
+        len = __ldg(lens + b);
+        len = len < 1 ? 1 : (len > S ? S : len);
+        nsb = (len + SB - 1) / SB;
+    };
+
+    if (warp < 4) {
+        // -------------------------------------------------------------------- TMA producer
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            int stage = 0;
+            uint32_t phase = 0, g = 0;
+            for (int u = blockIdx.x; u < n_units; u += gridDim.x, ++g) {
+                int b, h, t, len, nsb;
+                decode(u, b, h, t, len, nsb);
+                mbar_wait(&q_empty[g & 1], ((g >> 1) & 1) ^ 1);  // the unit two before this one has finished with the buffer
+                mbar_arrive_expect_tx(&q_full[g & 1], TILE_BYTES);
+                tma_load_3d(smem + OFF_Q + (g & 1) * TILE_BYTES, &tq, &q_full[g & 1], h * D, t * QT, b);
+                for (int j = 0; j < (nsb + 1) / 2; ++j) {
+                    mbar_wait(&kv_empty[stage], phase ^ 1);
+                    uint8_t* st = smem + OFF_KV + stage * 2 * TILE_BYTES;
+                    mbar_arrive_expect_tx(&kv_full[stage], 2 * TILE_BYTES);  // keys past S are zero-filled and still counted
+                    tma_load_3d(st, &tq, &kv_full[stage], HID + h * D, j * KB, b);
+                    tma_load_3d(st + TILE_BYTES, &tq, &kv_full[stage], 2 * HID + h * D, j * KB, b);
+                    if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+        __syncwarp();
+        return;
+    }
+
+    // ------------------------------------------------------------------------ consumers
+    setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1;  // which 64 query rows of a tile
+    const int w4 = warp & 3;         // rows 16 w4 .. 16 w4 + 15 of them
+    int stage = 0;
+    uint32_t phase = 0, g = 0;
+    for (int u = blockIdx.x; u < n_units; u += gridDim.x, ++g) {
+        int b, h, t, len, nsb;
+        decode(u, b, h, t, len, nsb);
+        mbar_wait(&q_full[g & 1], (g >> 1) & 1);
+        float o[NO];
+#pragma unroll
+        for (int i = 0; i < NO; ++i) o[i] = 0.f;
+        float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        const uint32_t q_addr = smem_u32(smem + OFF_Q + (g & 1) * TILE_BYTES) + wg * (64 * RB);
+#pragma unroll 1
+        for (int sb = 0; sb < nsb; ++sb) {
+            if ((sb & 1) == 0) mbar_wait(&kv_full[stage], phase);
+            const uint32_t k_addr = smem_u32(smem + OFF_KV + stage * 2 * TILE_BYTES) + (sb & 1) * (SB * RB);
+            float s[32];
+            wgmma_fence();
+            fence_operands(s);
+#pragma unroll
+            for (int k = 0; k < D / 16; ++k)
+                wgmma_m64n64k16_ss(s, make_desc<D>(q_addr + k * 32), make_desc<D>(k_addr + k * 32), k != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_operands(s);
+            const int valid = len - sb * SB;  // keys [0, valid) of this sub-block are real (>= 1)
+            if (valid < SB) {
+#pragma unroll
+                for (int i = 0; i < 32; ++i)
+                    if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) s[i] = -INFINITY;
+            }
+            uint32_t pa[4][4];  // P as the A fragments of the four 16-key steps
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * hf], s[4 * j + 2 * hf + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffff, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffff, mx, 2));
+                const float m_new = fmaxf(m_run[hf], mx);
+                const float alpha = ex2_approx((m_run[hf] - m_new) * kScaleLog2e);  // 0 on the first sub-block
+                m_run[hf] = m_new;
+                const float neg_ms = -m_new * kScaleLog2e;
+                float ls = 0.f;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float p0 = ex2_approx(fmaf(s[4 * j + 2 * hf], kScaleLog2e, neg_ms));
+                    const float p1 = ex2_approx(fmaf(s[4 * j + 2 * hf + 1], kScaleLog2e, neg_ms));
+                    ls += p0 + p1;
+                    pa[j >> 1][2 * (j & 1) + hf] = pack_half2(p0, p1);
+                    o[4 * j + 2 * hf] *= alpha;
+                    o[4 * j + 2 * hf + 1] *= alpha;
+                }
+                l_run[hf] = fmaf(l_run[hf], alpha, ls);
+            }
+            const uint32_t v_addr = smem_u32(smem + OFF_KV + stage * 2 * TILE_BYTES + TILE_BYTES) + (sb & 1) * (SB * RB);
+            wgmma_fence();
+            fence_operands(o);
+#pragma unroll
+            for (int kk = 0; kk < SB / 16; ++kk) wgmma_m64n64k16_rs_mn(o, pa[kk], make_desc<D>(v_addr + kk * (16 * RB)), 1);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_operands(o);
+            if ((sb & 1) || sb == nsb - 1) {  // the stage's last sub-block: hand it back to the producer
+                if (lane == 0) mbar_arrive(&kv_empty[stage]);
+                if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+            }
+        }
+        if (lane == 0) mbar_arrive(&q_empty[g & 1]);  // this warp's last MMA on the Q tile has completed
+        // ctx = O / l, straight from the registers: this thread's rows r and r + 8 of the tile, dims 8j + 2 (lane % 4) + {0, 1}
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            float l = l_run[hf];
+            l += __shfl_xor_sync(0xffffffff, l, 1);
+            l += __shfl_xor_sync(0xffffffff, l, 2);
+            const float inv_l = 1.0f / l;
+            const int r = t * QT + wg * 64 + w4 * 16 + (lane >> 2) + 8 * hf;
+            if (r < S) {
+                __half* row = ctx + (static_cast<size_t>(b) * S + r) * HID + h * D + 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < D / 8; ++j)
+                    *reinterpret_cast<uint32_t*>(row + 8 * j) = pack_half2(o[4 * j + 2 * hf] * inv_l, o[4 * j + 2 * hf + 1] * inv_l);
+            }
+        }
+    }
+}
+
 }  // namespace attn
 
 template <int D, int NH, bool CAUSAL = false>
@@ -283,7 +477,8 @@ cudaError_t attention_init_device() {
     if ((e = setup<64, 12>()) != cudaSuccess) return e;
     if ((e = setup<32, 12>()) != cudaSuccess) return e;
     if ((e = setup<64, 16>()) != cudaSuccess) return e;
-    return setup<64, 8, true>();
+    if ((e = setup<64, 8, true>()) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(attn::attention_stream_kernel<64, 12>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::stream::SMEM_BYTES);
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
@@ -294,6 +489,14 @@ cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, con
     if (head_dim == 32 && heads == 12) return launch_one<32, 12>(tq, tctx, lens, B, S, sm_count, stream);
     if (head_dim == 64 && heads == 16) return launch_one<64, 16>(tq, tctx, lens, B, S, sm_count, stream);
     return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_attention_stream(const CUtensorMap& tq, __half* ctx, const int32_t* lens, int B, int S, int sm_count, cudaStream_t stream) {
+    if (S < 64 || S % 64 != 0 || S > attn::stream::MAX_S || B < 1 || sm_count < 1 || ctx == nullptr || lens == nullptr) return cudaErrorInvalidValue;
+    const int n_units = B * 12 * ((S + attn::QT - 1) / attn::QT);
+    const int grid = n_units < sm_count ? n_units : sm_count;
+    return launch_pdl(attn::attention_stream_kernel<64, 12>, dim3(grid), dim3(attn::stream::NUM_THREADS), attn::stream::SMEM_BYTES, stream, tq,
+                      ctx, lens, S, n_units);
 }
 
 }  // namespace b200

@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <condition_variable>
 #include <cstdarg>
 #include <cstdio>
@@ -119,6 +120,7 @@ int make_map_qkv(CUtensorMap* m, const void* base, uint64_t B, uint64_t S, uint6
 constexpr int NSLOT = 4;
 constexpr int MIN_ITEMS_PER_REPLICA = 8;  // a wave uses fewer replicas rather than giving one fewer items than this
 constexpr int MAX_SEQ = 512;
+constexpr int MAX_SEQ_LONG = 8192;  // kind "nomic_bert" (streaming attention): max_pos and its longest bucket
 constexpr int VIT_WAVE_ITEMS = 64;  // images one replica takes per wave (64 x 197 tokens; 38.5 MB of pixels per wave slot)
 
 // The text geometries the kernels cover (hidden, heads, inter, causal): bge-base, bge-small and bge-large (kind "bert") and the
@@ -174,9 +176,13 @@ struct DevWeights {
     __half *mlm_t_w = nullptr, *mlm_dec_w = nullptr;
     CUtensorMap m_mlm_t, m_mlm_dec;
     float *mlm_t_c = nullptr, *mlm_dec_c = nullptr;
+    // nomic-bert (kind "nomic_bert"): pos = 64 zero rows (embed_kernel reads pos[t % 64]), zero_bias the zero bias of every
+    // projection, rope the (cos, sin) table [max_pos rounded up to 64][32]; LayerW::ff1_w holds gate and up interleaved
+    // (launch_gemm_swiglu) and ff1_c their folded c in the same order
+    float* rope = nullptr;  // float2 pairs
 };
 
-enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2 };
+enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2, KIND_NOMIC = 3 };
 
 struct Model {
     ModelKind kind = KIND_BERT;
@@ -393,12 +399,13 @@ int get_qkv_map(Dev& d, const Model& model, int S, const CUtensorMap** out, cons
 int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
                     LaunchHook* hook) {
     const DevWeights& w = m.per_dev[dev_index];
-    const bool vit = m.kind == KIND_VIT, clip_text = m.kind == KIND_CLIP_TEXT, pre_ln = m.kind != KIND_BERT;
+    const bool vit = m.kind == KIND_VIT, clip_text = m.kind == KIND_CLIP_TEXT, pre_ln = vit || clip_text;
     const int B = in.B, S = in.S, M = B * S;
     if (M > m.cap_rows || (vit && B > VIT_WAVE_ITEMS))
         return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the model's wave capacity (%d rows)", B, S, m.cap_rows);
-    if (m.splade_vpad > 0 && S % 64 != 0)
-        return fail(B200RT_E_INVALID, "a bert_splade forward runs at padded lengths that are multiples of 64 (got %d)", S);
+    if ((m.splade_vpad > 0 || m.kind == KIND_NOMIC) && S % 64 != 0)
+        return fail(B200RT_E_INVALID, "a %s forward runs at padded lengths that are multiples of 64 (got %d)",
+                    m.kind == KIND_NOMIC ? "nomic_bert" : "bert_splade", S);
     const int H = m.hidden, I = m.inter, P = H / 128;
     const Dev::ActMaps& am = d.act[text_geometry(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
@@ -429,31 +436,58 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             if (step("vit_embed")) return 0;
         } else {
             // clip_text: token + position, its zero type row leaves (word + 0) + pos bit-exact; no embedding LayerNorm
-            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, S, m.vocab, H, stream, in.segs));
+            // nomic_bert: no position table -- pos is 64 zero rows read as pos[t % 64], so the rows are (word + type0) + 0
+            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, m.kind == KIND_NOMIC ? 64 : S, m.vocab, H,
+                                  stream, in.segs));
             if (step("embed")) return 0;
         }
         const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // BERT: the LayerNorm that applies to the current residual rows
-        for (int l = 0; l < m.layers; ++l) {
-            const LayerW& lw = w.layers[l];
-            // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
-            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
-            if (step("gemm_qkv")) return 0;
-            CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, clip_text));
-            if (step("attention")) return 0;
-            // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
-            const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
-            if (step("gemm_attn_out")) return 0;
-            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
-            if (step(pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
-            // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
-            const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
-            if (step("gemm_ffn2")) return 0;
-            prev_g = lw.ln2_g;
-            prev_b = lw.ln2_b;
+        if (m.kind == KIND_NOMIC) {
+            // NomicBertModel, post-LN as BERT: h = LN_a(x + o(attn(rope(q), rope(k), v))), y = LN_m(h + down(silu(gate h) up h)).
+            // The embedding LN, then each layer's LN2, folds into QKV and is re-applied by attn-out; LN1 folds into FFN1 and is
+            // re-applied by FFN2.  No biases: the folded c vectors and a zero vector.
+            for (int l = 0; l < m.layers; ++l) {
+                const LayerW& lw = w.layers[l];
+                GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
+                CUDA_TRY(launch_gemm_rope(am.yhi, lw.m_qkv, d.qkv, e_qkv, RopeEpi{reinterpret_cast<const float2*>(w.rope), S, 2 * H}, M, 3 * H, H, d.sm_gemm, stream));
+                if (step("gemm_qkv_rope")) return 0;
+                CUDA_TRY(launch_attention_stream(*mq, d.ctx, lens, B, S, d.sm_attn, stream));
+                if (step("attention_stream")) return 0;
+                const GemmEpi e_ao = residual(w.zero_bias, d.pstats[0], prev_g, prev_b, d.pstats[1]);
+                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
+                if (step("gemm_attn_out")) return 0;
+                GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
+                CUDA_TRY(launch_gemm_swiglu(am.yhi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
+                if (step("gemm_ffn1_swiglu")) return 0;
+                const GemmEpi e_ff2 = residual(w.zero_bias, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
+                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
+                if (step("gemm_ffn2")) return 0;
+                prev_g = lw.ln2_g;
+                prev_b = lw.ln2_b;
+            }
+        } else {
+            for (int l = 0; l < m.layers; ++l) {
+                const LayerW& lw = w.layers[l];
+                // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
+                GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
+                CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
+                if (step("gemm_qkv")) return 0;
+                CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, clip_text));
+                if (step("attention")) return 0;
+                // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
+                const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
+                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
+                if (step("gemm_attn_out")) return 0;
+                GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
+                CUDA_TRY(launch_gemm(pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+                if (step(pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
+                // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
+                const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
+                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
+                if (step("gemm_ffn2")) return 0;
+                prev_g = lw.ln2_g;
+                prev_b = lw.ln2_b;
+            }
         }
         if (m.splade_vpad > 0) {
             // SPLADE (BertForMaskedLM + max pooling): u = gelu(LN2(y) W_t^T + b_t) into the idle ctx buffer; the partials of u's
@@ -620,7 +654,8 @@ bool is_pinned(const void* p, size_t nbytes) {
 
 // Padded lengths are bucketed to multiples of 64 tokens (the attention kernel's key sub-block): tickets whose max_len
 // falls into the same bucket share a wave, padded to the bucket size (at most 63 wasted tokens per item).
-inline int bucket_of(int S) { return std::min(MAX_SEQ, (S + 63) / 64 * 64); }
+// Kind "nomic_bert" keeps 64-token buckets up to its max_pos rounded up to 64 (`cap`); every other kind's stop at 512.
+inline int bucket_of(int S, int cap = MAX_SEQ) { return std::min(cap, (S + 63) / 64 * 64); }
 
 void launcher_main(Dev* dp) {
     Dev& d = *dp;
@@ -1490,6 +1525,92 @@ int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, si
     return register_model(rt, std::move(m), model_out);
 }
 
+// Kind "nomic_bert" (HF NomicBertModel): bge-base's geometry, rotary Q / K, SwiGLU MLP, no biases, max_pos <= 8192.
+int model_load_nomic(const b200rt_nomic_bert_config& nc, const float* blob, size_t nbytes, bool pool_mean, int* model_out) {
+    Runtime& rt = *g_rt;
+    const b200rt_bert_config& c = nc.bert;
+    if (c.hidden != HIDDEN || c.heads != HEADS || c.inter != 3072 || c.max_pos < 1 || c.max_pos > MAX_SEQ_LONG || c.layers < 1 || c.vocab < 1 ||
+        c.type_vocab < 1 || !(nc.rope_theta > 0.f) || !std::isfinite(nc.rope_theta))
+        return fail(B200RT_E_UNSUPPORTED,
+                    "kernels cover nomic-bert at hidden=768 heads=12 inter=3072, max_pos<=%d, rope_theta > 0 (got hidden %d heads %d inter "
+                    "%d max_pos %d rope_theta %g)", MAX_SEQ_LONG, c.hidden, c.heads, c.inter, c.max_pos, static_cast<double>(nc.rope_theta));
+    const int S_max = (c.max_pos + 63) / 64 * 64;
+    if (rt.cap_rows < S_max)
+        return fail(B200RT_E_INVALID, "a nomic_bert model with max_pos %d needs room for one %d-token item, and the workspace holds %d rows: "
+                    "initialise with a larger B200RT_INIT_WAVE_ITEMS (now %d)", c.max_pos, S_max, rt.cap_rows, rt.cap_items);
+
+    auto m = std::make_unique<Model>();
+    m->kind = KIND_NOMIC;
+    m->cfg = c;
+    m->vocab = c.vocab, m->max_pos = c.max_pos;
+    m->pool_mean = pool_mean;
+    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
+    m->cap_rows = rt.cap_rows;
+    m->out_dim = c.hidden;
+
+    // b200rt.weights.nomic_blob_layout.  QKV of layer l folds the previous layer's ln2 (the embedding LN for l = 0); gate and up
+    // (adjacent in the blob) are one [2I, H] entry folding the layer's ln1, interleaved below.  Then the arena-only vectors.
+    const size_t H = c.hidden, I = c.inter;
+    Layout L;
+    L.copy(c.vocab * H, &DevWeights::word);
+    L.copy(c.type_vocab * H, &DevWeights::type);
+    int ln_g = L.copy(H, &DevWeights::emb_g);
+    int ln_b = L.copy(H, &DevWeights::emb_b);
+    for (int l = 0; l < c.layers; ++l) {
+        const int qkv = L.half(l, 3 * H, H, &LayerW::qkv_w, &LayerW::m_qkv);
+        L.fold(qkv, ln_g, ln_b, -1, &LayerW::qkv_c);
+        L.half(l, H, H, &LayerW::ao_w, &LayerW::m_ao);
+        const int ln1_g = L.copy(l, H, &LayerW::ln1_g), ln1_b = L.copy(l, H, &LayerW::ln1_b);
+        const int ff1 = L.half(l, 2 * I, H, &LayerW::ff1_w, &LayerW::m_ff1);
+        L.fold(ff1, ln1_g, ln1_b, -1, &LayerW::ff1_c);
+        L.half(l, H, I, &LayerW::ff2_w, &LayerW::m_ff2);
+        ln_g = L.copy(l, H, &LayerW::ln2_g);
+        ln_b = L.copy(l, H, &LayerW::ln2_b);
+    }
+    L.zero(64 * H, &DevWeights::pos);
+    L.zero(H, &DevWeights::zero_bias);
+    L.zero(static_cast<size_t>(S_max) * 64, &DevWeights::rope);
+    if (int rc = load_weights(rt, *m, L, blob, nbytes)) return rc;
+
+    // The rotary table as HF builds it: inv_freq_i = fp32(1 / fp32(theta^(i/32))), f = fp32(inv_freq_i * pos), then cos / sin of f
+    // in double, rounded to fp32.
+    std::vector<float2> rope(static_cast<size_t>(S_max) * 32);
+    for (int i = 0; i < 32; ++i) {
+        const float inv_freq = 1.0f / powf(nc.rope_theta, static_cast<float>(2 * i) / 64.0f);
+        for (int p = 0; p < S_max; ++p) {
+            const float f = inv_freq * static_cast<float>(p);
+            rope[static_cast<size_t>(p) * 32 + i] = make_float2(static_cast<float>(cos(static_cast<double>(f))),
+                                                                static_cast<float>(sin(static_cast<double>(f))));
+        }
+    }
+    // gate rows 8k .. 8k+7 -> rows 16k .. 16k+7 and up rows 8k .. 8k+7 -> rows 16k+8 .. 16k+15, and their c alike, through a scratch
+    for (size_t g = 0; g < rt.devs.size(); ++g) {
+        Dev& d = *rt.devs[g];
+        DevWeights& w = m->per_dev[g];
+        CUDA_TRY(cudaSetDevice(d.id));
+        CUDA_TRY(cudaMemcpyAsync(w.rope, rope.data(), rope.size() * sizeof(float2), cudaMemcpyHostToDevice, d.compute));
+        __half* sw = nullptr;
+        float* sc = nullptr;
+        CUDA_TRY(cudaMalloc(&sw, 2 * I * H * 2));
+        std::unique_ptr<void, cudaError_t (*)(void*)> free_sw(sw, cudaFree);  // freed on every return (cudaFree waits for the device)
+        CUDA_TRY(cudaMalloc(&sc, 2 * I * 4));
+        std::unique_ptr<void, cudaError_t (*)(void*)> free_sc(sc, cudaFree);
+        for (int l = 0; l < c.layers; ++l) {
+            const LayerW& lw = w.layers[l];
+            for (int part = 0; part < 2; ++part) {  // 0: gate, 1: up
+                CUDA_TRY(cudaMemcpy2DAsync(sw + part * 8 * H, 16 * H * 2, lw.ff1_w + part * I * H, 8 * H * 2, 8 * H * 2, I / 8,
+                                           cudaMemcpyDeviceToDevice, d.compute));
+                CUDA_TRY(cudaMemcpy2DAsync(sc + part * 8, 16 * 4, lw.ff1_c + part * I, 8 * 4, 8 * 4, I / 8, cudaMemcpyDeviceToDevice, d.compute));
+            }
+            CUDA_TRY(cudaMemcpyAsync(lw.ff1_w, sw, 2 * I * H * 2, cudaMemcpyDeviceToDevice, d.compute));
+            CUDA_TRY(cudaMemcpyAsync(lw.ff1_c, sc, 2 * I * 4, cudaMemcpyDeviceToDevice, d.compute));
+        }
+        CUDA_TRY(cudaStreamSynchronize(d.compute));
+    }
+    CUDA_TRY(cudaSetDevice(rt.devs[0]->id));
+    return register_model(rt, std::move(m), model_out);
+}
+
 Runtime* live_rt() {
     if (g_poisoned.load()) {
         fail(B200RT_E_CUDA, "context poisoned by an earlier CUDA error%s%s", g_rt && !g_rt->async_error.empty() ? ": " : "",
@@ -1513,8 +1634,11 @@ const Model* get_model(Runtime& rt, int model) {
 }
 
 // The longest padded length a forward of this model runs at: the CLIP text tower's waves go up to the 128-token bucket (its
-// position table is padded to TEXT_POS_ROWS zero rows for that), a BERT model's up to max_pos.
-inline int max_wave_len(const Model& m) { return m.kind == KIND_CLIP_TEXT ? TEXT_POS_ROWS : m.max_pos; }
+// position table is padded to TEXT_POS_ROWS zero rows for that), a nomic-bert model's up to max_pos rounded up to 64 (its
+// rotary table has those rows), a BERT model's up to max_pos.
+inline int max_wave_len(const Model& m) {
+    return m.kind == KIND_CLIP_TEXT ? TEXT_POS_ROWS : m.kind == KIND_NOMIC ? (m.max_pos + 63) / 64 * 64 : m.max_pos;
+}
 
 // ids [n_items, max_len] with max_len <= S_cap (submit: max_pos; device-resident / debug forwards: max_wave_len) and every
 // item's length in [1, min(max_len, max_pos)], its ids inside the vocabulary.
@@ -1652,9 +1776,9 @@ int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights,
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0 && strcmp(kind, "clip_text") != 0 &&
-                  strcmp(kind, "bert_classifier") != 0 && strcmp(kind, "bert_splade") != 0))
-        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"bert_classifier\", \"bert_splade\", \"vit\" or \"clip_text\")",
-                    kind ? kind : "(null)");
+                  strcmp(kind, "bert_classifier") != 0 && strcmp(kind, "bert_splade") != 0 && strcmp(kind, "nomic_bert") != 0))
+        return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"bert_classifier\", \"bert_splade\", \"nomic_bert\", \"vit\" or "
+                    "\"clip_text\")", kind ? kind : "(null)");
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
     if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
     const bool pool_mean = (flags & B200RT_LOAD_POOL_MEAN) != 0;
@@ -1674,6 +1798,9 @@ int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights,
             return fail(B200RT_E_UNSUPPORTED, "num_labels %d outside [1, %d]", cc.num_labels, MAX_LABELS);
         return model_load(cc.bert, static_cast<const float*>(weights), nbytes, false, model_out, cc.num_labels);
     }
+    if (strcmp(kind, "nomic_bert") == 0)
+        return model_load_nomic(*static_cast<const b200rt_nomic_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean,
+                                model_out);
     if (strcmp(kind, "bert_splade") == 0) {
         if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"bert_splade\"", flags);
         return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, false, model_out, 0, true);
@@ -1727,6 +1854,8 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     // own length, so a ragged input wastes at most 63 tokens per item instead of max_len - len)
     std::vector<Run> runs;
     {
+        const int cap = m->kind == KIND_NOMIC ? max_wave_len(*m) : MAX_SEQ;
+        auto bucket_of = [cap](int S) { return ::bucket_of(S, cap); };
         bool one_bucket = true;
         const int b0 = bucket_of(t->lens[0]);
         for (int i = 1; i < n_items && one_bucket; ++i) one_bucket = bucket_of(t->lens[i]) == b0;
@@ -2309,6 +2438,109 @@ int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* 
     cudaEventElapsedTime(&ms, e0, e1);
     if (ms_out) *ms_out = ms / iters;
     CUDA_TRY(b.download(vmax_out, dmax, nmax * 4));
+    return 0;
+}
+
+int b200rt_debug_gemm_rope(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const float* table, int n_pos, int M,
+                           int N, int S, int rot_cols, float eps, int sms, uint16_t* out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!a || !w || !c || !table || !out || M < 1 || N < 256 || N % 256 || S < 64 || S % 64 || n_pos < S || rot_cols < 0 || rot_cols % 256 ||
+        rot_cols > N)
+        return fail(B200RT_E_INVALID, "bad gemm_rope arguments (N a multiple of 256, S of 64, n_pos >= S, rot_cols a multiple of 256 <= N)");
+    Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    constexpr size_t K = HIDDEN;
+    const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256;
+    DebugBuffers b(d.compute);
+    __half *da, *dw, *dout;
+    float *dc, *dt;
+    float2* dst = nullptr;
+    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));
+    CUDA_TRY(cudaMemcpyAsync(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, d.compute));
+    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
+    CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
+    CUDA_TRY(b.upload(&dt, table, static_cast<size_t>(n_pos) * 64 * 4));
+    if (stats) CUDA_TRY(b.upload(&dst, stats, static_cast<size_t>(M) * STAT_PARTS * sizeof(float2)));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(M) * N * 2));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, static_cast<size_t>(M) * N * 2, d.compute));
+    CUtensorMap ta, tb;
+    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
+    if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
+    const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
+    CUDA_TRY(launch_gemm_rope(ta, tb, dout, e, RopeEpi{reinterpret_cast<const float2*>(dt), S, rot_cols}, M, N, static_cast<int>(K),
+                              sms ? sms : d.sm_count, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * N * 2));
+    return 0;
+}
+
+int b200rt_debug_gemm_swiglu(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, int M, int N, float eps, int sms,
+                             uint16_t* out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!a || !w || !c || !out || M < 1 || N < 256 || N % 256) return fail(B200RT_E_INVALID, "bad gemm_swiglu arguments (N a multiple of 256)");
+    Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    constexpr size_t K = HIDDEN;
+    const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256, No = static_cast<size_t>(N) / 2;
+    DebugBuffers b(d.compute);
+    __half *da, *dw, *dout;
+    float* dc;
+    float2* dst = nullptr;
+    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));
+    CUDA_TRY(cudaMemcpyAsync(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, d.compute));
+    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
+    CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
+    if (stats) CUDA_TRY(b.upload(&dst, stats, static_cast<size_t>(M) * STAT_PARTS * sizeof(float2)));
+    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(M) * No * 2));
+    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, static_cast<size_t>(M) * No * 2, d.compute));
+    CUtensorMap ta, tb;
+    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
+    if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
+    const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
+    CUDA_TRY(launch_gemm_swiglu(ta, tb, dout, e, M, N, static_cast<int>(K), sms ? sms : d.sm_count, d.compute));
+    CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * No * 2));
+    return 0;
+}
+
+int b200rt_debug_attention_stream(const uint16_t* qkv, const int32_t* lens, int B, int S, uint16_t* ctx, int sms, int iters, float* ms_out) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    if (!qkv || !lens || !ctx || B < 1 || S < 64 || S % 64 || S > MAX_SEQ_LONG)
+        return fail(B200RT_E_INVALID, "bad attention_stream arguments (64 <= S <= %d, a multiple of 64)", MAX_SEQ_LONG);
+    Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    const int grid_sms = sms ? sms : d.sm_count;
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    const size_t M = static_cast<size_t>(B) * S, H = HIDDEN;
+    DebugBuffers b(d.compute);
+    __half *dq, *dc;
+    int32_t* dl_;
+    CUDA_TRY(b.upload(&dq, qkv, M * 3 * H * 2));
+    CUDA_TRY(b.upload(&dc, nullptr, M * H * 2));
+    CUDA_TRY(cudaMemsetAsync(dc, 0xFF, M * H * 2, d.compute));
+    CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));  // passed through unchecked: the kernel clamps to [1, S]
+    CUtensorMap tq;
+    if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, 64)) return rc;
+    CUDA_TRY(launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute));
+    CUDA_TRY(b.download(ctx, dc, M * H * 2));
+    if (iters > 0) {
+        cudaEvent_t e0, e1;
+        CUDA_TRY(b.event(&e0));
+        CUDA_TRY(b.event(&e1));
+        CUDA_TRY(cudaEventRecord(e0, d.compute));
+        for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute));
+        CUDA_TRY(cudaEventRecord(e1, d.compute));
+        CUDA_TRY(cudaStreamSynchronize(d.compute));
+        float ms = 0;
+        cudaEventElapsedTime(&ms, e0, e1);
+        if (ms_out) *ms_out = ms / iters;
+    }
     return 0;
 }
 

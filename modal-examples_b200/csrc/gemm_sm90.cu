@@ -28,7 +28,12 @@
 //                                  into fp16 hi + lo in place, and the (sum, M2) partial of each new 128-column row slice;
 //   EPI_SPLADE_MAX               : v = max(rstd * acc + c, 0) on the item's valid rows, max-reduced over the consumer's 64 rows
 //                                  (one item: S % 64 == 0) by shuffles and a 4 KB shared-memory pass, then one
-//                                  red.global.max.u32 per non-zero column < vocab into the item's row of the max buffer.
+//                                  red.global.max.u32 per non-zero column < vocab into the item's row of the max buffer;
+//   EPI_ROPE_F16                 : v = rstd * acc + c as EPI_BIAS_F16, then on columns < rp.rot_cols (Q and K) each pair
+//                                  (d, d + 32) of a 64-column head rotated by the angle of position row % rp.S; fp16 out;
+//   EPI_SWIGLU_F16               : W's rows are gate and up interleaved in 8-row groups (g on 16k .. 16k+7, u on 16k+8 ..
+//                                  16k+15), so accumulator groups 2m and 2m+1 hold matching g and u columns: fp16(silu(g) u)
+//                                  into out [M, N / 2].
 //
 // The accumulator fragment of thread (warp w of the consumer warpgroup, lane l) holds rows 16w + l/4 and 16w + l/4 + 8,
 // columns 8j + 2(l%4) + {0, 1} for j = 0..31: acc[4j + {0, 1}] on the first row, acc[4j + {2, 3}] on the second.
@@ -86,6 +91,15 @@ __device__ __forceinline__ float gelu_quick(float x) {
     float r;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(ex2_approx(x * (-1.702f * 1.4426950408889634f)) + 1.0f));
     return x * r;
+}
+
+// silu(g) = g / (1 + 2^(-g log2(e))): ex2.approx (relative error <= 2^-22) and rcp.approx (<= 1 ulp) put the result within
+// 4e-7 relative of silu(g) wherever it is finite and non-zero -- three orders of magnitude inside fp16's half ulp (2^-12).  For
+// g < -88 the exponential overflows to +inf, rcp gives 0 and silu(g) = -0 (the true value is below 1e-36).
+__device__ __forceinline__ float silu(float g) {
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(ex2_approx(g * -1.4426950408889634f) + 1.0f));
+    return g * r;
 }
 
 // LayerNorm statistics of a row from its PARTS (sum, M2) partials (Chan et al.): 8 for a 1024-wide row, 6 for a 768-wide one,
@@ -148,11 +162,12 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float e
 }
 
 // BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128).  sp is read by
-// EPI_SPLADE_MAX only; as the last parameter it leaves every other instantiation's parameter offsets as they were.
+// EPI_SPLADE_MAX only, rp by EPI_ROPE_F16 only; as the last parameters they leave every other instantiation's parameter
+// offsets as they were.
 template <int EPI, int BN, int PARTS>
 __global__ void __cluster_dims__(CM, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
-            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K, const SpladeEpi sp) {
+            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K, const SpladeEpi sp, const RopeEpi rp) {
     static_assert(BN == 256 || BN == 128, "tile width");
     constexpr int STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
     constexpr int NACC = BN / 2;     // fp32 accumulators per consumer thread
@@ -297,6 +312,64 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
                 }
                 named_bar_sync(1 + cw, 128);  // the next tile rewrites red
             }
+        } else if constexpr (EPI == EPI_ROPE_F16) {
+            // head column d < 32 of accumulator group j = 8 hh + jj (jj < 4) pairs with d + 32 in group j + 4 of the same thread;
+            // both take frequency d = 8 jj + 2 (lane % 4) + {0, 1}: one float4 (cos, sin, cos, sin) per row and jj.  Q / K / V
+            // boundaries fall on tile boundaries, so a tile is rotated whole (Q, K) or not at all (V).  S % 64 == 0, so the
+            // consumer's 64 rows are positions (m0 + 64 cw) % S on and this thread's two rows lie 8 positions apart.
+            if (n0 < rp.rot_cols) {
+                const float4* __restrict__ cs = reinterpret_cast<const float4*>(rp.table) +
+                                                ((m0 + cw * 64) % rp.S + w4 * 16 + (lane >> 2)) * 16 + (lane & 3);
+#pragma unroll
+                for (int hh = 0; hh < BN / 64; ++hh) {  // head by head; the table row is re-read (L1) for each
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int j0 = 8 * hh + jj, j1 = j0 + 4;
+                        const float2 b0 = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j0));
+                        const float2 b1 = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j1));
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int row = r0 + 8 * h;
+                            if (row >= M) continue;
+                            const float4 t = __ldg(cs + 128 * h + 4 * jj);
+                            const float x0 = fmaf(rstd[h], acc[4 * j0 + 2 * h], b0.x), x1 = fmaf(rstd[h], acc[4 * j0 + 2 * h + 1], b0.y);
+                            const float y0 = fmaf(rstd[h], acc[4 * j1 + 2 * h], b1.x), y1 = fmaf(rstd[h], acc[4 * j1 + 2 * h + 1], b1.y);
+                            // x_d cos - x_{d+32} sin,  x_{d+32} cos + x_d sin
+                            __half* o = out + static_cast<size_t>(row) * N + c0;
+                            *reinterpret_cast<uint32_t*>(o + 8 * j0) = pack_half2(fmaf(x0, t.x, -y0 * t.y), fmaf(x1, t.z, -y1 * t.w));
+                            *reinterpret_cast<uint32_t*>(o + 8 * j1) = pack_half2(fmaf(y0, t.x, x0 * t.y), fmaf(y1, t.z, x1 * t.w));
+                        }
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = r0 + 8 * h;
+                        if (row < M)
+                            *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * N + c0 + 8 * j) =
+                                pack_half2(fmaf(rstd[h], acc[4 * j + 2 * h], bv.x), fmaf(rstd[h], acc[4 * j + 2 * h + 1], bv.y));
+                    }
+                }
+            }
+        } else if constexpr (EPI == EPI_SWIGLU_F16) {
+            // groups 2m (gate) and 2m + 1 (up) -> output columns n0 / 2 + 8m + 2 (lane % 4) + {0, 1} of the N / 2 wide rows
+#pragma unroll
+            for (int m = 0; m < BN / 16; ++m) {
+                const float2 bg = __ldg(reinterpret_cast<const float2*>(bias + c0 + 16 * m));
+                const float2 bu = __ldg(reinterpret_cast<const float2*>(bias + c0 + 16 * m + 8));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float g0 = fmaf(rstd[h], acc[8 * m + 2 * h], bg.x), g1 = fmaf(rstd[h], acc[8 * m + 2 * h + 1], bg.y);
+                    const float u0 = fmaf(rstd[h], acc[8 * m + 4 + 2 * h], bu.x), u1 = fmaf(rstd[h], acc[8 * m + 4 + 2 * h + 1], bu.y);
+                    const int row = r0 + 8 * h;
+                    if (row < M)
+                        *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * (N / 2) + n0 / 2 + 8 * m + 2 * (lane & 3)) =
+                            pack_half2(silu(g0) * u0, silu(g1) * u1);
+                }
+            }
         } else if constexpr (EPI != EPI_BIAS_RES_SPLIT) {
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
@@ -386,13 +459,14 @@ static int& max_clusters() {
 
 template <int EPI, int BN, int PARTS>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                              int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{}) {
+                              int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{},
+                              const RopeEpi& rp = RopeEpi{}) {
     const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
     int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
     if (clusters < 1) clusters = 1;
     if (ctas) *ctas = clusters * gemm::CM;
     return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::smem_bytes<EPI, BN>(),
-                      stream, ta, tb, e, out, out_lo, M, N, K, sp);
+                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp);
 }
 
 // the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT / CLIP text
@@ -459,7 +533,9 @@ cudaError_t gemm_init_device() {
     if ((e = setup_epi<EPI_BIAS_RES_SPLIT>()) != cudaSuccess) return e;
     if ((e = setup<EPI_SPLADE_MAX, 256, 6>()) != cudaSuccess) return e;
     if ((e = setup<EPI_SPLADE_MAX, 256, 3>()) != cudaSuccess) return e;
-    return setup<EPI_SPLADE_MAX, 256, 8>();
+    if ((e = setup<EPI_SPLADE_MAX, 256, 8>()) != cudaSuccess) return e;
+    if ((e = setup<EPI_ROPE_F16, 256, 6>()) != cudaSuccess) return e;
+    return setup<EPI_SWIGLU_F16, 256, 6>();
 }
 
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
@@ -494,6 +570,22 @@ cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, con
         case 8: return launch_one<EPI_SPLADE_MAX, 256, 8>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
     }
     return cudaErrorInvalidValue;
+}
+
+
+cudaError_t launch_gemm_rope(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, const GemmEpi& e, const RopeEpi& rp, int M, int N,
+                             int K, int sm_count, cudaStream_t stream, int* ctas) {
+    if (N % 256 != 0 || K != 768 || M <= 0 || sm_count < 1 || out == nullptr || e.bias == nullptr || (e.stats_in != nullptr && e.parts_in != 6))
+        return cudaErrorInvalidValue;
+    if (rp.table == nullptr || rp.S < 64 || rp.S % 64 != 0 || rp.rot_cols < 0 || rp.rot_cols % 256 != 0 || rp.rot_cols > N) return cudaErrorInvalidValue;
+    return launch_one<EPI_ROPE_F16, 256, 6>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, rp);
+}
+
+cudaError_t launch_gemm_swiglu(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, const GemmEpi& e, int M, int N, int K, int sm_count,
+                               cudaStream_t stream, int* ctas) {
+    if (N % 256 != 0 || K != 768 || M <= 0 || sm_count < 1 || out == nullptr || e.bias == nullptr || (e.stats_in != nullptr && e.parts_in != 6))
+        return cudaErrorInvalidValue;
+    return launch_one<EPI_SWIGLU_F16, 256, 6>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
 }
 
 }  // namespace b200

@@ -13,6 +13,8 @@ enum GemmEpilogue : int {
     EPI_BIAS_RES_SPLIT = 2, // y (fp16 hi + fp16 lo, in place) = acc + bias + LN(y)  (attention-out / FFN down) + row statistics
     EPI_BIAS_QGELU_F16 = 3, // out fp16 = quick_gelu(LNfold(acc) + bias), x * sigmoid(1.702 x)   (CLIP MLP up-projection)
     EPI_SPLADE_MAX = 4,     // per item and column: max over the item's valid rows of relu(LNfold(acc) + bias)   (SPLADE decoder)
+    EPI_ROPE_F16 = 5,       // out fp16 = rotary(LNfold(acc) + bias) on the Q and K columns       (nomic-bert QKV projection)
+    EPI_SWIGLU_F16 = 6,     // out fp16 [M, N/2] = silu(g) u of interleaved gate / up columns    (nomic-bert FFN up-projection)
 };
 
 // Four text geometries: bge-base (hidden 768, 12 heads of 64, inter 3072), bge-small (hidden 384, 12 heads of 32, inter 1536),
@@ -78,6 +80,24 @@ struct SpladeEpi {
 cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi& e, const SpladeEpi& sp, int M, int N, int K,
                                int sm_count, cudaStream_t stream, int* ctas = nullptr);
 
+// Rotary embedding of the QKV projection (EPI_ROPE_F16): out = fp16 [M, N] of v = LNfold(acc) + bias (e.stats_in NULL: acc +
+// bias), and on columns n < rot_cols (Q | K; a multiple of 256) the pair (d, d + 32) of every 64-column head, v_d and
+// v_{d+32}, becomes (v_d cos - v_{d+32} sin, v_{d+32} cos + v_d sin) with (cos, sin) = table[(row % S) * 32 + d] (HF's
+// rotate_half, not interleaved).  table: fp32 [>= S rows][32] float2, one row per position.  K = 768 (6 partials), N % 256 == 0.
+struct RopeEpi {
+    const float2* table;
+    int S;         // padded length of the wave's items: row r is position r % S
+    int rot_cols;  // 2 H
+};
+cudaError_t launch_gemm_rope(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, const GemmEpi& e, const RopeEpi& rp, int M, int N,
+                             int K, int sm_count, cudaStream_t stream, int* ctas = nullptr);
+
+// SwiGLU up-projection (EPI_SWIGLU_F16): W [N, K] holds gate and up rows interleaved in groups of 8 (rows 16k .. 16k+7 = gate
+// rows 8k .. 8k+7, rows 16k+8 .. 16k+15 = up rows 8k .. 8k+7); out = fp16 [M, N / 2], out[r, 8k + i] = silu(g) u with g, u the
+// LNfold(acc) + bias of W rows 16k + i and 16k + 8 + i.  K = 768 (6 partials), N % 256 == 0.
+cudaError_t launch_gemm_swiglu(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, const GemmEpi& e, int M, int N, int K, int sm_count,
+                               cudaStream_t stream, int* ctas = nullptr);
+
 // gamma != NULL: w_out[n,k] = fp16(w[n,k] gamma[k] - mean_k(w[n,:] gamma)), cvec[n] = sum_k w[n,k] beta[k] + bias[n]
 // gamma == NULL: w_out = fp16(w) (cvec untouched)
 cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, __half* w_out, float* cvec,
@@ -89,6 +109,13 @@ cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta
 // or 64B (d = 32) swizzle.  Persistent: min(units, sm_count) CTAs walk the (item, head[, query tile]) units.
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
                              cudaStream_t stream, int head_dim, int heads, bool causal);
+
+// Streaming K/V attention (nomic-bert: 12 heads of 64, no mask but the length), any S with 64 <= S <= 8192 and S % 64 == 0.
+// qkv and tq as for launch_attention (tq: 3D map over qkv {3H, S, B}, box {64, 128, 1}, 128B swizzle); ctx fp16 [B*S, 768]
+// written directly (rows past S are not written).  Persistent: min(B 12 ceil(S / 128), sm_count) CTAs walk the (item, head,
+// 128-row query tile) units; a unit reads only its item's ceil(len / 128) key tiles.  At S <= 512 the result is bit-identical
+// to launch_attention's with (64, 12).
+cudaError_t launch_attention_stream(const CUtensorMap& tq, __half* ctx, const int32_t* lens, int B, int S, int sm_count, cudaStream_t stream);
 
 // Text row kernels on rows of `width` (768, 384 or 1024; embed also 512) columns.
 // word + position + token_type embedding gather -> y = hi + lo (pre-LN residual stream) + the row's statistic partials.

@@ -18,7 +18,9 @@ BGE_LARGE_ID = "BAAI/bge-large-en-v1.5"
 
 
 MINILM_L6_ID = "sentence-transformers/all-MiniLM-L6-v2"
-POOLING_BY_MODEL_ID = {MINILM_L6_ID: "mean"}  # models whose sentence-transformers config pools other than by [CLS]
+# long-context nomic-bert encoders (kind "nomic_bert", inputs up to 8192 tokens); their sentence-transformers config pools by mean
+NOMIC_MODEL_IDS = ("nomic-ai/nomic-embed-text-v1.5", "nomic-ai/nomic-embed-text-v1")
+POOLING_BY_MODEL_ID = {MINILM_L6_ID: "mean", **{i: "mean" for i in NOMIC_MODEL_IDS}}  # models whose sentence-transformers config pools other than by [CLS]
 POOLINGS = ("cls", "mean")  # TEI also knows splade and last-token; this runtime does not
 # SPLADE encoders served offline on seeded weights (bge-base's geometry) when no masked-LM snapshot is at hand; a snapshot
 # whose config names BertForMaskedLM, or whose weights carry cls.predictions.transform, serves --pooling splade under any id
@@ -30,13 +32,15 @@ MS_MARCO_L12_ID = "cross-encoder/ms-marco-MiniLM-L-12-v2"
 def geometry_for_model_id(model_id: str) -> dict:
     """Geometry of the offline seeded fallback and of a raw --weights blob (which carries no shapes): bge-small's for
     BAAI/bge-small-en-v1.5, bge-large's for BAAI/bge-large-en-v1.5, MiniLM-L6's (bge-small's with 6 layers) for
-    sentence-transformers/all-MiniLM-L6-v2, bge-base's for BAAI/bge-base-en-v1.5 and for any id this table does not know.
-    A hub snapshot takes its geometry from its own config.json instead."""
-    from b200rt.weights import BGE_BASE_GEOMETRY, BGE_LARGE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY, MS_MARCO_MINILM_L6_GEOMETRY
+    sentence-transformers/all-MiniLM-L6-v2, nomic-embed-text's (rotary, 8192 positions) for the NOMIC_MODEL_IDS, bge-base's for
+    BAAI/bge-base-en-v1.5 and for any id this table does not know.  A hub snapshot takes its geometry from its own config.json
+    instead."""
+    from b200rt.weights import (BGE_BASE_GEOMETRY, BGE_LARGE_GEOMETRY, BGE_SMALL_GEOMETRY, MINILM_L6_GEOMETRY, MS_MARCO_MINILM_L6_GEOMETRY,
+                                NOMIC_EMBED_TEXT_GEOMETRY)
 
     known = {"BAAI/bge-base-en-v1.5": BGE_BASE_GEOMETRY, BGE_SMALL_ID: BGE_SMALL_GEOMETRY, BGE_LARGE_ID: BGE_LARGE_GEOMETRY,
              MINILM_L6_ID: MINILM_L6_GEOMETRY, MS_MARCO_L6_ID: MS_MARCO_MINILM_L6_GEOMETRY,
-             MS_MARCO_L12_ID: dict(MS_MARCO_MINILM_L6_GEOMETRY, layers=12)}
+             MS_MARCO_L12_ID: dict(MS_MARCO_MINILM_L6_GEOMETRY, layers=12), **{i: NOMIC_EMBED_TEXT_GEOMETRY for i in NOMIC_MODEL_IDS}}
     return dict(known.get(model_id, BGE_BASE_GEOMETRY))
 
 
@@ -193,16 +197,22 @@ def load_weights(args):
                 return W.load_hf_classifier(sd, cfg) + (f"safetensors {args.weights}",)
             return W.load_safetensors(args.weights) + (f"safetensors {args.weights}",)
         if os.path.isdir(args.weights):
+            if W.is_nomic_dir(args.weights):
+                return W.load_hf_nomic_dir(args.weights) + (f"nomic-bert directory {args.weights}",)
             return W.load_hf_dir(args.weights) + (f"HF directory {args.weights}",)
         return geometry_for_model_id(args.model_id), np.fromfile(args.weights, np.float32), f"flat blob {args.weights}"
     cache = args.huggingface_hub_cache or os.environ.get("HUGGINGFACE_HUB_CACHE") or os.environ.get("HF_HUB_CACHE")
     if cache:
         snap = W.resolve_hub_snapshot(cache, args.model_id)
         if snap:
+            if W.is_nomic_dir(snap):
+                return W.load_hf_nomic_dir(snap) + (f"nomic-bert hub snapshot {snap}",)
             return W.load_hf_dir(snap) + (f"hub snapshot {snap}",)
     g = geometry_for_model_id(args.model_id)
     if "num_labels" in g:
         return g, W.random_classifier_blob(g, 0), None
+    if "rope_theta" in g:
+        return g, W.random_nomic_blob(g, 0), None
     return g, random_blob(geometry=g), None
 
 
@@ -261,6 +271,10 @@ class Engine:
             print("[text-embeddings-router/b200] SPLADE: BertForMaskedLM, sparse vectors over the vocabulary through /embed_sparse"
                   + (" -- SEEDED weights, vectors are not the real model's" if source is None else ""), file=sys.stderr)
             self.model = b200rt.SparseEmbedModel(geometry, blob)
+        elif self.long_context:
+            print(f"[text-embeddings-router/b200] nomic-bert: rotary positions, inputs up to {geometry['max_pos']} tokens"
+                  + (" -- SEEDED weights, vectors are not the real model's" if source is None else ""), file=sys.stderr)
+            self.model = b200rt.NomicEmbedModel(geometry, blob, pooling=self.pooling)
         else:
             self.model = b200rt.EmbedModel(geometry, blob, pooling=self.pooling)
         self.n_gpus = n_gpus
@@ -293,11 +307,17 @@ class Engine:
             ids[i, : len(r)] = r
         return self.model.classify(ids, lens, np.array(segs, np.int32))
 
+    @property
+    def long_context(self) -> bool:
+        """A nomic-bert model (kind "nomic_bert"): inputs up to its max_pos, up to 8192 tokens."""
+        return "rope_theta" in self.geometry
+
     def info(self) -> dict:
         """TEI's /info.  An embedding model's is what it always was; a classifier's reports model_type as TEI does."""
         args = self.args
         d = {"model_id": args.model_id, "model_dtype": "float16", "max_client_batch_size": args.max_client_batch_size,
-             "max_input_length": GEOMETRY["max_pos"], "backend": f"b200rt x{self.n_gpus}"}
+             "max_input_length": self.geometry["max_pos"] if self.long_context else GEOMETRY["max_pos"],
+             "backend": f"b200rt x{self.n_gpus}"}
         if not self.classifier:
             d["pooling"] = self.pooling
             return d
@@ -359,7 +379,9 @@ def make_handler(engine: Engine):
                     inputs = [inputs]
                 if not isinstance(inputs, list) or not inputs or not all(isinstance(t, str) for t in inputs):
                     raise TypeError("`inputs` must be a string or a non-empty list of strings")
-                truncate = bool(req.get("truncate", False)) if sparse else False
+                # TEI's `truncate`: honoured by /embed_sparse and by the long-context kind; other models' /embed answers stay as
+                # they were (413 past max_pos unless --auto-truncate)
+                truncate = bool(req.get("truncate", False)) if sparse or engine.long_context else False
             except Exception as e:  # noqa: BLE001
                 return self._send(422, {"error": f"Failed to deserialize the JSON body: {e}", "error_type": "Validation"})
             if len(inputs) > engine.args.max_client_batch_size:
