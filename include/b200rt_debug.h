@@ -82,23 +82,24 @@ int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* g
  *                   t < lens[i] (clamped to [0, S]), of rstd_r (a_r . w_n) + c[n]) for n < vocab, 0 for n >= vocab.  a fp16
  *                   [B S, K], w fp16 [vocab, K] (rows past vocab read as zeros), c fp32 [N], stats (sum, M2) [B S, K / 128],
  *                   vmax_out uint32 [B, N]; K = 768, 384 or 1024, N % 256 == 0, S % 64 == 0.  iters launches are timed into ms_out
- *                   (optional); the maxima come from one more launch on a zeroed buffer.  sms as for b200rt_debug_gemm: the result
- *                   must not depend on it.
+ *                   (optional); the maxima come from one more launch on a zeroed buffer.  sms and ctas_out (optional, the CTAs
+ *                   of that launch) as for b200rt_debug_gemm: the result must not depend on sms.
  *   mlm_ln_stats:   stats_out [n_rows, hidden / 128] (sum, M2) partials of the fp16 rows u [n_rows, hidden]; vmax_out [n_max]
  *                   is poisoned (0xFF) and comes back as the kernel leaves it (zeroed).
  *   splade_finalize: out[i, v] = log1p(fp32 bits vmax[i, v]) for v < vocab, vmax uint32 [n_items, vpad], out [n_items, vocab]. */
 int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const int32_t* lens, int B, int S,
-                             int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out);
+                             int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out, int* ctas_out);
 /* nomic-bert kernels (kernels.h: launch_gemm_rope, launch_gemm_swiglu, launch_attention_stream), one launch each behind host
  * buffers.  gemm_rope: a [M,768] fp16, w [N,768] fp16, c [N], stats [M][6] (NULL: plain acc + c), table float (cos, sin) pairs
  * [n_pos][32] with n_pos >= S, S % 64 == 0, rot_cols a multiple of 256 <= N; out fp16 [M, N].  gemm_swiglu: w [N,768] with
  * gate / up rows interleaved in groups of 8, out fp16 [M, N / 2].  attention_stream: qkv fp16 [B*S, 2304], 64 <= S <= 8192,
  * S % 64 == 0, ctx fp16 [B*S, 768]; ms_out (may be NULL) the mean time of `iters` further launches.  sms: the most CTAs of
- * the persistent launch (0 = every SM).                                                                                   */
+ * the persistent launch (0 = every SM); for the two GEMMs, as for b200rt_debug_gemm, with ctas_out (optional) receiving
+ * the number of CTAs launched.                                                                                             */
 int b200rt_debug_gemm_rope(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const float* table, int n_pos, int M,
-                           int N, int S, int rot_cols, float eps, int sms, uint16_t* out);
+                           int N, int S, int rot_cols, float eps, int sms, uint16_t* out, int* ctas_out);
 int b200rt_debug_gemm_swiglu(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, int M, int N, float eps, int sms,
-                             uint16_t* out);
+                             uint16_t* out, int* ctas_out);
 int b200rt_debug_attention_stream(const uint16_t* qkv, const int32_t* lens, int B, int S, uint16_t* ctx, int sms, int iters, float* ms_out);
 int b200rt_debug_mlm_ln_stats(const uint16_t* u, int n_rows, int hidden, size_t n_max, uint32_t* vmax_out, float* stats_out);
 int b200rt_debug_splade_finalize(const uint32_t* vmax, int n_items, int vpad, int vocab, float* out);

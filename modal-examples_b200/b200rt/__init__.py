@@ -145,11 +145,11 @@ def load_library():
         lib.b200rt_debug_forward_trace.argtypes = [ci, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_vit_forward_trace.argtypes = [ci, vp, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
         lib.b200rt_debug_forward_trace_segs.argtypes = [ci, vp, vp, vp, ci, ci, ci] + [vp] * 8 + [ctypes.c_char_p, ctypes.c_size_t, i32p]
-        lib.b200rt_debug_gemm_splade.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, ci, f32p, vp]
+        lib.b200rt_debug_gemm_splade.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, ci, f32p, vp, i32p]
         lib.b200rt_debug_mlm_ln_stats.argtypes = [vp, ci, ci, ctypes.c_size_t, vp, vp]
         lib.b200rt_debug_splade_finalize.argtypes = [vp, ci, ci, ci, vp]
-        lib.b200rt_debug_gemm_rope.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, vp]
-        lib.b200rt_debug_gemm_swiglu.argtypes = [vp] * 4 + [ci, ci, cf, ci, vp]
+        lib.b200rt_debug_gemm_rope.argtypes = [vp] * 5 + [ci] * 5 + [cf, ci, vp, i32p]
+        lib.b200rt_debug_gemm_swiglu.argtypes = [vp] * 4 + [ci, ci, cf, ci, vp, i32p]
         lib.b200rt_debug_attention_stream.argtypes = [vp, vp, ci, ci, vp, ci, ci, f32p]
         lib.b200rt_debug_profile_forward.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                      f32p, i32p, ctypes.c_int]
@@ -777,9 +777,11 @@ def debug_fold_ln(w: np.ndarray, gamma=None, beta=None, bias=None):
     return w_out, cvec
 
 
-def debug_gemm_splade(a16: np.ndarray, w16: np.ndarray, c, stats, lens, S: int, N: int, eps: float, sms: int = 0, iters: int = 1):
+def debug_gemm_splade(a16: np.ndarray, w16: np.ndarray, c, stats, lens, S: int, N: int, eps: float, sms: int = 0, iters: int = 1,
+                      want_ctas: bool = False):
     """The SPLADE decoder GEMM (b200rt_debug_gemm_splade): a16 [B S, K], w16 [vocab, K] float16, c [N], stats [B S, K / 128, 2],
-    lens [B]; returns (uint32 maxima [B, N] -- the fp32 bits of max(0, max over item i's valid rows) --, ms per launch)."""
+    lens [B]; returns (uint32 maxima [B, N] -- the fp32 bits of max(0, max over item i's valid rows) --, ms per launch), and
+    with ``want_ctas`` the number of CTAs launched appended."""
     a16 = np.ascontiguousarray(a16, dtype=np.float16)
     w16 = np.ascontiguousarray(w16, dtype=np.float16)
     lens = np.ascontiguousarray(lens, dtype=np.int32)
@@ -787,9 +789,10 @@ def debug_gemm_splade(a16: np.ndarray, w16: np.ndarray, c, stats, lens, S: int, 
     B, K, vocab = len(lens), a16.shape[1], w16.shape[0]
     out = np.empty((B, N), np.uint32)
     ms = ctypes.c_float(0)
+    ctas = ctypes.c_int(0)
     _check(load_library().b200rt_debug_gemm_splade(_ptr(a16), _ptr(w16), _ptr(c), _ptr(stats), _ptr(lens), B, S, N, K, vocab,
-                                                   eps, sms, iters, ctypes.byref(ms), _ptr(out)))
-    return out, ms.value
+                                                   eps, sms, iters, ctypes.byref(ms), _ptr(out), ctypes.byref(ctas)))
+    return (out, ms.value, ctas.value) if want_ctas else (out, ms.value)
 
 
 def debug_mlm_ln_stats(u16: np.ndarray, n_max: int = 0):
@@ -811,32 +814,35 @@ def debug_splade_finalize(vmax: np.ndarray, vocab: int) -> np.ndarray:
     return out
 
 
-def debug_gemm_rope(a16: np.ndarray, w16: np.ndarray, c, stats, table: np.ndarray, S: int, rot_cols: int, eps: float, sms: int = 0):
+def debug_gemm_rope(a16: np.ndarray, w16: np.ndarray, c, stats, table: np.ndarray, S: int, rot_cols: int, eps: float, sms: int = 0,
+                    want_ctas: bool = False):
     """nomic-bert's QKV epilogue (b200rt_debug_gemm_rope): a16 [M, 768], w16 [N, 768] float16, c [N], stats [M, 6, 2] or None,
-    table float32 [n_pos, 32, 2] (cos, sin); returns out float16 [M, N]."""
+    table float32 [n_pos, 32, 2] (cos, sin); returns out float16 [M, N], or (out, CTAs launched) with ``want_ctas``."""
     a16 = np.ascontiguousarray(a16, dtype=np.float16)
     w16 = np.ascontiguousarray(w16, dtype=np.float16)
     M, N = a16.shape[0], w16.shape[0]
     c, table = _f32(c), _f32(table)
     st = _f32(stats) if stats is not None else None
     out = np.empty((M, N), np.float16)
+    ctas = ctypes.c_int(0)
     _check(load_library().b200rt_debug_gemm_rope(_ptr(a16), _ptr(w16), _ptr(c), _ptr(st) if st is not None else None, _ptr(table),
-                                                 table.shape[0], M, N, S, rot_cols, eps, sms, _ptr(out)))
-    return out
+                                                 table.shape[0], M, N, S, rot_cols, eps, sms, _ptr(out), ctypes.byref(ctas)))
+    return (out, ctas.value) if want_ctas else out
 
 
-def debug_gemm_swiglu(a16: np.ndarray, w16: np.ndarray, c, stats, eps: float, sms: int = 0):
+def debug_gemm_swiglu(a16: np.ndarray, w16: np.ndarray, c, stats, eps: float, sms: int = 0, want_ctas: bool = False):
     """nomic-bert's FFN1 epilogue (b200rt_debug_gemm_swiglu): w16 [N, 768] with gate / up rows interleaved in groups of 8, c [N];
-    returns out float16 [M, N / 2] = silu(g) u."""
+    returns out float16 [M, N / 2] = silu(g) u, or (out, CTAs launched) with ``want_ctas``."""
     a16 = np.ascontiguousarray(a16, dtype=np.float16)
     w16 = np.ascontiguousarray(w16, dtype=np.float16)
     M, N = a16.shape[0], w16.shape[0]
     c = _f32(c)
     st = _f32(stats) if stats is not None else None
     out = np.empty((M, N // 2), np.float16)
+    ctas = ctypes.c_int(0)
     _check(load_library().b200rt_debug_gemm_swiglu(_ptr(a16), _ptr(w16), _ptr(c), _ptr(st) if st is not None else None, M, N, eps, sms,
-                                                   _ptr(out)))
-    return out
+                                                   _ptr(out), ctypes.byref(ctas)))
+    return (out, ctas.value) if want_ctas else out
 
 
 def debug_attention_stream(qkv16: np.ndarray, lens, B: int, S: int, sms: int = 0, iters: int = 0):

@@ -2394,7 +2394,7 @@ int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* g
 }
 
 int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const int32_t* lens, int B, int S,
-                             int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out) {
+                             int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out, int* ctas_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!a || !w || !c || !stats || !lens || !vmax_out || B < 1 || S < 64 || S % 64 || N % 256 || vocab < 1 || vocab > N)
@@ -2432,7 +2432,7 @@ int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* 
     for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute));
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(cudaMemsetAsync(dmax, 0, nmax * 4, d.compute));  // the returned maxima come from one launch on a zeroed buffer
-    CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute));
+    CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute, ctas_out));
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
@@ -2442,7 +2442,7 @@ int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* 
 }
 
 int b200rt_debug_gemm_rope(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const float* table, int n_pos, int M,
-                           int N, int S, int rot_cols, float eps, int sms, uint16_t* out) {
+                           int N, int S, int rot_cols, float eps, int sms, uint16_t* out, int* ctas_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!a || !w || !c || !table || !out || M < 1 || N < 256 || N % 256 || S < 64 || S % 64 || n_pos < S || rot_cols < 0 || rot_cols % 256 ||
@@ -2471,13 +2471,13 @@ int b200rt_debug_gemm_rope(const uint16_t* a, const uint16_t* w, const float* c,
     if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
     const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
     CUDA_TRY(launch_gemm_rope(ta, tb, dout, e, RopeEpi{reinterpret_cast<const float2*>(dt), S, rot_cols}, M, N, static_cast<int>(K),
-                              sms ? sms : d.sm_count, d.compute));
+                              sms ? sms : d.sm_count, d.compute, ctas_out));
     CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * N * 2));
     return 0;
 }
 
 int b200rt_debug_gemm_swiglu(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, int M, int N, float eps, int sms,
-                             uint16_t* out) {
+                             uint16_t* out, int* ctas_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     if (!a || !w || !c || !out || M < 1 || N < 256 || N % 256) return fail(B200RT_E_INVALID, "bad gemm_swiglu arguments (N a multiple of 256)");
@@ -2502,7 +2502,7 @@ int b200rt_debug_gemm_swiglu(const uint16_t* a, const uint16_t* w, const float* 
     if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
     if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
     const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
-    CUDA_TRY(launch_gemm_swiglu(ta, tb, dout, e, M, N, static_cast<int>(K), sms ? sms : d.sm_count, d.compute));
+    CUDA_TRY(launch_gemm_swiglu(ta, tb, dout, e, M, N, static_cast<int>(K), sms ? sms : d.sm_count, d.compute, ctas_out));
     CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * No * 2));
     return 0;
 }

@@ -6,11 +6,18 @@ of tests/kernel_refs.py at their tolerances:
     pairs to walk and on every SM, for every epilogue, at both tile widths;
   * many pairs per cluster, so that the ring phases of both CTAs cross tile boundaries in step;
   * launch widths that are not whole clusters, and the split-SM runtime at an odd SM split.
+
+The same three for the epilogues nomic-bert and SPLADE added -- the rotary QKV GEMM (tests/nomic_refs.rope_gemm_ref), the
+SwiGLU FFN1 GEMM (nomic_refs.swiglu_gemm_ref) and the SPLADE vocabulary max (tests/splade_refs.check_gemm_splade) -- with the
+split runtime's GEMM widths among the launch widths: SPLIT_SMS(k) gives GEMMs 132 - k SMs (21: 111, 66: 66) and attention k.
+Their debug entries report the CTAs they launched, so each case asserts the cluster shape it sets out to test.
 """
 import numpy as np
 import pytest
 
 import kernel_refs as KR
+import nomic_refs as NR
+import splade_refs as SR
 
 gpu = pytest.mark.gpu
 
@@ -57,7 +64,7 @@ def _run(rt, epi, args, kw, want_stats, sms=0):
 
 
 def _bits(x):
-    return x.view(np.uint32 if x.dtype == np.float32 else np.uint16)
+    return x.view(np.uint16 if x.dtype == np.float16 else np.uint32)
 
 
 def _same(a, b):
@@ -149,3 +156,164 @@ def test_split_sm_runtime_odd_split(rt):
     same = np.array_equal(whole.view(np.uint32), split.view(np.uint32))
     print(f"split SMs k=21: ragged text ({whole.shape[0]} items) bitwise equal to the whole-GPU runtime: {same}")
     assert same
+
+
+# ------------------------------------------------------------------------------------------------ rotary, SwiGLU, SPLADE
+#
+# Each case is (run, check): run(rt, sms) -> (out, ctas) through the debug entry, check(tag, out) -> the worst err/tol against
+# the fp64 reference at its tolerance.
+
+def _nomic_stats(rng, M):
+    """(sum, M2) partials of random 768-wide rows of mean ~0.3, sd ~1.5."""
+    return KR.partials(rng.standard_normal((M, 768)) * 1.5 + 0.3).astype(np.float32)
+
+
+def _rope_case(M, S, ln, seed):
+    """QKV of nomic-bert: N = 2304, the first rot_cols = 1536 columns (Q and K) rotated by position row % S, V not."""
+    rng = np.random.default_rng(seed)
+    a = (rng.standard_normal((M, 768)) * 1.2).astype(np.float16)
+    w = (rng.standard_normal((2304, 768)) * 0.05).astype(np.float16)
+    c = (rng.standard_normal(2304) * 0.1).astype(np.float32)
+    st = _nomic_stats(rng, M) if ln else None
+    table = NR.rope_table(S, 1000.0)
+
+    def run(rt, sms):
+        return rt.debug_gemm_rope(a, w, c, st, table, S, 1536, 1e-12, sms=sms, want_ctas=True)
+
+    def check(tag, out):
+        ref, tol = NR.rope_gemm_ref(a, w, c, st, table, S, 1536, 1e-12, pos=np.arange(M) % S)
+        return KR.check(tag, out.astype(np.float64), ref, tol)
+    return run, check
+
+
+def _swiglu_case(M, ln, seed):
+    """FFN1 of nomic-bert: gate and up (3072 rows each) interleaved in groups of 8, N = 6144, out [M, 3072]."""
+    rng = np.random.default_rng(seed)
+    a = (rng.standard_normal((M, 768)) * 1.2).astype(np.float16)
+    w = NR.interleave_rows(rng.standard_normal((3072, 768)) * 0.05, rng.standard_normal((3072, 768)) * 0.05).astype(np.float16)
+    c = (NR.interleave_rows(rng.standard_normal((3072, 1)), rng.standard_normal((3072, 1)))[:, 0] * 0.3).astype(np.float32)
+    st = _nomic_stats(rng, M) if ln else None
+
+    def run(rt, sms):
+        return rt.debug_gemm_swiglu(a, w, c, st, 1e-12, sms=sms, want_ctas=True)
+
+    def check(tag, out):
+        ref, tol = NR.swiglu_gemm_ref(a, w, c, st, 1e-12)
+        return KR.check(tag, out.astype(np.float64), ref, tol)
+    return run, check
+
+
+def _splade_lens(B, S, rng):
+    """Ragged lengths: S, 1, the 63 / 64 / 65 edges (65 clamps to S when S = 64), S - 1, then random."""
+    edges = np.array([S, 1, 63, 64, 65, S - 1], np.int32)
+    return np.concatenate([edges, rng.integers(1, S + 1, max(0, B - len(edges)))]).astype(np.int32)[:B]
+
+
+def _splade_case(B, S, K, vocab, seed):
+    """The decoder GEMM of B items of S rows: K = 384 / 768 / 1024 (PARTS 3 / 6 / 8), N = vocab tiled to 256.  Operands as
+    tests/test_gpu_splade.py's: ~60 % of the logits positive, a fifth of the columns' c so negative that they stay 0."""
+    rng = np.random.default_rng(seed)
+    lens = _splade_lens(B, S, rng)
+    x = rng.standard_normal((B * S, K))
+    u = (x * (x > -0.5) * 1.3 + 0.2 * rng.standard_normal(K)).astype(np.float16)
+    stats = KR.partials(u.astype(np.float64)).astype(np.float32)
+    w = (rng.standard_normal((vocab, K)) * (1.0 / np.sqrt(K))).astype(np.float16)
+    N = SR.vpad(vocab)
+    c = (rng.standard_normal(N) - 1.0).astype(np.float32)
+    c[rng.random(N) < 0.2] = -20.0
+
+    def run(rt, sms):
+        out, _, ctas = rt.debug_gemm_splade(u, w, c, stats, lens, S, N, 1e-12, sms=sms, want_ctas=True)
+        return out, ctas
+
+    def check(tag, out):
+        return SR.check_gemm_splade(tag, out, u, w, c, stats, lens, S, 1e-12)
+    return run, check
+
+
+def _bm_tiles(M):
+    return (M + 127) // 128
+
+
+# rotary: M = B S with an odd m-tile count or a partial last tile.  S = 64 puts two items in a 128-row tile; S = 192 never
+# splits a 64-row half across items.  M = 64, 192, 576 and 8256 (1, 2 -- the second partial --, 5 and 65 m-tiles).
+ROPE_PAST_M = [(B, S) for S, Bs in ((64, (1, 3, 129)), (192, (1, 3, 43))) for B in Bs]
+# SPLADE: (B, S, vocab).  30522 words (the last 256-column tile partial) at S = 64; elsewhere a narrower vocabulary, still
+# ending in a partial tile, keeps the fp64 reference's [B S, vocab] logits small.
+SPLADE_PAST_M = [(1, 64, 30522), (3, 64, 30522), (129, 64, 2000), (3, 192, 2000)]
+
+
+def _past_m(rt, tag, run, check):
+    one, ctas = run(rt, 2)
+    assert ctas == 2, ctas
+    margin = check(f"{tag} sms 2", one)
+    every, _ = run(rt, 0)
+    same = _same(every, one)
+    print(f"{tag}: sms 2 (worst err/tol {margin:.3f}) bitwise equal to every SM: {same}")
+    assert same
+
+
+@gpu
+@pytest.mark.parametrize("ln", [True, False])
+@pytest.mark.parametrize("B,S", ROPE_PAST_M)
+def test_rope_partner_tile_past_m(rt, B, S, ln):
+    M = B * S
+    run, check = _rope_case(M, S, ln, seed=M + S + ln)
+    _past_m(rt, f"rope M={M} S={S} ({_bm_tiles(M)} m-tiles) ln={ln}", run, check)
+
+
+@gpu
+@pytest.mark.parametrize("ln", [True, False])
+@pytest.mark.parametrize("M", [1, 129, 257, 8320])
+def test_swiglu_partner_tile_past_m(rt, M, ln):
+    run, check = _swiglu_case(M, ln, seed=M + 7 * ln)
+    _past_m(rt, f"swiglu M={M} ({_bm_tiles(M)} m-tiles) ln={ln}", run, check)
+
+
+@gpu
+@pytest.mark.parametrize("K", [384, 768, 1024])
+@pytest.mark.parametrize("B,S,vocab", SPLADE_PAST_M)
+def test_splade_partner_tile_past_m(rt, B, S, vocab, K):
+    """The maxima are an integer max of fp32 bits (order-independent), so any bitwise difference is a real bug."""
+    run, check = _splade_case(B, S, K, vocab, seed=B * S + K)
+    _past_m(rt, f"splade K={K} B={B} S={S} vocab={vocab} ({_bm_tiles(B * S)} m-tiles)", run, check)
+
+
+# M = 4096: 16 m-tile pairs.  rotary: 9 n-tiles, 144 pairs; SwiGLU: 24 n-tiles, 384 pairs; SPLADE: 8 items of 512 (each over
+# 4 m-tiles, so an item's maxima merge across tiles and both CTAs), vocabulary 4000 -> 16 n-tiles, 256 pairs.
+NEW_EPILOGUES = {
+    "rope": lambda M: _rope_case(M, 64 if M % 512 else 512, True, seed=M),
+    "swiglu": lambda M: _swiglu_case(M, True, seed=M + 1),
+    "splade": lambda M: _splade_case(M // 512 if M % 512 == 0 else M // 64, 512 if M % 512 == 0 else 64, 768, 4000, seed=M + 2),
+}
+
+
+@gpu
+@pytest.mark.parametrize("epi", list(NEW_EPILOGUES))
+def test_new_epilogues_many_pairs_per_cluster(rt, epi):
+    """Every pair of M = 4096 walked by one cluster (sms = 2), bitwise the launch on every SM; the reference once, on every SM."""
+    run, check = NEW_EPILOGUES[epi](4096)
+    base, ctas = run(rt, 0)
+    assert ctas % 2 == 0 and ctas > 2, ctas
+    margin = check(f"{epi} M=4096 every SM ({ctas} CTAs)", base)
+    one, one_ctas = run(rt, 2)
+    assert one_ctas == 2, one_ctas
+    same = _same(one, base)
+    print(f"{epi} M=4096: one cluster bitwise equal to {ctas} CTAs: {same} (worst err/tol {margin:.3f})")
+    assert same
+
+
+@gpu
+@pytest.mark.parametrize("epi", list(NEW_EPILOGUES))
+def test_new_epilogues_widths_that_are_not_whole_clusters(rt, epi):
+    """sms = 1, 3, 131 (not whole clusters) and 21, 66, 111 (the split runtime's attention and GEMM widths), each bitwise the
+    launch on every SM.  M = 4160 (33 m-tiles: the last pair's second tile past M); SPLADE: 65 items of 64."""
+    run, check = NEW_EPILOGUES[epi](4160)
+    base, base_ctas = run(rt, 0)
+    check(f"{epi} M=4160 every SM ({base_ctas} CTAs)", base)
+    for sms in (1, 3, 21, 66, 111, 131):
+        got, ctas = run(rt, sms)
+        assert ctas % 2 == 0 and 2 <= ctas <= max(2, sms), (sms, ctas)
+        same = _same(got, base)
+        print(f"{epi} M=4160: sms {sms} -> {ctas} CTAs, bitwise equal to every SM: {same}")
+        assert same, sms

@@ -4,7 +4,8 @@ oracle up to 8192 tokens, and bitwise invariance of an item's embedding.
   * kernels through the debug entries against their fp64 references (tests/nomic_refs.py): the rotary QKV GEMM and the SwiGLU
     GEMM for M from 1 to past a 128-row tile at several S; the streaming attention for S in {64, 576, 1024, 2048, 4096, 8192}
     with lengths on every tile boundary, one valid key and Q = 0;
-  * the streaming attention is bitwise the same on 1 and every SM, and bitwise attention_kernel<64, 12>'s for every S <= 512;
+  * the streaming attention is bitwise the same at every launch width from 1 CTA to every SM (many units per CTA, and fewer
+    units than CTAs), and bitwise attention_kernel<64, 12>'s for every S <= 512;
   * the forward launch by launch through run_chain (tests/test_gpu_forward_chain.py) with NomicChain, a TextChain for the
     kind's launches, on toy ragged batches and on a full wave of 8 x 8192 tokens (a row sample after
     tests/test_gpu_full_wave_chain.py's);
@@ -141,6 +142,98 @@ def test_attention_stream_grid_invariance(rt, S, lens):
     b, _ = rt.debug_attention_stream(qkv, l, len(lens), S, sms=0)
     c, _ = rt.debug_attention_stream(qkv, l, len(lens), S, sms=7)
     assert (_bits(a) == _bits(b)).all() and (_bits(a) == _bits(c)).all()
+
+
+# ---- the streaming kernel at every launch width the runtime uses
+#
+# A CTA walks units u = blockIdx.x, + gridDim.x, ... (grid = min(units, sms)); each unit pushes its item's ceil(len / 128)
+# key tiles through a 4-stage K/V ring whose phase bit flips on every wrap, and the ring carries over from one unit to the
+# next.  On one CTA every item starts at stage 0, because its 12 nq units are a multiple of 4: only odd tile counts, and
+# widths other than 1, move the stage a unit starts at.  stream_walk restates that walk (attention_sm90.cu,
+# attention_stream_kernel's producer loop), and test_stream_walk_covers_the_ring checks that the cases below start units at
+# every stage on both phases, wrap the ring inside a unit and change the tile count between a CTA's consecutive units.
+
+STREAM_NSTAGE = 4
+H100_SMS = 132
+
+
+def stream_walk(lens, S, sms):
+    """Per CTA, the units it walks in order, as (unit, key tiles, ring stage and phase the unit starts at)."""
+    nq = (S + 127) // 128
+    n_units = len(lens) * 12 * nq
+    grid = min(n_units, sms or H100_SMS)
+    walks = []
+    for cta in range(grid):
+        stage, phase, walk = 0, 0, []
+        for u in range(cta, n_units, grid):
+            tiles = (min(max(int(lens[u // nq // 12]), 1), S) + 127) // 128
+            walk.append((u, tiles, stage, phase))
+            stage += tiles
+            phase ^= (stage // STREAM_NSTAGE) & 1
+            stage %= STREAM_NSTAGE
+        walks.append(walk)
+    return walks
+
+
+# many units per CTA: 8 items of 1024 tokens, key tiles 1, 2, 3, 4, 5, 6, 8, 8
+STREAM_MANY = (1024, [1, 129, 300, 385, 640, 700, 897, 1024])
+STREAM_MANY_SMS = (1, 2, 3, 5, 12, 13, 21, 66, 111, 131)
+# fewer units than CTAs: 12 and 24 units
+STREAM_FEW = [(128, [128]), (256, [200])]
+STREAM_FEW_SMS = (0, 13, 23, 25)
+
+
+def _stream_cases():
+    yield from ((STREAM_MANY[0], STREAM_MANY[1], sms) for sms in (0,) + STREAM_MANY_SMS)
+    yield from ((S, lens, sms) for S, lens in STREAM_FEW for sms in STREAM_FEW_SMS)
+
+
+def test_stream_walk_covers_the_ring():
+    starts, wraps, changes = set(), False, False
+    for S, lens, sms in _stream_cases():
+        for walk in stream_walk(lens, S, sms):
+            for i, (u, tiles, stage, phase) in enumerate(walk):
+                starts.add((stage, phase))
+                wraps |= tiles == 3 and stage >= 2
+                changes |= i > 0 and walk[i - 1][1] != tiles
+    assert starts == {(st, ph) for st in range(STREAM_NSTAGE) for ph in (0, 1)}, starts
+    assert wraps and changes
+    # on one CTA every item's first unit starts at stage 0
+    walk = stream_walk(STREAM_MANY[1], STREAM_MANY[0], 1)[0]
+    assert {stage for u, _, stage, _ in walk if u % (12 * 8) == 0} == {0}
+
+
+@gpu
+def test_attention_stream_many_units_per_cta(rt):
+    """Every row of the 8 items on every SM against the fp64 reference; then bitwise the same at the widths of
+    STREAM_MANY_SMS, 1 (all 768 units on one CTA) to 131, the split runtime's 21 and 66 among them."""
+    S, lens = STREAM_MANY
+    B = len(lens)
+    qkv = N.synth_qkv(B, S, 17, q_scale=0.5)
+    l = np.array(lens, np.int32)
+    base, _ = rt.debug_attention_stream(qkv, l, B, S)
+    ref, tol = N.attention_rows_ref(qkv, lens, B, S, np.arange(S))
+    KR.check(f"attention_stream S={S} lens={lens} every SM", base.reshape(B, S, 768).astype(np.float64), ref, tol)
+    for sms in STREAM_MANY_SMS:
+        got, _ = rt.debug_attention_stream(qkv, l, B, S, sms=sms)
+        same = (_bits(got) == _bits(base)).all()
+        print(f"attention_stream S={S}: sms {sms} ({min(sms, B * 12 * 8)} CTAs) bitwise equal to every SM: {same}")
+        assert same, sms
+
+
+@gpu
+@pytest.mark.parametrize("S,lens", STREAM_FEW)
+def test_attention_stream_fewer_units_than_ctas(rt, S, lens):
+    B = len(lens)
+    qkv = N.synth_qkv(B, S, S + 3, q_scale=0.5)
+    l = np.array(lens, np.int32)
+    ref, tol = N.attention_rows_ref(qkv, lens, B, S, np.arange(S))
+    first = None
+    for sms in STREAM_FEW_SMS:
+        got, _ = rt.debug_attention_stream(qkv, l, B, S, sms=sms)
+        KR.check(f"attention_stream S={S} lens={lens} sms {sms}", got.reshape(B, S, 768).astype(np.float64), ref, tol)
+        first = got if first is None else first
+        assert (_bits(got) == _bits(first)).all(), sms
 
 
 @gpu
