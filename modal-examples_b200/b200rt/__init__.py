@@ -278,26 +278,37 @@ LOAD_POOL_MEAN = 1
 POOLINGS = ("cls", "mean")
 
 
+def _pool_flags(pooling: str) -> int:
+    """The load flags of a text encoder's ``pooling``."""
+    if pooling not in POOLINGS:
+        raise B200RTError(E_INVALID, f"pooling must be one of {POOLINGS}, got {pooling!r}")
+    return LOAD_POOL_MEAN if pooling == "mean" else 0
+
+
+def _load(model, kind: bytes, cfg, blob: np.ndarray, flags: int = 0):
+    """b200rt_model_load_ex of ``blob`` as a model of ``kind``; gives ``model`` its ``cfg``, ``handle`` and the library it calls."""
+    lib = load_library()
+    blob = np.ascontiguousarray(blob, dtype=np.float32)
+    h = ctypes.c_int32(-1)
+    _check(lib.b200rt_model_load_ex(kind, ctypes.byref(cfg), _ptr(blob), blob.nbytes, flags, ctypes.byref(h)))
+    model.cfg, model.handle, model._lib = cfg, h.value, lib
+
+
+def _bert_config(g: dict) -> BertConfig:
+    return BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"], g["eps"])
+
+
 class EmbedModel:
     """A loaded BERT-geometry encoder; ``submit``/``wait``/``poll_any`` are the .map() primitives.
     ``pooling``: "cls" (the [CLS] row: bge) or "mean" (the mean of the valid tokens' final hidden states, as
     sentence-transformers' Pooling(mean) computes it: all-MiniLM-L6-v2, e5, gte); either way the result is L2-normalised."""
 
     def __init__(self, geometry: dict, blob: np.ndarray, pooling: str = "cls"):
-        if pooling not in POOLINGS:
-            raise B200RTError(E_INVALID, f"pooling must be one of {POOLINGS}, got {pooling!r}")
-        lib = load_library()
-        blob = np.ascontiguousarray(blob, dtype=np.float32)
-        self.cfg = BertConfig(geometry["vocab"], geometry["hidden"], geometry["layers"], geometry["heads"], geometry["inter"],
-                              geometry["max_pos"], geometry["type_vocab"], geometry["eps"])
-        self.hidden, self.inter = geometry["hidden"], geometry["inter"]
+        g = geometry
+        self.hidden, self.inter = g["hidden"], g["inter"]
         self.out_dim = self.hidden
         self.pooling = pooling
-        h = ctypes.c_int32(-1)
-        flags = LOAD_POOL_MEAN if pooling == "mean" else 0
-        _check(lib.b200rt_model_load_ex(b"bert", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, flags, ctypes.byref(h)))
-        self.handle = h.value
-        self._lib = lib
+        _load(self, b"bert", _bert_config(g), blob, _pool_flags(pooling))
 
     def submit(self, ids: np.ndarray, lens=None, out: np.ndarray | None = None, tag=None, borrow_ids: bool = False) -> Ticket:
         """``borrow_ids``: the caller promises not to touch ``ids`` until the ticket completes; the library then takes
@@ -406,17 +417,12 @@ class ClipTextModel(EmbedModel):
     Token ids come from infinity_emb.clip_tokenizer (``<|startoftext|>`` ... ``<|endoftext|>``, at most ``max_pos``)."""
 
     def __init__(self, geometry: dict, blob: np.ndarray):
-        lib = load_library()
-        blob = np.ascontiguousarray(blob, dtype=np.float32)
         g = geometry
-        self.cfg = ClipTextConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["proj"], g["eos_id"], g["eps"])
         self.hidden, self.inter, self.proj = g["hidden"], g["inter"], g["proj"]
         self.out_dim = self.proj
         self.pooling = "eos"
-        h = ctypes.c_int32(-1)
-        _check(lib.b200rt_model_load(b"clip_text", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
-        self.handle = h.value
-        self._lib = lib
+        cfg = ClipTextConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["proj"], g["eos_id"], g["eps"])
+        _load(self, b"clip_text", cfg, blob)
 
 
 class ClassifierModel(EmbedModel):
@@ -427,18 +433,11 @@ class ClassifierModel(EmbedModel):
     :class:`EmbedModel`'s: same tickets, same scheduler, width ``num_labels``."""
 
     def __init__(self, geometry: dict, blob: np.ndarray):
-        lib = load_library()
-        blob = np.ascontiguousarray(blob, dtype=np.float32)
         g = geometry
-        self.cfg = BertClassifierConfig(BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"],
-                                                   g["eps"]), g["num_labels"])
         self.hidden, self.inter, self.num_labels = g["hidden"], g["inter"], g["num_labels"]
         self.out_dim = self.num_labels
         self.pooling = "cls_head"
-        h = ctypes.c_int32(-1)
-        _check(lib.b200rt_model_load(b"bert_classifier", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
-        self.handle = h.value
-        self._lib = lib
+        _load(self, b"bert_classifier", BertClassifierConfig(_bert_config(g), g["num_labels"]), blob)
 
     def submit(self, ids: np.ndarray, lens=None, out: np.ndarray | None = None, tag=None, borrow_ids: bool = False, segs=None) -> Ticket:
         """As :meth:`EmbedModel.submit`; ``segs`` [n_items]: where each item's second segment starts (0 <= segs[i] <= lens[i];
@@ -468,17 +467,11 @@ class SparseEmbedModel(EmbedModel):
     ``embed_device`` takes ``max_len`` a multiple of 64."""
 
     def __init__(self, geometry: dict, blob: np.ndarray):
-        lib = load_library()
-        blob = np.ascontiguousarray(blob, dtype=np.float32)
         g = geometry
-        self.cfg = BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"], g["eps"])
         self.hidden, self.inter, self.vocab = g["hidden"], g["inter"], g["vocab"]
         self.out_dim = self.vocab
         self.pooling = "splade"
-        h = ctypes.c_int32(-1)
-        _check(lib.b200rt_model_load(b"bert_splade", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
-        self.handle = h.value
-        self._lib = lib
+        _load(self, b"bert_splade", _bert_config(g), blob)
 
 
 class NomicEmbedModel(EmbedModel):
@@ -490,21 +483,11 @@ class NomicEmbedModel(EmbedModel):
     takes ``max_len`` a multiple of 64."""
 
     def __init__(self, geometry: dict, blob: np.ndarray, pooling: str = "mean"):
-        if pooling not in POOLINGS:
-            raise B200RTError(E_INVALID, f"pooling must be one of {POOLINGS}, got {pooling!r}")
-        lib = load_library()
-        blob = np.ascontiguousarray(blob, dtype=np.float32)
         g = geometry
-        self.cfg = NomicBertConfig(BertConfig(g["vocab"], g["hidden"], g["layers"], g["heads"], g["inter"], g["max_pos"], g["type_vocab"],
-                                              g["eps"]), g["rope_theta"])
         self.hidden, self.inter, self.max_pos = g["hidden"], g["inter"], g["max_pos"]
         self.out_dim = self.hidden
         self.pooling = pooling
-        h = ctypes.c_int32(-1)
-        _check(lib.b200rt_model_load_ex(b"nomic_bert", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, LOAD_POOL_MEAN if pooling == "mean" else 0,
-                                        ctypes.byref(h)))
-        self.handle = h.value
-        self._lib = lib
+        _load(self, b"nomic_bert", NomicBertConfig(_bert_config(g), g["rope_theta"]), blob, _pool_flags(pooling))
 
 
 class ImageEmbedModel:
@@ -513,17 +496,11 @@ class ImageEmbedModel:
     ``engine.image_embed(images=...)`` in the reference's image example (image_embeddings_infinity.py:330-350)."""
 
     def __init__(self, geometry: dict, blob: np.ndarray):
-        lib = load_library()
-        blob = np.ascontiguousarray(blob, dtype=np.float32)
         g = geometry
-        self.cfg = VitConfig(g["image"], g["patch"], g["hidden"], g["layers"], g["heads"], g["inter"], g["proj"], g["eps"])
         self.image, self.proj = g["image"], g["proj"]
         self.tokens = (g["image"] // g["patch"]) ** 2 + 1
         self.hidden, self.inter = g["hidden"], g["inter"]
-        h = ctypes.c_int32(-1)
-        _check(lib.b200rt_model_load(b"vit", ctypes.byref(self.cfg), _ptr(blob), blob.nbytes, ctypes.byref(h)))
-        self.handle = h.value
-        self._lib = lib
+        _load(self, b"vit", VitConfig(g["image"], g["patch"], g["hidden"], g["layers"], g["heads"], g["inter"], g["proj"], g["eps"]), blob)
 
     def submit(self, pixels: np.ndarray, out: np.ndarray | None = None, tag=None) -> Ticket:
         """``pixels`` (C-contiguous float32) and ``out`` stay lent to the library until the ticket completes."""

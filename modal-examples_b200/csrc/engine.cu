@@ -23,6 +23,7 @@
 #include <string>
 #include <thread>
 #include <tuple>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -122,6 +123,7 @@ constexpr int MIN_ITEMS_PER_REPLICA = 8;  // a wave uses fewer replicas rather t
 constexpr int MAX_SEQ = 512;
 constexpr int MAX_SEQ_LONG = 8192;  // kind "nomic_bert" (streaming attention): max_pos and its longest bucket
 constexpr int VIT_WAVE_ITEMS = 64;  // images one replica takes per wave (64 x 197 tokens; 38.5 MB of pixels per wave slot)
+constexpr int TEXT_POS_ROWS = 128;  // kind "clip_text": embed_kernel reads pos[t % S] for every row of a wave padded to its bucket
 
 // The text geometries the kernels cover (hidden, heads, inter, causal): bge-base, bge-small and bge-large (kind "bert") and the
 // CLIP text tower (kind "clip_text", causal attention).  The ViT tower is bge-base-wide.
@@ -182,14 +184,19 @@ struct DevWeights {
     float* rope = nullptr;  // float2 pairs
 };
 
-enum ModelKind { KIND_BERT = 0, KIND_VIT = 1, KIND_CLIP_TEXT = 2, KIND_NOMIC = 3 };
+// The model kinds.  What depends on the kind is answered by one switch without a default below (or in the loaders and the
+// forward's head), so that -Wswitch names every place a new kind has to answer.
+enum ModelKind { BERT, BERT_CLASSIFIER, BERT_SPLADE, NOMIC_BERT, VIT, CLIP_TEXT };
+// in ModelKind order: the name b200rt_model_load_ex takes the kind by, and whether it takes B200RT_LOAD_POOL_MEAN
+constexpr struct { const char* name; bool pool_mean_ok; } MODEL_KINDS[] = {
+    {"bert", true}, {"bert_classifier", false}, {"bert_splade", false}, {"nomic_bert", true}, {"vit", false}, {"clip_text", false}};
+static_assert(sizeof MODEL_KINDS / sizeof MODEL_KINDS[0] == CLIP_TEXT + 1, "one MODEL_KINDS entry per kind");
 
 struct Model {
-    ModelKind kind = KIND_BERT;
-    bool pool_mean = false;  // text: mean of the valid tokens' final hidden states (B200RT_LOAD_POOL_MEAN) instead of the CLS row
-    int num_labels = 0;      // > 0: a BERT classifier (kind "bert_classifier"): the head's L logits per item instead of a pool
-    int splade_vpad = 0;     // > 0: a SPLADE encoder (kind "bert_splade"): vocab-wide sparse vectors, the vocabulary tiled to this
-    b200rt_bert_config cfg{};
+    ModelKind kind = BERT;
+    bool pool_mean = false;  // bert, nomic_bert: mean of the valid tokens' final hidden states (B200RT_LOAD_POOL_MEAN) instead of the CLS row
+    int num_labels = 0;      // bert_classifier: the head's L logits per item
+    int splade_vpad = 0;     // bert_splade: the vocabulary tiled to a multiple of 256 (results are vocab-wide sparse vectors)
     b200rt_vit_config vcfg{};
     b200rt_clip_text_config tcfg{};
     int vocab = 0, max_pos = 0;  // token-id models (bert, clip_text): the bounds submit checks ids and lengths against
@@ -202,6 +209,54 @@ struct Model {
     size_t f32_elems = 0, f16_elems = 0;
     std::vector<DevWeights> per_dev;
 };
+
+int launches_per_forward(const Model& m) {  // the embedding (vit: 3 launches), 5 per layer, the head (bert_splade: 4)
+    switch (m.kind) {
+    case BERT: case BERT_CLASSIFIER: case NOMIC_BERT: case CLIP_TEXT: return 1 + 5 * m.layers + 1;
+    case BERT_SPLADE: return 1 + 5 * m.layers + 4;
+    case VIT: return 3 + 5 * m.layers + 1;
+    }
+    return 0;
+}
+int wave_items(const Model& m, int S) {  // items one replica takes in a wave padded to S tokens
+    switch (m.kind) { case VIT: return VIT_WAVE_ITEMS; case BERT: case BERT_CLASSIFIER: case BERT_SPLADE: case NOMIC_BERT: case CLIP_TEXT: break; }
+    return m.cap_rows / S;
+}
+bool takes_segments(const Model& m) {  // items carry segment starts (token types of sentence pairs)
+    switch (m.kind) { case BERT_CLASSIFIER: return true; case BERT: case BERT_SPLADE: case NOMIC_BERT: case VIT: case CLIP_TEXT: break; }
+    return false;
+}
+bool pads_to_64(const Model& m) {  // padded lengths are multiples of 64 (the SPLADE max epilogue's and streaming attention's blocks)
+    switch (m.kind) { case BERT_SPLADE: case NOMIC_BERT: return true; case BERT: case BERT_CLASSIFIER: case VIT: case CLIP_TEXT: break; }
+    return false;
+}
+// The longest padded length a forward runs at: clip_text's waves go up to the 128-token bucket (its position table is padded to
+// TEXT_POS_ROWS zero rows), nomic_bert's up to max_pos rounded up to 64 (its rotary table has those rows), the others' max_pos.
+int max_wave_len(const Model& m) {
+    switch (m.kind) {
+    case CLIP_TEXT: return TEXT_POS_ROWS;
+    case NOMIC_BERT: return (m.max_pos + 63) / 64 * 64;
+    case BERT: case BERT_CLASSIFIER: case BERT_SPLADE: case VIT: break;
+    }
+    return m.max_pos;
+}
+// Submit buckets items by length, to multiples of 64 tokens up to this cap; a wave takes one bucket, padded to the bucket size.
+int bucket_cap(const Model& m) {
+    switch (m.kind) { case NOMIC_BERT: return max_wave_len(m); case BERT: case BERT_CLASSIFIER: case BERT_SPLADE: case VIT: case CLIP_TEXT: break; }
+    return MAX_SEQ;
+}
+// The encoder layers: post-LN (a residual epilogue re-applies the LayerNorm of the rows it adds to) or pre-LN (quick-GELU FFN1),
+// causal attention, and rotary: rotary Q / K in the QKV epilogue, the streaming attention kernel and a SwiGLU FFN1.
+struct LayerStyle { bool pre_ln, causal, rotary; };
+LayerStyle layer_style(const Model& m) {
+    switch (m.kind) {
+    case BERT: case BERT_CLASSIFIER: case BERT_SPLADE: return {false, false, false};
+    case NOMIC_BERT: return {false, false, true};
+    case VIT: return {true, false, false};
+    case CLIP_TEXT: return {true, true, false};
+    }
+    return {};
+}
 
 struct Dev {
     int id = -1;
@@ -245,10 +300,8 @@ struct Dev {
     bool lstop = false;
 };
 
-struct Model;
 struct Ticket {
     uint64_t id;
-    int model;
     const Model* mp = nullptr;  // resolved at submit time (the models vector may grow while the ticket is queued)
     std::vector<int32_t> ids;   // private copy [n, S] (empty when the caller lent us its buffer: `borrowed`)
     const int32_t* ids_ext = nullptr;
@@ -391,21 +444,18 @@ int get_qkv_map(Dev& d, const Model& model, int S, const CUtensorMap** out, cons
 }
 
 // Enqueue the forward of one padded batch on `stream` and add the launches it enqueued to `launches`.  out: fp32 [B, out_dim],
-// may be peer memory.  Widths, statistic partials and the attention head size follow the model's geometry.
-// BERT is post-LN: a residual epilogue re-applies the LayerNorm of the rows it adds to (the embedding LN or LN2 of the layer
-// before, then LN1).  CLIPVisionTransformer and CLIPTextTransformer are pre-LN: LayerNorm1 / LayerNorm2 are folded into QKV /
-// FFN1, the residual epilogues add the raw stream and emit the statistics the next fold needs.  The text tower's attention is
-// causal and its pooled row is chosen per item from its ids (launch_clip_text_pool).
+// may be peer memory.  Widths, statistic partials and the attention head size follow the model's geometry: three stages, the
+// embedding, the encoder layers as the kind's layer_style runs them, and the kind's head.
 int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
                     LaunchHook* hook) {
     const DevWeights& w = m.per_dev[dev_index];
-    const bool vit = m.kind == KIND_VIT, clip_text = m.kind == KIND_CLIP_TEXT, pre_ln = vit || clip_text;
+    const bool vit = m.kind == VIT;
+    const LayerStyle ls = layer_style(m);
     const int B = in.B, S = in.S, M = B * S;
-    if (M > m.cap_rows || (vit && B > VIT_WAVE_ITEMS))
+    if (M > m.cap_rows || B > wave_items(m, S))
         return fail(B200RT_E_INVALID, "batch of %d x %d tokens exceeds the model's wave capacity (%d rows)", B, S, m.cap_rows);
-    if ((m.splade_vpad > 0 || m.kind == KIND_NOMIC) && S % 64 != 0)
-        return fail(B200RT_E_INVALID, "a %s forward runs at padded lengths that are multiples of 64 (got %d)",
-                    m.kind == KIND_NOMIC ? "nomic_bert" : "bert_splade", S);
+    if (pads_to_64(m) && S % 64 != 0)
+        return fail(B200RT_E_INVALID, "a %s forward runs at padded lengths that are multiples of 64 (got %d)", MODEL_KINDS[m.kind].name, S);
     const int H = m.hidden, I = m.inter, P = H / 128;
     const Dev::ActMaps& am = d.act[text_geometry(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
@@ -413,13 +463,17 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
     const int32_t* lens = vit ? d.lens_const : in.lens;
     // residual epilogue: y <- acc + bias + LN(y), LN given by (stats, gamma, beta) -- or + y (pre-LN); new statistics to stats_out
     auto residual = [&](const float* bias, const float2* stats, const float* gamma, const float* beta, float2* stats_out) {
-        return pre_ln ? GemmEpi{bias, nullptr, P, nullptr, nullptr, stats_out, m.eps} : GemmEpi{bias, stats, P, gamma, beta, stats_out, m.eps};
+        return ls.pre_ln ? GemmEpi{bias, nullptr, P, nullptr, nullptr, stats_out, m.eps} : GemmEpi{bias, stats, P, gamma, beta, stats_out, m.eps};
     };
     uint64_t nl = 0;
     // counts the launch just enqueued; true once the hook wants no more
     auto step = [&](const char* name) {
         ++nl;
         return hook && hook->at(name, stream);
+    };
+    auto last = [&](const char* name) {  // the head's last launch
+        step(name);
+        return 0;
     };
     auto enqueue = [&]() -> int {
         if (hook && hook->at(nullptr, stream)) return 0;
@@ -437,59 +491,49 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
         } else {
             // clip_text: token + position, its zero type row leaves (word + 0) + pos bit-exact; no embedding LayerNorm
             // nomic_bert: no position table -- pos is 64 zero rows read as pos[t % 64], so the rows are (word + type0) + 0
-            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, m.kind == KIND_NOMIC ? 64 : S, m.vocab, H,
+            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, m.kind == NOMIC_BERT ? 64 : S, m.vocab, H,
                                   stream, in.segs));
             if (step("embed")) return 0;
         }
-        const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // BERT: the LayerNorm that applies to the current residual rows
-        if (m.kind == KIND_NOMIC) {
-            // NomicBertModel, post-LN as BERT: h = LN_a(x + o(attn(rope(q), rope(k), v))), y = LN_m(h + down(silu(gate h) up h)).
-            // The embedding LN, then each layer's LN2, folds into QKV and is re-applied by attn-out; LN1 folds into FFN1 and is
-            // re-applied by FFN2.  No biases: the folded c vectors and a zero vector.
-            for (int l = 0; l < m.layers; ++l) {
-                const LayerW& lw = w.layers[l];
-                GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
+        // Post-LN: the embedding LN, then each layer's LN2, folds into QKV and is re-applied by attn-out; LN1 folds into FFN1 and is
+        // re-applied by FFN2.  NomicBertModel: h = LN_a(x + o(attn(rope(q), rope(k), v))), y = LN_m(h + down(silu(gate h) up h)).
+        const float *prev_g = w.emb_g, *prev_b = w.emb_b;  // post-LN: the LayerNorm that applies to the current residual rows
+        for (int l = 0; l < m.layers; ++l) {
+            const LayerW& lw = w.layers[l];
+            // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
+            GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
+            if (ls.rotary) {
                 CUDA_TRY(launch_gemm_rope(am.yhi, lw.m_qkv, d.qkv, e_qkv, RopeEpi{reinterpret_cast<const float2*>(w.rope), S, 2 * H}, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv_rope")) return 0;
                 CUDA_TRY(launch_attention_stream(*mq, d.ctx, lens, B, S, d.sm_attn, stream));
                 if (step("attention_stream")) return 0;
-                const GemmEpi e_ao = residual(w.zero_bias, d.pstats[0], prev_g, prev_b, d.pstats[1]);
-                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
-                if (step("gemm_attn_out")) return 0;
-                GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
-                CUDA_TRY(launch_gemm_swiglu(am.yhi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
-                if (step("gemm_ffn1_swiglu")) return 0;
-                const GemmEpi e_ff2 = residual(w.zero_bias, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
-                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
-                if (step("gemm_ffn2")) return 0;
-                prev_g = lw.ln2_g;
-                prev_b = lw.ln2_b;
-            }
-        } else {
-            for (int l = 0; l < m.layers; ++l) {
-                const LayerW& lw = w.layers[l];
-                // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
-                GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
+            } else {
                 CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv")) return 0;
-                CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, clip_text));
+                CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, ls.causal));
                 if (step("attention")) return 0;
-                // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
-                const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
-                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
-                if (step("gemm_attn_out")) return 0;
-                GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
-                CUDA_TRY(launch_gemm(pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
-                if (step(pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
-                // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
-                const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
-                CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
-                if (step("gemm_ffn2")) return 0;
-                prev_g = lw.ln2_g;
-                prev_b = lw.ln2_b;
             }
+            // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
+            const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
+            if (step("gemm_attn_out")) return 0;
+            GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
+            if (ls.rotary) {
+                CUDA_TRY(launch_gemm_swiglu(am.yhi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
+                if (step("gemm_ffn1_swiglu")) return 0;
+            } else {
+                CUDA_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+                if (step(ls.pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
+            }
+            // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
+            const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
+            if (step("gemm_ffn2")) return 0;
+            prev_g = lw.ln2_g;
+            prev_b = lw.ln2_b;
         }
-        if (m.splade_vpad > 0) {
+        switch (m.kind) {
+        case BERT_SPLADE: {
             // SPLADE (BertForMaskedLM + max pooling): u = gelu(LN2(y) W_t^T + b_t) into the idle ctx buffer; the partials of u's
             // LayerNorm into the idle pstats[1] and the wave's max buffer (uint32 [B, vpad] in the idle ffn buffer) zeroed; the
             // decoder GEMM max-reduces relu(LN_t(u) W_dec^T + b) over each item's valid tokens into it, and never stores the
@@ -505,19 +549,27 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
                                         stream));
             if (step("gemm_splade")) return 0;
             CUDA_TRY(launch_splade_finalize(vmax, out, B, m.splade_vpad, m.vocab, stream));
-            step("splade_finalize");
-            return 0;
+            return last("splade_finalize");
         }
-        if (vit) CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
-        else if (clip_text)
+        case VIT:
+            CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
+            return last("vit_pool");
+        case CLIP_TEXT:
             CUDA_TRY(launch_clip_text_pool(d.yhi, d.ylo, in.ids, in.lens, w.post_g, w.post_b, w.proj_w, out, B, S, m.tcfg.proj, m.eps,
                                            m.tcfg.eos_id, stream));
-        else if (m.num_labels > 0)
+            return last("clip_text_pool");
+        case BERT_CLASSIFIER:
             CUDA_TRY(launch_cls_head(d.yhi, d.ylo, prev_g, prev_b, w.pool_w, w.pool_b, w.cls_w, w.cls_b, out, B, S, m.num_labels, m.eps, H,
                                      stream));
-        else if (m.pool_mean) CUDA_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
-        else CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
-        step(vit ? "vit_pool" : clip_text ? "clip_text_pool" : m.num_labels > 0 ? "cls_head" : (m.pool_mean ? "mean_pool_normalize" : "pool_normalize"));
+            return last("cls_head");
+        case BERT: case NOMIC_BERT:
+            if (m.pool_mean) {
+                CUDA_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
+                return last("mean_pool_normalize");
+            }
+            CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
+            return last("pool_normalize");
+        }
         return 0;
     };
     if (int rc = enqueue()) return rc;
@@ -570,7 +622,7 @@ void drop_graphs(Dev& d) {  // the replica is going away: its cached launches po
 int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
             LaunchHook* hook = nullptr) {
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(stream, d.ev_ws, 0));
-    if (hook || m.kind == KIND_VIT || in.B * in.S > GRAPH_MAX_ROWS) {
+    if (hook || m.kind == VIT || in.B * in.S > GRAPH_MAX_ROWS) {
         if (int rc = forward_enqueue(d, m, dev_index, in, out, stream, launches, hook)) return rc;
     } else {
         GraphCache& cache = graph_cache(d);
@@ -652,11 +704,6 @@ bool is_pinned(const void* p, size_t nbytes) {
     return a >= it->first && a + nbytes <= it->first + it->second;
 }
 
-// Padded lengths are bucketed to multiples of 64 tokens (the attention kernel's key sub-block): tickets whose max_len
-// falls into the same bucket share a wave, padded to the bucket size (at most 63 wasted tokens per item).
-// Kind "nomic_bert" keeps 64-token buckets up to its max_pos rounded up to 64 (`cap`); every other kind's stop at 512.
-inline int bucket_of(int S, int cap = MAX_SEQ) { return std::min(cap, (S + 63) / 64 * 64); }
-
 void launcher_main(Dev* dp) {
     Dev& d = *dp;
     cudaSetDevice(d.id);
@@ -696,7 +743,7 @@ void dispatcher_main(Runtime* rtp) {
             {
                 const int S0 = rt.pending.front().bucket;
                 const Model* m0 = rt.pending.front().t->mp;
-                const int cap0 = (m0->kind == KIND_VIT ? VIT_WAVE_ITEMS : m0->cap_rows / S0) * G;
+                const int cap0 = wave_items(*m0, S0) * G;
                 auto queued = [&] {
                     int n = 0;
                     for (auto& r : rt.pending)
@@ -723,7 +770,7 @@ void dispatcher_main(Runtime* rtp) {
             wv.n_items = 0;
             const Model* model = rt.pending.front().t->mp;
             // token capacity scales with 512/S: a wave holds the model's cap_rows tokens per replica
-            const int cap_items_S = (model->kind == KIND_VIT ? VIT_WAVE_ITEMS : model->cap_rows / wv.S) * G;
+            const int cap_items_S = wave_items(*model, wv.S) * G;
             for (auto it = rt.pending.begin(); it != rt.pending.end() && wv.n_items < cap_items_S;) {
                 if (it->bucket != wv.S || it->t->mp != model) {
                     ++it;
@@ -744,7 +791,7 @@ void dispatcher_main(Runtime* rtp) {
         // Stage the wave's ids on the root GPU.  A segment whose ids the caller lent us in pinned memory, at the
         // wave's own padded length, is DMA'd from where it lies; anything else goes through the slot's pinned buffer
         // (re-strided to the bucket length when the ticket's max_len is shorter).
-        const bool vit = model.kind == KIND_VIT;
+        const bool vit = model.kind == VIT;
         const int out_dim = model.out_dim;
         bool staged = false;
         auto direct_ids = [&](const Segment& sg) {  // lent, pinned, already at the wave's padded length, items in place
@@ -778,7 +825,7 @@ void dispatcher_main(Runtime* rtp) {
             for (const Segment& sg : wv.segs)
                 for (int i = 0; i < sg.count; ++i) rt.h_lens[slot][sg.wave_off + i] = sg.t->lens[sg.t->item_at(sg.ticket_off + i)];
         // a classifier wave carries every item's segment start; an item submitted without one is a single segment (start = len)
-        const bool pairs = model.num_labels > 0;
+        const bool pairs = takes_segments(model);
         if (pairs)
             for (const Segment& sg : wv.segs)
                 for (int i = 0; i < sg.count; ++i) {
@@ -1354,12 +1401,24 @@ constexpr int CLS_B_FLOATS = 128;  // the classifier bias is padded to 128 float
 constexpr int SPLADE_MAX_VOCAB = 64 * HIDDEN;
 static_assert(static_cast<size_t>((SPLADE_MAX_VOCAB + 255) / 256 * 256) * 4 <= static_cast<size_t>(64) * 3072 * 2, "SPLADE maxima in ffn");
 
-// num_labels > 0: kind "bert_classifier" -- the BERT layout followed by the pooler and the classifier, and the head as the last
-// launch instead of a pool.  splade: kind "bert_splade" -- the BERT layout followed by BertForMaskedLM's head, and the four
-// SPLADE launches instead of a pool.
-int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bool pool_mean, int* model_out, int num_labels = 0,
-               bool splade = false) {
+// A model of `kind` with its config's geometry (and token-id bounds), cap_rows rows per wave and out_dim floats per result.
+template <class Config>
+std::unique_ptr<Model> new_model(ModelKind kind, const Config& c, int cap_rows, int out_dim) {
+    auto m = std::make_unique<Model>();
+    m->kind = kind, m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
+    if constexpr (!std::is_same<Config, b200rt_vit_config>::value) m->vocab = c.vocab, m->max_pos = c.max_pos;
+    m->cap_rows = cap_rows, m->out_dim = out_dim;
+    return m;
+}
+
+// Kinds "bert", "bert_classifier" (num_labels: its logits per item) and "bert_splade".  The classifier is the BERT layout
+// followed by the pooler and the classifier, with the head as the last launch instead of a pool; the SPLADE encoder is the BERT
+// layout followed by BertForMaskedLM's head, with the four SPLADE launches instead of a pool.
+int model_load(ModelKind kind, const b200rt_bert_config& c, int num_labels, const float* blob, size_t nbytes, bool pool_mean,
+               int* model_out) {
     Runtime& rt = *g_rt;
+    if (kind == BERT_CLASSIFIER && (num_labels < 1 || num_labels > MAX_LABELS))
+        return fail(B200RT_E_UNSUPPORTED, "num_labels %d outside [1, %d]", num_labels, MAX_LABELS);
     bool known = false;
     for (const TextGeometry& tg : TEXT_GEOMETRIES) known |= !tg.causal && c.hidden == tg.hidden && c.heads == tg.heads && c.inter == tg.inter;
     if (!known || c.max_pos > MAX_SEQ || c.max_pos < 1 || c.layers < 1 || c.vocab < 1 || c.type_vocab < 1)
@@ -1367,10 +1426,10 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
                     "kernels cover three geometries, bge-base (hidden=768 heads=12 inter=3072), bge-small (hidden=384 heads=12 "
                     "inter=1536) and bge-large (hidden=1024 heads=16 inter=4096), with max_pos<=512 (got hidden %d heads %d inter %d "
                     "max_pos %d)", c.hidden, c.heads, c.inter, c.max_pos);
-    if (splade && c.vocab > SPLADE_MAX_VOCAB)
+    if (kind == BERT_SPLADE && c.vocab > SPLADE_MAX_VOCAB)
         return fail(B200RT_E_UNSUPPORTED, "a SPLADE vocabulary of %d words exceeds %d (one vocab-wide result per 64 tokens must fit the "
                     "wave's result buffers)", c.vocab, SPLADE_MAX_VOCAB);
-    if (num_labels > 0 && c.type_vocab != 2)
+    if (kind == BERT_CLASSIFIER && c.type_vocab != 2)
         return fail(B200RT_E_UNSUPPORTED, "a classifier takes sentence pairs through two token types: type_vocab must be 2, got %d",
                     c.type_vocab);
     const int cap_rows = model_cap_rows(rt.cap_rows, c.hidden);
@@ -1379,19 +1438,9 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
                     "a hidden=%d model needs room for one %d-token item, and the workspace holds %d of its rows: initialise with a "
                     "larger B200RT_INIT_WAVE_ITEMS (now %d)", c.hidden, MAX_SEQ, cap_rows, rt.cap_items);
 
-    auto m = std::make_unique<Model>();
-    m->cfg = c;
-    m->vocab = c.vocab, m->max_pos = c.max_pos;
-    m->pool_mean = pool_mean;
-    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
-    m->cap_rows = cap_rows;
-    m->out_dim = c.hidden;
-    m->num_labels = num_labels;
-    if (num_labels > 0) m->out_dim = num_labels;
-    if (splade) {
-        m->splade_vpad = (c.vocab + 255) / 256 * 256;
-        m->out_dim = c.vocab;
-    }
+    auto m = new_model(kind, c, cap_rows, kind == BERT_CLASSIFIER ? num_labels : kind == BERT_SPLADE ? c.vocab : c.hidden);
+    m->pool_mean = pool_mean, m->num_labels = num_labels;  // num_labels: 0 but for a classifier
+    if (kind == BERT_SPLADE) m->splade_vpad = (c.vocab + 255) / 256 * 256;
 
     // b200rt.weights.blob_layout.  QKV of layer l folds the LayerNorm in front of it, the previous layer's ln2 (the embedding
     // LN for l = 0); FFN1 folds the layer's own ln1.
@@ -1415,14 +1464,14 @@ int model_load(const b200rt_bert_config& c, const float* blob, size_t nbytes, bo
         ln_g = L.copy(l, H, &LayerW::ln2_g);
         ln_b = L.copy(l, H, &LayerW::ln2_b);
     }
-    if (num_labels > 0) {  // b200rt.weights.classifier_blob_layout: pool.w [H,H] | pool.b [H] | cls.w [L,H] | cls.b [128]
+    if (kind == BERT_CLASSIFIER) {  // b200rt.weights.classifier_blob_layout: pool.w [H,H] | pool.b [H] | cls.w [L,H] | cls.b [128]
         L.copy(H * H, &DevWeights::pool_w);
         L.copy(H, &DevWeights::pool_b);
         L.copy(static_cast<size_t>(num_labels) * H, &DevWeights::cls_w);
         L.copy(CLS_B_FLOATS, &DevWeights::cls_b);
         if (int rc = alloc_seg_slots(rt)) return rc;
     }
-    if (splade) {  // b200rt.weights.splade_blob_layout: mlm.t.w [H,H] | mlm.t.b [H] | mlm.ln.g [H] | mlm.ln.b [H] | mlm.dec.w [V,H] | mlm.dec.b
+    if (kind == BERT_SPLADE) {  // b200rt.weights.splade_blob_layout: mlm.t.w [H,H] | mlm.t.b [H] | mlm.ln.g [H] | mlm.ln.b [H] | mlm.dec.w [V,H] | mlm.dec.b
         // [V rounded up to 128]; the transform folds the last layer's LN2, the decoder the transform's LayerNorm
         const int tw = L.half(H, H, &DevWeights::mlm_t_w, &DevWeights::m_mlm_t);
         L.fold(tw, ln_g, ln_b, L.copy(H, nullptr), &DevWeights::mlm_t_c, H);
@@ -1443,15 +1492,12 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
         PD != HIDDEN || c.patch % 2 != 0 || c.proj < 1 || c.proj > 1024)
         return fail(B200RT_E_UNSUPPORTED, "kernels are specialised for ViT-B: hidden=768 heads=12 inter=3072, <= 512 tokens, 3*patch^2 %% 64 == 0, proj <= 1024 "
                                           "(got hidden %d heads %d inter %d image %d patch %d proj %d)", c.hidden, c.heads, c.inter, c.image, c.patch, c.proj);
+    const size_t item_bytes = static_cast<size_t>(3) * c.image * c.image * 4;
+    if (rt.vit_item_bytes != 0 && rt.vit_item_bytes != item_bytes)
+        return fail(B200RT_E_UNSUPPORTED, "a second vit model with a different image size is not supported in one runtime");
 
-    auto m = std::make_unique<Model>();
-    m->kind = KIND_VIT;
-    m->vcfg = c;
-    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
-    m->cap_rows = rt.cap_rows;
-    m->tokens = T;
-    m->out_dim = c.proj;
-    m->item_bytes = static_cast<size_t>(3) * c.image * c.image * 4;
+    auto m = new_model(VIT, c, rt.cap_rows, c.proj);
+    m->vcfg = c, m->tokens = T, m->item_bytes = item_bytes;
 
     // b200rt.weights.vit_blob_layout, plus the patch projection's zero bias
     Layout L;
@@ -1483,13 +1529,10 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
             if (!d.ev_pix[sl]) CUDA_TRY(cudaEventCreateWithFlags(&d.ev_pix[sl], cudaEventDisableTiming));
         }
     }
-    if (rt.vit_item_bytes != 0 && rt.vit_item_bytes != m->item_bytes)
-        return fail(B200RT_E_UNSUPPORTED, "a second vit model with a different image size is not supported in one runtime");
-    rt.vit_item_bytes = m->item_bytes;
+    rt.vit_item_bytes = item_bytes;
     return register_model(rt, std::move(m), model_out);
 }
 
-constexpr int TEXT_POS_ROWS = 128;  // embed_kernel reads pos[t % S] for every row of a wave padded to its bucket (<= 128)
 int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, size_t nbytes, int* model_out) {
     Runtime& rt = *g_rt;
     const TextGeometry* tgp = TEXT_GEOMETRIES;
@@ -1502,13 +1545,8 @@ int model_load_clip_text(const b200rt_clip_text_config& c, const float* blob, si
         return fail(B200RT_E_UNSUPPORTED, "max_pos %d outside [1, %d]", c.max_pos, TEXT_POS_ROWS);
     if (c.eos_id < 0 || c.eos_id >= c.vocab) return fail(B200RT_E_INVALID, "eos_id %d outside the vocabulary [0, %d)", c.eos_id, c.vocab);
 
-    auto m = std::make_unique<Model>();
-    m->kind = KIND_CLIP_TEXT;
+    auto m = new_model(CLIP_TEXT, c, model_cap_rows(rt.cap_rows, c.hidden), c.proj);
     m->tcfg = c;
-    m->vocab = c.vocab, m->max_pos = c.max_pos;
-    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
-    m->cap_rows = model_cap_rows(rt.cap_rows, c.hidden);
-    m->out_dim = c.proj;
 
     // b200rt.weights.clip_text_blob_layout, with pos padded to TEXT_POS_ROWS zero rows and a zero type row
     const size_t H = c.hidden, I = c.inter;
@@ -1539,14 +1577,8 @@ int model_load_nomic(const b200rt_nomic_bert_config& nc, const float* blob, size
         return fail(B200RT_E_INVALID, "a nomic_bert model with max_pos %d needs room for one %d-token item, and the workspace holds %d rows: "
                     "initialise with a larger B200RT_INIT_WAVE_ITEMS (now %d)", c.max_pos, S_max, rt.cap_rows, rt.cap_items);
 
-    auto m = std::make_unique<Model>();
-    m->kind = KIND_NOMIC;
-    m->cfg = c;
-    m->vocab = c.vocab, m->max_pos = c.max_pos;
+    auto m = new_model(NOMIC_BERT, c, rt.cap_rows, c.hidden);
     m->pool_mean = pool_mean;
-    m->hidden = c.hidden, m->inter = c.inter, m->heads = c.heads, m->layers = c.layers, m->eps = c.eps;
-    m->cap_rows = rt.cap_rows;
-    m->out_dim = c.hidden;
 
     // b200rt.weights.nomic_blob_layout.  QKV of layer l folds the previous layer's ln2 (the embedding LN for l = 0); gate and up
     // (adjacent in the blob) are one [2I, H] entry folding the layer's ln1, interleaved below.  Then the arena-only vectors.
@@ -1596,7 +1628,8 @@ int model_load_nomic(const b200rt_nomic_bert_config& nc, const float* blob, size
         CUDA_TRY(cudaMalloc(&sc, 2 * I * 4));
         std::unique_ptr<void, cudaError_t (*)(void*)> free_sc(sc, cudaFree);
         for (int l = 0; l < c.layers; ++l) {
-            const LayerW& lw = w.layers[l];
+            LayerW& lw = w.layers[l];
+            lw.ao_b = lw.ff2_b = w.zero_bias;  // no biases
             for (int part = 0; part < 2; ++part) {  // 0: gate, 1: up
                 CUDA_TRY(cudaMemcpy2DAsync(sw + part * 8 * H, 16 * H * 2, lw.ff1_w + part * I * H, 8 * H * 2, 8 * H * 2, I / 8,
                                            cudaMemcpyDeviceToDevice, d.compute));
@@ -1631,13 +1664,6 @@ const Model* get_model(Runtime& rt, int model) {
         return nullptr;
     }
     return rt.models[model].get();
-}
-
-// The longest padded length a forward of this model runs at: the CLIP text tower's waves go up to the 128-token bucket (its
-// position table is padded to TEXT_POS_ROWS zero rows for that), a nomic-bert model's up to max_pos rounded up to 64 (its
-// rotary table has those rows), a BERT model's up to max_pos.
-inline int max_wave_len(const Model& m) {
-    return m.kind == KIND_CLIP_TEXT ? TEXT_POS_ROWS : m.kind == KIND_NOMIC ? (m.max_pos + 63) / 64 * 64 : m.max_pos;
 }
 
 // ids [n_items, max_len] with max_len <= S_cap (submit: max_pos; device-resident / debug forwards: max_wave_len) and every
@@ -1699,11 +1725,26 @@ struct TraceOut {
     size_t names_cap;
 };
 
-// Runs the first n_launches launches of the forward of `in` on replica d (the caller holds d.mu): every workspace buffer and
-// the pooled output are set to 0xFF bytes (NaN in fp16 and fp32) behind the previous forward, the launches run on d.compute
-// through forward(), and once the stream has drained, rows = min(M + 256, the model's cap_rows) rows of every buffer, at the
-// model's widths (the buffers are used densely at those widths), and the pooled output are copied out.
-int trace_forward(DebugBuffers& b, Dev& d, const Model& m, const Input& in, int n_launches, const TraceOut& o) {
+// Runs the first n_launches launches of the forward of host input `in` (ids, lens, segs or pixels) on the root replica: every
+// workspace buffer and the pooled output are set to 0xFF bytes (NaN in fp16 and fp32) behind the previous forward, the launches
+// run on d.compute through forward(), and once the stream has drained, rows = min(M + 256, the model's cap_rows) rows of every
+// buffer, at the model's widths (the buffers are used densely at those widths), and the pooled output are copied out.
+int trace_forward(Runtime& rt, const Model& m, const Input& in, int n_launches, const TraceOut& o, int* n_total) {
+    const int total = launches_per_forward(m);
+    if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
+    if (!o.yhi || !o.ylo || !o.pstats0 || !o.pstats1 || !o.qkv || !o.ctx || !o.ffn || !o.out) return fail(B200RT_E_INVALID, "null output buffer");
+    if (n_total) *n_total = total;
+    Dev& d = *rt.devs[0];
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    DebugBuffers b(d.compute);
+    Input din = in;
+    if (in.pixels) CUDA_TRY(b.upload(&din.pixels, in.pixels, static_cast<size_t>(in.B) * m.item_bytes));
+    else {
+        CUDA_TRY(b.upload(&din.ids, in.ids, static_cast<size_t>(in.B) * in.S * 4));
+        CUDA_TRY(b.upload(&din.lens, in.lens, static_cast<size_t>(in.B) * 4));
+        if (in.segs) CUDA_TRY(b.upload(&din.segs, in.segs, static_cast<size_t>(in.B) * 4));
+    }
     const size_t R = g_rt->cap_rows, rows = std::min(static_cast<size_t>(in.B) * in.S + 256, static_cast<size_t>(m.cap_rows));
     const size_t H = m.hidden, I = m.inter, P = H / 128, out_floats = static_cast<size_t>(in.B) * m.out_dim;
     float* dout = nullptr;
@@ -1719,7 +1760,7 @@ int trace_forward(DebugBuffers& b, Dev& d, const Model& m, const Input& in, int 
     LaunchHook hook;
     hook.stop_after = n_launches;
     uint64_t launches = 0;
-    if (int rc = forward(d, m, 0, in, dout, d.compute, launches, &hook)) return rc;
+    if (int rc = forward(d, m, 0, din, dout, d.compute, launches, &hook)) return rc;
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     CUDA_TRY(cudaMemcpy(o.yhi, d.yhi, rows * H * 2, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(o.ylo, d.ylo, rows * H * 2, cudaMemcpyDeviceToHost));
@@ -1765,7 +1806,7 @@ int b200rt_model_wave_capacity_items(int model) {
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    return m->kind == KIND_VIT ? VIT_WAVE_ITEMS : m->cap_rows / MAX_SEQ;
+    return wave_items(*m, MAX_SEQ);
 }
 
 int b200rt_model_load(const char* kind, const void* cfg, const void* weights, size_t nbytes, int* model_out) {
@@ -1775,48 +1816,65 @@ int b200rt_model_load(const char* kind, const void* cfg, const void* weights, si
 int b200rt_model_load_ex(const char* kind, const void* cfg, const void* weights, size_t nbytes, uint32_t flags, int* model_out) {
     Runtime* rt = live_rt();
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!kind || (strcmp(kind, "bert") != 0 && strcmp(kind, "vit") != 0 && strcmp(kind, "clip_text") != 0 &&
-                  strcmp(kind, "bert_classifier") != 0 && strcmp(kind, "bert_splade") != 0 && strcmp(kind, "nomic_bert") != 0))
+    int k = 0;
+    while (k <= CLIP_TEXT && !(kind && strcmp(kind, MODEL_KINDS[k].name) == 0)) ++k;
+    if (k > CLIP_TEXT)
         return fail(B200RT_E_UNSUPPORTED, "unknown model kind '%s' (\"bert\", \"bert_classifier\", \"bert_splade\", \"nomic_bert\", \"vit\" or "
                     "\"clip_text\")", kind ? kind : "(null)");
     if (!cfg || !weights || !model_out) return fail(B200RT_E_INVALID, "null argument");
     if (flags & ~B200RT_LOAD_POOL_MEAN) return fail(B200RT_E_INVALID, "unknown load flags 0x%x", flags & ~B200RT_LOAD_POOL_MEAN);
+    if (flags && !MODEL_KINDS[k].pool_mean_ok)
+        return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\" or \"nomic_bert\", not \"%s\"", flags,
+                    MODEL_KINDS[k].name);
     const bool pool_mean = (flags & B200RT_LOAD_POOL_MEAN) != 0;
+    const float* blob = static_cast<const float*>(weights);
     std::lock_guard<std::mutex> dl(rt->devs[0]->mu);  // a load enqueues on the root's compute stream
-    if (strcmp(kind, "vit") == 0) {
-        if (pool_mean) return fail(B200RT_E_INVALID, "B200RT_LOAD_POOL_MEAN applies to text encoders (kind \"bert\"), not \"vit\"");
-        return model_load_vit(*static_cast<const b200rt_vit_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
+    switch (static_cast<ModelKind>(k)) {
+    case BERT: case BERT_SPLADE: return model_load(static_cast<ModelKind>(k), *static_cast<const b200rt_bert_config*>(cfg), 0, blob, nbytes, pool_mean, model_out);
+    case BERT_CLASSIFIER: {
+        const auto& cc = *static_cast<const b200rt_bert_classifier_config*>(cfg);
+        return model_load(BERT_CLASSIFIER, cc.bert, cc.num_labels, blob, nbytes, false, model_out);
     }
-    if (strcmp(kind, "clip_text") == 0) {
-        if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"clip_text\"", flags);
-        return model_load_clip_text(*static_cast<const b200rt_clip_text_config*>(cfg), static_cast<const float*>(weights), nbytes, model_out);
+    case NOMIC_BERT: return model_load_nomic(*static_cast<const b200rt_nomic_bert_config*>(cfg), blob, nbytes, pool_mean, model_out);
+    case VIT: return model_load_vit(*static_cast<const b200rt_vit_config*>(cfg), blob, nbytes, model_out);
+    case CLIP_TEXT: return model_load_clip_text(*static_cast<const b200rt_clip_text_config*>(cfg), blob, nbytes, model_out);
     }
-    if (strcmp(kind, "bert_classifier") == 0) {
-        if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"bert_classifier\"", flags);
-        const b200rt_bert_classifier_config& cc = *static_cast<const b200rt_bert_classifier_config*>(cfg);
-        if (cc.num_labels < 1 || cc.num_labels > MAX_LABELS)
-            return fail(B200RT_E_UNSUPPORTED, "num_labels %d outside [1, %d]", cc.num_labels, MAX_LABELS);
-        return model_load(cc.bert, static_cast<const float*>(weights), nbytes, false, model_out, cc.num_labels);
-    }
-    if (strcmp(kind, "nomic_bert") == 0)
-        return model_load_nomic(*static_cast<const b200rt_nomic_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean,
-                                model_out);
-    if (strcmp(kind, "bert_splade") == 0) {
-        if (flags) return fail(B200RT_E_INVALID, "load flags 0x%x apply to text encoders of kind \"bert\", not \"bert_splade\"", flags);
-        return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, false, model_out, 0, true);
-    }
-    return model_load(*static_cast<const b200rt_bert_config*>(cfg), static_cast<const float*>(weights), nbytes, pool_mean, model_out);
+    return fail(B200RT_E_STATE, "internal: no loader for kind \"%s\"", MODEL_KINDS[k].name);
 }
 
 // segs [n_items] (b200rt_submit_pairs, classifier models only): item i's second segment starts at token segs[i], 0 <= segs[i] <=
 // lens[i]; NULL: one segment.
 int check_segs(const Model& m, const int32_t* lens, const int32_t* segs, int n_items, int max_len) {
     if (!segs) return 0;
-    if (m.num_labels == 0) return fail(B200RT_E_INVALID, "token segments (segs) apply to classifier models (kind \"bert_classifier\")");
+    if (!takes_segments(m)) return fail(B200RT_E_INVALID, "token segments (segs) apply to classifier models (kind \"bert_classifier\")");
     for (int i = 0; i < n_items; ++i) {
         const int L = lens ? lens[i] : max_len;
         if (segs[i] < 0 || segs[i] > L) return fail(B200RT_E_INVALID, "segs[%d] = %d outside [0, lens[%d] = %d]", i, segs[i], i, L);
     }
+    return 0;
+}
+
+// A ticket of n_items results of model m, into `out`, for inputs padded to S tokens.
+static std::shared_ptr<Ticket> new_ticket(const Model* m, int n_items, int S, float* out) {
+    auto t = std::make_shared<Ticket>();
+    t->mp = m, t->n_items = n_items, t->S = S, t->out = out;
+    t->remaining.store(n_items);
+    t->out_pinned = is_pinned(out, static_cast<size_t>(n_items) * m->out_dim * 4);
+    return t;
+}
+
+// Registers ticket t and queues its runs for the dispatcher.
+static int queue_ticket(Runtime& rt, const std::shared_ptr<Ticket>& t, const std::vector<Run>& runs, uint64_t* ticket_out) {
+    {
+        std::lock_guard<std::mutex> lk(rt.mu);
+        if (rt.stopping) return fail(B200RT_E_STATE, "runtime is shutting down");
+        t->id = rt.next_ticket++;
+        rt.tickets.emplace(t->id, t);
+        for (const Run& r : runs) rt.pending.push_back(r);
+        rt.last_submit = std::chrono::steady_clock::now();
+        *ticket_out = t->id;
+    }
+    rt.cv_submit.notify_one();
     return 0;
 }
 
@@ -1827,17 +1885,11 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
     if (!out || !ticket_out) return fail(B200RT_E_INVALID, "null out / ticket_out");
-    if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d takes pixels (b200rt_submit_pixels), not token ids", model);
+    if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d takes pixels (b200rt_submit_pixels), not token ids", model);
     if (flags & ~static_cast<uint32_t>(B200RT_SUBMIT_BORROW_IDS)) return fail(B200RT_E_INVALID, "unknown submit flags 0x%x", flags);
     if (int rc = check_ids(*m, ids, lens, n_items, max_len, m->max_pos)) return rc;
     if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
-    auto t = std::make_shared<Ticket>();
-    t->model = model;
-    t->mp = m;
-    t->n_items = n_items;
-    t->S = max_len;
-    t->out = out;
-    t->remaining.store(n_items);
+    auto t = new_ticket(m, n_items, max_len, out);
     const size_t id_bytes = static_cast<size_t>(n_items) * max_len * 4;
     if (flags & B200RT_SUBMIT_BORROW_IDS) {  // the caller keeps ids valid and unchanged until the ticket completes
         t->borrowed = true;
@@ -1846,7 +1898,6 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     } else {
         t->ids.assign(ids, ids + static_cast<size_t>(n_items) * max_len);
     }
-    t->out_pinned = is_pinned(out, static_cast<size_t>(n_items) * m->out_dim * 4);
     if (lens) t->lens.assign(lens, lens + n_items);
     else t->lens.assign(n_items, max_len);
     if (segs) t->segs.assign(segs, segs + n_items);
@@ -1854,8 +1905,7 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
     // own length, so a ragged input wastes at most 63 tokens per item instead of max_len - len)
     std::vector<Run> runs;
     {
-        const int cap = m->kind == KIND_NOMIC ? max_wave_len(*m) : MAX_SEQ;
-        auto bucket_of = [cap](int S) { return ::bucket_of(S, cap); };
+        auto bucket_of = [cap = bucket_cap(*m)](int S) { return std::min(cap, (S + 63) / 64 * 64); };
         bool one_bucket = true;
         const int b0 = bucket_of(t->lens[0]);
         for (int i = 1; i < n_items && one_bucket; ++i) one_bucket = bucket_of(t->lens[i]) == b0;
@@ -1874,17 +1924,7 @@ static int submit_impl(int model, const int32_t* ids, const int32_t* lens, int n
             }
         }
     }
-    {
-        std::lock_guard<std::mutex> lk(rt->mu);
-        if (rt->stopping) return fail(B200RT_E_STATE, "runtime is shutting down");
-        t->id = rt->next_ticket++;
-        rt->tickets.emplace(t->id, t);
-        for (auto& r : runs) rt->pending.push_back(r);
-        rt->last_submit = std::chrono::steady_clock::now();
-        *ticket_out = t->id;
-    }
-    rt->cv_submit.notify_one();
-    return 0;
+    return queue_ticket(*rt, t, runs, ticket_out);
 }
 
 int b200rt_submit(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, float* out,
@@ -1907,29 +1947,11 @@ int b200rt_submit_pixels(int model, const float* pixels, int n_items, float* out
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    if (m->kind != KIND_VIT) return fail(B200RT_E_INVALID, "model %d takes token ids (b200rt_submit), not pixels", model);
+    if (m->kind != VIT) return fail(B200RT_E_INVALID, "model %d takes token ids (b200rt_submit), not pixels", model);
     if (!pixels || !out || !ticket_out || n_items < 1) return fail(B200RT_E_INVALID, "null / empty argument");
-    auto t = std::make_shared<Ticket>();
-    t->model = model;
-    t->mp = m;
-    t->n_items = n_items;
-    t->S = m->tokens;
-    t->out = out;
-    t->pixels = pixels;
-    t->borrowed = true;
-    t->remaining.store(n_items);
-    t->out_pinned = is_pinned(out, static_cast<size_t>(n_items) * m->out_dim * 4);
-    {
-        std::lock_guard<std::mutex> lk(rt->mu);
-        if (rt->stopping) return fail(B200RT_E_STATE, "runtime is shutting down");
-        t->id = rt->next_ticket++;
-        rt->tickets.emplace(t->id, t);
-        rt->pending.push_back(Run{t, 0, n_items, -m->tokens});  // negative bucket keys: image waves never mix with text waves
-        rt->last_submit = std::chrono::steady_clock::now();
-        *ticket_out = t->id;
-    }
-    rt->cv_submit.notify_one();
-    return 0;
+    auto t = new_ticket(m, n_items, m->tokens, out);
+    t->pixels = pixels, t->borrowed = true;
+    return queue_ticket(*rt, t, {Run{t, 0, n_items, -m->tokens}}, ticket_out);  // negative bucket keys: image waves never mix with text waves
 }
 
 static int reap_locked(Runtime& rt, uint64_t id, const std::shared_ptr<Ticket>& t) {
@@ -2018,9 +2040,9 @@ int b200rt_embed_device_pairs(int model, int gpu, const int32_t* d_ids, const in
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
     if (gpu < 0 || gpu >= static_cast<int>(rt->devs.size())) return fail(B200RT_E_INVALID, "gpu index %d outside the pool", gpu);
-    if (m->kind == KIND_VIT) return fail(B200RT_E_UNSUPPORTED, "b200rt_embed_device takes token ids: model %d is not a text encoder", model);
+    if (m->kind == VIT) return fail(B200RT_E_UNSUPPORTED, "b200rt_embed_device takes token ids: model %d is not a text encoder", model);
     if (!d_ids || !d_lens || !d_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
-    if (d_segs && m->num_labels == 0)
+    if (d_segs && !takes_segments(*m))
         return fail(B200RT_E_INVALID, "token segments (d_segs) apply to classifier models (kind \"bert_classifier\")");
     Dev& d = *rt->devs[gpu];
     std::lock_guard<std::mutex> dl(d.mu);
@@ -2766,28 +2788,15 @@ int b200rt_debug_forward_trace_segs(int model, const int32_t* ids, const int32_t
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+    if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (int rc = check_ids(*m, ids, lens, n_items, max_len, max_wave_len(*m))) return rc;
     if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
-    const int total = 5 * m->layers + (m->splade_vpad > 0 ? 5 : 2);
-    if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
-    if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
-    const size_t M = static_cast<size_t>(n_items) * max_len;
-    if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
-    if (n_total) *n_total = total;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
+    if (static_cast<size_t>(n_items) * max_len > static_cast<size_t>(m->cap_rows))
+        return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
     std::vector<int32_t> l(n_items, max_len);
     if (lens) l.assign(lens, lens + n_items);
-    DebugBuffers b(d.compute);
-    int32_t *dids = nullptr, *dlens = nullptr;
-    CUDA_TRY(b.upload(&dids, ids, M * 4));
-    CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
-    int32_t* dsegs = nullptr;
-    if (segs) CUDA_TRY(b.upload(&dsegs, segs, static_cast<size_t>(n_items) * 4));
     const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(b, d, *m, Input{dids, dlens, nullptr, n_items, max_len, dsegs}, n_launches, o);
+    return trace_forward(*rt, *m, Input{ids, l.data(), nullptr, n_items, max_len, segs}, n_launches, o, n_total);
 }
 
 int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
@@ -2797,19 +2806,9 @@ int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, 
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    if (m->kind != KIND_VIT || !pixels || n_items < 1 || n_items > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "bad arguments");
-    const int total = 5 * m->layers + 4;
-    if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
-    if (!yhi || !ylo || !pstats0 || !pstats1 || !qkv || !ctx || !ffn || !out) return fail(B200RT_E_INVALID, "null output buffer");
-    if (n_total) *n_total = total;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    DebugBuffers b(d.compute);
-    float* dpix = nullptr;
-    CUDA_TRY(b.upload(&dpix, pixels, static_cast<size_t>(n_items) * m->item_bytes));
+    if (m->kind != VIT || !pixels || n_items < 1 || n_items > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "bad arguments");
     const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(b, d, *m, Input{nullptr, nullptr, dpix, n_items, m->tokens}, n_launches, o);
+    return trace_forward(*rt, *m, Input{nullptr, nullptr, pixels, n_items, m->tokens}, n_launches, o, n_total);
 }
 
 int b200rt_debug_model_cap_rows(int model) {
@@ -2826,7 +2825,7 @@ int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters,
     if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
     const Model* m = get_model(*rt, model);
     if (!m) return B200RT_E_INVALID;
-    if (m->kind == KIND_VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+    if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
     if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
     const size_t M = static_cast<size_t>(n_items) * max_len;
     if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");

@@ -103,6 +103,24 @@ def test_scheduler_waves_pool_and_text_model_side_by_side(rt):
         model.submit(np.zeros((1, 3, 32, 32), np.float32))
 
 
+def test_second_image_size_is_refused_before_loading_weights(rt):
+    """A second ViT with another image size is refused with E_UNSUPPORTED ahead of the blob-size check (E_INVALID), so before
+    any of its weights are allocated on a replica; the loaded model embeds exactly as before."""
+    import ctypes
+
+    g, flat, model = get_model(rt, 2, "trained", 1)
+    px = C.synth_pixels(2, g, 2)
+    before = model.embed(px)
+    cfg = rt.VitConfig(g.image // 2, g.patch, g.hidden, g.layers, g.heads, g.inter, g.proj, g.eps)
+    wrong = np.zeros(16, np.float32)
+    h = ctypes.c_int32(-1)
+    assert model._lib.b200rt_model_load_ex(b"vit", ctypes.byref(cfg), rt._ptr(wrong), wrong.nbytes, 0, ctypes.byref(h)) == rt.E_UNSUPPORTED
+    assert b"image size" in model._lib.b200rt_last_error()
+    after = model.embed(px)
+    assert np.array_equal(after, before)
+    assert C.rel_l2(after, C.forward_np(flat, px, g)).max() <= 1e-3
+
+
 def test_infinity_emb_adapter_matches_the_oracle_on_pil_images(rt, tmp_path):
     """The product's `infinity_emb` stand-in (what image_embeddings_infinity.py:296-306, 340-350 drives): engines started the
     reference's way -- several per process, one per concurrent input -- share one loaded model; PIL images go through
