@@ -25,6 +25,7 @@
 #include <tuple>
 #include <type_traits>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200rt.h"
@@ -116,6 +117,67 @@ int make_map_qkv(CUtensorMap* m, const void* base, uint64_t B, uint64_t S, uint6
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------ owned CUDA resources
+
+// One CUDA resource and the device it was made on.  Move-only; it releases the resource on that device when it goes, so a
+// runtime, a replica or a model frees what it made on shutdown and on every early return of init or a load alike.  It converts
+// to the raw pointer or handle.
+template <class H, auto Release>
+class Owned {
+  public:
+    Owned() = default;
+    Owned(Owned&& o) noexcept : h_(std::exchange(o.h_, H{})), dev_(o.dev_) {}
+    Owned& operator=(Owned&& o) noexcept { std::swap(h_, o.h_); std::swap(dev_, o.dev_); return *this; }
+    ~Owned() { reset(); }
+    operator H() const { return h_; }
+    H get() const { return h_; }
+    cudaError_t reset() {  // releases the resource now, and leaves the calling thread on the device it was on
+        if (!h_) return cudaSuccess;
+        int cur = 0;
+        cudaError_t e = cudaGetDevice(&cur);
+        if (e == cudaSuccess) e = cudaSetDevice(dev_);
+        if (e == cudaSuccess) {
+            e = Release(h_);
+            cudaSetDevice(cur);
+        }
+        h_ = H{};
+        return e;
+    }
+  protected:
+    template <class Create>
+    cudaError_t make(Create create) {  // create(&h) on the current device; on success this holds h instead of what it held
+        int dev = 0;
+        H h{};
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e == cudaSuccess) e = create(&h);
+        if (e != cudaSuccess) return e;
+        reset();
+        h_ = h, dev_ = dev;
+        return cudaSuccess;
+    }
+  private:
+    H h_{};
+    int dev_ = 0;
+};
+
+template <class T>
+struct DevMem : Owned<T*, cudaFree> {
+    cudaError_t alloc(size_t bytes) { return this->make([&](T** p) { return cudaMalloc(p, bytes); }); }
+};
+template <class T>
+struct HostMem : Owned<T*, cudaFreeHost> {  // pinned
+    cudaError_t alloc(size_t bytes) { return this->make([&](T** p) { return cudaMallocHost(p, bytes); }); }
+};
+struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
+    cudaError_t create() { return make([](cudaStream_t* s) { return cudaStreamCreateWithFlags(s, cudaStreamNonBlocking); }); }
+};
+struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
+    cudaError_t create(unsigned flags = cudaEventDefault) { return make([&](cudaEvent_t* e) { return cudaEventCreateWithFlags(e, flags); }); }
+};
+struct GraphExec : Owned<cudaGraphExec_t, cudaGraphExecDestroy> {
+    cudaError_t instantiate(cudaGraph_t g) { return make([&](cudaGraphExec_t* x) { return cudaGraphInstantiate(x, g, 0); }); }
+};
+
 // ------------------------------------------------------------------------------------------ model / device state
 
 constexpr int NSLOT = 4;
@@ -159,8 +221,8 @@ struct LayerW {
 };
 
 struct DevWeights {
-    float* f32_arena = nullptr;  // embeddings, biases, LayerNorm params
-    __half* f16_arena = nullptr; // GEMM weights
+    DevMem<float> f32_arena;   // embeddings, biases, LayerNorm params
+    DevMem<__half> f16_arena;  // GEMM weights
     float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;
     std::vector<LayerW> layers;
     // ViT (kind "vit"): patch projection (fp16, the stride-p convolution as a [H, 3 p p] matrix), class / position embeddings,
@@ -258,15 +320,31 @@ LayerStyle layer_style(const Model& m) {
     return {};
 }
 
+// A forward captured as a CUDA graph (see forward), by the model, buffers, stream and shape it was captured with.
+struct GraphKey {
+    const void *model, *ids, *lens, *out;
+    cudaStream_t stream;
+    int B, S;
+    const void* segs;
+    bool operator<(const GraphKey& o) const {
+        return std::tie(model, ids, lens, out, stream, B, S, segs) < std::tie(o.model, o.ids, o.lens, o.out, o.stream, o.B, o.S, o.segs);
+    }
+};
+struct GraphEntry {
+    GraphExec exec;
+    uint64_t launches;
+    uint64_t last_use;
+};
+
 struct Dev {
     int id = -1;
     int sm_count = 0;
     int sm_gemm = 0, sm_attn = 0;  // SMs a GEMM / an attention launch of this replica asks for (see B200RT_INIT_SPLIT_SMS)
-    cudaStream_t compute = nullptr;
+    Stream compute;
     // workspace (capacity cap_rows rows)
-    __half *yhi = nullptr, *ylo = nullptr;  // residual stream y = hi + lo, PRE-LayerNorm; hi doubles as the GEMM A operand
-    float2* pstats[2] = {nullptr, nullptr};  // [rows][STAT_PARTS] (sum, M2) partials: [0] embedding LN / LN2 inputs, [1] LN1 inputs
-    __half *qkv = nullptr, *ctx = nullptr, *ffn = nullptr;
+    DevMem<__half> yhi, ylo;  // residual stream y = hi + lo, PRE-LayerNorm; hi doubles as the GEMM A operand
+    DevMem<float2> pstats[2];  // [rows][STAT_PARTS] (sum, M2) partials: [0] embedding LN / LN2 inputs, [1] LN1 inputs
+    DevMem<__half> qkv, ctx, ffn;
     // fp16 [rows, *] box {64,128}: GEMM A operands, per TEXT_GEOMETRIES entry, each over that geometry's model_cap_rows rows
     // (a model reads the same buffers densely at its own widths)
     struct ActMaps {
@@ -274,23 +352,24 @@ struct Dev {
     } act[N_TEXT_GEOMETRIES];
     std::map<std::pair<int, int>, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per (padded length, hidden)
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
-    int32_t* ids_in[NSLOT] = {};
-    int32_t* lens_in[NSLOT] = {};
-    int32_t* segs_in[NSLOT] = {};  // classifier waves' segment starts (allocated when the first classifier model loads)
-    float* pix_in[NSLOT] = {};     // vit: this replica's share of a wave's pixels (allocated when the first vit model loads)
-    cudaStream_t copy = nullptr;   // vit: H2D of wave k+1's pixels runs here, under the forward of wave k on `compute`
-    cudaEvent_t ev_pix[NSLOT] = {};
-    int32_t* lens_const = nullptr; // vit: every item has `tokens` keys
-    CUtensorMap m_im2col;          // vit: the ffn buffer viewed as the im2col matrix [rows, 768]
-    cudaEvent_t ev_done[NSLOT];
-    cudaEvent_t ev_begin[NSLOT], ev_end[NSLOT];  // timing: the forward itself on this replica's compute stream
-    int last_slot = -1;                          // completer only: slot of this replica's previous wave (gap statistics)
+    DevMem<int32_t> ids_in[NSLOT], lens_in[NSLOT];
+    DevMem<int32_t> segs_in[NSLOT];  // classifier waves' segment starts (allocated when the first classifier model loads)
+    DevMem<float> pix_in[NSLOT];     // vit: this replica's share of a wave's pixels (allocated when the first vit model loads)
+    Stream copy;                     // vit: H2D of wave k+1's pixels runs here, under the forward of wave k on `compute`
+    Event ev_pix[NSLOT];
+    DevMem<int32_t> lens_const;      // vit: every item has `tokens` keys
+    CUtensorMap m_im2col;            // vit: the ffn buffer viewed as the im2col matrix [rows, 768]
+    Event ev_done[NSLOT];
+    Event ev_begin[NSLOT], ev_end[NSLOT];  // timing: the forward itself on this replica's compute stream
+    int last_slot = -1;                    // completer only: slot of this replica's previous wave (gap statistics)
     std::mutex mu;  // serialises host-side enqueue on this replica (scheduler vs. embed_device/debug)
     // Every forward on this replica uses the same workspace (yhi, ylo, qkv, ctx, ffn, pstats), whichever stream it is
     // enqueued on: ev_ws is recorded behind each forward and waited on ahead of the next one, so forwards from the
     // scheduler's stream and from callers' streams (b200rt_embed_device) execute one after the other on the device.
-    cudaEvent_t ev_ws = nullptr;
+    Event ev_ws;
     bool ev_ws_armed = false;
+    std::map<GraphKey, GraphEntry> graphs;  // cached forwards (see forward); guarded by mu
+    uint64_t graph_tick = 0;
     // launcher thread: enqueues this replica's share of a wave (the ~85 launches per replica would otherwise be issued
     // by the one dispatcher thread for all replicas in turn)
     std::thread launcher;
@@ -351,13 +430,14 @@ struct Runtime {
     int cap_rows = 0;    // cap_items*512 rounded up to 128
     std::vector<std::unique_ptr<Model>> models;
     // root staging per slot
-    int32_t *h_ids[NSLOT], *h_lens[NSLOT];
-    float* h_out[NSLOT];
-    int32_t *d_ids_stage[NSLOT], *d_lens_stage[NSLOT];
-    int32_t *h_segs[NSLOT] = {}, *d_segs_stage[NSLOT] = {};  // classifier waves only (allocated with the first classifier model)
-    float* d_out_gather[NSLOT];
-    cudaStream_t s_in = nullptr, s_out = nullptr;  // on root
-    cudaEvent_t ev_scatter[NSLOT], ev_wave[NSLOT], ev_t0[NSLOT], ev_fwd_end[NSLOT];
+    HostMem<int32_t> h_ids[NSLOT], h_lens[NSLOT];
+    HostMem<float> h_out[NSLOT];
+    DevMem<int32_t> d_ids_stage[NSLOT], d_lens_stage[NSLOT];
+    HostMem<int32_t> h_segs[NSLOT];  // classifier waves only (allocated with the first classifier model)
+    DevMem<int32_t> d_segs_stage[NSLOT];
+    DevMem<float> d_out_gather[NSLOT];
+    Stream s_in, s_out;  // on root
+    Event ev_scatter[NSLOT], ev_wave[NSLOT], ev_t0[NSLOT], ev_fwd_end[NSLOT];
     // queues
     std::mutex mu;
     std::condition_variable cv_submit, cv_done, cv_slot, cv_wave, cv_idle;
@@ -402,23 +482,14 @@ struct LaunchHook {
     int stop_after = -1;
     bool timing = false;
     std::vector<std::string> names;
-    std::vector<cudaEvent_t> evs;
+    std::vector<Event> evs;
     cudaError_t error = cudaSuccess;  // of the first timing event that could not be created or recorded (ends the enqueue)
-    LaunchHook() = default;
-    LaunchHook(const LaunchHook&) = delete;
-    LaunchHook& operator=(const LaunchHook&) = delete;
-    ~LaunchHook() {
-        for (cudaEvent_t e : evs) cudaEventDestroy(e);
-    }
     bool at(const char* name, cudaStream_t stream) {  // true: enqueue nothing more
         if (name) names.push_back(name);
         if (timing && error == cudaSuccess) {
-            cudaEvent_t e;
-            error = cudaEventCreate(&e);
-            if (error == cudaSuccess) {
-                evs.push_back(e);
-                error = cudaEventRecord(e, stream);
-            }
+            evs.emplace_back();
+            error = evs.back().create();
+            if (error == cudaSuccess) error = cudaEventRecord(evs.back(), stream);
         }
         return error != cudaSuccess || (stop_after >= 0 && names.size() >= static_cast<size_t>(stop_after));
     }
@@ -541,7 +612,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             GemmEpi e_t{w.mlm_t_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
             CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, w.m_mlm_t, d.ctx, nullptr, e_t, M, H, H, d.sm_gemm, stream));
             if (step("gemm_mlm_transform")) return 0;
-            uint32_t* vmax = reinterpret_cast<uint32_t*>(d.ffn);
+            uint32_t* vmax = reinterpret_cast<uint32_t*>(d.ffn.get());
             CUDA_TRY(launch_mlm_ln_stats(d.ctx, d.pstats[1], vmax, M, static_cast<size_t>(B) * m.splade_vpad, H, stream));
             if (step("mlm_ln_stats")) return 0;
             GemmEpi e_dec{w.mlm_dec_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
@@ -585,38 +656,6 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
 constexpr int GRAPH_MAX_ROWS = 8192;
 constexpr size_t GRAPH_CACHE_MAX = 96;
 
-struct GraphKey {
-    const void *model, *ids, *lens, *out;
-    cudaStream_t stream;
-    int B, S;
-    const void* segs;
-    bool operator<(const GraphKey& o) const {
-        return std::tie(model, ids, lens, out, stream, B, S, segs) < std::tie(o.model, o.ids, o.lens, o.out, o.stream, o.B, o.S, o.segs);
-    }
-};
-struct GraphEntry {
-    cudaGraphExec_t exec;
-    uint64_t launches;
-    uint64_t last_use;
-};
-struct GraphCache {
-    std::map<GraphKey, GraphEntry> entries;
-    uint64_t tick = 0;
-};
-std::mutex g_graph_mu;
-std::map<Dev*, GraphCache> g_graphs;
-GraphCache& graph_cache(Dev& d) {
-    std::lock_guard<std::mutex> lk(g_graph_mu);
-    return g_graphs[&d];
-}
-void drop_graphs(Dev& d) {  // the replica is going away: its cached launches point into freed buffers
-    std::lock_guard<std::mutex> lk(g_graph_mu);
-    auto it = g_graphs.find(&d);
-    if (it == g_graphs.end()) return;
-    for (auto& kv : it->second.entries) cudaGraphExecDestroy(kv.second.exec);
-    g_graphs.erase(it);
-}
-
 // The caller holds d.mu.  Orders this forward behind the previous one on the replica's workspace (see Dev::ev_ws) and adds
 // its launches to `launches`.  Text batches of at most GRAPH_MAX_ROWS rows without a hook replay their CUDA graph.
 int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, cudaStream_t stream, uint64_t& launches,
@@ -625,16 +664,14 @@ int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, 
     if (hook || m.kind == VIT || in.B * in.S > GRAPH_MAX_ROWS) {
         if (int rc = forward_enqueue(d, m, dev_index, in, out, stream, launches, hook)) return rc;
     } else {
-        GraphCache& cache = graph_cache(d);
         const GraphKey key{&m, in.ids, in.lens, out, stream, in.B, in.S, in.segs};
-        auto it = cache.entries.find(key);
-        if (it == cache.entries.end()) {
-            if (cache.entries.size() >= GRAPH_CACHE_MAX) {  // evict the least recently replayed graph
-                auto victim = cache.entries.begin();
-                for (auto j = cache.entries.begin(); j != cache.entries.end(); ++j)
+        auto it = d.graphs.find(key);
+        if (it == d.graphs.end()) {
+            if (d.graphs.size() >= GRAPH_CACHE_MAX) {  // evict the least recently replayed graph
+                auto victim = d.graphs.begin();
+                for (auto j = d.graphs.begin(); j != d.graphs.end(); ++j)
                     if (j->second.last_use < victim->second.last_use) victim = j;
-                cudaGraphExecDestroy(victim->second.exec);
-                cache.entries.erase(victim);
+                d.graphs.erase(victim);
             }
             const CUtensorMap *mq = nullptr, *mc = nullptr;
             if (int rc = get_qkv_map(d, m, in.S, &mq, &mc)) return rc;  // host-side map creation happens outside the capture
@@ -648,12 +685,12 @@ int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, 
                 return rc;
             }
             CUDA_TRY(ce);
-            GraphEntry ent{nullptr, nl, 0};
-            CUDA_TRY(cudaGraphInstantiate(&ent.exec, graph, 0));
+            GraphEntry ent{{}, nl, 0};
+            CUDA_TRY(ent.exec.instantiate(graph));
             cudaGraphDestroy(graph);
-            it = cache.entries.emplace(key, ent).first;
+            it = d.graphs.emplace(key, std::move(ent)).first;
         }
-        it->second.last_use = ++cache.tick;
+        it->second.last_use = ++d.graph_tick;
         CUDA_TRY(cudaGraphLaunch(it->second.exec, stream));
         launches += it->second.launches;
     }
@@ -877,7 +914,7 @@ void dispatcher_main(Runtime* rtp) {
             plan.item_count[g] = b1 - b0;
             if (g != 0) peer_bytes += static_cast<uint64_t>(b1 - b0) * (vit ? out_dim * 4 : S * 4 + 4 + (pairs ? 4 : 0) + out_dim * 4);
         }
-        if (!vit) SCHED_TRY(launch_scatter(rt.d_ids_stage[slot], rt.d_lens_stage[slot], plan, rt.s_in, pairs ? rt.d_segs_stage[slot] : nullptr));
+        if (!vit) SCHED_TRY(launch_scatter(rt.d_ids_stage[slot], rt.d_lens_stage[slot], plan, rt.s_in, pairs ? rt.d_segs_stage[slot].get() : nullptr));
         SCHED_TRY(cudaEventRecord(rt.ev_scatter[slot], rt.s_in));
         // every participating replica's launcher thread enqueues its own forward (~85 launches each, in parallel)
         std::atomic<uint64_t> launches{1};
@@ -926,7 +963,7 @@ void dispatcher_main(Runtime* rtp) {
                                              dd.compute, nl);
                         } else {
                             rc = forward(dd, model, g, Input{dd.ids_in[slot], dd.lens_in[slot], nullptr, plan.item_count[g], S,
-                                                             pairs ? dd.segs_in[slot] : nullptr}, dst, dd.compute, nl);
+                                                             pairs ? dd.segs_in[slot].get() : nullptr}, dst, dd.compute, nl);
                         }
                         if (rc) { e = t_last_error; code = rc; }
                         else {
@@ -1095,18 +1132,18 @@ int alloc_dev(Runtime& rt, Dev& d) {
         d.sm_gemm = d.sm_count - d.sm_attn;
     }
     CUDA_TRY(kernels_init_device());
-    CUDA_TRY(cudaStreamCreateWithFlags(&d.compute, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&d.ev_ws, cudaEventDisableTiming));
+    CUDA_TRY(d.compute.create());
+    CUDA_TRY(d.ev_ws.create(cudaEventDisableTiming));
     const size_t R = rt.cap_rows;
     for (int i = 0; i < 2; ++i) {
-        CUDA_TRY(cudaMalloc(&d.pstats[i], R * STAT_PARTS * sizeof(float2)));
+        CUDA_TRY(d.pstats[i].alloc(R * STAT_PARTS * sizeof(float2)));
         CUDA_TRY(cudaMemset(d.pstats[i], 0, R * STAT_PARTS * sizeof(float2)));
     }
-    CUDA_TRY(cudaMalloc(&d.yhi, R * HIDDEN * 2));
-    CUDA_TRY(cudaMalloc(&d.ylo, R * HIDDEN * 2));
-    CUDA_TRY(cudaMalloc(&d.qkv, R * QKV_DIM * 2));
-    CUDA_TRY(cudaMalloc(&d.ctx, R * HIDDEN * 2));
-    CUDA_TRY(cudaMalloc(&d.ffn, R * 3072 * 2));
+    CUDA_TRY(d.yhi.alloc(R * HIDDEN * 2));
+    CUDA_TRY(d.ylo.alloc(R * HIDDEN * 2));
+    CUDA_TRY(d.qkv.alloc(R * QKV_DIM * 2));
+    CUDA_TRY(d.ctx.alloc(R * HIDDEN * 2));
+    CUDA_TRY(d.ffn.alloc(R * 3072 * 2));
     // padded / stale rows must stay finite (0 * NaN would leak through masked attention probabilities)
     CUDA_TRY(cudaMemset(d.yhi, 0, R * HIDDEN * 2));
     CUDA_TRY(cudaMemset(d.ylo, 0, R * HIDDEN * 2));
@@ -1122,12 +1159,12 @@ int alloc_dev(Runtime& rt, Dev& d) {
         if (int rc = make_map_2d(&d.act[g].ffn, d.ffn, rows, tg.inter, 128)) return rc;
     }
     for (int s = 0; s < NSLOT; ++s) {
-        CUDA_TRY(cudaMalloc(&d.ids_in[s], R * 4));
-        CUDA_TRY(cudaMalloc(&d.lens_in[s], R * 4));
+        CUDA_TRY(d.ids_in[s].alloc(R * 4));
+        CUDA_TRY(d.lens_in[s].alloc(R * 4));
         CUDA_TRY(cudaMemset(d.ids_in[s], 0, R * 4));
-        CUDA_TRY(cudaEventCreateWithFlags(&d.ev_done[s], cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreate(&d.ev_begin[s]));
-        CUDA_TRY(cudaEventCreate(&d.ev_end[s]));
+        CUDA_TRY(d.ev_done[s].create(cudaEventDisableTiming));
+        CUDA_TRY(d.ev_begin[s].create());
+        CUDA_TRY(d.ev_end[s].create());
     }
     return 0;
 }
@@ -1154,7 +1191,7 @@ int rt_init(const int* devices, int n, uint32_t flags) {
     if (rt->cap_items > 1024) return fail(B200RT_E_INVALID, "wave capacity of %d items per replica is out of range (1..1024)", rt->cap_items);
     rt->cap_rows = ((rt->cap_items * MAX_SEQ + 255) / 256) * 256;
     g_rt = rt.get();  // forward() and friends read capacity through g_rt
-    auto bail = [&](int rc) { g_rt = nullptr; return rc; };
+    auto bail = [&](int rc) { g_rt = nullptr; return rc; };  // rt goes with the return, and frees what it allocated
     if (int rc = load_driver_entry()) return bail(rc);
     const int split_sms = static_cast<int>((flags >> 16) & 0xFFu);  // B200RT_INIT_SPLIT_SMS(k): two replicas per GPU
     if (split_sms && 2 * n > ScatterPlan::MAX_SHARDS) return bail(fail(B200RT_E_INVALID, "split replicas: at most %d GPUs", ScatterPlan::MAX_SHARDS / 2));
@@ -1185,19 +1222,17 @@ int rt_init(const int* devices, int n, uint32_t flags) {
     if (cudaSetDevice(root.id) != cudaSuccess) return bail(fail(B200RT_E_CUDA, "cudaSetDevice(root)"));
     const size_t wave_rows = static_cast<size_t>(rt->cap_rows) * n;
     auto ck = [&](cudaError_t ce, const char* what) { return ce == cudaSuccess ? 0 : fail(B200RT_E_CUDA, "%s: %s", what, cudaGetErrorString(ce)); };
-    if (int rc = ck(cudaStreamCreateWithFlags(&rt->s_in, cudaStreamNonBlocking), "stream")) return bail(rc);
-    if (int rc = ck(cudaStreamCreateWithFlags(&rt->s_out, cudaStreamNonBlocking), "stream")) return bail(rc);
+    if (int rc = ck(rt->s_in.create(), "stream")) return bail(rc);
+    if (int rc = ck(rt->s_out.create(), "stream")) return bail(rc);
     for (int s = 0; s < NSLOT; ++s) {
-        if (int rc = ck(cudaMallocHost(&rt->h_ids[s], wave_rows * 4), "cudaMallocHost ids")) return bail(rc);
-        if (int rc = ck(cudaMallocHost(&rt->h_lens[s], wave_rows * 4), "cudaMallocHost lens")) return bail(rc);
-        if (int rc = ck(cudaMallocHost(&rt->h_out[s], wave_rows * HIDDEN * 4), "cudaMallocHost out")) return bail(rc);
-        if (int rc = ck(cudaMalloc(&rt->d_ids_stage[s], wave_rows * 4), "cudaMalloc")) return bail(rc);
-        if (int rc = ck(cudaMalloc(&rt->d_lens_stage[s], wave_rows * 4), "cudaMalloc")) return bail(rc);
-        if (int rc = ck(cudaMalloc(&rt->d_out_gather[s], wave_rows * HIDDEN * 4), "cudaMalloc")) return bail(rc);
-        cudaEventCreate(&rt->ev_scatter[s]);
-        cudaEventCreate(&rt->ev_wave[s]);
-        cudaEventCreate(&rt->ev_t0[s]);
-        cudaEventCreate(&rt->ev_fwd_end[s]);
+        if (int rc = ck(rt->h_ids[s].alloc(wave_rows * 4), "cudaMallocHost ids")) return bail(rc);
+        if (int rc = ck(rt->h_lens[s].alloc(wave_rows * 4), "cudaMallocHost lens")) return bail(rc);
+        if (int rc = ck(rt->h_out[s].alloc(wave_rows * HIDDEN * 4), "cudaMallocHost out")) return bail(rc);
+        if (int rc = ck(rt->d_ids_stage[s].alloc(wave_rows * 4), "cudaMalloc")) return bail(rc);
+        if (int rc = ck(rt->d_lens_stage[s].alloc(wave_rows * 4), "cudaMalloc")) return bail(rc);
+        if (int rc = ck(rt->d_out_gather[s].alloc(wave_rows * HIDDEN * 4), "cudaMalloc")) return bail(rc);
+        for (Event* ev : {&rt->ev_scatter[s], &rt->ev_wave[s], &rt->ev_t0[s], &rt->ev_fwd_end[s]})
+            if (int rc = ck(ev->create(), "cudaEventCreate")) return bail(rc);
     }
     for (auto& d : rt->devs) {
         cudaSetDevice(d->id);
@@ -1287,15 +1322,15 @@ void pre_ln_layer(Layout& L, int l, size_t H, size_t I) {
 }
 
 // the fp32 blob onto the root, an fp32 and an fp16 arena (m.f32_elems, m.f16_elems) on every replica; leaves the root current
-int upload_blob(Runtime& rt, Model& m, const float* blob, size_t nbytes, float** d_blob) {
+int upload_blob(Runtime& rt, Model& m, const float* blob, size_t nbytes, DevMem<float>& d_blob) {
     Dev& root = *rt.devs[0];
     CUDA_TRY(cudaSetDevice(root.id));
-    CUDA_TRY(cudaMalloc(d_blob, nbytes));
-    CUDA_TRY(cudaMemcpy(*d_blob, blob, nbytes, cudaMemcpyHostToDevice));
+    CUDA_TRY(d_blob.alloc(nbytes));
+    CUDA_TRY(cudaMemcpy(d_blob, blob, nbytes, cudaMemcpyHostToDevice));
     for (size_t g = 0; g < rt.devs.size(); ++g) {
         CUDA_TRY(cudaSetDevice(rt.devs[g]->id));
-        CUDA_TRY(cudaMalloc(&m.per_dev[g].f32_arena, m.f32_elems * 4));
-        CUDA_TRY(cudaMalloc(&m.per_dev[g].f16_arena, m.f16_elems * 2));
+        CUDA_TRY(m.per_dev[g].f32_arena.alloc(m.f32_elems * 4));
+        CUDA_TRY(m.per_dev[g].f16_arena.alloc(m.f16_elems * 2));
     }
     CUDA_TRY(cudaSetDevice(root.id));
     return 0;
@@ -1303,10 +1338,10 @@ int upload_blob(Runtime& rt, Model& m, const float* blob, size_t nbytes, float**
 
 // once the root's carve (enqueued on its compute stream) is done: free the blob, then the one-time broadcast of the root's
 // arenas to the other replicas over NVLink
-int broadcast_arenas(Runtime& rt, Model& m, float* d_blob) {
+int broadcast_arenas(Runtime& rt, Model& m, DevMem<float>& d_blob) {
     Dev& root = *rt.devs[0];
     CUDA_TRY(cudaStreamSynchronize(root.compute));
-    CUDA_TRY(cudaFree(d_blob));
+    CUDA_TRY(d_blob.reset());
     for (size_t g = 1; g < rt.devs.size(); ++g) {
         CUDA_TRY(cudaMemcpyPeerAsync(m.per_dev[g].f32_arena, rt.devs[g]->id, m.per_dev[0].f32_arena, root.id, m.f32_elems * 4, root.compute));
         CUDA_TRY(cudaMemcpyPeerAsync(m.per_dev[g].f16_arena, rt.devs[g]->id, m.per_dev[0].f16_arena, root.id, m.f16_elems * 2, root.compute));
@@ -1333,8 +1368,8 @@ int load_weights(Runtime& rt, Model& m, Layout& L, const float* blob, size_t nby
 
     m.per_dev.resize(rt.devs.size());
     Dev& root = *rt.devs[0];
-    float* d_blob = nullptr;
-    if (int rc = upload_blob(rt, m, blob, nbytes, &d_blob)) return rc;
+    DevMem<float> d_blob;
+    if (int rc = upload_blob(rt, m, blob, nbytes, d_blob)) return rc;
     const DevWeights& rw = m.per_dev[0];
     auto blob_at = [&](int i) -> const float* { return i < 0 ? nullptr : d_blob + L.e[i].src; };
     // a DERIVED entry may be longer than the fold that writes it (the SPLADE decoder's c, padded to its tiles): zeros past it
@@ -1383,12 +1418,12 @@ int alloc_seg_slots(Runtime& rt) {
     const size_t wave_rows = static_cast<size_t>(rt.cap_rows) * rt.devs.size();
     for (auto& d : rt.devs) {
         CUDA_TRY(cudaSetDevice(d->id));
-        for (int s = 0; s < NSLOT; ++s) CUDA_TRY(cudaMalloc(&d->segs_in[s], rt.cap_rows * 4));
+        for (int s = 0; s < NSLOT; ++s) CUDA_TRY(d->segs_in[s].alloc(rt.cap_rows * 4));
     }
     CUDA_TRY(cudaSetDevice(rt.devs[0]->id));
     for (int s = 0; s < NSLOT; ++s) {
-        CUDA_TRY(cudaMalloc(&rt.d_segs_stage[s], wave_rows * 4));
-        CUDA_TRY(cudaMallocHost(&rt.h_segs[s], wave_rows * 4));
+        CUDA_TRY(rt.d_segs_stage[s].alloc(wave_rows * 4));
+        CUDA_TRY(rt.h_segs[s].alloc(wave_rows * 4));
     }
     return 0;
 }
@@ -1519,14 +1554,14 @@ int model_load_vit(const b200rt_vit_config& c, const float* blob, size_t nbytes,
         // per-replica image input slots and constants, once
         if (!d.lens_const) {
             std::vector<int32_t> lens(VIT_WAVE_ITEMS, T);
-            CUDA_TRY(cudaMalloc(&d.lens_const, VIT_WAVE_ITEMS * 4));
+            CUDA_TRY(d.lens_const.alloc(VIT_WAVE_ITEMS * 4));
             CUDA_TRY(cudaMemcpy(d.lens_const, lens.data(), VIT_WAVE_ITEMS * 4, cudaMemcpyHostToDevice));
             if (int rc = make_map_2d(&d.m_im2col, d.ffn, static_cast<uint64_t>(rt.cap_rows) * 4, HIDDEN, 128)) return rc;
         }
-        if (!d.copy) CUDA_TRY(cudaStreamCreateWithFlags(&d.copy, cudaStreamNonBlocking));
+        if (!d.copy) CUDA_TRY(d.copy.create());
         for (int sl = 0; sl < NSLOT; ++sl) {
-            if (!d.pix_in[sl]) CUDA_TRY(cudaMalloc(&d.pix_in[sl], VIT_WAVE_ITEMS * m->item_bytes));
-            if (!d.ev_pix[sl]) CUDA_TRY(cudaEventCreateWithFlags(&d.ev_pix[sl], cudaEventDisableTiming));
+            if (!d.pix_in[sl]) CUDA_TRY(d.pix_in[sl].alloc(VIT_WAVE_ITEMS * m->item_bytes));
+            if (!d.ev_pix[sl]) CUDA_TRY(d.ev_pix[sl].create(cudaEventDisableTiming));
         }
     }
     rt.vit_item_bytes = item_bytes;
@@ -1621,12 +1656,10 @@ int model_load_nomic(const b200rt_nomic_bert_config& nc, const float* blob, size
         DevWeights& w = m->per_dev[g];
         CUDA_TRY(cudaSetDevice(d.id));
         CUDA_TRY(cudaMemcpyAsync(w.rope, rope.data(), rope.size() * sizeof(float2), cudaMemcpyHostToDevice, d.compute));
-        __half* sw = nullptr;
-        float* sc = nullptr;
-        CUDA_TRY(cudaMalloc(&sw, 2 * I * H * 2));
-        std::unique_ptr<void, cudaError_t (*)(void*)> free_sw(sw, cudaFree);  // freed on every return (cudaFree waits for the device)
-        CUDA_TRY(cudaMalloc(&sc, 2 * I * 4));
-        std::unique_ptr<void, cudaError_t (*)(void*)> free_sc(sc, cudaFree);
+        DevMem<__half> sw;  // freed on every return (freeing waits for the device)
+        DevMem<float> sc;
+        CUDA_TRY(sw.alloc(2 * I * H * 2));
+        CUDA_TRY(sc.alloc(2 * I * 4));
         for (int l = 0; l < c.layers; ++l) {
             LayerW& lw = w.layers[l];
             lw.ao_b = lw.ff2_b = w.zero_bias;  // no biases
@@ -1683,37 +1716,25 @@ int check_ids(const Model& m, const int32_t* ids, const int32_t* lens, int n_ite
     return 0;
 }
 
-// Device buffers and timing events of one debug entry (b200rt_debug_embed & co.): buffers are filled from the host (or
-// zeroed) in stream order on allocation, and everything is freed when the entry returns, on success or on error.
+// Device buffers of one debug entry (b200rt_debug_embed & co.): buffers are filled from the host (or zeroed) in stream order
+// on allocation, and freed once the stream has drained when the entry returns, on success or on error.
 struct DebugBuffers {
     cudaStream_t stream;
-    std::vector<void*> ptrs;
-    std::vector<cudaEvent_t> evs;
+    std::vector<DevMem<void>> ptrs;
     explicit DebugBuffers(cudaStream_t s) : stream(s) {}
-    DebugBuffers(const DebugBuffers&) = delete;
-    DebugBuffers& operator=(const DebugBuffers&) = delete;
-    ~DebugBuffers() {
-        cudaStreamSynchronize(stream);
-        for (void* p : ptrs) cudaFree(p);
-        for (cudaEvent_t e : evs) cudaEventDestroy(e);
-    }
+    ~DebugBuffers() { cudaStreamSynchronize(stream); }
     template <typename T>
     cudaError_t upload(T** dp, const void* host, size_t bytes) {  // host NULL: zeros
-        void* p = nullptr;
-        cudaError_t e = cudaMalloc(&p, bytes);
+        ptrs.emplace_back();
+        cudaError_t e = ptrs.back().alloc(bytes);
         if (e != cudaSuccess) return e;
-        ptrs.push_back(p);
+        void* p = ptrs.back();
         *dp = static_cast<T*>(p);
         return host ? cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, stream) : cudaMemsetAsync(p, 0, bytes, stream);
     }
     cudaError_t download(void* host, const void* dev, size_t bytes) {
         cudaError_t e = cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, stream);
         return e != cudaSuccess ? e : cudaStreamSynchronize(stream);
-    }
-    cudaError_t event(cudaEvent_t* ev) {
-        cudaError_t e = cudaEventCreate(ev);
-        if (e == cudaSuccess) evs.push_back(*ev);
-        return e;
     }
 };
 
@@ -2132,34 +2153,8 @@ void b200rt_shutdown(void) {
         cudaSetDevice(d->id);
         cudaDeviceSynchronize();
     }
-    for (auto& m : rt->models)
-        for (size_t g = 0; g < m->per_dev.size(); ++g) {
-            cudaSetDevice(rt->devs[g]->id);
-            cudaFree(m->per_dev[g].f32_arena);
-            cudaFree(m->per_dev[g].f16_arena);
-        }
-    for (auto& d : rt->devs) {
-        cudaSetDevice(d->id);
-        drop_graphs(*d);
-        cudaFree(d->pstats[0]); cudaFree(d->pstats[1]); cudaFree(d->yhi); cudaFree(d->ylo); cudaFree(d->qkv); cudaFree(d->ctx); cudaFree(d->ffn);
-        cudaFree(d->lens_const);
-        if (d->copy) cudaStreamDestroy(d->copy);
-        for (int s = 0; s < NSLOT; ++s) if (d->ev_pix[s]) cudaEventDestroy(d->ev_pix[s]);
-        for (int s = 0; s < NSLOT; ++s) { cudaFree(d->pix_in[s]); cudaFree(d->ids_in[s]); cudaFree(d->lens_in[s]); cudaFree(d->segs_in[s]); cudaEventDestroy(d->ev_done[s]); cudaEventDestroy(d->ev_begin[s]); cudaEventDestroy(d->ev_end[s]); }
-        cudaEventDestroy(d->ev_ws);
-        cudaStreamDestroy(d->compute);
-    }
-    cudaSetDevice(rt->devs[0]->id);
-    for (int s = 0; s < NSLOT; ++s) {
-        cudaFreeHost(rt->h_ids[s]); cudaFreeHost(rt->h_lens[s]); cudaFreeHost(rt->h_out[s]);
-        cudaFree(rt->d_ids_stage[s]); cudaFree(rt->d_lens_stage[s]); cudaFree(rt->d_out_gather[s]);
-        if (rt->h_segs[s]) cudaFreeHost(rt->h_segs[s]);
-        cudaFree(rt->d_segs_stage[s]);
-        cudaEventDestroy(rt->ev_scatter[s]); cudaEventDestroy(rt->ev_wave[s]); cudaEventDestroy(rt->ev_t0[s]); cudaEventDestroy(rt->ev_fwd_end[s]);
-    }
-    cudaStreamDestroy(rt->s_in);
-    cudaStreamDestroy(rt->s_out);
-    delete rt;
+    cudaSetDevice(rt->devs[0]->id);  // the caller's thread is left on the root device
+    delete rt;  // with every buffer, stream, event and graph of its replicas and models, each released on its own device
     g_rt = nullptr;
 }
 
@@ -2240,9 +2235,9 @@ int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const fl
         cudaError_t ce = cudaMemcpyAsync(dhi, dhi0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute);
         return ce != cudaSuccess ? ce : cudaMemcpyAsync(dlo, dlo0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute);
     };
-    cudaEvent_t e0, e1;
-    CUDA_TRY(b.event(&e0));
-    CUDA_TRY(b.event(&e1));
+    Event e0, e1;
+    CUDA_TRY(e0.create());
+    CUDA_TRY(e1.create());
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
     for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
@@ -2300,9 +2295,9 @@ int b200rt_debug_attention_ex(const uint16_t* qkv, const int32_t* lens, uint16_t
     CUtensorMap tq, tc;
     if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, head_dim)) return rc;
     if (int rc = make_map_qkv(&tc, dc, B, S, H, head_dim)) return rc;
-    cudaEvent_t e0, e1;
-    CUDA_TRY(b.event(&e0));
-    CUDA_TRY(b.event(&e1));
+    Event e0, e1;
+    CUDA_TRY(e0.create());
+    CUDA_TRY(e1.create());
     if (iters < 1) iters = 1;
     CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads, causal));
     CUDA_TRY(cudaEventRecord(e0, d.compute));
@@ -2446,9 +2441,9 @@ int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* 
     const GemmEpi e{dc, dst, static_cast<int>(P), nullptr, nullptr, nullptr, eps};
     const SpladeEpi sp{dl_, S, dmax, vocab};
     const int grid_sms = sms ? sms : d.sm_count;
-    cudaEvent_t e0, e1;
-    CUDA_TRY(b.event(&e0));
-    CUDA_TRY(b.event(&e1));
+    Event e0, e1;
+    CUDA_TRY(e0.create());
+    CUDA_TRY(e1.create());
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
     for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute));
@@ -2552,9 +2547,9 @@ int b200rt_debug_attention_stream(const uint16_t* qkv, const int32_t* lens, int 
     CUDA_TRY(launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute));
     CUDA_TRY(b.download(ctx, dc, M * H * 2));
     if (iters > 0) {
-        cudaEvent_t e0, e1;
-        CUDA_TRY(b.event(&e0));
-        CUDA_TRY(b.event(&e1));
+        Event e0, e1;
+        CUDA_TRY(e0.create());
+        CUDA_TRY(e1.create());
         CUDA_TRY(cudaEventRecord(e0, d.compute));
         for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute));
         CUDA_TRY(cudaEventRecord(e1, d.compute));
