@@ -490,8 +490,12 @@ static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __ha
         return cudaErrorInvalidValue;
     }
     const bool six = e.stats_in == nullptr || e.parts_in == 6;
-    if (wide) return six ? launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas)
-                         : launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+    if (wide) {
+        if (six) return launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+        // three partials re-applied by the residual epilogue mean N = 384, never a multiple of 256: no <RES_SPLIT, 256, 3>
+        if constexpr (EPI != EPI_BIAS_RES_SPLIT) return launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+        return cudaErrorInvalidValue;
+    }
     return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas)
                : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
 }
@@ -516,7 +520,8 @@ template <int EPI>
 static cudaError_t setup_epi() {
     cudaError_t e;
     if ((e = setup<EPI, 256, 6>()) != cudaSuccess) return e;
-    if ((e = setup<EPI, 256, 3>()) != cudaSuccess) return e;
+    if constexpr (EPI != EPI_BIAS_RES_SPLIT)
+        if ((e = setup<EPI, 256, 3>()) != cudaSuccess) return e;
     if ((e = setup<EPI, 128, 6>()) != cudaSuccess) return e;
     if ((e = setup<EPI, 128, 3>()) != cudaSuccess) return e;
     if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16)

@@ -166,7 +166,10 @@ def test_gemm_small_geometry_epilogues(rt, epi, N, K, M):
         KR.check_gemm(f"epi {epi} M={M} N={N} K={K}", out, epi, *args, **kw)
 
 
-@pytest.mark.parametrize("K", [384, 1536])
+RESIDUAL_NO_LN_KS = [384, 1536]
+
+
+@pytest.mark.parametrize("K", RESIDUAL_NO_LN_KS)
 def test_residual_epilogue_three_partials_without_stats_in(rt, K):
     """stats_in = NULL (the residual added as is) at N = 384: 3 partials of the new rows, including rows of mean 150."""
     M, N = 300, 384

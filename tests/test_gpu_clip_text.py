@@ -78,13 +78,16 @@ def test_plain_debug_gemm_keeps_refusing_a_512_wide_layernorm(rt):
     assert e.value.code == rt.E_INVALID
 
 
+LN512_CASES = ((0, 1536), (3, 2048))  # (epi, N): the tower's QKV and quick-GELU FFN1, K = 512 (4 partials)
+
+
 @pytest.mark.parametrize("M", [1, 127, 128, 129, 300])
 def test_gemm_512_wide_layernorm_epilogues(rt, M):
     rng = np.random.default_rng(M)
     y = (rng.standard_normal((M, 512)) * 3 + 0.5).astype(np.float32)
     st = KR.partials(y.astype(np.float64)).astype(np.float32)
     a16 = y.astype(np.float16)
-    for epi, N in ((0, 1536), (3, 2048)):
+    for epi, N in LN512_CASES:
         w = (rng.standard_normal((N, 512)) * 0.03).astype(np.float32)
         w16 = (w - w.mean(1, keepdims=True)).astype(np.float16)
         bias = (rng.standard_normal(N) * 0.1).astype(np.float32)

@@ -72,8 +72,10 @@ def _same(a, b):
 
 
 # (epi, N, K, stats_out): every epilogue at BN = 256 (N = 768) and BN = 128 (N = 384), the residual one with and without
-# the row statistics of its output
-EPILOGUES = [(e, n, n, st) for n in (768, 384) for e, st in ((0, False), (1, False), (3, False), (2, True), (2, False))]
+# the row statistics of its output; then the folded epilogues' other pairings of tile width and partials: BN = 128 with a
+# 768-wide LayerNorm (6 partials) and BN = 256 with a 384-wide one (3 partials)
+EPILOGUES = ([(e, n, n, st) for n in (768, 384) for e, st in ((0, False), (1, False), (3, False), (2, True), (2, False))]
+             + [(e, 384, 768, False) for e in (0, 1, 3)] + [(e, 768, 384, False) for e in (0, 1, 3)])
 
 
 @gpu
@@ -270,8 +272,11 @@ def test_swiglu_partner_tile_past_m(rt, M, ln):
     _past_m(rt, f"swiglu M={M} ({_bm_tiles(M)} m-tiles) ln={ln}", run, check)
 
 
+SPLADE_KS = [384, 768, 1024]  # PARTS 3, 6, 8
+
+
 @gpu
-@pytest.mark.parametrize("K", [384, 768, 1024])
+@pytest.mark.parametrize("K", SPLADE_KS)
 @pytest.mark.parametrize("B,S,vocab", SPLADE_PAST_M)
 def test_splade_partner_tile_past_m(rt, B, S, vocab, K):
     """The maxima are an integer max of fp32 bits (order-independent), so any bitwise difference is a real bug."""
