@@ -345,10 +345,11 @@ struct Dev {
     DevMem<__half> yhi, ylo;  // residual stream y = hi + lo, PRE-LayerNorm; hi doubles as the GEMM A operand
     DevMem<float2> pstats[2];  // [rows][STAT_PARTS] (sum, M2) partials: [0] embedding LN / LN2 inputs, [1] LN1 inputs
     DevMem<__half> qkv, ctx, ffn;
-    // fp16 [rows, *] box {64,128}: GEMM A operands, per TEXT_GEOMETRIES entry, each over that geometry's model_cap_rows rows
-    // (a model reads the same buffers densely at its own widths)
+    // fp16 [rows, *] box {64,128}: GEMM A operands and the residual stream (res: hi, lo), per TEXT_GEOMETRIES entry, each over
+    // that geometry's model_cap_rows rows (a model reads the same buffers densely at its own widths)
     struct ActMaps {
-        CUtensorMap yhi, ctx, ffn;
+        ResEpi res;  // res.hi doubles as the A operand of QKV and FFN1
+        CUtensorMap ctx, ffn;
     } act[N_TEXT_GEOMETRIES];
     std::map<std::pair<int, int>, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per (padded length, hidden)
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
@@ -555,7 +556,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             CUDA_TRY(launch_im2col(in.pixels, d.ffn, B, c.image, c.patch, stream));
             if (step("im2col")) return 0;
             GemmEpi e_patch{w.zero_bias, nullptr, P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, nullptr, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
             if (step("gemm_patch")) return 0;
             CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, S, m.eps, stream));
             if (step("vit_embed")) return 0;
@@ -574,31 +575,31 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
             GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
             if (ls.rotary) {
-                CUDA_TRY(launch_gemm_rope(am.yhi, lw.m_qkv, d.qkv, e_qkv, RopeEpi{reinterpret_cast<const float2*>(w.rope), S, 2 * H}, M, 3 * H, H, d.sm_gemm, stream));
+                CUDA_TRY(launch_gemm_rope(am.res.hi, lw.m_qkv, d.qkv, e_qkv, RopeEpi{reinterpret_cast<const float2*>(w.rope), S, 2 * H}, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv_rope")) return 0;
                 CUDA_TRY(launch_attention_stream(*mq, d.ctx, lens, B, S, d.sm_attn, stream));
                 if (step("attention_stream")) return 0;
             } else {
-                CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.yhi, lw.m_qkv, d.qkv, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
+                CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.res.hi, lw.m_qkv, d.qkv, nullptr, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv")) return 0;
                 CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, ls.causal));
                 if (step("attention")) return 0;
             }
             // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
             const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, e_ao, M, H, H, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, &am.res, e_ao, M, H, H, d.sm_gemm, stream));
             if (step("gemm_attn_out")) return 0;
             GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
             if (ls.rotary) {
-                CUDA_TRY(launch_gemm_swiglu(am.yhi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
+                CUDA_TRY(launch_gemm_swiglu(am.res.hi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
                 if (step("gemm_ffn1_swiglu")) return 0;
             } else {
-                CUDA_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.yhi, lw.m_ff1, d.ffn, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+                CUDA_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.res.hi, lw.m_ff1, d.ffn, nullptr, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
                 if (step(ls.pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
             }
             // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
             const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, e_ff2, M, H, I, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, &am.res, e_ff2, M, H, I, d.sm_gemm, stream));
             if (step("gemm_ffn2")) return 0;
             prev_g = lw.ln2_g;
             prev_b = lw.ln2_b;
@@ -610,7 +611,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             // decoder GEMM max-reduces relu(LN_t(u) W_dec^T + b) over each item's valid tokens into it, and never stores the
             // [M, vocab] logits; log1p once per (item, word) into out
             GemmEpi e_t{w.mlm_t_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.yhi, w.m_mlm_t, d.ctx, nullptr, e_t, M, H, H, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.res.hi, w.m_mlm_t, d.ctx, nullptr, nullptr, e_t, M, H, H, d.sm_gemm, stream));
             if (step("gemm_mlm_transform")) return 0;
             uint32_t* vmax = reinterpret_cast<uint32_t*>(d.ffn.get());
             CUDA_TRY(launch_mlm_ln_stats(d.ctx, d.pstats[1], vmax, M, static_cast<size_t>(B) * m.splade_vpad, H, stream));
@@ -1154,7 +1155,8 @@ int alloc_dev(Runtime& rt, Dev& d) {
         const TextGeometry& tg = TEXT_GEOMETRIES[g];
         const size_t rows = model_cap_rows(rt.cap_rows, tg.hidden);
         if (rows < 128) continue;  // no model of this width can be loaded (model_load refuses it)
-        if (int rc = make_map_2d(&d.act[g].yhi, d.yhi, rows, tg.hidden, 128)) return rc;
+        if (int rc = make_map_2d(&d.act[g].res.hi, d.yhi, rows, tg.hidden, 128)) return rc;
+        if (int rc = make_map_2d(&d.act[g].res.lo, d.ylo, rows, tg.hidden, 128)) return rc;
         if (int rc = make_map_2d(&d.act[g].ctx, d.ctx, rows, tg.hidden, 128)) return rc;
         if (int rc = make_map_2d(&d.act[g].ffn, d.ffn, rows, tg.inter, 128)) return rc;
     }
@@ -2210,6 +2212,7 @@ int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const fl
     if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
     if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
     std::vector<__half> hhi, hlo;
+    ResEpi res{};  // epi 2: TMA maps over the residual's hi and lo
     if (epi == 2) {
         // the residual travels as hi + lo (fp16 + fp16): split on the host, keep a pristine copy for the final launch
         hhi.assign(Mp * N, __float2half_rn(0.f));
@@ -2223,6 +2226,8 @@ int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const fl
         CUDA_TRY(b.upload(&dhi, hhi.data(), Mp * N * 2));
         CUDA_TRY(b.upload(&dlo, hlo.data(), Mp * N * 2));
         CUDA_TRY(b.upload(&dso, nullptr, Mp * parts_out * sizeof(float2)));
+        if (int rc = make_map_2d(&res.hi, dhi, Mp, N, 128)) return rc;
+        if (int rc = make_map_2d(&res.lo, dlo, Mp, N, 128)) return rc;
     } else {
         CUDA_TRY(b.upload(&dout, nullptr, Mp * N * 2));
         CUDA_TRY(cudaMemsetAsync(dout, 0xFF, Mp * N * 2, d.compute));
@@ -2240,10 +2245,10 @@ int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const fl
     CUDA_TRY(e1.create());
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(reload());
-    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, e, M, N, K, grid_sms, d.compute, ctas_out));  // the result that is returned
+    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, e, M, N, K, grid_sms, d.compute, ctas_out));  // the result that is returned
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);

@@ -22,6 +22,22 @@
 // A cluster barrier after the barrier init (before any remote arrive or multicast) and one before exit (so that no CTA leaves
 // while the peer may still arrive on its barriers) bracket the protocol; every thread of both warpgroups takes both.
 //
+// EPI_BIAS_RES_SPLIT brings the tile's residual in through the same ring: after the tile's last k-block the producer takes
+// BN / 64 more entries, one per 64-column chunk q, each the hi box [128 rows x 64 columns] at (n0 + 64q, m0) at the stage's
+// offset 0 and the lo box at 16 KB (expect_tx 32 KB; own rows only, not multicast).  The consumers wait on full[s], read the
+// chunk from shared memory, store it and arrive on empty[s] exactly as for an operand stage (8 CM arrivals).  Both CTAs walk
+// the same pairs with the same K and BN, so both add the same entries at the same points and the rings stay in lockstep; a
+// tile past M loads the map's rows there or out-of-bounds zeros, with the full byte count either way, and stores nothing.
+// Each thread writes hi' and lo' over the very values it read; a named barrier over the consumer warpgroup then lets its 128
+// threads copy the warpgroup's 64 rows of the chunk to global memory as 16-byte pieces of whole 128-byte rows (rows < M).
+//   * The stage is read and written by the generic proxy (ld/st.shared), and its next write is a TMA (async proxy) of this
+//     CTA's producer or, for a W box, the peer's.  Every consumer thread issues fence.proxy.async after its last access,
+//     so its shared-memory writes are ordered before any later async-proxy write; its reads have returned their values
+//     (they were stored to global memory) before the __syncwarp ahead of its warp's arrive; the arrive releases both, and a
+//     producer issues the TMA only after its wait on empty[s] has acquired all 8 CM arrivals.
+//   * Each element of y is written in place by the one tile that owns it, after that tile's TMA has read it (the consumer
+//     stores only after its wait on full[s] saw the read complete).  Tiles are disjoint, so no tile reads what another wrote.
+//
 // Epilogues (see kernels.h for the residual-stream format):
 //   EPI_BIAS(_GELU / _QGELU)_F16 : folded LayerNorm  rstd * acc + c  (c = W beta + b), optional GELU, fp16 out;
 //   EPI_BIAS_RES_SPLIT           : y' = acc + bias + LN(y) with the LayerNorm re-applied from the row's statistics, y' split
@@ -55,6 +71,7 @@ constexpr int A_BYTES = BM * BK * 2;            // 16 KB
 constexpr int W_BOX_BYTES = 128 * BK * 2;       // one 128-row TMA box of W: 16 KB
 constexpr int NUM_THREADS = 384;
 constexpr int CM = 2;  // CTAs per cluster, along M, sharing every W tile
+constexpr int RES_BOX_BYTES = BM * 64 * 2;      // EPI_BIAS_RES_SPLIT: one [128 x 64] box of hi or lo, 16 KB
 
 // ring layout of the BN-column kernel
 template <int BN>
@@ -162,12 +179,13 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float e
 }
 
 // BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128).  sp is read by
-// EPI_SPLADE_MAX only, rp by EPI_ROPE_F16 only; as the last parameters they leave every other instantiation's parameter
-// offsets as they were.
+// EPI_SPLADE_MAX only, rp by EPI_ROPE_F16 only, res by EPI_BIAS_RES_SPLIT only; as the last parameters they leave every other
+// instantiation's parameter offsets as they were.
 template <int EPI, int BN, int PARTS>
 __global__ void __cluster_dims__(CM, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
-            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K, const SpladeEpi sp, const RopeEpi rp) {
+            __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K, const SpladeEpi sp, const RopeEpi rp,
+            const __grid_constant__ ResEpi res) {
     static_assert(BN == 256 || BN == 128, "tile width");
     constexpr int STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
     constexpr int NACC = BN / 2;     // fp32 accumulators per consumer thread
@@ -191,6 +209,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     if (threadIdx.x == 0) {
         prefetch_tmap(&tma_a);
         prefetch_tmap(&tma_b);
+        if constexpr (EPI == EPI_BIAS_RES_SPLIT) {
+            prefetch_tmap(&res.hi);
+            prefetch_tmap(&res.lo);
+        }
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 8 * CM);  // the 8 consumer warps of every CTA of the cluster
@@ -218,6 +240,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
                         tma_load_2d_multicast(sa + A_BYTES + b * W_BOX_BYTES, &tma_b, &full[stage], kb * BK, n0 + 128 * b,
                                               (1u << CM) - 1);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+                if constexpr (EPI == EPI_BIAS_RES_SPLIT) {
+                    for (int q = 0; q < BN / 64; ++q) {  // the tile's residual, one 64-column chunk of hi and lo per entry
+                        mbar_wait(&empty[stage], phase ^ 1);
+                        uint8_t* sr = smem + stage * STAGE_BYTES;
+                        mbar_arrive_expect_tx(&full[stage], 2 * RES_BOX_BYTES);
+                        tma_load_2d(sr, &res.hi, &full[stage], n0 + 64 * q, m0);
+                        tma_load_2d(sr + RES_BOX_BYTES, &res.lo, &full[stage], n0 + 64 * q, m0);
+                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                    }
                 }
             }
         }
@@ -390,33 +422,64 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             // y' = acc + bias + LN(y); LN(y) = fmaf((y - mean) * rstd, gamma, beta) (stats_in NULL: the residual is added as is)
             float csum[2][NSLICE] = {};  // [row][128-column slice of the tile]
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int col = c0 + 8 * j;
-                const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + col));
-                float2 gm = make_float2(1.f, 1.f), bt = make_float2(0.f, 0.f);
-                if (has_ln) {
-                    gm = __ldg(reinterpret_cast<const float2*>(ep.ln_gamma + col));
-                    bt = __ldg(reinterpret_cast<const float2*>(ep.ln_beta + col));
-                }
+            for (int q = 0; q < BN / 64; ++q) {
+                // the ring entry of columns n0 + 64q ..: this thread's rows of the boxes are 64 cw + 16 w4 + lane / 4 + 8 h, and
+                // 128B swizzle puts 16-byte column group jj of box row r at (jj ^ r % 8) * 16 -- r % 8 = lane / 4 for both rows,
+                // so a warp's 32 reads fall in 32 distinct banks.  hi' and lo' go back over the values they replace, and the
+                // warpgroup then stores its 64 rows of the chunk as whole 128-byte rows instead of 4-byte fragments.
+                mbar_wait(&full[stage], phase);
+                const uint32_t sbase = smem_u32(smem + stage * STAGE_BYTES);
+                const uint32_t box = sbase + (cw * 64 + w4 * 16 + (lane >> 2)) * 128 + 4 * (lane & 3);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = r0 + 8 * h;
-                    float& v0 = acc[4 * j + 2 * h];
-                    float& v1 = acc[4 * j + 2 * h + 1];
-                    if (row < M) {
-                        const size_t off = static_cast<size_t>(row) * N + col;
-                        const float2 hv = __half22float2(*reinterpret_cast<const __half2*>(out + off));
-                        const float2 lv = __half22float2(*reinterpret_cast<const __half2*>(out_lo + off));
-                        v0 = v0 + bv.x + fmaf((hv.x + lv.x - mean[h]) * rstd[h], gm.x, bt.x);
-                        v1 = v1 + bv.y + fmaf((hv.y + lv.y - mean[h]) * rstd[h], gm.y, bt.y);
-                        // split y' = hi' + lo' and write both back in place
-                        const __half2 hp = __floats2half2_rn(v0, v1);
-                        const float2 hb = __half22float2(hp);
-                        *reinterpret_cast<__half2*>(out + off) = hp;
-                        *reinterpret_cast<uint32_t*>(out_lo + off) = pack_half2(v0 - hb.x, v1 - hb.y);
+                for (int j = 8 * q; j < 8 * q + 8; ++j) {
+                    const int col = c0 + 8 * j;
+                    const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + col));
+                    float2 gm = make_float2(1.f, 1.f), bt = make_float2(0.f, 0.f);
+                    if (has_ln) {
+                        gm = __ldg(reinterpret_cast<const float2*>(ep.ln_gamma + col));
+                        bt = __ldg(reinterpret_cast<const float2*>(ep.ln_beta + col));
                     }
-                    csum[h][j >> 4] += v0 + v1;
+                    const uint32_t sw = static_cast<uint32_t>((j & 7) ^ (lane >> 2)) << 4;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = r0 + 8 * h;
+                        float& v0 = acc[4 * j + 2 * h];
+                        float& v1 = acc[4 * j + 2 * h + 1];
+                        if (row < M) {
+                            const uint32_t a = box + h * (8 * 128) + sw;
+                            const float2 hv = __half22float2(lds_half2(a));
+                            const float2 lv = __half22float2(lds_half2(a + RES_BOX_BYTES));
+                            v0 = v0 + bv.x + fmaf((hv.x + lv.x - mean[h]) * rstd[h], gm.x, bt.x);
+                            v1 = v1 + bv.y + fmaf((hv.y + lv.y - mean[h]) * rstd[h], gm.y, bt.y);
+                            // split y' = hi' + lo'
+                            const __half2 hp = __floats2half2_rn(v0, v1);
+                            const float2 hb = __half22float2(hp);
+                            sts32(a, *reinterpret_cast<const uint32_t*>(&hp));
+                            sts32(a + RES_BOX_BYTES, pack_half2(v0 - hb.x, v1 - hb.y));
+                        }
+                        csum[h][j >> 4] += v0 + v1;
+                    }
                 }
+                named_bar_sync(1 + cw, 128);  // the warpgroup's 64 rows of hi' and lo' are in the stage
+                {
+                    // 128 threads x 16 bytes: 16 rows per pass, a warp covering 4 whole rows; unit u = row 8 + column group
+                    const int t = threadIdx.x - 128 * (cw + 1);
+#pragma unroll 1
+                    for (int pass = 0; pass < 8; ++pass) {  // rolled: the 128 accumulators leave room for one value in flight
+                        const int u = (pass & 3) * 128 + t, lr = u >> 3, cg = u & 7;
+                        const int row = m0 + cw * 64 + lr;
+                        const uint32_t a = sbase + (pass >> 2) * RES_BOX_BYTES + (cw * 64 + lr) * 128 + ((cg ^ (lr & 7)) << 4);
+                        const uint4 v = lds128(a);
+                        if (row < M)
+                            *reinterpret_cast<uint4*>(((pass >> 2) ? out_lo : out) + static_cast<size_t>(row) * N + n0 + 64 * q + 8 * cg) = v;
+                    }
+                }
+                // every lane's reads of the stage are done, and its shared-memory writes ordered before the TMA that will
+                // overwrite the stage, before its warp's arrivals hand it back
+                fence_proxy_async_smem();
+                __syncwarp();
+                if (lane < CM) mbar_arrive_cluster(&empty[stage], lane);
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
             if (ep.stats_out != nullptr) {
                 // (sum, M2 about the slice mean) of each 128-column slice of the new rows: the four threads of a quad share a row
@@ -460,13 +523,13 @@ static int& max_clusters() {
 template <int EPI, int BN, int PARTS>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                               int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{},
-                              const RopeEpi& rp = RopeEpi{}) {
+                              const RopeEpi& rp = RopeEpi{}, const ResEpi& res = ResEpi{}) {
     const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
     int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
     if (clusters < 1) clusters = 1;
     if (ctas) *ctas = clusters * gemm::CM;
     return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::smem_bytes<EPI, BN>(),
-                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp);
+                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp, res);
 }
 
 // the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT / CLIP text
@@ -474,30 +537,30 @@ static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __ha
 // bge-large N is a multiple of 256.  Four partials (the CLIP text tower's 512-wide LayerNorm, folded into QKV and the quick-GELU
 // FFN1) exist for BN = 256 and EPI 0 / 3 only; its residual epilogues take no statistics (pre-LN, stats_in NULL).
 template <int EPI>
-static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                              int K, int sm_count, cudaStream_t stream, int* ctas) {
+static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi& res, const GemmEpi& e,
+                              int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
     const bool wide = N % 256 == 0;
     if (e.stats_in != nullptr && e.parts_in == 8) {
         if constexpr (EPI != EPI_BIAS_QGELU_F16) {
-            if (wide) return launch_one<EPI, 256, 8>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+            if (wide) return launch_one<EPI, 256, 8>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
         }
         return cudaErrorInvalidValue;
     }
     if (e.stats_in != nullptr && e.parts_in == 4) {
         if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16) {
-            if (wide) return launch_one<EPI, 256, 4>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+            if (wide) return launch_one<EPI, 256, 4>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
         }
         return cudaErrorInvalidValue;
     }
     const bool six = e.stats_in == nullptr || e.parts_in == 6;
     if (wide) {
-        if (six) return launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+        if (six) return launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
         // three partials re-applied by the residual epilogue mean N = 384, never a multiple of 256: no <RES_SPLIT, 256, 3>
-        if constexpr (EPI != EPI_BIAS_RES_SPLIT) return launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+        if constexpr (EPI != EPI_BIAS_RES_SPLIT) return launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
         return cudaErrorInvalidValue;
     }
-    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas)
-               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res)
+               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
 }
 
 template <int EPI, int BN, int PARTS>
@@ -543,8 +606,8 @@ cudaError_t gemm_init_device() {
     return setup<EPI_SWIGLU_F16, 256, 6>();
 }
 
-cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                        int K, int sm_count, cudaStream_t stream, int* ctas) {
+cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi* res,
+                        const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
     if (N % 128 != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
     // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 1024, 768,
     // 512 or 384
@@ -552,13 +615,14 @@ cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, _
     if (e.stats_in != nullptr && ((e.parts_in != 8 && e.parts_in != 6 && e.parts_in != 4 && e.parts_in != 3) || e.parts_in * 128 != ln_width))
         return cudaErrorInvalidValue;
     switch (epi) {
-        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, ResEpi{}, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, ResEpi{}, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, ResEpi{}, e, M, N, K, sm_count, stream, ctas);
         case EPI_BIAS_RES_SPLIT:
-            if (out_lo == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr))) return cudaErrorInvalidValue;
+            if (out_lo == nullptr || res == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr)))
+                return cudaErrorInvalidValue;
             if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
-            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas);
+            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, *res, e, M, N, K, sm_count, stream, ctas);
     }
     return cudaErrorInvalidValue;
 }

@@ -331,6 +331,19 @@ __device__ __forceinline__ float4 lds128f(uint32_t addr) {
 __device__ __forceinline__ void sts32f(uint32_t addr, float a) {
     asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(a) : "memory");
 }
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t a) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
+}
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ __half2 lds_half2(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return *reinterpret_cast<__half2*>(&v);
+}
 
 // ------------------------------------------------------------------------------------ thread-block clusters
 
