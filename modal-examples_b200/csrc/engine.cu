@@ -352,6 +352,7 @@ struct Dev {
         CUtensorMap ctx, ffn;
     } act[N_TEXT_GEOMETRIES];
     std::map<std::pair<int, int>, std::pair<CUtensorMap, CUtensorMap>> m_qkv_by_S;  // (qkv, ctx) 3D maps per (padded length, hidden)
+    std::map<std::tuple<const void*, int, int>, OutEpi> m_out_by_M;  // EPI 0/1/3 output maps per (buffer, width, rows): see get_out_maps
     // wave input slots (written by the root's scatter kernel, possibly over NVLink)
     DevMem<int32_t> ids_in[NSLOT], lens_in[NSLOT];
     DevMem<int32_t> segs_in[NSLOT];  // classifier waves' segment starts (allocated when the first classifier model loads)
@@ -515,6 +516,33 @@ int get_qkv_map(Dev& d, const Model& model, int S, const CUtensorMap** out, cons
     return 0;
 }
 
+// The output maps of a forward's EPI 0/1/3 GEMMs (kernels.h: {width, M} over the buffer each writes, exactly M rows), made once
+// per (buffer, width, M) -- as many as the wave shapes a replica meets -- and kept on the replica.  Making a map is host work:
+// forward() makes a forward's maps ahead of a graph capture, as for get_qkv_map.
+struct OutMaps {
+    const OutEpi *qkv = nullptr, *ffn = nullptr, *ctx = nullptr;  // QKV; GELU / quick-GELU FFN1; ViT patch, SPLADE transform
+};
+int get_out_maps(Dev& d, const Model& m, int M, OutMaps* om) {
+    auto get = [&](const __half* buf, int width, const OutEpi** out) {
+        const auto key = std::make_tuple(static_cast<const void*>(buf), width, M);
+        auto it = d.m_out_by_M.find(key);
+        if (it == d.m_out_by_M.end()) {
+            OutEpi oe;
+            if (int rc = make_map_2d(&oe.out, buf, M, width, 64)) return rc;
+            it = d.m_out_by_M.emplace(key, oe).first;
+        }
+        *out = &it->second;
+        return 0;
+    };
+    if (!layer_style(m).rotary) {
+        if (int rc = get(d.qkv, 3 * m.hidden, &om->qkv)) return rc;
+        if (int rc = get(d.ffn, m.inter, &om->ffn)) return rc;
+    }
+    if (m.kind == VIT || m.kind == BERT_SPLADE)
+        if (int rc = get(d.ctx, m.hidden, &om->ctx)) return rc;
+    return 0;
+}
+
 // Enqueue the forward of one padded batch on `stream` and add the launches it enqueued to `launches`.  out: fp32 [B, out_dim],
 // may be peer memory.  Widths, statistic partials and the attention head size follow the model's geometry: three stages, the
 // embedding, the encoder layers as the kind's layer_style runs them, and the kind's head.
@@ -532,6 +560,8 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
     const Dev::ActMaps& am = d.act[text_geometry(H)];
     const CUtensorMap *mq = nullptr, *mc = nullptr;
     if (int rc = get_qkv_map(d, m, S, &mq, &mc)) return rc;
+    OutMaps om;
+    if (int rc = get_out_maps(d, m, M, &om)) return rc;
     const int32_t* lens = vit ? d.lens_const : in.lens;
     // residual epilogue: y <- acc + bias + LN(y), LN given by (stats, gamma, beta) -- or + y (pre-LN); new statistics to stats_out
     auto residual = [&](const float* bias, const float2* stats, const float* gamma, const float* beta, float2* stats_out) {
@@ -556,7 +586,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             CUDA_TRY(launch_im2col(in.pixels, d.ffn, B, c.image, c.patch, stream));
             if (step("im2col")) return 0;
             GemmEpi e_patch{w.zero_bias, nullptr, P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, nullptr, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, nullptr, om.ctx, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
             if (step("gemm_patch")) return 0;
             CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, S, m.eps, stream));
             if (step("vit_embed")) return 0;
@@ -580,26 +610,26 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
                 CUDA_TRY(launch_attention_stream(*mq, d.ctx, lens, B, S, d.sm_attn, stream));
                 if (step("attention_stream")) return 0;
             } else {
-                CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.res.hi, lw.m_qkv, d.qkv, nullptr, nullptr, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
+                CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.res.hi, lw.m_qkv, d.qkv, nullptr, nullptr, om.qkv, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv")) return 0;
                 CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, ls.causal));
                 if (step("attention")) return 0;
             }
             // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
             const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, &am.res, e_ao, M, H, H, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, &am.res, nullptr, e_ao, M, H, H, d.sm_gemm, stream));
             if (step("gemm_attn_out")) return 0;
             GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
             if (ls.rotary) {
                 CUDA_TRY(launch_gemm_swiglu(am.res.hi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
                 if (step("gemm_ffn1_swiglu")) return 0;
             } else {
-                CUDA_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.res.hi, lw.m_ff1, d.ffn, nullptr, nullptr, e_ff1, M, I, H, d.sm_gemm, stream));
+                CUDA_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.res.hi, lw.m_ff1, d.ffn, nullptr, nullptr, om.ffn, e_ff1, M, I, H, d.sm_gemm, stream));
                 if (step(ls.pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
             }
             // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
             const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, &am.res, e_ff2, M, H, I, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, &am.res, nullptr, e_ff2, M, H, I, d.sm_gemm, stream));
             if (step("gemm_ffn2")) return 0;
             prev_g = lw.ln2_g;
             prev_b = lw.ln2_b;
@@ -611,7 +641,7 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             // decoder GEMM max-reduces relu(LN_t(u) W_dec^T + b) over each item's valid tokens into it, and never stores the
             // [M, vocab] logits; log1p once per (item, word) into out
             GemmEpi e_t{w.mlm_t_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.res.hi, w.m_mlm_t, d.ctx, nullptr, nullptr, e_t, M, H, H, d.sm_gemm, stream));
+            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.res.hi, w.m_mlm_t, d.ctx, nullptr, nullptr, om.ctx, e_t, M, H, H, d.sm_gemm, stream));
             if (step("gemm_mlm_transform")) return 0;
             uint32_t* vmax = reinterpret_cast<uint32_t*>(d.ffn.get());
             CUDA_TRY(launch_mlm_ln_stats(d.ctx, d.pstats[1], vmax, M, static_cast<size_t>(B) * m.splade_vpad, H, stream));
@@ -676,6 +706,8 @@ int forward(Dev& d, const Model& m, int dev_index, const Input& in, float* out, 
             }
             const CUtensorMap *mq = nullptr, *mc = nullptr;
             if (int rc = get_qkv_map(d, m, in.S, &mq, &mc)) return rc;  // host-side map creation happens outside the capture
+            OutMaps om;
+            if (int rc = get_out_maps(d, m, in.B * in.S, &om)) return rc;
             uint64_t nl = 0;
             CUDA_TRY(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
             const int rc = forward_enqueue(d, m, dev_index, in, out, stream, nl, nullptr);
@@ -2232,6 +2264,9 @@ int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const fl
         CUDA_TRY(b.upload(&dout, nullptr, Mp * N * 2));
         CUDA_TRY(cudaMemsetAsync(dout, 0xFF, Mp * N * 2, d.compute));
     }
+    OutEpi oe{};  // epi 0/1/3: the TMA map the output is stored through, M rows (the poisoned rows past M stay so)
+    if (epi != 2)
+        if (int rc = make_map_2d(&oe.out, dout, M, N, 64)) return rc;
     __half* const o_hi = epi == 2 ? dhi : dout;
     GemmEpi e{db, dsi, parts_in, dg, dbt, dso, eps};
     // epi 2 updates hi / lo in place (y = acc + bias + LN(y)): reload the residual before the launch whose result is returned
@@ -2245,10 +2280,10 @@ int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const fl
     CUDA_TRY(e1.create());
     if (iters < 1) iters = 1;
     CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
+    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, epi == 2 ? nullptr : &oe, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
     CUDA_TRY(cudaEventRecord(e1, d.compute));
     CUDA_TRY(reload());
-    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, e, M, N, K, grid_sms, d.compute, ctas_out));  // the result that is returned
+    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, epi == 2 ? nullptr : &oe, e, M, N, K, grid_sms, d.compute, ctas_out));  // the result that is returned
     CUDA_TRY(cudaStreamSynchronize(d.compute));
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);

@@ -12,7 +12,8 @@
 //                  consumers are in their epilogue;
 //   warpgroups 1-2: consumer c owns rows 64c .. 64c+63 of the tile and all 256 columns: four wgmma.m64n256k16 per k-block
 //                  into 128 fp32 accumulator registers per thread, one k-block's MMAs kept in flight while the previous
-//                  stage is handed back to the producers; then the epilogue runs straight from the registers.
+//                  stage is handed back to the producers; then the epilogue runs from the registers (EPI_BIAS(_GELU /
+//                  _QGELU)_F16: into shared memory, and TMA stores it, see below).
 //
 //   full[s]  : own producer arrive.expect_tx(48 KB); own A, own W share and the peer's W share complete_tx on it
 //   empty[s] : one arrival per consumer warp of EVERY CTA of the cluster once the wgmma that read stage s have completed
@@ -37,6 +38,23 @@
 //     producer issues the TMA only after its wait on empty[s] has acquired all 8 CM arrivals.
 //   * Each element of y is written in place by the one tile that owns it, after that tile's TMA has read it (the consumer
 //     stores only after its wait on full[s] saw the read complete).  Tiles are disjoint, so no tile reads what another wrote.
+//
+// EPI_BIAS(_GELU / _QGELU)_F16 store their output by TMA through a staging area behind the barriers, outside the ring: two
+// [64 rows x 64 columns] fp16 boxes (8 KB, 128B-swizzled) per consumer warpgroup.  For each 64-column chunk q of the tile the
+// warpgroup writes its 64 rows of the chunk into box q % 2, and its first thread (the issuer) stores the box to (n0 + 64q,
+// m0 + 64 cw) with one TMA store and commits it as one bulk group.  Nothing waits for the stores to land: the warpgroup goes
+// on to its next chunk and its next tile's main loop while the TMA engine drains them.  A warpgroup whose 64 rows all lie
+// past M writes no box and stores nothing.
+//   * The output map is {N, M}: exactly M rows, so TMA clips a box's rows past M and rows past M are never written.
+//   * Before box q % 2 is rewritten, the issuer's cp.async.bulk.wait_group.read 1 leaves only the other box's store (chunk
+//     q - 1) pending, so the store of chunk q - 2 has finished reading it; a named barrier over the warpgroup then lets its
+//     128 threads write.  BN / 64 is even and a tile stores all of its chunks or none, so every store's box alternates
+//     with the one before it across tiles as well.
+//   * Every thread issues fence.proxy.async after its writes (generic proxy) and before a second named barrier, after
+//     which the issuer's TMA (async proxy) reads the box.
+//   * The issuer waits for all its stores to complete (cp.async.bulk.wait_group 0) before the final cluster barrier: the
+//     staging area must outlive their reads, and the output must be in global memory when the grid ends, since the next
+//     kernel's griddepcontrol.wait only waits for the grid.
 //
 // Epilogues (see kernels.h for the residual-stream format):
 //   EPI_BIAS(_GELU / _QGELU)_F16 : folded LayerNorm  rstd * acc + c  (c = W beta + b), optional GELU, fp16 out;
@@ -72,6 +90,10 @@ constexpr int W_BOX_BYTES = 128 * BK * 2;       // one 128-row TMA box of W: 16 
 constexpr int NUM_THREADS = 384;
 constexpr int CM = 2;  // CTAs per cluster, along M, sharing every W tile
 constexpr int RES_BOX_BYTES = BM * 64 * 2;      // EPI_BIAS_RES_SPLIT: one [128 x 64] box of hi or lo, 16 KB
+constexpr int OUT_BOX_BYTES = 64 * 64 * 2;      // EPI_BIAS(_GELU / _QGELU)_F16: one [64 x 64] staging box of the output, 8 KB
+
+// the epilogues that stage their fp16 output in shared memory and store it by TMA
+constexpr bool tma_store_epi(int epi) { return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_QGELU_F16; }
 
 // ring layout of the BN-column kernel
 template <int BN>
@@ -85,9 +107,15 @@ struct Tiles {
     static constexpr int OFF_RED = OFF_BAR + 256;
     static constexpr int SPLADE_SMEM_BYTES = SMEM_BYTES + 2 * 4 * BN * 4;
     static_assert(SPLADE_SMEM_BYTES <= 232448, "shared memory");
+    // tma_store_epi: behind the barriers, 1024-aligned for the 128B swizzle, each consumer warpgroup's two staging boxes
+    static constexpr int OFF_OUT = OFF_BAR + 1024;
+    static constexpr int OUT_SMEM_BYTES = OFF_OUT + 2 * 2 * OUT_BOX_BYTES + 1024;  // 231 424 / 165 888
+    static_assert(OUT_SMEM_BYTES <= 232448, "shared memory");
 };
 template <int EPI, int BN>
-constexpr int smem_bytes() { return EPI == EPI_SPLADE_MAX ? Tiles<BN>::SPLADE_SMEM_BYTES : Tiles<BN>::SMEM_BYTES; }
+constexpr int smem_bytes() {
+    return EPI == EPI_SPLADE_MAX ? Tiles<BN>::SPLADE_SMEM_BYTES : tma_store_epi(EPI) ? Tiles<BN>::OUT_SMEM_BYTES : Tiles<BN>::SMEM_BYTES;
+}
 
 // erf-GELU x * Phi(x), erf by Abramowitz-Stegun 7.1.26 (abs err <= 1.5e-7): 2 MUFU (rcp, ex2) per value
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -179,13 +207,13 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ st, float e
 }
 
 // BN: tile width (256 or 128); PARTS: partials per row of ep.stats_in (the LayerNorm'd width / 128).  sp is read by
-// EPI_SPLADE_MAX only, rp by EPI_ROPE_F16 only, res by EPI_BIAS_RES_SPLIT only; as the last parameters they leave every other
-// instantiation's parameter offsets as they were.
+// EPI_SPLADE_MAX only, rp by EPI_ROPE_F16 only, res by EPI_BIAS_RES_SPLIT only, oe by tma_store_epi only; as the last
+// parameters they leave every other instantiation's parameter offsets as they were.
 template <int EPI, int BN, int PARTS>
 __global__ void __cluster_dims__(CM, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmEpi ep,
             __half* __restrict__ out, __half* __restrict__ out_lo, int M, int N, int K, const SpladeEpi sp, const RopeEpi rp,
-            const __grid_constant__ ResEpi res) {
+            const __grid_constant__ ResEpi res, const __grid_constant__ OutEpi oe) {
     static_assert(BN == 256 || BN == 128, "tile width");
     constexpr int STAGE_BYTES = Tiles<BN>::STAGE_BYTES, OFF_BAR = Tiles<BN>::OFF_BAR;
     constexpr int NACC = BN / 2;     // fp32 accumulators per consumer thread
@@ -213,6 +241,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             prefetch_tmap(&res.hi);
             prefetch_tmap(&res.lo);
         }
+        if constexpr (tma_store_epi(EPI)) prefetch_tmap(&oe.out);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 8 * CM);  // the 8 consumer warps of every CTA of the cluster
@@ -403,19 +432,40 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
                 }
             }
         } else if constexpr (EPI != EPI_BIAS_RES_SPLIT) {
+            // one 64-column chunk q at a time through staging box q % 2 (see the top of the file): this thread's rows of the box
+            // are lr and lr + 8, and 128B swizzle puts 16-byte column group jj of box row r at (jj ^ r % 8) * 16 -- r % 8 =
+            // lane / 4 for both rows, so a warp's 32 writes fall in 32 distinct banks
+            const bool issuer = (threadIdx.x & 127) == 0;
+            const int lr = w4 * 16 + (lane >> 2);
+            uint8_t* const stg = smem + Tiles<BN>::OFF_OUT + cw * (2 * OUT_BOX_BYTES);
+            if (m0 + 64 * cw < M) {
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
+                for (int q = 0; q < BN / 64; ++q) {
+                    uint8_t* const box = stg + (q & 1) * OUT_BOX_BYTES;
+                    if (issuer) tma_store_wait_read<1>();  // the store of chunk q - 2 has read the box
+                    named_bar_sync(1 + cw, 128);
+                    const uint32_t row_addr = smem_u32(box) + lr * 128 + 4 * (lane & 3);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    // folded LayerNorm: rstd * acc + c -- the weight rows are centred at load time (sum_k W''[n,k] = 0), so the
-                    // row mean cancels inside the tensor core: sum_k (y_k - mean) W''_nk = sum_k y_k W''_nk
-                    float v0 = fmaf(rstd[h], acc[4 * j + 2 * h], bv.x);
-                    float v1 = fmaf(rstd[h], acc[4 * j + 2 * h + 1], bv.y);
-                    if constexpr (EPI == EPI_BIAS_GELU_F16) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-                    if constexpr (EPI == EPI_BIAS_QGELU_F16) { v0 = gelu_quick(v0); v1 = gelu_quick(v1); }
-                    const int row = r0 + 8 * h;
-                    if (row < M) *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * N + c0 + 8 * j) = pack_half2(v0, v1);
+                    for (int j = 8 * q; j < 8 * q + 8; ++j) {
+                        const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0 + 8 * j));
+                        const uint32_t a = row_addr + (static_cast<uint32_t>((j & 7) ^ (lane >> 2)) << 4);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            // folded LayerNorm: rstd * acc + c -- the weight rows are centred at load time (sum_k W''[n,k] = 0),
+                            // so the row mean cancels inside the tensor core: sum_k (y_k - mean) W''_nk = sum_k y_k W''_nk
+                            float v0 = fmaf(rstd[h], acc[4 * j + 2 * h], bv.x);
+                            float v1 = fmaf(rstd[h], acc[4 * j + 2 * h + 1], bv.y);
+                            if constexpr (EPI == EPI_BIAS_GELU_F16) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                            if constexpr (EPI == EPI_BIAS_QGELU_F16) { v0 = gelu_quick(v0); v1 = gelu_quick(v1); }
+                            sts32(a + h * (8 * 128), pack_half2(v0, v1));
+                        }
+                    }
+                    fence_proxy_async_smem();     // the writes are ordered before the TMA store's reads
+                    named_bar_sync(1 + cw, 128);  // the warpgroup's 64 rows of the chunk are in the box
+                    if (issuer) {
+                        tma_store_2d(&oe.out, box, n0 + 64 * q, m0 + 64 * cw);
+                        tma_store_commit();
+                    }
                 }
             }
         } else {
@@ -507,6 +557,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             }
         }
     }
+    if constexpr (tma_store_epi(EPI))
+        if ((threadIdx.x & 127) == 0) tma_store_wait<0>();  // the stores have read the staging boxes and written the output
     cluster_sync();  // the peer's consumers have made their last arrival on this CTA's barriers
 }
 
@@ -523,13 +575,13 @@ static int& max_clusters() {
 template <int EPI, int BN, int PARTS>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
                               int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{},
-                              const RopeEpi& rp = RopeEpi{}, const ResEpi& res = ResEpi{}) {
+                              const RopeEpi& rp = RopeEpi{}, const ResEpi& res = ResEpi{}, const OutEpi& oe = OutEpi{}) {
     const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
     int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
     if (clusters < 1) clusters = 1;
     if (ctas) *ctas = clusters * gemm::CM;
     return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::smem_bytes<EPI, BN>(),
-                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp, res);
+                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp, res, oe);
 }
 
 // the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT / CLIP text
@@ -537,30 +589,30 @@ static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __ha
 // bge-large N is a multiple of 256.  Four partials (the CLIP text tower's 512-wide LayerNorm, folded into QKV and the quick-GELU
 // FFN1) exist for BN = 256 and EPI 0 / 3 only; its residual epilogues take no statistics (pre-LN, stats_in NULL).
 template <int EPI>
-static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi& res, const GemmEpi& e,
-                              int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
+static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi& res, const OutEpi& oe,
+                              const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
     const bool wide = N % 256 == 0;
     if (e.stats_in != nullptr && e.parts_in == 8) {
         if constexpr (EPI != EPI_BIAS_QGELU_F16) {
-            if (wide) return launch_one<EPI, 256, 8>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
+            if (wide) return launch_one<EPI, 256, 8>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
         }
         return cudaErrorInvalidValue;
     }
     if (e.stats_in != nullptr && e.parts_in == 4) {
         if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16) {
-            if (wide) return launch_one<EPI, 256, 4>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
+            if (wide) return launch_one<EPI, 256, 4>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
         }
         return cudaErrorInvalidValue;
     }
     const bool six = e.stats_in == nullptr || e.parts_in == 6;
     if (wide) {
-        if (six) return launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
+        if (six) return launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
         // three partials re-applied by the residual epilogue mean N = 384, never a multiple of 256: no <RES_SPLIT, 256, 3>
-        if constexpr (EPI != EPI_BIAS_RES_SPLIT) return launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
+        if constexpr (EPI != EPI_BIAS_RES_SPLIT) return launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
         return cudaErrorInvalidValue;
     }
-    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res)
-               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res);
+    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe)
+               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
 }
 
 template <int EPI, int BN, int PARTS>
@@ -607,22 +659,23 @@ cudaError_t gemm_init_device() {
 }
 
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi* res,
-                        const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
+                        const OutEpi* oe, const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
     if (N % 128 != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
     // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 1024, 768,
     // 512 or 384
     const int ln_width = epi == EPI_BIAS_RES_SPLIT ? N : K;
     if (e.stats_in != nullptr && ((e.parts_in != 8 && e.parts_in != 6 && e.parts_in != 4 && e.parts_in != 3) || e.parts_in * 128 != ln_width))
         return cudaErrorInvalidValue;
+    if (gemm::tma_store_epi(epi) && oe == nullptr) return cudaErrorInvalidValue;
     switch (epi) {
-        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, ResEpi{}, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, ResEpi{}, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, ResEpi{}, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, ResEpi{}, *oe, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, ResEpi{}, *oe, e, M, N, K, sm_count, stream, ctas);
+        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, ResEpi{}, *oe, e, M, N, K, sm_count, stream, ctas);
         case EPI_BIAS_RES_SPLIT:
             if (out_lo == nullptr || res == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr)))
                 return cudaErrorInvalidValue;
             if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
-            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, *res, e, M, N, K, sm_count, stream, ctas);
+            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, *res, OutEpi{}, e, M, N, K, sm_count, stream, ctas);
     }
     return cudaErrorInvalidValue;
 }

@@ -41,12 +41,14 @@ cudaError_t kernels_init_device();
 //
 // C[M,N] = epi(A[M,K] . W[N,K]^T).  A and W move by TMA:
 //   ta  : fp16 A   {K, rows>=M}  box {64,128} SW128     tb  : fp16 W {K, N} box {64,128} SW128
-//   EPI 0/1/3: out = fp16 [M, N] row-major; e.stats_in (or NULL: plain acc + bias), e.bias
+//   EPI 0/1/3: out = fp16 [M, N] row-major, written by TMA stores through oe (required): a map over out, {N, M} -- exactly M
+//              rows, so that the stores clip the last tile's rows past M -- box {64, 64} SW128; e.stats_in (or NULL: plain
+//              acc + bias), e.bias
 //   EPI 2    : out = hi, out_lo = lo, both fp16 [M, N] row-major (read and written in place); res (required) holds TMA maps
 //              over the same hi and lo, {N, rows>=M} box {64,128} SW128 like ta, through which the tile's residual is read;
 //              e.stats_in + e.ln_gamma/e.ln_beta describe the LayerNorm of the residual (stats_in NULL: the residual is added
 //              as is); e.stats_out receives the partials of the new rows (N / 128 per row; must not alias stats_in: other tiles
-//              still read those).  EPI 0/1/3 take out_lo and res NULL.
+//              still read those).  EPI 0/1/3 take out_lo and res NULL, EPI 2 oe NULL.
 //   N % 128 == 0, K % 64 == 0; rows past M are neither read from out nor written.  Tiles are 128 x 256 when N % 256 == 0,
 //   else 128 x 128.  e.parts_in (with stats_in) must be the LayerNorm'd width / 128, that width being 768 or 384 (K for
 //   EPI 0/1/3, N for EPI 2), 1024 for EPI 0/1/2 with N % 256 == 0, or 512 for EPI 0/3 with N % 256 == 0.  ta's map may end at M rows or run past them: a tile's A rows past M only feed rows no store
@@ -68,8 +70,12 @@ struct GemmEpi {
 struct ResEpi {
     CUtensorMap hi, lo;
 };
+// EPI 0/1/3's output as the kernel stores it: {N, M} box {64, 64} SW128
+struct OutEpi {
+    CUtensorMap out;
+};
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi* res,
-                        const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas = nullptr);
+                        const OutEpi* oe, const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas = nullptr);
 
 // SPLADE's vocabulary max (EPI_SPLADE_MAX): the decoder GEMM C = LNfold(A . W^T) + bias over rows of items padded to S tokens
 // (S % 64 == 0, M = B S), never stored.  Instead, for item i and column n < vocab,

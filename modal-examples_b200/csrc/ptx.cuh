@@ -183,6 +183,11 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
+// as tma_store_wait_read, and the writes of the completed groups have been made to global memory
+template <int N>
+__device__ __forceinline__ void tma_store_wait() {
+    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
 
 // Warpgroup register re-allocation: every warp of an aligned group of four must execute the same one.
 template <int N>
