@@ -35,6 +35,8 @@
 //
 // Restates BertSelfAttention.forward (HF modeling_bert.py:143-207) for the TEI /embed path the
 // reference calls at 06_gpu_and_ml/embeddings/text_embeddings_inference.py:100.
+#include <tuple>
+
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -454,14 +456,23 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tq, __half* __restri
 
 }  // namespace attn
 
-template <int D, int NH, bool CAUSAL = false>
-static cudaError_t setup() {
+// Every attention_kernel<D, NH, CAUSAL> launch_attention can select, each set up at init and launched from this one list:
+// (head_dim, heads) = (64, 12) bge-base and ViT, (32, 12) bge-small, (64, 16) bge-large, and (64, 8) causal, the CLIP text tower.
+template <int D, int NH, bool CAUSAL>
+struct Inst {
+    static constexpr int d = D, nh = NH;
+    static constexpr bool causal = CAUSAL;
+};
+constexpr std::tuple<Inst<64, 12, false>, Inst<32, 12, false>, Inst<64, 16, false>, Inst<64, 8, true>> INSTANTIATIONS{};
+
+template <int D, int NH, bool CAUSAL>
+static cudaError_t setup(Inst<D, NH, CAUSAL>) {
     return cudaFuncSetAttribute(attn::attention_kernel<D, NH, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Layout<D>::SMEM_BYTES);
 }
 
-template <int D, int NH, bool CAUSAL = false>
-static cudaError_t launch_one(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
-                              cudaStream_t stream) {
+template <int D, int NH, bool CAUSAL>
+static cudaError_t launch_one(Inst<D, NH, CAUSAL>, const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S,
+                              int sm_count, cudaStream_t stream) {
     // fewer (item, head) units than SMs: split them by query tile (K and V are then loaded once per tile, but a single item
     // spreads over 4 NH SMs instead of NH)
     const int nq = (S + attn::QT - 1) / attn::QT;
@@ -473,22 +484,21 @@ static cudaError_t launch_one(const CUtensorMap& tq, const CUtensorMap& tctx, co
 }
 
 cudaError_t attention_init_device() {
-    cudaError_t e;
-    if ((e = setup<64, 12>()) != cudaSuccess) return e;
-    if ((e = setup<32, 12>()) != cudaSuccess) return e;
-    if ((e = setup<64, 16>()) != cudaSuccess) return e;
-    if ((e = setup<64, 8, true>()) != cudaSuccess) return e;
+    cudaError_t e = cudaSuccess;
+    std::apply([&](auto... inst) { (((e = setup(inst)) == cudaSuccess) && ...); }, INSTANTIATIONS);
+    if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(attn::attention_stream_kernel<64, 12>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::stream::SMEM_BYTES);
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
                              cudaStream_t stream, int head_dim, int heads, bool causal) {
     if (S < 1 || S > attn::MAX_KB * attn::KB || B < 1 || sm_count < 1) return cudaErrorInvalidValue;
-    if (causal) return head_dim == 64 && heads == 8 ? launch_one<64, 8, true>(tq, tctx, lens, B, S, sm_count, stream) : cudaErrorInvalidValue;
-    if (head_dim == 64 && heads == 12) return launch_one<64, 12>(tq, tctx, lens, B, S, sm_count, stream);
-    if (head_dim == 32 && heads == 12) return launch_one<32, 12>(tq, tctx, lens, B, S, sm_count, stream);
-    if (head_dim == 64 && heads == 16) return launch_one<64, 16>(tq, tctx, lens, B, S, sm_count, stream);
-    return cudaErrorInvalidValue;
+    cudaError_t r = cudaErrorInvalidValue;
+    std::apply([&](auto... inst) {
+        ((inst.d == head_dim && inst.nh == heads && inst.causal == causal && (r = launch_one(inst, tq, tctx, lens, B, S, sm_count, stream), true)) ||
+         ...);
+    }, INSTANTIATIONS);
+    return r;
 }
 
 cudaError_t launch_attention_stream(const CUtensorMap& tq, __half* ctx, const int32_t* lens, int B, int S, int sm_count, cudaStream_t stream) {

@@ -69,6 +69,17 @@ int fail(int code, const char* fmt, ...) {
             return fail(B200RT_E_CUDA, "%s:%d: %s failed: %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
     } while (0)
 
+// A launch_* call (kernels.h): a launcher refuses operands outside its contract with cudaErrorInvalidValue before any CUDA call,
+// and the runtime's own cudaErrorInvalidValue is a non-sticky argument error, so a refusal is the caller's B200RT_E_INVALID and
+// leaves the runtime usable; any other error is handled as by CUDA_TRY.
+#define LAUNCH_TRY(expr)                                                                                    \
+    do {                                                                                                    \
+        cudaError_t _e = (expr);                                                                            \
+        if (_e == cudaErrorInvalidValue) return fail(B200RT_E_INVALID, "%s refused its operands", #expr);   \
+        if (_e != cudaSuccess)                                                                              \
+            return fail(B200RT_E_CUDA, "%s:%d: %s failed: %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
+    } while (0)
+
 // ------------------------------------------------------------------------------------------ tensor maps
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -87,6 +98,10 @@ int load_driver_entry() {
     return 0;
 }
 
+// Encoding a map is host work on no context: CUDA_ERROR_INVALID_VALUE means these operands have no map of this layout (a row
+// pitch that is not a multiple of 16 bytes, a head too wide for its swizzle), which is the caller's B200RT_E_INVALID.
+int map_error(CUresult r) { return r == CUDA_ERROR_INVALID_VALUE ? B200RT_E_INVALID : B200RT_E_CUDA; }
+
 // fp16 2D row-major [rows, cols] -> box {64, box_rows}, 128B swizzle
 int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
     cuuint64_t dims[2] = {cols, rows};
@@ -96,7 +111,7 @@ int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, 
     CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(B200RT_E_CUDA, "cuTensorMapEncodeTiled(2d %llu x %llu) -> %d",
+    if (r != CUDA_SUCCESS) return fail(map_error(r), "cuTensorMapEncodeTiled(2d %llu x %llu) -> %d",
                                        (unsigned long long)rows, (unsigned long long)cols, (int)r);
     return 0;
 }
@@ -112,7 +127,7 @@ int make_map_qkv(CUtensorMap* m, const void* base, uint64_t B, uint64_t S, uint6
                           CU_TENSOR_MAP_INTERLEAVE_NONE, head_dim == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(B200RT_E_CUDA, "cuTensorMapEncodeTiled(qkv B=%llu S=%llu) -> %d",
+    if (r != CUDA_SUCCESS) return fail(map_error(r), "cuTensorMapEncodeTiled(qkv B=%llu S=%llu) -> %d",
                                        (unsigned long long)B, (unsigned long long)S, (int)r);
     return 0;
 }
@@ -583,17 +598,17 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             // patches -> im2col rows in the (idle) ffn buffer -> patch projection into the (idle) ctx buffer -> + class / position
             // embeddings, pre_layrnorm -> residual stream + statistics
             const b200rt_vit_config& c = m.vcfg;
-            CUDA_TRY(launch_im2col(in.pixels, d.ffn, B, c.image, c.patch, stream));
+            LAUNCH_TRY(launch_im2col(in.pixels, d.ffn, B, c.image, c.patch, stream));
             if (step("im2col")) return 0;
             GemmEpi e_patch{w.zero_bias, nullptr, P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, nullptr, om.ctx, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
+            LAUNCH_TRY(launch_gemm(EPI_BIAS_F16, d.m_im2col, w.m_patch, d.ctx, nullptr, nullptr, om.ctx, e_patch, M, H, 3 * c.patch * c.patch, d.sm_gemm, stream));
             if (step("gemm_patch")) return 0;
-            CUDA_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, S, m.eps, stream));
+            LAUNCH_TRY(launch_vit_embed(d.ctx, w.cls, w.pos, w.pre_g, w.pre_b, d.yhi, d.ylo, d.pstats[0], M, S, m.eps, stream));
             if (step("vit_embed")) return 0;
         } else {
             // clip_text: token + position, its zero type row leaves (word + 0) + pos bit-exact; no embedding LayerNorm
             // nomic_bert: no position table -- pos is 64 zero rows read as pos[t % 64], so the rows are (word + type0) + 0
-            CUDA_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, m.kind == NOMIC_BERT ? 64 : S, m.vocab, H,
+            LAUNCH_TRY(launch_embed(in.ids, w.word, w.pos, w.type, d.yhi, d.ylo, d.pstats[0], M, m.kind == NOMIC_BERT ? 64 : S, m.vocab, H,
                                   stream, in.segs));
             if (step("embed")) return 0;
         }
@@ -605,31 +620,31 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             // QKV = LN_prev(y) Wqkv^T + b, the LayerNorm folded into the epilogue
             GemmEpi e_qkv{lw.qkv_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
             if (ls.rotary) {
-                CUDA_TRY(launch_gemm_rope(am.res.hi, lw.m_qkv, d.qkv, e_qkv, RopeEpi{reinterpret_cast<const float2*>(w.rope), S, 2 * H}, M, 3 * H, H, d.sm_gemm, stream));
+                LAUNCH_TRY(launch_gemm_rope(am.res.hi, lw.m_qkv, d.qkv, e_qkv, RopeEpi{reinterpret_cast<const float2*>(w.rope), S, 2 * H}, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv_rope")) return 0;
-                CUDA_TRY(launch_attention_stream(*mq, d.ctx, lens, B, S, d.sm_attn, stream));
+                LAUNCH_TRY(launch_attention_stream(*mq, d.ctx, lens, B, S, d.sm_attn, stream));
                 if (step("attention_stream")) return 0;
             } else {
-                CUDA_TRY(launch_gemm(EPI_BIAS_F16, am.res.hi, lw.m_qkv, d.qkv, nullptr, nullptr, om.qkv, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
+                LAUNCH_TRY(launch_gemm(EPI_BIAS_F16, am.res.hi, lw.m_qkv, d.qkv, nullptr, nullptr, om.qkv, e_qkv, M, 3 * H, H, d.sm_gemm, stream));
                 if (step("gemm_qkv")) return 0;
-                CUDA_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, ls.causal));
+                LAUNCH_TRY(launch_attention(*mq, *mc, lens, B, S, d.sm_attn, stream, H / m.heads, m.heads, ls.causal));
                 if (step("attention")) return 0;
             }
             // y <- ctx Wao^T + b + LN_prev(y) (pre-LN: + y); new row statistics (LN1's) into pstats[1]
             const GemmEpi e_ao = residual(lw.ao_b, d.pstats[0], prev_g, prev_b, d.pstats[1]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, &am.res, nullptr, e_ao, M, H, H, d.sm_gemm, stream));
+            LAUNCH_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ctx, lw.m_ao, d.yhi, d.ylo, &am.res, nullptr, e_ao, M, H, H, d.sm_gemm, stream));
             if (step("gemm_attn_out")) return 0;
             GemmEpi e_ff1{lw.ff1_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
             if (ls.rotary) {
-                CUDA_TRY(launch_gemm_swiglu(am.res.hi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
+                LAUNCH_TRY(launch_gemm_swiglu(am.res.hi, lw.m_ff1, d.ffn, e_ff1, M, 2 * I, H, d.sm_gemm, stream));
                 if (step("gemm_ffn1_swiglu")) return 0;
             } else {
-                CUDA_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.res.hi, lw.m_ff1, d.ffn, nullptr, nullptr, om.ffn, e_ff1, M, I, H, d.sm_gemm, stream));
+                LAUNCH_TRY(launch_gemm(ls.pre_ln ? EPI_BIAS_QGELU_F16 : EPI_BIAS_GELU_F16, am.res.hi, lw.m_ff1, d.ffn, nullptr, nullptr, om.ffn, e_ff1, M, I, H, d.sm_gemm, stream));
                 if (step(ls.pre_ln ? "gemm_ffn1_qgelu" : "gemm_ffn1_gelu")) return 0;
             }
             // y <- ffn W2^T + b + LN1(y) (pre-LN: + y); LN2's statistics into pstats[0]
             const GemmEpi e_ff2 = residual(lw.ff2_b, d.pstats[1], lw.ln1_g, lw.ln1_b, d.pstats[0]);
-            CUDA_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, &am.res, nullptr, e_ff2, M, H, I, d.sm_gemm, stream));
+            LAUNCH_TRY(launch_gemm(EPI_BIAS_RES_SPLIT, am.ffn, lw.m_ff2, d.yhi, d.ylo, &am.res, nullptr, e_ff2, M, H, I, d.sm_gemm, stream));
             if (step("gemm_ffn2")) return 0;
             prev_g = lw.ln2_g;
             prev_b = lw.ln2_b;
@@ -641,35 +656,35 @@ int forward_enqueue(Dev& d, const Model& m, int dev_index, const Input& in, floa
             // decoder GEMM max-reduces relu(LN_t(u) W_dec^T + b) over each item's valid tokens into it, and never stores the
             // [M, vocab] logits; log1p once per (item, word) into out
             GemmEpi e_t{w.mlm_t_c, d.pstats[0], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.res.hi, w.m_mlm_t, d.ctx, nullptr, nullptr, om.ctx, e_t, M, H, H, d.sm_gemm, stream));
+            LAUNCH_TRY(launch_gemm(EPI_BIAS_GELU_F16, am.res.hi, w.m_mlm_t, d.ctx, nullptr, nullptr, om.ctx, e_t, M, H, H, d.sm_gemm, stream));
             if (step("gemm_mlm_transform")) return 0;
             uint32_t* vmax = reinterpret_cast<uint32_t*>(d.ffn.get());
-            CUDA_TRY(launch_mlm_ln_stats(d.ctx, d.pstats[1], vmax, M, static_cast<size_t>(B) * m.splade_vpad, H, stream));
+            LAUNCH_TRY(launch_mlm_ln_stats(d.ctx, d.pstats[1], vmax, M, static_cast<size_t>(B) * m.splade_vpad, H, stream));
             if (step("mlm_ln_stats")) return 0;
             GemmEpi e_dec{w.mlm_dec_c, d.pstats[1], P, nullptr, nullptr, nullptr, m.eps};
-            CUDA_TRY(launch_gemm_splade(am.ctx, w.m_mlm_dec, e_dec, SpladeEpi{in.lens, S, vmax, m.vocab}, M, m.splade_vpad, H, d.sm_gemm,
+            LAUNCH_TRY(launch_gemm_splade(am.ctx, w.m_mlm_dec, e_dec, SpladeEpi{in.lens, S, vmax, m.vocab}, M, m.splade_vpad, H, d.sm_gemm,
                                         stream));
             if (step("gemm_splade")) return 0;
-            CUDA_TRY(launch_splade_finalize(vmax, out, B, m.splade_vpad, m.vocab, stream));
+            LAUNCH_TRY(launch_splade_finalize(vmax, out, B, m.splade_vpad, m.vocab, stream));
             return last("splade_finalize");
         }
         case VIT:
-            CUDA_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
+            LAUNCH_TRY(launch_vit_pool(d.yhi, d.ylo, w.post_g, w.post_b, w.proj_w, out, B, S, m.vcfg.proj, m.eps, stream));
             return last("vit_pool");
         case CLIP_TEXT:
-            CUDA_TRY(launch_clip_text_pool(d.yhi, d.ylo, in.ids, in.lens, w.post_g, w.post_b, w.proj_w, out, B, S, m.tcfg.proj, m.eps,
+            LAUNCH_TRY(launch_clip_text_pool(d.yhi, d.ylo, in.ids, in.lens, w.post_g, w.post_b, w.proj_w, out, B, S, m.tcfg.proj, m.eps,
                                            m.tcfg.eos_id, stream));
             return last("clip_text_pool");
         case BERT_CLASSIFIER:
-            CUDA_TRY(launch_cls_head(d.yhi, d.ylo, prev_g, prev_b, w.pool_w, w.pool_b, w.cls_w, w.cls_b, out, B, S, m.num_labels, m.eps, H,
+            LAUNCH_TRY(launch_cls_head(d.yhi, d.ylo, prev_g, prev_b, w.pool_w, w.pool_b, w.cls_w, w.cls_b, out, B, S, m.num_labels, m.eps, H,
                                      stream));
             return last("cls_head");
         case BERT: case NOMIC_BERT:
             if (m.pool_mean) {
-                CUDA_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
+                LAUNCH_TRY(launch_mean_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, in.lens, out, B, S, m.eps, H, stream));
                 return last("mean_pool_normalize");
             }
-            CUDA_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
+            LAUNCH_TRY(launch_pool_normalize(d.yhi, d.ylo, prev_g, prev_b, out, B, S, m.eps, H, stream));
             return last("pool_normalize");
         }
         return 0;
@@ -1414,7 +1429,7 @@ int load_weights(Runtime& rt, Model& m, Layout& L, const float* blob, size_t nby
         else if (e.op == LayoutEntry::ZERO)
             CUDA_TRY(cudaMemsetAsync(rw.f32_arena + e.off, 0, e.n * 4, root.compute));
         else if (e.op == LayoutEntry::HALF)
-            CUDA_TRY(launch_fold_ln(d_blob + e.src, blob_at(e.gamma), blob_at(e.beta), blob_at(e.bias), rw.f16_arena + e.off,
+            LAUNCH_TRY(launch_fold_ln(d_blob + e.src, blob_at(e.gamma), blob_at(e.beta), blob_at(e.bias), rw.f16_arena + e.off,
                                     e.cvec < 0 ? nullptr : rw.f32_arena + L.e[e.cvec].off, static_cast<int>(e.n), static_cast<int>(e.k),
                                     root.compute));
     }
@@ -1750,27 +1765,77 @@ int check_ids(const Model& m, const int32_t* ids, const int32_t* lens, int n_ite
     return 0;
 }
 
-// Device buffers of one debug entry (b200rt_debug_embed & co.): buffers are filled from the host (or zeroed) in stream order
-// on allocation, and freed once the stream has drained when the entry returns, on success or on error.
+// Device buffers of one debug entry (b200rt_debug_embed & co.): buffers are filled from the host, zeroed or poisoned in stream
+// order on allocation, and freed once the stream has drained when the entry returns, on success or on error.
 struct DebugBuffers {
     cudaStream_t stream;
     std::vector<DevMem<void>> ptrs;
     explicit DebugBuffers(cudaStream_t s) : stream(s) {}
     ~DebugBuffers() { cudaStreamSynchronize(stream); }
     template <typename T>
-    cudaError_t upload(T** dp, const void* host, size_t bytes) {  // host NULL: zeros
-        ptrs.emplace_back();
-        cudaError_t e = ptrs.back().alloc(bytes);
-        if (e != cudaSuccess) return e;
-        void* p = ptrs.back();
+    cudaError_t upload(T** dp, const void* host, size_t bytes, size_t padded = 0) {  // host NULL: zeros; then zeros up to `padded` bytes
+        const size_t total = std::max(bytes, padded);
+        void* p = nullptr;
+        cudaError_t e = alloc(&p, total);
         *dp = static_cast<T*>(p);
-        return host ? cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, stream) : cudaMemsetAsync(p, 0, bytes, stream);
+        if (e == cudaSuccess && p && (!host || padded > bytes)) e = cudaMemsetAsync(p, 0, total, stream);
+        if (e == cudaSuccess && host && bytes) e = cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, stream);
+        return e;
+    }
+    template <typename T>
+    cudaError_t poisoned(T** dp, size_t bytes) {  // 0xFF bytes, NaN in fp16 and fp32: whatever a kernel leaves unwritten shows
+        void* p = nullptr;
+        cudaError_t e = alloc(&p, bytes);
+        *dp = static_cast<T*>(p);
+        return e == cudaSuccess && p ? cudaMemsetAsync(p, 0xFF, bytes, stream) : e;
     }
     cudaError_t download(void* host, const void* dev, size_t bytes) {
         cudaError_t e = cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, stream);
         return e != cudaSuccess ? e : cudaStreamSynchronize(stream);
     }
+
+  private:
+    cudaError_t alloc(void** p, size_t bytes) {  // 0 bytes: no buffer, NULL (a launcher judges a NULL operand)
+        if (bytes == 0) return cudaSuccess;
+        ptrs.emplace_back();
+        cudaError_t e = ptrs.back().alloc(bytes);
+        if (e == cudaSuccess) *p = ptrs.back();
+        return e;
+    }
 };
+
+// The frame of a debug entry: body(d, b, sms) runs on the live runtime's root replica d, under its lock and with its device
+// current, with b a DebugBuffers on d.compute and sms the launch width -- the entry's `sms` (0 = every SM, else 1..SM count;
+// an entry without one passes 0).
+template <class Body>
+int on_root(int sms, Body&& body) {
+    Runtime* rt = live_rt();
+    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
+    Dev& d = *rt->devs[0];
+    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
+    std::lock_guard<std::mutex> dl(d.mu);
+    CUDA_TRY(cudaSetDevice(d.id));
+    DebugBuffers b(d.compute);
+    return body(d, b, sms ? sms : d.sm_count);
+}
+
+// The mean device time of `iters` (at least one) back-to-back launch() calls on `stream` into *ms_out (may be NULL): one event
+// pair around them, synchronised.
+template <class Launch>
+int time_launches(cudaStream_t stream, int iters, float* ms_out, Launch&& launch) {
+    Event e0, e1;
+    CUDA_TRY(e0.create());
+    CUDA_TRY(e1.create());
+    if (iters < 1) iters = 1;
+    CUDA_TRY(cudaEventRecord(e0, stream));
+    for (int i = 0; i < iters; ++i) LAUNCH_TRY(launch());
+    CUDA_TRY(cudaEventRecord(e1, stream));
+    CUDA_TRY(cudaEventSynchronize(e1));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    if (ms_out) *ms_out = ms / iters;
+    return 0;
+}
 
 // Host buffers of a forward trace (b200rt_debug_forward_trace / b200rt_debug_vit_forward_trace, include/b200rt_debug.h).
 struct TraceOut {
@@ -1780,19 +1845,16 @@ struct TraceOut {
     size_t names_cap;
 };
 
-// Runs the first n_launches launches of the forward of host input `in` (ids, lens, segs or pixels) on the root replica: every
-// workspace buffer and the pooled output are set to 0xFF bytes (NaN in fp16 and fp32) behind the previous forward, the launches
-// run on d.compute through forward(), and once the stream has drained, rows = min(M + 256, the model's cap_rows) rows of every
-// buffer, at the model's widths (the buffers are used densely at those widths), and the pooled output are copied out.
-int trace_forward(Runtime& rt, const Model& m, const Input& in, int n_launches, const TraceOut& o, int* n_total) {
+// Runs the first n_launches launches of the forward of host input `in` (ids, lens, segs or pixels) on the root replica d (an
+// on_root frame): every workspace buffer and the pooled output are set to 0xFF bytes (NaN in fp16 and fp32) behind the previous
+// forward, the launches run on d.compute through forward(), and once the stream has drained, rows = min(M + 256, the model's
+// cap_rows) rows of every buffer, at the model's widths (the buffers are used densely at those widths), and the pooled output
+// are copied out.
+int trace_forward(Dev& d, DebugBuffers& b, const Model& m, const Input& in, int n_launches, const TraceOut& o, int* n_total) {
     const int total = launches_per_forward(m);
     if (n_launches < 0 || n_launches > total) return fail(B200RT_E_INVALID, "n_launches %d outside [0, %d]", n_launches, total);
     if (!o.yhi || !o.ylo || !o.pstats0 || !o.pstats1 || !o.qkv || !o.ctx || !o.ffn || !o.out) return fail(B200RT_E_INVALID, "null output buffer");
     if (n_total) *n_total = total;
-    Dev& d = *rt.devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    DebugBuffers b(d.compute);
     Input din = in;
     if (in.pixels) CUDA_TRY(b.upload(&din.pixels, in.pixels, static_cast<size_t>(in.B) * m.item_bytes));
     else {
@@ -1803,8 +1865,7 @@ int trace_forward(Runtime& rt, const Model& m, const Input& in, int n_launches, 
     const size_t R = g_rt->cap_rows, rows = std::min(static_cast<size_t>(in.B) * in.S + 256, static_cast<size_t>(m.cap_rows));
     const size_t H = m.hidden, I = m.inter, P = H / 128, out_floats = static_cast<size_t>(in.B) * m.out_dim;
     float* dout = nullptr;
-    CUDA_TRY(b.upload(&dout, nullptr, out_floats * 4));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, out_floats * 4, d.compute));
+    CUDA_TRY(b.poisoned(&dout, out_floats * 4));
     if (d.ev_ws_armed) CUDA_TRY(cudaStreamWaitEvent(d.compute, d.ev_ws, 0));
     for (int i = 0; i < 2; ++i) CUDA_TRY(cudaMemsetAsync(d.pstats[i], 0xFF, R * STAT_PARTS * sizeof(float2), d.compute));
     CUDA_TRY(cudaMemsetAsync(d.yhi, 0xFF, R * HIDDEN * 2, d.compute));
@@ -2193,6 +2254,7 @@ void b200rt_shutdown(void) {
 }
 
 // ------------------------------------------------------------------------------------------ debug entry points
+// Each entry checks what its own host copies need and the debug ABI's policy; the launchers judge every other operand.
 
 int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid, void* out,
                       int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
@@ -2204,100 +2266,72 @@ int b200rt_debug_gemm(int epi, const uint16_t* a, const uint16_t* w, const float
 int b200rt_debug_gemm_ex(int epi, const uint16_t* a, const uint16_t* w, const float* bias, const float* resid, void* out,
                          int M, int N, int K, int iters, float* ms_out, const float* ln_stats,
                          const float* ln_gamma, const float* ln_beta, float eps, float* stats_out, int sms, int* ctas_out, uint32_t flags) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (flags & ~B200RT_DEBUG_GEMM_LN512) return fail(B200RT_E_INVALID, "unknown gemm flags 0x%x", flags);
-    if (!a || !w || !bias || !out || M < 1 || N % 128 || K % 64 || epi < 0 || epi > 3) return fail(B200RT_E_INVALID, "bad gemm arguments");
-    if (epi == 2 && !resid) return fail(B200RT_E_INVALID, "epi 2 needs resid");
-    const int ln_w = epi == 2 ? N : K;
-    const bool ln512 = (flags & B200RT_DEBUG_GEMM_LN512) != 0;
-    if (ln_stats && ln_w != 768 && ln_w != 384 && ln_w != 1024 && !(ln512 && ln_w == 512))
-        return fail(B200RT_E_INVALID, ln512 ? "the LayerNorm'd width must be 768, 384, 1024 or 512" : "the LayerNorm'd width must be 768, 384 or 1024");
-    if (ln_stats && ln_w == 1024 && (epi == 3 || N % 256 != 0))
-        return fail(B200RT_E_INVALID, "a 1024-wide LayerNorm needs epi 0, 1 or 2 and N %% 256 == 0");
-    if (ln_stats && ln_w == 512 && ((epi != 0 && epi != 3) || N % 256 != 0))
-        return fail(B200RT_E_INVALID, "a 512-wide LayerNorm needs epi 0 or 3 and N %% 256 == 0");
-    if (ln_stats && epi == 2 && (!ln_gamma || !ln_beta)) return fail(B200RT_E_INVALID, "LayerNorm re-apply needs gamma and beta");
-    Dev& d = *rt->devs[0];
-    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
-    const int grid_sms = sms ? sms : d.sm_count;
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256;
-    const int parts_in = epi == 2 ? N / 128 : K / 128;
-    const int parts_out = N / 128;
-    DebugBuffers b(d.compute);
-    __half *da, *dw, *dhi = nullptr, *dlo = nullptr, *dhi0 = nullptr, *dlo0 = nullptr, *dout = nullptr;
-    float *db, *dg = nullptr, *dbt = nullptr;
-    float2 *dsi = nullptr, *dso = nullptr;
-    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));  // rows past M stay zero
-    CUDA_TRY(cudaMemcpyAsync(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, d.compute));
-    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
-    CUDA_TRY(b.upload(&db, bias, static_cast<size_t>(N) * 4));
-    if (ln_stats) {
-        CUDA_TRY(b.upload(&dsi, nullptr, Mp * parts_in * sizeof(float2)));
-        CUDA_TRY(cudaMemcpyAsync(dsi, ln_stats, static_cast<size_t>(M) * parts_in * sizeof(float2), cudaMemcpyHostToDevice, d.compute));
-    }
-    if (ln_gamma) CUDA_TRY(b.upload(&dg, ln_gamma, static_cast<size_t>(N) * 4));
-    if (ln_beta) CUDA_TRY(b.upload(&dbt, ln_beta, static_cast<size_t>(N) * 4));
-    CUtensorMap ta, tb;
-    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
-    if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
-    std::vector<__half> hhi, hlo;
-    ResEpi res{};  // epi 2: TMA maps over the residual's hi and lo
-    if (epi == 2) {
-        // the residual travels as hi + lo (fp16 + fp16): split on the host, keep a pristine copy for the final launch
-        hhi.assign(Mp * N, __float2half_rn(0.f));
-        hlo.assign(Mp * N, __float2half_rn(0.f));
-        for (size_t i = 0; i < static_cast<size_t>(M) * N; ++i) {
-            hhi[i] = __float2half_rn(resid[i]);
-            hlo[i] = __float2half_rn(resid[i] - __half2float(hhi[i]));
+    return on_root(sms, [&](Dev& d, DebugBuffers& b, int grid_sms) {
+        if (flags & ~B200RT_DEBUG_GEMM_LN512) return fail(B200RT_E_INVALID, "unknown gemm flags 0x%x", flags);
+        if (!a || !w || !bias || !out || M < 1 || N < 1 || K < 1) return fail(B200RT_E_INVALID, "bad gemm arguments");
+        if (epi == 2 && !resid) return fail(B200RT_E_INVALID, "epi 2 needs resid");
+        const int ln_w = epi == 2 ? N : K;
+        if (ln_stats && ln_w == 512 && !(flags & B200RT_DEBUG_GEMM_LN512))
+            return fail(B200RT_E_INVALID, "a 512-wide LayerNorm needs B200RT_DEBUG_GEMM_LN512");
+        const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256;
+        const int parts_in = ln_w / 128, parts_out = N / 128;
+        __half *da, *dw, *dhi = nullptr, *dlo = nullptr, *dhi0 = nullptr, *dlo0 = nullptr, *dout = nullptr;
+        float *db, *dg = nullptr, *dbt = nullptr;
+        float2 *dsi = nullptr, *dso = nullptr;
+        CUDA_TRY(b.upload(&da, a, static_cast<size_t>(M) * K * 2, Mp * K * 2));  // rows past M stay zero
+        CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
+        CUDA_TRY(b.upload(&db, bias, static_cast<size_t>(N) * 4));
+        if (ln_stats)  // at least one partial wide, so that a LayerNorm'd width under 128 still reaches the launcher as one
+            CUDA_TRY(b.upload(&dsi, ln_stats, static_cast<size_t>(M) * parts_in * sizeof(float2), Mp * std::max(parts_in, 1) * sizeof(float2)));
+        if (ln_gamma) CUDA_TRY(b.upload(&dg, ln_gamma, static_cast<size_t>(N) * 4));
+        if (ln_beta) CUDA_TRY(b.upload(&dbt, ln_beta, static_cast<size_t>(N) * 4));
+        CUtensorMap ta, tb;
+        if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
+        if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
+        std::vector<__half> hhi, hlo;
+        ResEpi res{};  // epi 2: TMA maps over the residual's hi and lo
+        OutEpi oe{};   // otherwise: the TMA map the output is stored through, M rows (the poisoned rows past M stay so)
+        if (epi == 2) {
+            // the residual travels as hi + lo (fp16 + fp16): split on the host, keep a pristine copy for the final launch
+            hhi.assign(Mp * N, __float2half_rn(0.f));
+            hlo.assign(Mp * N, __float2half_rn(0.f));
+            for (size_t i = 0; i < static_cast<size_t>(M) * N; ++i) {
+                hhi[i] = __float2half_rn(resid[i]);
+                hlo[i] = __float2half_rn(resid[i] - __half2float(hhi[i]));
+            }
+            CUDA_TRY(b.upload(&dhi0, hhi.data(), Mp * N * 2));
+            CUDA_TRY(b.upload(&dlo0, hlo.data(), Mp * N * 2));
+            CUDA_TRY(b.upload(&dhi, hhi.data(), Mp * N * 2));
+            CUDA_TRY(b.upload(&dlo, hlo.data(), Mp * N * 2));
+            CUDA_TRY(b.upload(&dso, nullptr, Mp * parts_out * sizeof(float2)));
+            if (int rc = make_map_2d(&res.hi, dhi, Mp, N, 128)) return rc;
+            if (int rc = make_map_2d(&res.lo, dlo, Mp, N, 128)) return rc;
+        } else {
+            CUDA_TRY(b.poisoned(&dout, Mp * N * 2));
+            if (int rc = make_map_2d(&oe.out, dout, M, N, 64)) return rc;
         }
-        CUDA_TRY(b.upload(&dhi0, hhi.data(), Mp * N * 2));
-        CUDA_TRY(b.upload(&dlo0, hlo.data(), Mp * N * 2));
-        CUDA_TRY(b.upload(&dhi, hhi.data(), Mp * N * 2));
-        CUDA_TRY(b.upload(&dlo, hlo.data(), Mp * N * 2));
-        CUDA_TRY(b.upload(&dso, nullptr, Mp * parts_out * sizeof(float2)));
-        if (int rc = make_map_2d(&res.hi, dhi, Mp, N, 128)) return rc;
-        if (int rc = make_map_2d(&res.lo, dlo, Mp, N, 128)) return rc;
-    } else {
-        CUDA_TRY(b.upload(&dout, nullptr, Mp * N * 2));
-        CUDA_TRY(cudaMemsetAsync(dout, 0xFF, Mp * N * 2, d.compute));
-    }
-    OutEpi oe{};  // epi 0/1/3: the TMA map the output is stored through, M rows (the poisoned rows past M stay so)
-    if (epi != 2)
-        if (int rc = make_map_2d(&oe.out, dout, M, N, 64)) return rc;
-    __half* const o_hi = epi == 2 ? dhi : dout;
-    GemmEpi e{db, dsi, parts_in, dg, dbt, dso, eps};
-    // epi 2 updates hi / lo in place (y = acc + bias + LN(y)): reload the residual before the launch whose result is returned
-    auto reload = [&]() -> cudaError_t {
-        if (epi != 2) return cudaSuccess;
-        cudaError_t ce = cudaMemcpyAsync(dhi, dhi0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute);
-        return ce != cudaSuccess ? ce : cudaMemcpyAsync(dlo, dlo0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute);
-    };
-    Event e0, e1;
-    CUDA_TRY(e0.create());
-    CUDA_TRY(e1.create());
-    if (iters < 1) iters = 1;
-    CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, epi == 2 ? nullptr : &oe, e, M, N, K, grid_sms, d.compute));  // timing (values drift in place)
-    CUDA_TRY(cudaEventRecord(e1, d.compute));
-    CUDA_TRY(reload());
-    CUDA_TRY(launch_gemm(epi, ta, tb, o_hi, dlo, epi == 2 ? &res : nullptr, epi == 2 ? nullptr : &oe, e, M, N, K, grid_sms, d.compute, ctas_out));  // the result that is returned
-    CUDA_TRY(cudaStreamSynchronize(d.compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    if (ms_out) *ms_out = ms / iters;
-    if (epi == 2) {
-        CUDA_TRY(b.download(hhi.data(), dhi, Mp * N * 2));
-        CUDA_TRY(b.download(hlo.data(), dlo, Mp * N * 2));
-        float* o = static_cast<float*>(out);
-        for (size_t i = 0; i < static_cast<size_t>(M) * N; ++i) o[i] = __half2float(hhi[i]) + __half2float(hlo[i]);
-        if (stats_out) CUDA_TRY(b.download(stats_out, dso, static_cast<size_t>(M) * parts_out * sizeof(float2)));
-    } else {
-        CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * N * 2));
-    }
-    return 0;
+        const GemmEpi e{db, dsi, parts_in, dg, dbt, dso, eps};
+        auto gemm = [&](int* ctas) {
+            return launch_gemm(epi, ta, tb, epi == 2 ? dhi : dout, dlo, epi == 2 ? &res : nullptr, epi == 2 ? nullptr : &oe, e, M, N, K, grid_sms,
+                               d.compute, ctas);
+        };
+        if (int rc = time_launches(d.compute, iters, ms_out, [&] { return gemm(nullptr); })) return rc;  // values drift in place
+        if (epi == 2) {  // y = acc + bias + LN(y) in place: reload the residual before the launch whose result is returned
+            CUDA_TRY(cudaMemcpyAsync(dhi, dhi0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute));
+            CUDA_TRY(cudaMemcpyAsync(dlo, dlo0, Mp * N * 2, cudaMemcpyDeviceToDevice, d.compute));
+        }
+        LAUNCH_TRY(gemm(ctas_out));
+        if (epi == 2) {
+            CUDA_TRY(b.download(hhi.data(), dhi, Mp * N * 2));
+            CUDA_TRY(b.download(hlo.data(), dlo, Mp * N * 2));
+            float* o = static_cast<float*>(out);
+            for (size_t i = 0; i < static_cast<size_t>(M) * N; ++i) o[i] = __half2float(hhi[i]) + __half2float(hlo[i]);
+            if (stats_out) CUDA_TRY(b.download(stats_out, dso, static_cast<size_t>(M) * parts_out * sizeof(float2)));
+        } else {
+            CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * N * 2));
+        }
+        return 0;
+    });
 }
 
 int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms,
@@ -2307,506 +2341,334 @@ int b200rt_debug_attention(const uint16_t* qkv, const int32_t* lens, uint16_t* c
 
 int b200rt_debug_attention_ex(const uint16_t* qkv, const int32_t* lens, uint16_t* ctx, int B, int S, int iters, float* ms_out, int sms,
                               int head_dim, int heads, uint32_t flags) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!qkv || !lens || !ctx || B < 1 || S < 1 || S > MAX_SEQ) return fail(B200RT_E_INVALID, "bad attention arguments");
-    if (flags & ~B200RT_DEBUG_ATTN_CAUSAL) return fail(B200RT_E_INVALID, "unknown attention flags 0x%x", flags);
-    const bool causal = (flags & B200RT_DEBUG_ATTN_CAUSAL) != 0;
-    if (head_dim == 0) head_dim = 64;
-    if (heads == 0) heads = HEADS;
-    if (causal && !(head_dim == 64 && heads == 8))
-        return fail(B200RT_E_INVALID, "causal attention exists for (head_dim, heads) = (64, 8), got (%d, %d)", head_dim, heads);
-    if (!causal && !((head_dim == 64 && heads == 12) || (head_dim == 32 && heads == 12) || (head_dim == 64 && heads == 16)))
-        return fail(B200RT_E_INVALID, "(head_dim, heads) must be (64, 12), (32, 12) or (64, 16) (0 = 64, 12), got (%d, %d)", head_dim, heads);
-    const size_t H = static_cast<size_t>(heads) * head_dim;
-    Dev& d = *rt->devs[0];
-    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
-    const int grid_sms = sms ? sms : d.sm_count;
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t M = static_cast<size_t>(B) * S;
-    DebugBuffers b(d.compute);
-    __half *dq, *dc;
-    int32_t* dl_;
-    CUDA_TRY(b.upload(&dq, qkv, M * 3 * H * 2));
-    CUDA_TRY(b.upload(&dc, nullptr, M * H * 2));
-    CUDA_TRY(cudaMemsetAsync(dc, 0xFF, M * H * 2, d.compute));
-    CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));
-    CUtensorMap tq, tc;
-    if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, head_dim)) return rc;
-    if (int rc = make_map_qkv(&tc, dc, B, S, H, head_dim)) return rc;
-    Event e0, e1;
-    CUDA_TRY(e0.create());
-    CUDA_TRY(e1.create());
-    if (iters < 1) iters = 1;
-    CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads, causal));
-    CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads, causal));
-    CUDA_TRY(cudaEventRecord(e1, d.compute));
-    CUDA_TRY(cudaStreamSynchronize(d.compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    if (ms_out) *ms_out = ms / iters;
-    CUDA_TRY(b.download(ctx, dc, M * H * 2));
-    return 0;
+    return on_root(sms, [&](Dev& d, DebugBuffers& b, int grid_sms) {
+        if (flags & ~B200RT_DEBUG_ATTN_CAUSAL) return fail(B200RT_E_INVALID, "unknown attention flags 0x%x", flags);
+        if (head_dim == 0) head_dim = 64;
+        if (heads == 0) heads = HEADS;
+        if (!qkv || !lens || !ctx || B < 1 || S < 1 || head_dim < 1 || heads < 1) return fail(B200RT_E_INVALID, "bad attention arguments");
+        const bool causal = (flags & B200RT_DEBUG_ATTN_CAUSAL) != 0;
+        const size_t H = static_cast<size_t>(heads) * head_dim, M = static_cast<size_t>(B) * S;
+        __half *dq, *dc;
+        int32_t* dl_;
+        CUDA_TRY(b.upload(&dq, qkv, M * 3 * H * 2));
+        CUDA_TRY(b.poisoned(&dc, M * H * 2));
+        CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));
+        CUtensorMap tq, tc;
+        if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, head_dim)) return rc;
+        if (int rc = make_map_qkv(&tc, dc, B, S, H, head_dim)) return rc;
+        auto attention = [&] { return launch_attention(tq, tc, dl_, B, S, grid_sms, d.compute, head_dim, heads, causal); };
+        LAUNCH_TRY(attention());
+        if (int rc = time_launches(d.compute, iters, ms_out, attention)) return rc;
+        CUDA_TRY(b.download(ctx, dc, M * H * 2));
+        return 0;
+    });
+}
+
+// embed (segs NULL: type holds one row) and embed_segs (type holds two)
+static int debug_embed(const int32_t* ids, const int32_t* segs, const float* word, const float* pos, const float* type, int n_tokens, int S,
+                       int vocab, uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden) {
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!ids || !word || !pos || !type || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1 || hidden < 1 ||
+            (segs && n_tokens % S))
+            return fail(B200RT_E_INVALID, "bad embed arguments (with segs, n_tokens must be a multiple of S)");
+        const size_t H = hidden, P = H / 128, rows = static_cast<size_t>(n_tokens);
+        int32_t *dids, *dsegs = nullptr;
+        float *dw, *dp, *dt;
+        __half *dhi, *dlo;
+        float2* dst;
+        CUDA_TRY(b.upload(&dids, ids, rows * 4));
+        if (segs) CUDA_TRY(b.upload(&dsegs, segs, rows / S * 4));  // passed through unchecked: the kernel clamps to [0, S]
+        CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * H * 4));
+        CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * H * 4));
+        CUDA_TRY(b.upload(&dt, type, (segs ? 2 : 1) * H * 4));
+        CUDA_TRY(b.upload(&dhi, nullptr, rows * H * 2));
+        CUDA_TRY(b.upload(&dlo, nullptr, rows * H * 2));
+        CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
+        LAUNCH_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, hidden, d.compute, dsegs));
+        CUDA_TRY(b.download(hi_out, dhi, rows * H * 2));
+        CUDA_TRY(b.download(lo_out, dlo, rows * H * 2));
+        CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
+        return 0;
+    });
 }
 
 int b200rt_debug_embed(const int32_t* ids, const float* word, const float* pos, const float* type0, int n_tokens, int S, int vocab,
                        uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!ids || !word || !pos || !type0 || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1)
-        return fail(B200RT_E_INVALID, "bad embed arguments");
-    if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384 && hidden != 1024 && hidden != 512)
-        return fail(B200RT_E_INVALID, "row width must be 768, 384, 1024 or 512 (0 = 768), got %d", hidden);
-    const size_t H = hidden, P = H / 128;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_tokens);
-    DebugBuffers b(d.compute);
-    int32_t* dids;
-    float *dw, *dp, *dt;
-    __half *dhi, *dlo;
-    float2* dst;
-    CUDA_TRY(b.upload(&dids, ids, rows * 4));
-    CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * H * 4));
-    CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * H * 4));
-    CUDA_TRY(b.upload(&dt, type0, H * 4));
-    CUDA_TRY(b.upload(&dhi, nullptr, rows * H * 2));
-    CUDA_TRY(b.upload(&dlo, nullptr, rows * H * 2));
-    CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
-    CUDA_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, hidden, d.compute));
-    CUDA_TRY(b.download(hi_out, dhi, rows * H * 2));
-    CUDA_TRY(b.download(lo_out, dlo, rows * H * 2));
-    CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
-    return 0;
+    return debug_embed(ids, nullptr, word, pos, type0, n_tokens, S, vocab, hi_out, lo_out, stats_out, hidden == 0 ? 768 : hidden);
 }
 
 int b200rt_debug_embed_segs(const int32_t* ids, const int32_t* segs, const float* word, const float* pos, const float* type, int n_tokens,
                             int S, int vocab, uint16_t* hi_out, uint16_t* lo_out, float* stats_out, int hidden) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!ids || !segs || !word || !pos || !type || !hi_out || !lo_out || !stats_out || n_tokens < 1 || S < 1 || vocab < 1 || n_tokens % S)
-        return fail(B200RT_E_INVALID, "bad embed_segs arguments (n_tokens must be a multiple of S)");
-    if (hidden != 768 && hidden != 384 && hidden != 1024)
-        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024, got %d", hidden);
-    const size_t H = hidden, P = H / 128;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_tokens);
-    DebugBuffers b(d.compute);
-    int32_t *dids, *dsegs;
-    float *dw, *dp, *dt;
-    __half *dhi, *dlo;
-    float2* dst;
-    CUDA_TRY(b.upload(&dids, ids, rows * 4));
-    CUDA_TRY(b.upload(&dsegs, segs, rows / S * 4));  // passed through unchecked: the kernel clamps to [0, S]
-    CUDA_TRY(b.upload(&dw, word, static_cast<size_t>(vocab) * H * 4));
-    CUDA_TRY(b.upload(&dp, pos, static_cast<size_t>(S) * H * 4));
-    CUDA_TRY(b.upload(&dt, type, 2 * H * 4));
-    CUDA_TRY(b.upload(&dhi, nullptr, rows * H * 2));
-    CUDA_TRY(b.upload(&dlo, nullptr, rows * H * 2));
-    CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
-    CUDA_TRY(launch_embed(dids, dw, dp, dt, dhi, dlo, dst, n_tokens, S, vocab, hidden, d.compute, dsegs));
-    CUDA_TRY(b.download(hi_out, dhi, rows * H * 2));
-    CUDA_TRY(b.download(lo_out, dlo, rows * H * 2));
-    CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
-    return 0;
+    if (!segs) return fail(B200RT_E_INVALID, "embed_segs needs segs");
+    return debug_embed(ids, segs, word, pos, type, n_tokens, S, vocab, hi_out, lo_out, stats_out, hidden);
 }
 
 int b200rt_debug_cls_head(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* pool_w,
                           const float* pool_b, const float* cls_w, const float* cls_b, int n_items, int S, int L, float eps, float* out,
                           int hidden, int ctas) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!hi || !lo || !gamma || !beta || !pool_w || !pool_b || !cls_w || !cls_b || !out || n_items < 1 || S < 1 || ctas < 0)
-        return fail(B200RT_E_INVALID, "bad cls_head arguments");
-    if (L < 1 || L > MAX_LABELS) return fail(B200RT_E_INVALID, "num_labels %d outside [1, %d]", L, MAX_LABELS);
-    if (hidden != 768 && hidden != 384 && hidden != 1024)
-        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024, got %d", hidden);
-    const size_t H = hidden;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_items) * S;
-    DebugBuffers b(d.compute);
-    __half *dhi, *dlo;
-    float *dg, *dbt, *dpw, *dpb, *dcw, *dcb, *dout;
-    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
-    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
-    CUDA_TRY(b.upload(&dg, gamma, H * 4));
-    CUDA_TRY(b.upload(&dbt, beta, H * 4));
-    CUDA_TRY(b.upload(&dpw, pool_w, H * H * 4));
-    CUDA_TRY(b.upload(&dpb, pool_b, H * 4));
-    CUDA_TRY(b.upload(&dcw, cls_w, static_cast<size_t>(L) * H * 4));
-    CUDA_TRY(b.upload(&dcb, cls_b, static_cast<size_t>(L) * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * L * 4));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, static_cast<size_t>(n_items) * L * 4, d.compute));
-    CUDA_TRY(launch_cls_head(dhi, dlo, dg, dbt, dpw, dpb, dcw, dcb, dout, n_items, S, L, eps, hidden, d.compute, ctas));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * L * 4));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!hi || !lo || !gamma || !beta || !pool_w || !pool_b || !cls_w || !cls_b || !out || n_items < 1 || S < 1 || L < 1 || hidden < 1)
+            return fail(B200RT_E_INVALID, "bad cls_head arguments");
+        const size_t H = hidden, rows = static_cast<size_t>(n_items) * S;
+        __half *dhi, *dlo;
+        float *dg, *dbt, *dpw, *dpb, *dcw, *dcb, *dout;
+        CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+        CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+        CUDA_TRY(b.upload(&dg, gamma, H * 4));
+        CUDA_TRY(b.upload(&dbt, beta, H * 4));
+        CUDA_TRY(b.upload(&dpw, pool_w, H * H * 4));
+        CUDA_TRY(b.upload(&dpb, pool_b, H * 4));
+        CUDA_TRY(b.upload(&dcw, cls_w, static_cast<size_t>(L) * H * 4));
+        CUDA_TRY(b.upload(&dcb, cls_b, static_cast<size_t>(L) * 4));
+        CUDA_TRY(b.poisoned(&dout, static_cast<size_t>(n_items) * L * 4));
+        LAUNCH_TRY(launch_cls_head(dhi, dlo, dg, dbt, dpw, dpb, dcw, dcb, dout, n_items, S, L, eps, hidden, d.compute, ctas));
+        CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * L * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_gemm_splade(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const int32_t* lens, int B, int S,
                              int N, int K, int vocab, float eps, int sms, int iters, float* ms_out, uint32_t* vmax_out, int* ctas_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!a || !w || !c || !stats || !lens || !vmax_out || B < 1 || S < 64 || S % 64 || N % 256 || vocab < 1 || vocab > N)
-        return fail(B200RT_E_INVALID, "bad gemm_splade arguments (S a multiple of 64, N of 256, 1 <= vocab <= N)");
-    if (K != 768 && K != 384 && K != 1024) return fail(B200RT_E_INVALID, "K (the LayerNorm'd width) must be 768, 384 or 1024, got %d", K);
-    Dev& d = *rt->devs[0];
-    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t M = static_cast<size_t>(B) * S, Mp = (M + 255) / 256 * 256, P = K / 128, nmax = static_cast<size_t>(B) * N;
-    DebugBuffers b(d.compute);
-    __half *da, *dw;
-    float *dc;
-    float2* dst;
-    int32_t* dl_;
-    uint32_t* dmax;
-    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));
-    CUDA_TRY(cudaMemcpyAsync(da, a, M * K * 2, cudaMemcpyHostToDevice, d.compute));
-    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(vocab) * K * 2));  // [vocab, K]: the map reads rows past vocab as zeros, as a model's
-    CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
-    CUDA_TRY(b.upload(&dst, stats, M * P * sizeof(float2)));
-    CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));
-    CUDA_TRY(b.upload(&dmax, nullptr, nmax * 4));
-    CUtensorMap ta, tb;
-    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
-    if (int rc = make_map_2d(&tb, dw, vocab, K, 128)) return rc;
-    const GemmEpi e{dc, dst, static_cast<int>(P), nullptr, nullptr, nullptr, eps};
-    const SpladeEpi sp{dl_, S, dmax, vocab};
-    const int grid_sms = sms ? sms : d.sm_count;
-    Event e0, e1;
-    CUDA_TRY(e0.create());
-    CUDA_TRY(e1.create());
-    if (iters < 1) iters = 1;
-    CUDA_TRY(cudaEventRecord(e0, d.compute));
-    for (int i = 0; i < iters; ++i) CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute));
-    CUDA_TRY(cudaEventRecord(e1, d.compute));
-    CUDA_TRY(cudaMemsetAsync(dmax, 0, nmax * 4, d.compute));  // the returned maxima come from one launch on a zeroed buffer
-    CUDA_TRY(launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute, ctas_out));
-    CUDA_TRY(cudaStreamSynchronize(d.compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    if (ms_out) *ms_out = ms / iters;
-    CUDA_TRY(b.download(vmax_out, dmax, nmax * 4));
-    return 0;
+    return on_root(sms, [&](Dev& d, DebugBuffers& b, int grid_sms) {
+        if (!a || !w || !c || !stats || !lens || !vmax_out || B < 1 || S < 1 || N < 1 || K < 1 || vocab < 1)
+            return fail(B200RT_E_INVALID, "bad gemm_splade arguments");
+        const size_t M = static_cast<size_t>(B) * S, Mp = (M + 255) / 256 * 256, P = K / 128, nmax = static_cast<size_t>(B) * N;
+        __half *da, *dw;
+        float* dc;
+        float2* dst;
+        int32_t* dl_;
+        uint32_t* dmax;
+        CUDA_TRY(b.upload(&da, a, M * K * 2, Mp * K * 2));
+        CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(vocab) * K * 2));  // [vocab, K]: the map reads rows past vocab as zeros, as a model's
+        CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
+        CUDA_TRY(b.upload(&dst, stats, M * P * sizeof(float2)));
+        CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));
+        CUDA_TRY(b.upload(&dmax, nullptr, nmax * 4));
+        CUtensorMap ta, tb;
+        if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
+        if (int rc = make_map_2d(&tb, dw, vocab, K, 128)) return rc;
+        const GemmEpi e{dc, dst, static_cast<int>(P), nullptr, nullptr, nullptr, eps};
+        const SpladeEpi sp{dl_, S, dmax, vocab};
+        auto splade = [&](int* ctas) { return launch_gemm_splade(ta, tb, e, sp, static_cast<int>(M), N, K, grid_sms, d.compute, ctas); };
+        if (int rc = time_launches(d.compute, iters, ms_out, [&] { return splade(nullptr); })) return rc;
+        CUDA_TRY(cudaMemsetAsync(dmax, 0, nmax * 4, d.compute));  // the returned maxima come from one launch on a zeroed buffer
+        LAUNCH_TRY(splade(ctas_out));
+        CUDA_TRY(b.download(vmax_out, dmax, nmax * 4));
+        return 0;
+    });
+}
+
+// gemm_rope (table non-NULL) and gemm_swiglu: nomic-bert's fused epilogues over a [M, 768] and w [N, 768]
+static int debug_nomic_gemm(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const float* table, int n_pos, int M,
+                            int N, int S, int rot_cols, float eps, int sms, uint16_t* out, int* ctas_out) {
+    return on_root(sms, [&](Dev& d, DebugBuffers& b, int grid_sms) {
+        if (!a || !w || !c || !out || M < 1 || N < 1 || (table && (S < 1 || n_pos < S)))
+            return fail(B200RT_E_INVALID, "bad fused GEMM arguments (gemm_rope: n_pos >= S)");
+        constexpr size_t K = HIDDEN;
+        const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256, out_cols = table ? N : N / 2;
+        __half *da, *dw, *dout;
+        float *dc, *dt = nullptr;
+        float2* dst = nullptr;
+        CUDA_TRY(b.upload(&da, a, static_cast<size_t>(M) * K * 2, Mp * K * 2));
+        CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
+        CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
+        if (table) CUDA_TRY(b.upload(&dt, table, static_cast<size_t>(n_pos) * 64 * 4));
+        if (stats) CUDA_TRY(b.upload(&dst, stats, static_cast<size_t>(M) * STAT_PARTS * sizeof(float2)));
+        CUDA_TRY(b.poisoned(&dout, static_cast<size_t>(M) * out_cols * 2));
+        CUtensorMap ta, tb;
+        if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
+        if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
+        const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
+        LAUNCH_TRY(table ? launch_gemm_rope(ta, tb, dout, e, RopeEpi{reinterpret_cast<const float2*>(dt), S, rot_cols}, M, N, static_cast<int>(K),
+                                            grid_sms, d.compute, ctas_out)
+                         : launch_gemm_swiglu(ta, tb, dout, e, M, N, static_cast<int>(K), grid_sms, d.compute, ctas_out));
+        CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * out_cols * 2));
+        return 0;
+    });
 }
 
 int b200rt_debug_gemm_rope(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, const float* table, int n_pos, int M,
                            int N, int S, int rot_cols, float eps, int sms, uint16_t* out, int* ctas_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!a || !w || !c || !table || !out || M < 1 || N < 256 || N % 256 || S < 64 || S % 64 || n_pos < S || rot_cols < 0 || rot_cols % 256 ||
-        rot_cols > N)
-        return fail(B200RT_E_INVALID, "bad gemm_rope arguments (N a multiple of 256, S of 64, n_pos >= S, rot_cols a multiple of 256 <= N)");
-    Dev& d = *rt->devs[0];
-    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    constexpr size_t K = HIDDEN;
-    const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256;
-    DebugBuffers b(d.compute);
-    __half *da, *dw, *dout;
-    float *dc, *dt;
-    float2* dst = nullptr;
-    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));
-    CUDA_TRY(cudaMemcpyAsync(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, d.compute));
-    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
-    CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
-    CUDA_TRY(b.upload(&dt, table, static_cast<size_t>(n_pos) * 64 * 4));
-    if (stats) CUDA_TRY(b.upload(&dst, stats, static_cast<size_t>(M) * STAT_PARTS * sizeof(float2)));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(M) * N * 2));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, static_cast<size_t>(M) * N * 2, d.compute));
-    CUtensorMap ta, tb;
-    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
-    if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
-    const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
-    CUDA_TRY(launch_gemm_rope(ta, tb, dout, e, RopeEpi{reinterpret_cast<const float2*>(dt), S, rot_cols}, M, N, static_cast<int>(K),
-                              sms ? sms : d.sm_count, d.compute, ctas_out));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * N * 2));
-    return 0;
+    if (!table) return fail(B200RT_E_INVALID, "gemm_rope needs its table");
+    return debug_nomic_gemm(a, w, c, stats, table, n_pos, M, N, S, rot_cols, eps, sms, out, ctas_out);
 }
 
 int b200rt_debug_gemm_swiglu(const uint16_t* a, const uint16_t* w, const float* c, const float* stats, int M, int N, float eps, int sms,
                              uint16_t* out, int* ctas_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!a || !w || !c || !out || M < 1 || N < 256 || N % 256) return fail(B200RT_E_INVALID, "bad gemm_swiglu arguments (N a multiple of 256)");
-    Dev& d = *rt->devs[0];
-    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    constexpr size_t K = HIDDEN;
-    const size_t Mp = (static_cast<size_t>(M) + 255) / 256 * 256, No = static_cast<size_t>(N) / 2;
-    DebugBuffers b(d.compute);
-    __half *da, *dw, *dout;
-    float* dc;
-    float2* dst = nullptr;
-    CUDA_TRY(b.upload(&da, nullptr, Mp * K * 2));
-    CUDA_TRY(cudaMemcpyAsync(da, a, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, d.compute));
-    CUDA_TRY(b.upload(&dw, w, static_cast<size_t>(N) * K * 2));
-    CUDA_TRY(b.upload(&dc, c, static_cast<size_t>(N) * 4));
-    if (stats) CUDA_TRY(b.upload(&dst, stats, static_cast<size_t>(M) * STAT_PARTS * sizeof(float2)));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(M) * No * 2));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, static_cast<size_t>(M) * No * 2, d.compute));
-    CUtensorMap ta, tb;
-    if (int rc = make_map_2d(&ta, da, Mp, K, 128)) return rc;
-    if (int rc = make_map_2d(&tb, dw, N, K, 128)) return rc;
-    const GemmEpi e{dc, dst, STAT_PARTS, nullptr, nullptr, nullptr, eps};
-    CUDA_TRY(launch_gemm_swiglu(ta, tb, dout, e, M, N, static_cast<int>(K), sms ? sms : d.sm_count, d.compute, ctas_out));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(M) * No * 2));
-    return 0;
+    return debug_nomic_gemm(a, w, c, stats, nullptr, 0, M, N, 0, 0, eps, sms, out, ctas_out);
 }
 
 int b200rt_debug_attention_stream(const uint16_t* qkv, const int32_t* lens, int B, int S, uint16_t* ctx, int sms, int iters, float* ms_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!qkv || !lens || !ctx || B < 1 || S < 64 || S % 64 || S > MAX_SEQ_LONG)
-        return fail(B200RT_E_INVALID, "bad attention_stream arguments (64 <= S <= %d, a multiple of 64)", MAX_SEQ_LONG);
-    Dev& d = *rt->devs[0];
-    if (sms < 0 || sms > d.sm_count) return fail(B200RT_E_INVALID, "sms must be 0 (every SM) or 1..%d, got %d", d.sm_count, sms);
-    const int grid_sms = sms ? sms : d.sm_count;
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t M = static_cast<size_t>(B) * S, H = HIDDEN;
-    DebugBuffers b(d.compute);
-    __half *dq, *dc;
-    int32_t* dl_;
-    CUDA_TRY(b.upload(&dq, qkv, M * 3 * H * 2));
-    CUDA_TRY(b.upload(&dc, nullptr, M * H * 2));
-    CUDA_TRY(cudaMemsetAsync(dc, 0xFF, M * H * 2, d.compute));
-    CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));  // passed through unchecked: the kernel clamps to [1, S]
-    CUtensorMap tq;
-    if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, 64)) return rc;
-    CUDA_TRY(launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute));
-    CUDA_TRY(b.download(ctx, dc, M * H * 2));
-    if (iters > 0) {
-        Event e0, e1;
-        CUDA_TRY(e0.create());
-        CUDA_TRY(e1.create());
-        CUDA_TRY(cudaEventRecord(e0, d.compute));
-        for (int i = 0; i < iters; ++i) CUDA_TRY(launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute));
-        CUDA_TRY(cudaEventRecord(e1, d.compute));
-        CUDA_TRY(cudaStreamSynchronize(d.compute));
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
-        if (ms_out) *ms_out = ms / iters;
-    }
-    return 0;
+    return on_root(sms, [&](Dev& d, DebugBuffers& b, int grid_sms) {
+        if (!qkv || !lens || !ctx || B < 1 || S < 1) return fail(B200RT_E_INVALID, "bad attention_stream arguments");
+        const size_t M = static_cast<size_t>(B) * S, H = HIDDEN;
+        __half *dq, *dc;
+        int32_t* dl_;
+        CUDA_TRY(b.upload(&dq, qkv, M * 3 * H * 2));
+        CUDA_TRY(b.poisoned(&dc, M * H * 2));
+        CUDA_TRY(b.upload(&dl_, lens, static_cast<size_t>(B) * 4));  // passed through unchecked: the kernel clamps to [1, S]
+        CUtensorMap tq;
+        if (int rc = make_map_qkv(&tq, dq, B, S, 3 * H, 64)) return rc;
+        auto attention = [&] { return launch_attention_stream(tq, dc, dl_, B, S, grid_sms, d.compute); };
+        LAUNCH_TRY(attention());
+        CUDA_TRY(b.download(ctx, dc, M * H * 2));
+        return iters > 0 ? time_launches(d.compute, iters, ms_out, attention) : 0;
+    });
 }
 
 int b200rt_debug_mlm_ln_stats(const uint16_t* u, int n_rows, int hidden, size_t n_max, uint32_t* vmax_out, float* stats_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!u || !stats_out || n_rows < 1 || (n_max > 0 && !vmax_out)) return fail(B200RT_E_INVALID, "bad mlm_ln_stats arguments");
-    if (hidden != 768 && hidden != 384 && hidden != 1024) return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024, got %d", hidden);
-    const size_t rows = static_cast<size_t>(n_rows), H = hidden, P = H / 128;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    DebugBuffers b(d.compute);
-    __half* du;
-    float2* dst;
-    uint32_t* dmax = nullptr;
-    CUDA_TRY(b.upload(&du, u, rows * H * 2));
-    CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
-    if (n_max > 0) {
-        CUDA_TRY(b.upload(&dmax, nullptr, n_max * 4));
-        CUDA_TRY(cudaMemsetAsync(dmax, 0xFF, n_max * 4, d.compute));
-    }
-    CUDA_TRY(launch_mlm_ln_stats(du, dst, dmax, n_rows, n_max, hidden, d.compute));
-    CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
-    if (n_max > 0) CUDA_TRY(b.download(vmax_out, dmax, n_max * 4));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!u || !stats_out || n_rows < 1 || hidden < 1 || (n_max > 0 && !vmax_out)) return fail(B200RT_E_INVALID, "bad mlm_ln_stats arguments");
+        const size_t rows = static_cast<size_t>(n_rows), H = hidden, P = H / 128;
+        __half* du;
+        float2* dst;
+        uint32_t* dmax = nullptr;
+        CUDA_TRY(b.upload(&du, u, rows * H * 2));
+        CUDA_TRY(b.upload(&dst, nullptr, rows * P * sizeof(float2)));
+        if (n_max > 0) CUDA_TRY(b.poisoned(&dmax, n_max * 4));
+        LAUNCH_TRY(launch_mlm_ln_stats(du, dst, dmax, n_rows, n_max, hidden, d.compute));
+        CUDA_TRY(b.download(stats_out, dst, rows * P * sizeof(float2)));
+        if (n_max > 0) CUDA_TRY(b.download(vmax_out, dmax, n_max * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_splade_finalize(const uint32_t* vmax, int n_items, int vpad, int vocab, float* out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!vmax || !out || n_items < 1 || vocab < 1 || vpad < vocab) return fail(B200RT_E_INVALID, "bad splade_finalize arguments");
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t n_out = static_cast<size_t>(n_items) * vocab;
-    DebugBuffers b(d.compute);
-    uint32_t* dmax;
-    float* dout;
-    CUDA_TRY(b.upload(&dmax, vmax, static_cast<size_t>(n_items) * vpad * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, n_out * 4));
-    CUDA_TRY(cudaMemsetAsync(dout, 0xFF, n_out * 4, d.compute));
-    CUDA_TRY(launch_splade_finalize(dmax, dout, n_items, vpad, vocab, d.compute));
-    CUDA_TRY(b.download(out, dout, n_out * 4));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!vmax || !out || n_items < 1 || vocab < 1 || vpad < 1) return fail(B200RT_E_INVALID, "bad splade_finalize arguments");
+        const size_t n_out = static_cast<size_t>(n_items) * vocab;
+        uint32_t* dmax;
+        float* dout;
+        CUDA_TRY(b.upload(&dmax, vmax, static_cast<size_t>(n_items) * vpad * 4));
+        CUDA_TRY(b.poisoned(&dout, n_out * 4));
+        LAUNCH_TRY(launch_splade_finalize(dmax, dout, n_items, vpad, vocab, d.compute));
+        CUDA_TRY(b.download(out, dout, n_out * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_vit_embed(const uint16_t* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                            int n_rows, int T, float eps, uint16_t* hi_out, uint16_t* lo_out, float* stats_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!patch_out || !cls || !pos || !gamma || !beta || !hi_out || !lo_out || !stats_out || n_rows < 1 || T < 1)
-        return fail(B200RT_E_INVALID, "bad vit_embed arguments");
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_rows);
-    DebugBuffers b(d.compute);
-    __half *dpatch, *dhi, *dlo;
-    float *dcls, *dpos, *dg, *dbt;
-    float2* dst;
-    CUDA_TRY(b.upload(&dpatch, patch_out, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dcls, cls, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dpos, pos, static_cast<size_t>(T) * HIDDEN * 4));
-    CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dhi, nullptr, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dlo, nullptr, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dst, nullptr, rows * STAT_PARTS * sizeof(float2)));
-    CUDA_TRY(launch_vit_embed(dpatch, dcls, dpos, dg, dbt, dhi, dlo, dst, n_rows, T, eps, d.compute));
-    CUDA_TRY(b.download(hi_out, dhi, rows * HIDDEN * 2));
-    CUDA_TRY(b.download(lo_out, dlo, rows * HIDDEN * 2));
-    CUDA_TRY(b.download(stats_out, dst, rows * STAT_PARTS * sizeof(float2)));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!patch_out || !cls || !pos || !gamma || !beta || !hi_out || !lo_out || !stats_out || n_rows < 1 || T < 1)
+            return fail(B200RT_E_INVALID, "bad vit_embed arguments");
+        const size_t rows = static_cast<size_t>(n_rows);
+        __half *dpatch, *dhi, *dlo;
+        float *dcls, *dpos, *dg, *dbt;
+        float2* dst;
+        CUDA_TRY(b.upload(&dpatch, patch_out, rows * HIDDEN * 2));
+        CUDA_TRY(b.upload(&dcls, cls, HIDDEN * 4));
+        CUDA_TRY(b.upload(&dpos, pos, static_cast<size_t>(T) * HIDDEN * 4));
+        CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
+        CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
+        CUDA_TRY(b.upload(&dhi, nullptr, rows * HIDDEN * 2));
+        CUDA_TRY(b.upload(&dlo, nullptr, rows * HIDDEN * 2));
+        CUDA_TRY(b.upload(&dst, nullptr, rows * STAT_PARTS * sizeof(float2)));
+        LAUNCH_TRY(launch_vit_embed(dpatch, dcls, dpos, dg, dbt, dhi, dlo, dst, n_rows, T, eps, d.compute));
+        CUDA_TRY(b.download(hi_out, dhi, rows * HIDDEN * 2));
+        CUDA_TRY(b.download(lo_out, dlo, rows * HIDDEN * 2));
+        CUDA_TRY(b.download(stats_out, dst, rows * STAT_PARTS * sizeof(float2)));
+        return 0;
+    });
+}
+
+// pool_normalize (lens NULL) and mean_pool_normalize
+static int debug_pool(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const int32_t* lens, int n_items, int S,
+                      float eps, float* out, int hidden) {
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!hi || !lo || !gamma || !beta || !out || n_items < 1 || S < 1 || hidden < 1) return fail(B200RT_E_INVALID, "bad pool arguments");
+        const size_t H = hidden, rows = static_cast<size_t>(n_items) * S;
+        __half *dhi, *dlo;
+        float *dg, *dbt, *dout;
+        int32_t* dlens = nullptr;
+        CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+        CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+        CUDA_TRY(b.upload(&dg, gamma, H * 4));
+        CUDA_TRY(b.upload(&dbt, beta, H * 4));
+        if (lens) CUDA_TRY(b.upload(&dlens, lens, static_cast<size_t>(n_items) * 4));  // passed through unchecked: the kernel clamps to [1, S]
+        CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * H * 4));
+        LAUNCH_TRY(lens ? launch_mean_pool_normalize(dhi, dlo, dg, dbt, dlens, dout, n_items, S, eps, hidden, d.compute)
+                        : launch_pool_normalize(dhi, dlo, dg, dbt, dout, n_items, S, eps, hidden, d.compute));
+        CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * H * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, int n_items, int S,
                                 float eps, float* out, int hidden) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!hi || !lo || !gamma || !beta || !out || n_items < 1 || S < 1) return fail(B200RT_E_INVALID, "bad pool_normalize arguments");
-    if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384 && hidden != 1024)
-        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024 (0 = 768), got %d", hidden);
-    const size_t H = hidden;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_items) * S;
-    DebugBuffers b(d.compute);
-    __half *dhi, *dlo;
-    float *dg, *dbt, *dout;
-    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
-    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
-    CUDA_TRY(b.upload(&dg, gamma, H * 4));
-    CUDA_TRY(b.upload(&dbt, beta, H * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * H * 4));
-    CUDA_TRY(launch_pool_normalize(dhi, dlo, dg, dbt, dout, n_items, S, eps, hidden, d.compute));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * H * 4));
-    return 0;
+    return debug_pool(hi, lo, gamma, beta, nullptr, n_items, S, eps, out, hidden == 0 ? 768 : hidden);
 }
 
 int b200rt_debug_mean_pool_normalize(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const int32_t* lens,
                                      int n_items, int S, float eps, float* out, int hidden) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!hi || !lo || !gamma || !beta || !lens || !out || n_items < 1 || S < 1)
-        return fail(B200RT_E_INVALID, "bad mean_pool_normalize arguments");
-    if (hidden == 0) hidden = 768;
-    if (hidden != 768 && hidden != 384 && hidden != 1024)
-        return fail(B200RT_E_INVALID, "row width must be 768, 384 or 1024 (0 = 768), got %d", hidden);
-    const size_t H = hidden;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_items) * S;
-    DebugBuffers b(d.compute);
-    __half *dhi, *dlo;
-    float *dg, *dbt, *dout;
-    int32_t* dlens;
-    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
-    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
-    CUDA_TRY(b.upload(&dg, gamma, H * 4));
-    CUDA_TRY(b.upload(&dbt, beta, H * 4));
-    CUDA_TRY(b.upload(&dlens, lens, static_cast<size_t>(n_items) * 4));  // passed through unchecked: the kernel clamps to [1, S]
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * H * 4));
-    CUDA_TRY(launch_mean_pool_normalize(dhi, dlo, dg, dbt, dlens, dout, n_items, S, eps, hidden, d.compute));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * H * 4));
-    return 0;
+    if (!lens) return fail(B200RT_E_INVALID, "mean_pool_normalize needs lens");
+    return debug_pool(hi, lo, gamma, beta, lens, n_items, S, eps, out, hidden == 0 ? 768 : hidden);
 }
 
 int b200rt_debug_vit_pool(const uint16_t* hi, const uint16_t* lo, const float* gamma, const float* beta, const float* proj, int n_items,
                           int T, int P, float eps, float* out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!hi || !lo || !gamma || !beta || !proj || !out || n_items < 1 || T < 1) return fail(B200RT_E_INVALID, "bad vit_pool arguments");
-    if (P < 1 || P > 1024) return fail(B200RT_E_INVALID, "projection width %d outside [1, 1024]", P);
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_items) * T;
-    DebugBuffers b(d.compute);
-    __half *dhi, *dlo;
-    float *dg, *dbt, *dproj, *dout;
-    CUDA_TRY(b.upload(&dhi, hi, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dlo, lo, rows * HIDDEN * 2));
-    CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
-    CUDA_TRY(b.upload(&dproj, proj, static_cast<size_t>(P) * HIDDEN * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * P * 4));
-    CUDA_TRY(launch_vit_pool(dhi, dlo, dg, dbt, dproj, dout, n_items, T, P, eps, d.compute));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * P * 4));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!hi || !lo || !gamma || !beta || !proj || !out || n_items < 1 || T < 1 || P < 1) return fail(B200RT_E_INVALID, "bad vit_pool arguments");
+        const size_t rows = static_cast<size_t>(n_items) * T;
+        __half *dhi, *dlo;
+        float *dg, *dbt, *dproj, *dout;
+        CUDA_TRY(b.upload(&dhi, hi, rows * HIDDEN * 2));
+        CUDA_TRY(b.upload(&dlo, lo, rows * HIDDEN * 2));
+        CUDA_TRY(b.upload(&dg, gamma, HIDDEN * 4));
+        CUDA_TRY(b.upload(&dbt, beta, HIDDEN * 4));
+        CUDA_TRY(b.upload(&dproj, proj, static_cast<size_t>(P) * HIDDEN * 4));
+        CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * P * 4));
+        LAUNCH_TRY(launch_vit_pool(dhi, dlo, dg, dbt, dproj, dout, n_items, T, P, eps, d.compute));
+        CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * P * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_clip_text_pool(const uint16_t* hi, const uint16_t* lo, const int32_t* ids, const int32_t* lens, const float* gamma,
                                 const float* beta, const float* proj, int n_items, int S, int P, float eps, int eos_id, float* out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!hi || !lo || !ids || !lens || !gamma || !beta || !proj || !out || n_items < 1 || S < 1)
-        return fail(B200RT_E_INVALID, "bad clip_text_pool arguments");
-    if (P < 1 || P > 1024) return fail(B200RT_E_INVALID, "projection width %d outside [1, 1024]", P);
-    constexpr size_t H = 512;
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t rows = static_cast<size_t>(n_items) * S;
-    DebugBuffers b(d.compute);
-    __half *dhi, *dlo;
-    int32_t *dids, *dlens;
-    float *dg, *dbt, *dproj, *dout;
-    CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
-    CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
-    CUDA_TRY(b.upload(&dids, ids, rows * 4));
-    CUDA_TRY(b.upload(&dlens, lens, static_cast<size_t>(n_items) * 4));  // passed through unchecked: the kernel clamps to [1, S]
-    CUDA_TRY(b.upload(&dg, gamma, H * 4));
-    CUDA_TRY(b.upload(&dbt, beta, H * 4));
-    CUDA_TRY(b.upload(&dproj, proj, static_cast<size_t>(P) * H * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * P * 4));
-    CUDA_TRY(launch_clip_text_pool(dhi, dlo, dids, dlens, dg, dbt, dproj, dout, n_items, S, P, eps, eos_id, d.compute));
-    CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * P * 4));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!hi || !lo || !ids || !lens || !gamma || !beta || !proj || !out || n_items < 1 || S < 1 || P < 1)
+            return fail(B200RT_E_INVALID, "bad clip_text_pool arguments");
+        constexpr size_t H = 512;
+        const size_t rows = static_cast<size_t>(n_items) * S;
+        __half *dhi, *dlo;
+        int32_t *dids, *dlens;
+        float *dg, *dbt, *dproj, *dout;
+        CUDA_TRY(b.upload(&dhi, hi, rows * H * 2));
+        CUDA_TRY(b.upload(&dlo, lo, rows * H * 2));
+        CUDA_TRY(b.upload(&dids, ids, rows * 4));
+        CUDA_TRY(b.upload(&dlens, lens, static_cast<size_t>(n_items) * 4));  // passed through unchecked: the kernel clamps to [1, S]
+        CUDA_TRY(b.upload(&dg, gamma, H * 4));
+        CUDA_TRY(b.upload(&dbt, beta, H * 4));
+        CUDA_TRY(b.upload(&dproj, proj, static_cast<size_t>(P) * H * 4));
+        CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * P * 4));
+        LAUNCH_TRY(launch_clip_text_pool(dhi, dlo, dids, dlens, dg, dbt, dproj, dout, n_items, S, P, eps, eos_id, d.compute));
+        CUDA_TRY(b.download(out, dout, static_cast<size_t>(n_items) * P * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, int N, int K, uint16_t* w_out,
                          float* cvec_out) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    if (!w || !w_out || N < 1 || K < 64 || K % 64) return fail(B200RT_E_INVALID, "bad fold_ln arguments (K must be a multiple of 64)");
-    if (gamma && (!beta || !cvec_out)) return fail(B200RT_E_INVALID, "a LayerNorm fold needs beta and cvec_out");
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    const size_t n = static_cast<size_t>(N) * K;
-    DebugBuffers b(d.compute);
-    float *dw, *dg = nullptr, *dbt = nullptr, *dbias = nullptr, *dc = nullptr;
-    __half* dout;
-    CUDA_TRY(b.upload(&dw, w, n * 4));
-    if (gamma) {
-        CUDA_TRY(b.upload(&dg, gamma, static_cast<size_t>(K) * 4));
-        CUDA_TRY(b.upload(&dbt, beta, static_cast<size_t>(K) * 4));
-        if (bias) CUDA_TRY(b.upload(&dbias, bias, static_cast<size_t>(N) * 4));
-        CUDA_TRY(b.upload(&dc, nullptr, static_cast<size_t>(N) * 4));
-    }
-    CUDA_TRY(b.upload(&dout, nullptr, n * 2));
-    CUDA_TRY(launch_fold_ln(dw, dg, dbt, dbias, dout, dc, N, K, d.compute));
-    CUDA_TRY(b.download(w_out, dout, n * 2));
-    if (gamma) CUDA_TRY(b.download(cvec_out, dc, static_cast<size_t>(N) * 4));
-    return 0;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        if (!w || !w_out || N < 1 || K < 1) return fail(B200RT_E_INVALID, "bad fold_ln arguments");
+        if (gamma && (!beta || !cvec_out)) return fail(B200RT_E_INVALID, "a LayerNorm fold needs beta and cvec_out");
+        const size_t n = static_cast<size_t>(N) * K;
+        float *dw, *dg = nullptr, *dbt = nullptr, *dbias = nullptr, *dc = nullptr;
+        __half* dout;
+        CUDA_TRY(b.upload(&dw, w, n * 4));
+        if (gamma) {
+            CUDA_TRY(b.upload(&dg, gamma, static_cast<size_t>(K) * 4));
+            CUDA_TRY(b.upload(&dbt, beta, static_cast<size_t>(K) * 4));
+            if (bias) CUDA_TRY(b.upload(&dbias, bias, static_cast<size_t>(N) * 4));
+            CUDA_TRY(b.upload(&dc, nullptr, static_cast<size_t>(N) * 4));
+        }
+        CUDA_TRY(b.upload(&dout, nullptr, n * 2));
+        LAUNCH_TRY(launch_fold_ln(dw, dg, dbt, dbias, dout, dc, N, K, d.compute));
+        CUDA_TRY(b.download(w_out, dout, n * 2));
+        if (gamma) CUDA_TRY(b.download(cvec_out, dc, static_cast<size_t>(N) * 4));
+        return 0;
+    });
 }
 
 int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* lens, int n_items, int max_len, int n_launches,
@@ -2819,31 +2681,31 @@ int b200rt_debug_forward_trace(int model, const int32_t* ids, const int32_t* len
 int b200rt_debug_forward_trace_segs(int model, const int32_t* ids, const int32_t* lens, const int32_t* segs, int n_items, int max_len,
                                     int n_launches, uint16_t* yhi, uint16_t* ylo, float* pstats0, float* pstats1, uint16_t* qkv,
                                     uint16_t* ctx, uint16_t* ffn, float* out, char* names_out, size_t names_cap, int* n_total) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    const Model* m = get_model(*rt, model);
-    if (!m) return B200RT_E_INVALID;
-    if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
-    if (int rc = check_ids(*m, ids, lens, n_items, max_len, max_wave_len(*m))) return rc;
-    if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
-    if (static_cast<size_t>(n_items) * max_len > static_cast<size_t>(m->cap_rows))
-        return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
-    std::vector<int32_t> l(n_items, max_len);
-    if (lens) l.assign(lens, lens + n_items);
-    const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(*rt, *m, Input{ids, l.data(), nullptr, n_items, max_len, segs}, n_launches, o, n_total);
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        const Model* m = get_model(*g_rt, model);
+        if (!m) return B200RT_E_INVALID;
+        if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+        if (int rc = check_ids(*m, ids, lens, n_items, max_len, max_wave_len(*m))) return rc;
+        if (int rc = check_segs(*m, lens, segs, n_items, max_len)) return rc;
+        if (static_cast<size_t>(n_items) * max_len > static_cast<size_t>(m->cap_rows))
+            return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
+        std::vector<int32_t> l(n_items, max_len);
+        if (lens) l.assign(lens, lens + n_items);
+        const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
+        return trace_forward(d, b, *m, Input{ids, l.data(), nullptr, n_items, max_len, segs}, n_launches, o, n_total);
+    });
 }
 
 int b200rt_debug_vit_forward_trace(int model, const float* pixels, int n_items, int n_launches, uint16_t* yhi, uint16_t* ylo,
                                    float* pstats0, float* pstats1, uint16_t* qkv, uint16_t* ctx, uint16_t* ffn, float* out,
                                    char* names_out, size_t names_cap, int* n_total) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    const Model* m = get_model(*rt, model);
-    if (!m) return B200RT_E_INVALID;
-    if (m->kind != VIT || !pixels || n_items < 1 || n_items > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "bad arguments");
-    const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
-    return trace_forward(*rt, *m, Input{nullptr, nullptr, pixels, n_items, m->tokens}, n_launches, o, n_total);
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        const Model* m = get_model(*g_rt, model);
+        if (!m) return B200RT_E_INVALID;
+        if (m->kind != VIT || !pixels || n_items < 1 || n_items > VIT_WAVE_ITEMS) return fail(B200RT_E_INVALID, "bad arguments");
+        const TraceOut o{yhi, ylo, qkv, ctx, ffn, pstats0, pstats1, out, names_out, names_cap};
+        return trace_forward(d, b, *m, Input{nullptr, nullptr, pixels, n_items, m->tokens}, n_launches, o, n_total);
+    });
 }
 
 int b200rt_debug_model_cap_rows(int model) {
@@ -2856,52 +2718,48 @@ int b200rt_debug_model_cap_rows(int model) {
 
 int b200rt_debug_profile_forward(int model, int n_items, int max_len, int iters, char* names_out, size_t names_cap,
                                  float* ms_out, int* n_out, int cap) {
-    Runtime* rt = live_rt();
-    if (!rt) return g_poisoned.load() ? B200RT_E_CUDA : B200RT_E_STATE;
-    const Model* m = get_model(*rt, model);
-    if (!m) return B200RT_E_INVALID;
-    if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
-    if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
-    const size_t M = static_cast<size_t>(n_items) * max_len;
-    if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
-    Dev& d = *rt->devs[0];
-    std::lock_guard<std::mutex> dl(d.mu);
-    CUDA_TRY(cudaSetDevice(d.id));
-    std::vector<int32_t> ids(M), l(n_items, std::min(max_len, m->max_pos));  // a clip_text wave may be longer than its items
-    uint32_t x = 12345;
-    for (auto& v : ids) { x = x * 1664525u + 1013904223u; v = 1000 + static_cast<int32_t>((x >> 8) % (m->vocab - 1000)); }
-    DebugBuffers b(d.compute);
-    int32_t *dids = nullptr, *dlens = nullptr;
-    float* dout = nullptr;
-    CUDA_TRY(b.upload(&dids, ids.data(), M * 4));
-    CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
-    CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * m->out_dim * 4));
-    if (iters < 1) iters = 1;
-    std::map<std::string, double> acc;
-    std::vector<std::string> order;
-    for (int it = 0; it < iters + 1; ++it) {
-        LaunchHook hook;
-        hook.timing = true;
-        uint64_t launches = 0;
-        if (int rc = forward(d, *m, 0, Input{dids, dlens, nullptr, n_items, max_len}, dout, d.compute, launches, &hook)) return rc;
-        CUDA_TRY(cudaStreamSynchronize(d.compute));
-        for (size_t i = 0; it > 0 && i < hook.names.size(); ++i) {  // the first forward warms up
-            float ms = 0;
-            cudaEventElapsedTime(&ms, hook.evs[i], hook.evs[i + 1]);
-            if (!acc.count(hook.names[i])) order.push_back(hook.names[i]);
-            acc[hook.names[i]] += ms;
+    return on_root(0, [&](Dev& d, DebugBuffers& b, int) {
+        const Model* m = get_model(*g_rt, model);
+        if (!m) return B200RT_E_INVALID;
+        if (m->kind == VIT) return fail(B200RT_E_INVALID, "model %d is not a text encoder", model);
+        if (!names_out || !ms_out || !n_out || n_items < 1 || max_len < 1 || max_len > max_wave_len(*m)) return fail(B200RT_E_INVALID, "bad argument");
+        const size_t M = static_cast<size_t>(n_items) * max_len;
+        if (M > static_cast<size_t>(m->cap_rows)) return fail(B200RT_E_INVALID, "batch exceeds the model's wave capacity");
+        std::vector<int32_t> ids(M), l(n_items, std::min(max_len, m->max_pos));  // a clip_text wave may be longer than its items
+        uint32_t x = 12345;
+        for (auto& v : ids) { x = x * 1664525u + 1013904223u; v = 1000 + static_cast<int32_t>((x >> 8) % (m->vocab - 1000)); }
+        int32_t *dids = nullptr, *dlens = nullptr;
+        float* dout = nullptr;
+        CUDA_TRY(b.upload(&dids, ids.data(), M * 4));
+        CUDA_TRY(b.upload(&dlens, l.data(), static_cast<size_t>(n_items) * 4));
+        CUDA_TRY(b.upload(&dout, nullptr, static_cast<size_t>(n_items) * m->out_dim * 4));
+        if (iters < 1) iters = 1;
+        std::map<std::string, double> acc;
+        std::vector<std::string> order;
+        for (int it = 0; it < iters + 1; ++it) {
+            LaunchHook hook;
+            hook.timing = true;
+            uint64_t launches = 0;
+            if (int rc = forward(d, *m, 0, Input{dids, dlens, nullptr, n_items, max_len}, dout, d.compute, launches, &hook)) return rc;
+            CUDA_TRY(cudaStreamSynchronize(d.compute));
+            for (size_t i = 0; it > 0 && i < hook.names.size(); ++i) {  // the first forward warms up
+                float ms = 0;
+                cudaEventElapsedTime(&ms, hook.evs[i], hook.evs[i + 1]);
+                if (!acc.count(hook.names[i])) order.push_back(hook.names[i]);
+                acc[hook.names[i]] += ms;
+            }
         }
-    }
-    size_t off = 0;
-    int n = 0;
-    for (const auto& name : order) {
-        if (n >= cap || off + name.size() + 1 > names_cap) break;
-        memcpy(names_out + off, name.c_str(), name.size() + 1);
-        off += name.size() + 1;
-        ms_out[n++] = static_cast<float>(acc[name] / iters);
-    }
-    *n_out = n;
-    return 0;
+        size_t off = 0;
+        int n = 0;
+        for (const auto& name : order) {
+            if (n >= cap || off + name.size() + 1 > names_cap) break;
+            memcpy(names_out + off, name.c_str(), name.size() + 1);
+            off += name.size() + 1;
+            ms_out[n++] = static_cast<float>(acc[name] / iters);
+        }
+        *n_out = n;
+        return 0;
+    });
 }
 
 }  // extern "C"

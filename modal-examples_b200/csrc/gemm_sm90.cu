@@ -76,6 +76,7 @@
 // BertSelfAttention :143-207 (fused QKV), BertSelfOutput.dense :287-298, BertIntermediate :330-342
 // (dense + GELU) and BertOutput.dense :345-356.
 #include <algorithm>
+#include <tuple>
 
 #include "kernels.h"
 #include "ptx.cuh"
@@ -572,51 +573,32 @@ static int& max_clusters() {
     return n;
 }
 
+// Every gemm_kernel<EPI, BN, PARTS> the launchers can select, each set up at init and launched from this one list.  A launch
+// selects BN = 256 when N % 256 == 0, else 128, and PARTS = e.parts_in with statistics, else 6 (not read), and is refused with
+// cudaErrorInvalidValue when that instantiation is not listed.  Eight partials (bge-large's 1024-wide LayerNorm) exist for BN =
+// 256 and every epilogue but quick-GELU: every bge-large N is a multiple of 256.  Four partials (the CLIP text tower's 512-wide
+// LayerNorm, folded into QKV and the quick-GELU FFN1) exist for BN = 256 and EPI 0 / 3 only; its residual epilogues take no
+// statistics (pre-LN).  Three partials re-applied by the residual epilogue mean N = 384, never a multiple of 256: no
+// <RES_SPLIT, 256, 3>.
 template <int EPI, int BN, int PARTS>
-static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M, int N,
-                              int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{},
-                              const RopeEpi& rp = RopeEpi{}, const ResEpi& res = ResEpi{}, const OutEpi& oe = OutEpi{}) {
-    const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
-    int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
-    if (clusters < 1) clusters = 1;
-    if (ctas) *ctas = clusters * gemm::CM;
-    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::smem_bytes<EPI, BN>(),
-                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp, res, oe);
-}
-
-// the tile width and statistic count of a launch: BN = 256 whenever N allows it (every bge-base / bge-large / ViT / CLIP text
-// launch), else 128.  Eight partials (bge-large's 1024-wide LayerNorm) exist for BN = 256 and the text epilogues only: every
-// bge-large N is a multiple of 256.  Four partials (the CLIP text tower's 512-wide LayerNorm, folded into QKV and the quick-GELU
-// FFN1) exist for BN = 256 and EPI 0 / 3 only; its residual epilogues take no statistics (pre-LN, stats_in NULL).
-template <int EPI>
-static cudaError_t launch_epi(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi& res, const OutEpi& oe,
-                              const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
-    const bool wide = N % 256 == 0;
-    if (e.stats_in != nullptr && e.parts_in == 8) {
-        if constexpr (EPI != EPI_BIAS_QGELU_F16) {
-            if (wide) return launch_one<EPI, 256, 8>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
-        }
-        return cudaErrorInvalidValue;
-    }
-    if (e.stats_in != nullptr && e.parts_in == 4) {
-        if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16) {
-            if (wide) return launch_one<EPI, 256, 4>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
-        }
-        return cudaErrorInvalidValue;
-    }
-    const bool six = e.stats_in == nullptr || e.parts_in == 6;
-    if (wide) {
-        if (six) return launch_one<EPI, 256, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
-        // three partials re-applied by the residual epilogue mean N = 384, never a multiple of 256: no <RES_SPLIT, 256, 3>
-        if constexpr (EPI != EPI_BIAS_RES_SPLIT) return launch_one<EPI, 256, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
-        return cudaErrorInvalidValue;
-    }
-    return six ? launch_one<EPI, 128, 6>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe)
-               : launch_one<EPI, 128, 3>(ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, res, oe);
-}
+struct Inst {
+    static constexpr int epi = EPI, bn = BN, parts = PARTS;
+};
+constexpr std::tuple<
+    Inst<EPI_BIAS_F16, 256, 6>, Inst<EPI_BIAS_F16, 256, 3>, Inst<EPI_BIAS_F16, 128, 6>, Inst<EPI_BIAS_F16, 128, 3>,
+    Inst<EPI_BIAS_F16, 256, 4>, Inst<EPI_BIAS_F16, 256, 8>,
+    Inst<EPI_BIAS_GELU_F16, 256, 6>, Inst<EPI_BIAS_GELU_F16, 256, 3>, Inst<EPI_BIAS_GELU_F16, 128, 6>, Inst<EPI_BIAS_GELU_F16, 128, 3>,
+    Inst<EPI_BIAS_GELU_F16, 256, 8>,
+    Inst<EPI_BIAS_QGELU_F16, 256, 6>, Inst<EPI_BIAS_QGELU_F16, 256, 3>, Inst<EPI_BIAS_QGELU_F16, 128, 6>, Inst<EPI_BIAS_QGELU_F16, 128, 3>,
+    Inst<EPI_BIAS_QGELU_F16, 256, 4>,
+    Inst<EPI_BIAS_RES_SPLIT, 256, 6>, Inst<EPI_BIAS_RES_SPLIT, 128, 6>, Inst<EPI_BIAS_RES_SPLIT, 128, 3>, Inst<EPI_BIAS_RES_SPLIT, 256, 8>,
+    Inst<EPI_SPLADE_MAX, 256, 6>, Inst<EPI_SPLADE_MAX, 256, 3>, Inst<EPI_SPLADE_MAX, 256, 8>,
+    Inst<EPI_ROPE_F16, 256, 6>,
+    Inst<EPI_SWIGLU_F16, 256, 6>>
+    INSTANTIATIONS{};
 
 template <int EPI, int BN, int PARTS>
-static cudaError_t setup() {
+static cudaError_t setup(Inst<EPI, BN, PARTS>) {
     auto kernel = gemm::gemm_kernel<EPI, BN, PARTS>;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::smem_bytes<EPI, BN>());
     if (e != cudaSuccess) return e;
@@ -631,53 +613,52 @@ static cudaError_t setup() {
     m = m == 0 ? n : std::min(m, n);
     return cudaSuccess;
 }
-template <int EPI>
-static cudaError_t setup_epi() {
-    cudaError_t e;
-    if ((e = setup<EPI, 256, 6>()) != cudaSuccess) return e;
-    if constexpr (EPI != EPI_BIAS_RES_SPLIT)
-        if ((e = setup<EPI, 256, 3>()) != cudaSuccess) return e;
-    if ((e = setup<EPI, 128, 6>()) != cudaSuccess) return e;
-    if ((e = setup<EPI, 128, 3>()) != cudaSuccess) return e;
-    if constexpr (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_QGELU_F16)
-        if ((e = setup<EPI, 256, 4>()) != cudaSuccess) return e;
-    if constexpr (EPI != EPI_BIAS_QGELU_F16) return setup<EPI, 256, 8>();
-    return cudaSuccess;
-}
 
 cudaError_t gemm_init_device() {
-    cudaError_t e;
-    if ((e = setup_epi<EPI_BIAS_F16>()) != cudaSuccess) return e;
-    if ((e = setup_epi<EPI_BIAS_GELU_F16>()) != cudaSuccess) return e;
-    if ((e = setup_epi<EPI_BIAS_QGELU_F16>()) != cudaSuccess) return e;
-    if ((e = setup_epi<EPI_BIAS_RES_SPLIT>()) != cudaSuccess) return e;
-    if ((e = setup<EPI_SPLADE_MAX, 256, 6>()) != cudaSuccess) return e;
-    if ((e = setup<EPI_SPLADE_MAX, 256, 3>()) != cudaSuccess) return e;
-    if ((e = setup<EPI_SPLADE_MAX, 256, 8>()) != cudaSuccess) return e;
-    if ((e = setup<EPI_ROPE_F16, 256, 6>()) != cudaSuccess) return e;
-    return setup<EPI_SWIGLU_F16, 256, 6>();
+    cudaError_t e = cudaSuccess;
+    std::apply([&](auto... inst) { (((e = setup(inst)) == cudaSuccess) && ...); }, INSTANTIATIONS);
+    return e;
+}
+
+template <int EPI, int BN, int PARTS>
+static cudaError_t launch_one(Inst<EPI, BN, PARTS>, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo,
+                              const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp,
+                              const RopeEpi& rp, const ResEpi& res, const OutEpi& oe) {
+    const int pairs = ((M + gemm::CM * gemm::BM - 1) / (gemm::CM * gemm::BM)) * (N / BN);
+    int clusters = std::min({pairs, sm_count / gemm::CM, max_clusters<EPI, BN, PARTS>()});
+    if (clusters < 1) clusters = 1;
+    if (ctas) *ctas = clusters * gemm::CM;
+    return launch_pdl(gemm::gemm_kernel<EPI, BN, PARTS>, dim3(clusters * gemm::CM), dim3(gemm::NUM_THREADS), gemm::smem_bytes<EPI, BN>(),
+                      stream, ta, tb, e, out, out_lo, M, N, K, sp, rp, res, oe);
+}
+
+// launches the listed instantiation that epilogue `epi` selects for these operands (see INSTANTIATIONS)
+static cudaError_t launch_listed(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const GemmEpi& e, int M,
+                                 int N, int K, int sm_count, cudaStream_t stream, int* ctas, const SpladeEpi& sp = SpladeEpi{},
+                                 const RopeEpi& rp = RopeEpi{}, const ResEpi& res = ResEpi{}, const OutEpi& oe = OutEpi{}) {
+    const int bn = N % 256 == 0 ? 256 : 128, parts = e.stats_in != nullptr ? e.parts_in : 6;
+    cudaError_t r = cudaErrorInvalidValue;
+    std::apply([&](auto... inst) {
+        ((inst.epi == epi && inst.bn == bn && inst.parts == parts && (r = launch_one(inst, ta, tb, out, out_lo, e, M, N, K, sm_count, stream,
+                                                                                  ctas, sp, rp, res, oe), true)) || ...);
+    }, INSTANTIATIONS);
+    return r;
 }
 
 cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, __half* out, __half* out_lo, const ResEpi* res,
                         const OutEpi* oe, const GemmEpi& e, int M, int N, int K, int sm_count, cudaStream_t stream, int* ctas) {
     if (N % 128 != 0 || K % gemm::BK != 0 || M <= 0 || e.bias == nullptr || out == nullptr || sm_count < 1) return cudaErrorInvalidValue;
-    // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply; 1024, 768,
-    // 512 or 384
-    const int ln_width = epi == EPI_BIAS_RES_SPLIT ? N : K;
-    if (e.stats_in != nullptr && ((e.parts_in != 8 && e.parts_in != 6 && e.parts_in != 4 && e.parts_in != 3) || e.parts_in * 128 != ln_width))
-        return cudaErrorInvalidValue;
-    if (gemm::tma_store_epi(epi) && oe == nullptr) return cudaErrorInvalidValue;
-    switch (epi) {
-        case EPI_BIAS_F16: return launch_epi<EPI_BIAS_F16>(ta, tb, out, nullptr, ResEpi{}, *oe, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_GELU_F16: return launch_epi<EPI_BIAS_GELU_F16>(ta, tb, out, nullptr, ResEpi{}, *oe, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_QGELU_F16: return launch_epi<EPI_BIAS_QGELU_F16>(ta, tb, out, nullptr, ResEpi{}, *oe, e, M, N, K, sm_count, stream, ctas);
-        case EPI_BIAS_RES_SPLIT:
-            if (out_lo == nullptr || res == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr)))
-                return cudaErrorInvalidValue;
-            if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
-            return launch_epi<EPI_BIAS_RES_SPLIT>(ta, tb, out, out_lo, *res, OutEpi{}, e, M, N, K, sm_count, stream, ctas);
+    // the statistics describe the LayerNorm'd row: K wide for a folded LayerNorm, N wide for the residual re-apply
+    const bool resid = epi == EPI_BIAS_RES_SPLIT;
+    if (e.stats_in != nullptr && e.parts_in * 128 != (resid ? N : K)) return cudaErrorInvalidValue;
+    if (gemm::tma_store_epi(epi)) {
+        if (oe == nullptr) return cudaErrorInvalidValue;
+        return launch_listed(epi, ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, ResEpi{}, *oe);
     }
-    return cudaErrorInvalidValue;
+    if (!resid || out_lo == nullptr || res == nullptr || (e.stats_in != nullptr && (e.ln_gamma == nullptr || e.ln_beta == nullptr)))
+        return cudaErrorInvalidValue;
+    if (e.stats_out != nullptr && e.stats_out == e.stats_in) return cudaErrorInvalidValue;
+    return launch_listed(epi, ta, tb, out, out_lo, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, RopeEpi{}, *res);
 }
 
 cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi& e, const SpladeEpi& sp, int M, int N, int K,
@@ -686,28 +667,20 @@ cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, con
         return cudaErrorInvalidValue;
     if (sp.lens == nullptr || sp.vmax == nullptr || sp.S < 64 || sp.S % 64 != 0 || M % sp.S != 0 || sp.vocab < 1 || sp.vocab > N)
         return cudaErrorInvalidValue;
-    switch (e.parts_in) {
-        case 6: return launch_one<EPI_SPLADE_MAX, 256, 6>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
-        case 3: return launch_one<EPI_SPLADE_MAX, 256, 3>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
-        case 8: return launch_one<EPI_SPLADE_MAX, 256, 8>(ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
-    }
-    return cudaErrorInvalidValue;
+    return launch_listed(EPI_SPLADE_MAX, ta, tb, nullptr, nullptr, e, M, N, K, sm_count, stream, ctas, sp);
 }
-
 
 cudaError_t launch_gemm_rope(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, const GemmEpi& e, const RopeEpi& rp, int M, int N,
                              int K, int sm_count, cudaStream_t stream, int* ctas) {
-    if (N % 256 != 0 || K != 768 || M <= 0 || sm_count < 1 || out == nullptr || e.bias == nullptr || (e.stats_in != nullptr && e.parts_in != 6))
-        return cudaErrorInvalidValue;
+    if (N % 256 != 0 || K != 768 || M <= 0 || sm_count < 1 || out == nullptr || e.bias == nullptr) return cudaErrorInvalidValue;
     if (rp.table == nullptr || rp.S < 64 || rp.S % 64 != 0 || rp.rot_cols < 0 || rp.rot_cols % 256 != 0 || rp.rot_cols > N) return cudaErrorInvalidValue;
-    return launch_one<EPI_ROPE_F16, 256, 6>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, rp);
+    return launch_listed(EPI_ROPE_F16, ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas, SpladeEpi{}, rp);
 }
 
 cudaError_t launch_gemm_swiglu(const CUtensorMap& ta, const CUtensorMap& tb, __half* out, const GemmEpi& e, int M, int N, int K, int sm_count,
                                cudaStream_t stream, int* ctas) {
-    if (N % 256 != 0 || K != 768 || M <= 0 || sm_count < 1 || out == nullptr || e.bias == nullptr || (e.stats_in != nullptr && e.parts_in != 6))
-        return cudaErrorInvalidValue;
-    return launch_one<EPI_SWIGLU_F16, 256, 6>(ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
+    if (N % 256 != 0 || K != 768 || M <= 0 || sm_count < 1 || out == nullptr || e.bias == nullptr) return cudaErrorInvalidValue;
+    return launch_listed(EPI_SWIGLU_F16, ta, tb, out, nullptr, e, M, N, K, sm_count, stream, ctas);
 }
 
 }  // namespace b200

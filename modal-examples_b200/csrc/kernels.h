@@ -1,4 +1,6 @@
 // Internal launch interface between the engine (host C++) and the sm_90a kernels.
+// Every launch_* function refuses operands outside the contract its comment documents with cudaErrorInvalidValue, having
+// enqueued nothing.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -82,7 +84,8 @@ cudaError_t launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, _
 //   vmax[i * N + n] = max(vmax[i * N + n], bits(max over rows r of item i with r % S < lens[i] of max(C[r, n], 0)))
 // by red.global.max.u32 on the fp32 bits (exact and order-independent for values >= 0), one per 64-row consumer half and
 // column, none for a zero.  vmax must hold zeros (or earlier maxima) for the B items; columns >= vocab are never written.
-// e.stats_in is required (the LayerNorm of A, K wide: 768, 384 or 1024); N % 256 == 0.  lens[i] is clamped to [0, S].
+// e.stats_in is required (the LayerNorm of A, K wide: 768, 384 or 1024); N % 256 == 0, 1 <= vocab <= N, S >= 64 a multiple of 64
+// dividing M.  lens[i] is clamped to [0, S].
 struct SpladeEpi {
     const int32_t* lens;  // [B]
     int S;
@@ -95,7 +98,8 @@ cudaError_t launch_gemm_splade(const CUtensorMap& ta, const CUtensorMap& tb, con
 // Rotary embedding of the QKV projection (EPI_ROPE_F16): out = fp16 [M, N] of v = LNfold(acc) + bias (e.stats_in NULL: acc +
 // bias), and on columns n < rot_cols (Q | K; a multiple of 256) the pair (d, d + 32) of every 64-column head, v_d and
 // v_{d+32}, becomes (v_d cos - v_{d+32} sin, v_{d+32} cos + v_d sin) with (cos, sin) = table[(row % S) * 32 + d] (HF's
-// rotate_half, not interleaved).  table: fp32 [>= S rows][32] float2, one row per position.  K = 768 (6 partials), N % 256 == 0.
+// rotate_half, not interleaved).  table: fp32 [>= S rows][32] float2, one row per position.  K = 768 (6 partials), N % 256 == 0,
+// S >= 64 a multiple of 64, rot_cols <= N.
 struct RopeEpi {
     const float2* table;
     int S;         // padded length of the wave's items: row r is position r % S
@@ -111,12 +115,12 @@ cudaError_t launch_gemm_swiglu(const CUtensorMap& ta, const CUtensorMap& tb, __h
                                cudaStream_t stream, int* ctas = nullptr);
 
 // gamma != NULL: w_out[n,k] = fp16(w[n,k] gamma[k] - mean_k(w[n,:] gamma)), cvec[n] = sum_k w[n,k] beta[k] + bias[n]
-// gamma == NULL: w_out = fp16(w) (cvec untouched)
+// gamma == NULL: w_out = fp16(w) (cvec untouched).  N >= 1, K % 64 == 0.
 cudaError_t launch_fold_ln(const float* w, const float* gamma, const float* beta, const float* bias, __half* w_out, float* cvec,
                            int N, int K, cudaStream_t stream);
 
 // Multi-head self-attention over a padded batch of `heads` heads of head_dim, H = heads head_dim: (head_dim, heads) is
-// (64, 12), (32, 12) or (64, 16); causal (key k masked for query row q when k > q, CLIP's text tower): (64, 8) only.  qkv fp16 [B, S, 3H] (Q | K | V, head-major within each), lens[B] valid keys per item, ctx
+// (64, 12), (32, 12) or (64, 16); causal (key k masked for query row q when k > q, CLIP's text tower): (64, 8) only.  1 <= S <= 512.  qkv fp16 [B, S, 3H] (Q | K | V, head-major within each), lens[B] valid keys per item, ctx
 // fp16 [B*S, H].  tq: 3D map over qkv {3H, S, B}, tctx: 3D map over ctx {H, S, B}; both box {head_dim, 128, 1}, 128B (d = 64)
 // or 64B (d = 32) swizzle.  Persistent: min(units, sm_count) CTAs walk the (item, head[, query tile]) units.
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tctx, const int32_t* lens, int B, int S, int sm_count,
@@ -150,7 +154,7 @@ cudaError_t launch_cls_head(const __half* yhi, const __half* ylo, const float* g
 cudaError_t launch_mlm_ln_stats(const __half* u, float2* stats, uint32_t* vmax, int n_rows, size_t n_max, int width, cudaStream_t stream);
 
 // out[i * vocab + v] = log1pf(fp32 bits vmax[i * vpad + v]) for v < vocab: SPLADE's log(1 + relu) applied once per (item, word)
-// after the max (both are monotone).  `out` may be peer memory.
+// after the max (both are monotone).  1 <= n_items <= 65535 (the grid's y), 1 <= vocab <= vpad.  `out` may be peer memory.
 cudaError_t launch_splade_finalize(const uint32_t* vmax, float* out, int n_items, int vpad, int vocab, cudaStream_t stream);
 
 // final LayerNorm of the CLS row of every item + L2 normalise; row i is stored at out + i * width,
@@ -166,7 +170,7 @@ cudaError_t launch_mean_pool_normalize(const __half* yhi, const __half* ylo, con
 
 // ViT image tower (CLIP): pixels fp32 [n, 3, img, img] -> im2col A fp16 [n*T, 3 p p] (class-token rows zero); patch GEMM output +
 // class / position embeddings + pre_layrnorm -> residual stream + statistics; pooled head: post_layernorm(class token) ->
-// projection [P, 768] -> L2 normalise, stored at out + i * P (possibly peer memory).
+// projection [P, 768] -> L2 normalise, stored at out + i * P (possibly peer memory), 1 <= P <= 1024.
 cudaError_t launch_im2col(const float* pixels, __half* a, int n_items, int img, int p, cudaStream_t stream);
 cudaError_t launch_vit_embed(const __half* patch_out, const float* cls, const float* pos, const float* gamma, const float* beta,
                              __half* yhi, __half* ylo, float2* stats, int n_rows, int T, float eps, cudaStream_t stream);

@@ -19,7 +19,7 @@ EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RES_SPLIT, EPI_BIAS_QGELU_F16, EPI_SPL
 # ------------------------------------------------------------------------------------------------ GEMM
 
 def gemm(epi, N, K, stats_in, parts_in=6):
-    """launch_gemm -> launch_epi: (GEMM, EPI, BN, PARTS), or None.  `stats_in`: whether e.stats_in is non-NULL (parts_in is
+    """launch_gemm: (GEMM, EPI, BN, PARTS), or None.  `stats_in`: whether e.stats_in is non-NULL (parts_in is
     read only then)."""
     if epi not in (0, 1, 2, 3) or N % 128 or K % 64 or N < 128 or K < 64:
         return None
